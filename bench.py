@@ -2,14 +2,14 @@
 """bench.py -- frames/sec of the per-frame keypoint-voting hot path on synthetic 12288-pt RGB-D clouds.
 
     python bench.py [--gpus N] [--steps K] [--warmup W] [--impl reference] [--config linemod|ycb]
-                    [--ms-mode certified|early_exit|strict] [--quick]
+                    [--ms-mode certified|early_exit|strict] [--quick] [--dump-outputs DIR]
 
 Metric / config (BASELINE.json): frames/sec; headline workload = configs[1]: LineMOD-shape synthetic,
 12288 pts, 1 instance, 8 kps, batch 32 per GPU.  A step = one pass of hot path A (Pointnet2MSG.forward)
 + hot path B (cal_frame_poses_lm) over one batch.  N > 1 (launched by torchrun): every rank owns its
 own frames (weak scaling, frames sharded across ranks, no data-path collective) and a step ends with
 ONE NCCL all_gather of the poses.  Timing: CUDA events around exactly K steps, barrier + synchronize
-on both sides, max over ranks.  Inputs: 4 rotating device-resident batches (252 MB > the 126 MB L2).
+on both sides, max over ranks.  Inputs: 4 rotating device-resident batches (252 MB > the 50 MB L2).
 
 The ONE JSON line also carries (rank 0):
   e2e                 same metric through FramePipeline.run_host (pinned host in, H2D + D2H inside the
@@ -26,7 +26,9 @@ The ONE JSON line also carries (rank 0):
   stock_gpu_baseline  the UNMODIFIED reference on this GPU: reference `_ext` (oracle/_ref/_ext.so) under the
                       reference Pointnet2MSG + reference cal_frame_poses_lm / MeanShiftTorch on CUDA tensors
 `--impl reference` times the CPU implementation of the same path (oracle port; the reference's
-PointNet++ ops have no CPU path and /root/reference is absent on the GPU box) on the host cores.
+PointNet++ ops have no CPU path) on the host cores.
+`--dump-outputs DIR` writes the outputs of the last timed step (rank 0): poses, present and a seeded sample of
+the point features, as .npy; the inputs are seeded, so two builds can be compared output for output.
 """
 from __future__ import annotations
 
@@ -66,7 +68,7 @@ def load_peaks():
             return float(json.load(open(p))["hbm_gbs"]), "measured"
         except Exception:
             pass
-    return 6650.0, "fallback (B200_PROFILING.md copy bandwidth)"
+    return 3350.0, "fallback (H100 SXM data sheet HBM3 bandwidth)"
 
 
 class ClockSampler:
@@ -305,11 +307,14 @@ class Runner:
         self.rot_bytes = sum(v.numel() * v.element_size() for v in self.dev_rot[0].values()) * n_rot
         self.gather_buf = (torch.empty((world * B * self.pipe.n_cls * 12,), dtype=torch.float32, device=dev)
                            if world > 1 else None)
+        self.last = None           # (poses, present) of the latest step_device call
+        self.last_outputs = None   # host copies of the last timed device step (measure(..., keep_outputs=True))
 
     def step_device(self, i):
         d = self.dev_rot[i % self.n_rot]
         nxt = self.dev_rot[(i + 1) % self.n_rot]["cld_rgb_nrm"] if self.lookahead else None
-        poses, _ = self.pipe.run_device(d["cld_rgb_nrm"], d["pcld"], d["labels"], d["ctr_of"], d["kp_of"], next_cloud=nxt)
+        self.last = self.pipe.run_device(d["cld_rgb_nrm"], d["pcld"], d["labels"], d["ctr_of"], d["kp_of"], next_cloud=nxt)
+        poses = self.last[0]
         if self.world > 1:   # the single collective of the path: ~1.5 kB per frame
             self.torch.distributed.all_gather_into_tensor(self.gather_buf, poses.reshape(-1))
 
@@ -338,7 +343,16 @@ class Runner:
         ms = e0.elapsed_time(e1)
         return pdist.max_over_ranks(ms, self.dev), (lib.pvn3d_launch_count() - l0 if lib is not None else 0)
 
-    def measure(self, steps, warmup, lib, e2e=True, clocks=True):
+    def outputs(self, n_sample=2048):
+        """host copies of what the last step_device call returned, plus a seeded sample of its point features"""
+        poses, present = self.last
+        feats = self.pipe.features
+        pts = np.sort(np.random.default_rng(0).choice(feats.size(-1), size=min(n_sample, feats.size(-1)), replace=False))
+        return {"poses": poses.float().cpu().numpy(), "present": present.float().cpu().numpy(),
+                "features_sample": feats[..., self.torch.from_numpy(pts).to(feats.device)].float().cpu().numpy(),
+                "features_sample_points": pts.astype(np.float64)}
+
+    def measure(self, steps, warmup, lib, e2e=True, clocks=True, keep_outputs=False):
         # W untimed steps of exactly the loop that is timed next (indices -W..-1, so that the look-ahead of the
         # last warm-up step names the first timed batch), then K timed steps; first the device-resident loop,
         # then the same for the host loop
@@ -346,6 +360,8 @@ class Runner:
             self.step_device(i)
         sampler = ClockSampler(self.dev.index or 0).start() if (clocks and self.rank == 0) else None
         ms_dev, launches = self.timed(self.step_device, steps, lib)
+        if keep_outputs:
+            self.last_outputs = self.outputs()
         ms_e2e = None
         if e2e:
             for i in range(-warmup, 0):
@@ -459,9 +475,6 @@ def roofline_query_group(torch, _ext, dev, B, cloud, peak, peak_kind):
                       "of a level per call: 4 calls of one batch)",
             "on_timed_step": False, "where": "module-graph API (QueryAndGroup.forward); the fused step never writes the grouped tensor",
             "bound": "hbm", "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak, "peak_kind": peak_kind,
-            # dram bytes of the same four calls (8 kernels) from one `ncu --set full` capture (profiles/ncu_qgsplit_r01u.md,
-            # kernels unchanged since): below the algorithmic bytes -- the descriptor tables are L2 hits
-            "traffic": 2005.4 if B == 32 else None, "traffic_unit": "MB per batch (ncu, profiles/ncu_qgsplit_r01u.md)",
             "algorithmic_MB_per_batch": total_bytes / 1e6, "us_per_batch": total_ms * 1e3, "per_launch": per}
 
 
@@ -498,7 +511,7 @@ def stock_gpu_baseline(torch, runner, dev):
     ref_ext = load_ref_ext()
     ref = load_reference_python()
     if ref_ext is None or ref is None:
-        return {"unavailable": "oracle/_ref/_ext.so or oracle/_ref/py missing (built where /root/reference exists)"}
+        return {"unavailable": "oracle/_ref/_ext.so or oracle/_ref/py missing (built where a reference checkout exists)"}
     from pvn3d_b200 import _ext as our_ext, testing
 
     d = runner.dev_rot[0]
@@ -524,7 +537,7 @@ def stock_gpu_baseline(torch, runner, dev):
     ms_step = ms_a + B * s_b * 1e3
     return {"value": B / (ms_step * 1e-3), "unit": "frames/s", "ms_per_step": ms_step,
             "path_a_ms_per_batch": ms_a, "path_b_s_per_frame": s_b,
-            "what": "UNMODIFIED reference: reference _ext kernels (compiled -O2 for sm_100a) + cuDNN (TF32 allowed, torch default) "
+            "what": "UNMODIFIED reference: reference _ext kernels (compiled -O2 for sm_90a) + cuDNN (TF32 allowed, torch default) "
                     "under the reference Pointnet2MSG on the whole batch; reference cal_frame_poses_lm + MeanShiftTorch on CUDA "
                     "tensors, one complete frame timed (wall clock around a synchronised call) and scaled by the batch size"}
 
@@ -545,7 +558,11 @@ def b200_arm(args, json_out):
 
     la = not args.no_lookahead
     run = Runner(torch, cfg, dev, rank, world, args.ms_mode, overlap=overlap, engine=args.engine, lookahead=la)
-    head = run.measure(args.steps, args.warmup, lib)
+    head = run.measure(args.steps, args.warmup, lib, keep_outputs=bool(args.dump_outputs) and rank == 0)
+    if run.last_outputs is not None:
+        os.makedirs(args.dump_outputs, exist_ok=True)
+        for name, arr in run.last_outputs.items():
+            np.save(os.path.join(args.dump_outputs, f"{name}.npy"), arr)
     B = run.B
     line = None
     if rank == 0:
@@ -555,7 +572,7 @@ def b200_arm(args, json_out):
                 "config": {"workload": workload_name(cfg), "n_points": cfg["n_points"], "global_batch": B * world,
                            "parallelism": (f"frame-sharded x{world}, one NCCL all_gather of poses per step" if world > 1 else "1 GPU"),
                            "l2": f"{run.n_rot} rotating device-resident input batches ({run.rot_bytes / 1e6:.0f} MB) > L2",
-                           "mlp": ("tcgen05.mma kind::tf32 shared-MLP layers, grouping/interpolation fused into the operand producer"
+                           "mlp": ("wgmma tf32 shared-MLP layers, grouping/interpolation fused into the operand producer"
                                    if args.engine == "fused" else "cuDNN/cuBLAS 1x1 conv (TF32 allowed, the reference's torch default)"),
                            "meanshift": {"certified": "certified (headline): returned seed + witness seeds, provably within 1e-5*bandwidth of "
                                                       "the reference's centre; iteration count not computed (include/pvn3d_b200.h)",
@@ -602,10 +619,6 @@ def b200_arm(args, json_out):
                                   "gather + second layer, third layer + max-pool), 4 FP modules, the last one storing [B,128,N] directly) + factor tables",
                         "on_timed_step": True, "bound": "hbm", "achieved": MLP_IO_BYTES * B / t_mlp / 1e6, "peak": peak,
                         "unit": "GB/s", "frac": MLP_IO_BYTES * B / t_mlp / 1e6 / peak, "peak_kind": peak_kind,
-                        # dram__bytes_read.sum + dram__bytes_write.sum over the 33 launches of one batch, `ncu --set full`
-                        # (profiles/ncu_mlp_r02c.md): 1.5x the algorithmic bytes -- the second-layer activations
-                        "traffic": 4964.1 if (B == 32 and cfg["shape"] == "linemod" and run.pipe.fused.factor) else None,
-                        "traffic_unit": "MB per batch (ncu, profiles/ncu_mlp_r02c.md)",
                         "ms_per_batch": t_mlp, "algorithmic_MB_per_batch": MLP_IO_BYTES * B / 1e6,
                         "useful_TFLOPs": MLP_FLOPS * B / t_mlp / 1e9,
                         "note": "algorithmic bytes = SURVEY 8d MLP stage I/O with every SharedMLP(+max-pool) fused (100.2 MB/frame); "
@@ -630,8 +643,8 @@ def b200_arm(args, json_out):
             run.set_mode("early_exit")
             ms_b_early = run.path_b_ms()
             run.set_mode(args.ms_mode)
-            sm_clock = (head["clocks"] or {}).get("sm_mhz") or 1965.0
-            mufu_peak = 148 * 16 * sm_clock * 1e6
+            sm_clock = (head["clocks"] or {}).get("sm_mhz") or (head["clocks"] or {}).get("sm_max_mhz") or 1980.0
+            mufu_peak = torch.cuda.get_device_properties(dev).multi_processor_count * 16 * sm_clock * 1e6
             rooflines.append({"kernel": "ms_iterate_kernel + ms_density_kernel, strict mode (all seeds, reference iteration counts)",
                               "on_timed_step": args.ms_mode == "strict", "bound": "mufu (16 ex2/clk/SM)",
                               "pair_evaluations_per_batch": pairs, "ms_per_batch_path_b": ms_b_strict,
@@ -734,7 +747,9 @@ def main():
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--quick", action="store_true", help="headline + stage split only (development runs, ncu)")
     ap.add_argument("--engine", default="fused", choices=["fused", "modules"],
-                    help="hot path A: fused tcgen05 engine (default) or module graph with cuDNN/cuBLAS MLPs")
+                    help="hot path A: fused wgmma engine (default) or module graph with cuDNN/cuBLAS MLPs")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the outputs of the last timed step as DIR/<name>.npy (see the module docstring)")
     args = ap.parse_args()
     # stdout carries exactly ONE line (the JSON): everything any library prints to fd 1 from here on
     # (NCCL prints its version there) goes to stderr; the JSON is written to the saved descriptor

@@ -1,5 +1,5 @@
 /*
- * pvn3d_b200.h -- C ABI of libpvn3d_b200.so (hand-written sm_100a kernels).
+ * pvn3d_b200.h -- C ABI of libpvn3d_b200.so (hand-written sm_90a kernels).
  *
  * This is the drop-in boundary of the PVN3D per-frame keypoint-voting hot path:
  *   Boundary 1  the nine PointNet++ ops the reference exports from its pybind11 module
@@ -143,14 +143,14 @@ int pvn3d_three_nn_interpolate(const float *unknown, const float *known, const f
                                float *dist2, int *idx, pvn3d_stream_t stream);
 
 /* ------------------------------------------------------------------------------------------
- * Shared-MLP layers of set abstraction / feature propagation on the tcgen05 tensor cores
+ * Shared-MLP layers of set abstraction / feature propagation on the Hopper tensor cores (wgmma)
  * (reference: SharedMLP = Conv2d 1x1 (no bias) + BatchNorm2d + ReLU, pytorch_utils.py:25-50, and the
  * max-pool over nsample of pointnet2_modules.py:64-67).  One call = one layer:
  *      out[p, col0 + 0:n_pad] = act( A[p, 0:k_pad] . W^T + bias ),   optionally max over `pool` rows
  *   w    [n_pad, k_pad] f32, BN folded into rows, values rounded to TF32, zero padded
  *        (k_pad multiple of 32, n_pad multiple of 16); bias [n_pad] (folded BN shift, 0 in the pad)
  *   out  point-major rows of length ldo (ldo, col0 multiples of 4); pool in {0, 8, 16, 32}
- * Arithmetic: TF32 operands (round-to-nearest), fp32 accumulation in TMEM.
+ * Arithmetic: TF32 operands (round-to-nearest), fp32 accumulation.
  * flags: PVN3D_MLP_RELU       apply ReLU (flags = 1 / 0 is the plain relu switch)
  *        PVN3D_MLP_ROUND_OUT  store the activations (pooled or not) already rounded to TF32
  *        PVN3D_MLP_A_TF32     (mlp_dense) `a` / (mlp_sa_first) `feat_pm` was produced with ROUND_OUT and is

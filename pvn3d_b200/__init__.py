@@ -1,4 +1,4 @@
-"""pvn3d_b200 -- B200-native (sm_100a) implementation of PVN3D's per-frame keypoint-voting hot path.
+"""pvn3d_b200 -- H100-native (sm_90a) implementation of PVN3D's per-frame keypoint-voting hot path.
 
   _ext            drop-in for the reference's `lib.pointnet2_utils._ext` (9 PointNet++ ops)
   pointnet2       host-side mirror of pointnet2_utils / pointnet2_modules / Pointnet2MSG

@@ -2,7 +2,7 @@
 
 Same nine functions, argument order, dtypes, output allocation and error text as
 pvn3d/_ext-src/src/bindings.cpp:6-19 and the host wrappers in pvn3d/_ext-src/src/*.cpp, but every
-call lands in a hand-written sm_100a kernel of libpvn3d_b200.so through the C ABI
+call lands in a hand-written sm_90a kernel of libpvn3d_b200.so through the C ABI
 (include/pvn3d_b200.h).  Install it with `pvn3d_b200.compat.install()` and the reference's
 `pointnet2_utils.py` / `pointnet2_modules.py` / `demo.py` / `train_*.py` run on it unchanged.
 

@@ -109,7 +109,7 @@ def load() -> ctypes.CDLL:
         return _lib
     if not os.path.exists(LIB_PATH):
         raise Pvn3dError(
-            f"{LIB_PATH} not found: the sm_100a kernel library is not built "
+            f"{LIB_PATH} not found: the sm_90a kernel library is not built "
             "(run `python -m pvn3d_b200.build`); pvn3d_b200 has no CPU / PyTorch fallback")
     try:
         lib = ctypes.CDLL(LIB_PATH)

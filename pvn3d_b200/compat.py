@@ -5,7 +5,7 @@
 
 What install() does (SURVEY section 8b, App. D):
   1. registers pvn3d_b200._ext as `lib.pointnet2_utils._ext`, so the reference's
-     pointnet2_utils.py:19 (`from lib.pointnet2_utils import _ext`) binds the sm_100a kernels;
+     pointnet2_utils.py:19 (`from lib.pointnet2_utils import _ext`) binds the sm_90a kernels;
   2. adds the small import shims the 2019 code needs on torch 2.x / PyYAML 6 (`torch._six`,
      `yaml.load` default Loader, empty `neupeak.utils.webcv2`, `plyfile`, `pcl` modules);
   3. with patch_post=True, after the reference modules are imported, rebinds
@@ -82,7 +82,7 @@ def install(reference_root: str | None = None, patch_post: bool = False) -> None
 
 
 def patch_post_modules(import_missing: bool = False) -> None:
-    """Rebind the reference's post-processing entry points to the B200 implementations."""
+    """Rebind the reference's post-processing entry points to the implementations of this package."""
     from . import eval_utils, meanshift
 
     targets = {

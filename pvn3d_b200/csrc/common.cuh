@@ -1,4 +1,4 @@
-// common.cuh -- shared helpers for the sm_100a kernels of libpvn3d_b200.so
+// common.cuh -- shared helpers for the sm_90a kernels of libpvn3d_b200.so
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -87,6 +87,17 @@ __device__ __forceinline__ float ref_sqdist(float dx, float dy, float dz) {
 // mean-shift path.
 __device__ __forceinline__ float torch_sqnorm(float dx, float dy, float dz) {
   return __fmaf_rn(dz, dz, __fmaf_rn(dy, dy, __fmul_rn(dx, dx)));
+}
+
+// float2 arithmetic, one correctly rounded fp32 operation per component (same bits as the scalar forms)
+__device__ __forceinline__ float2 f2_add(float2 a, float2 b) {
+  return make_float2(__fadd_rn(a.x, b.x), __fadd_rn(a.y, b.y));
+}
+__device__ __forceinline__ float2 f2_mul(float2 a, float2 b) {
+  return make_float2(__fmul_rn(a.x, b.x), __fmul_rn(a.y, b.y));
+}
+__device__ __forceinline__ float2 f2_fma(float2 a, float2 b, float2 c) {
+  return make_float2(__fmaf_rn(a.x, b.x, c.x), __fmaf_rn(a.y, b.y, c.y));
 }
 
 __device__ __forceinline__ unsigned lane_id() { return threadIdx.x & 31u; }

@@ -1,4 +1,4 @@
-// fps.cu -- furthest point sampling for sm_100a.
+// fps.cu -- furthest point sampling for sm_90a.
 //
 // Replaces furthest_point_sampling (reference pvn3d/_ext-src/src/sampling.cpp:65-86 and
 // sampling_gpu.cu:69-229).  Same result bit for bit, different machine mapping:

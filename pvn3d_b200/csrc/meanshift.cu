@@ -1,4 +1,4 @@
-// meanshift.cu -- batched Gaussian mean-shift vote clustering for sm_100a.
+// meanshift.cu -- batched Gaussian mean-shift vote clustering for sm_90a.
 //
 // Replaces MeanShiftTorch.fit (reference pvn3d/lib/utils/meanshift_pytorch.py:13-51), which per
 // iteration materialises four [n,n,3] float32 tensors with ~10 torch kernels and one host sync,
@@ -165,10 +165,9 @@ __global__ void __launch_bounds__(1024) ms_setup_kernel(MsArgs a) {
 
 // ------------------------------------------------------------------------------------------------
 // exact density pass: one thread per input point, all points of the fit swept from shared memory.
-// The tile holds point PAIRS (x0,x1,y0,y1 | z0,z1) so that the distance of one seed to two points is
-// three FADD2 + FMUL2 + two FFMA2 on the packed fp32 pipe: per lane these are the same IEEE operations in
-// the same order as torch_sqnorm (fma(dz,dz, fma(dy,dy, dx*dx)) on p - me), so counts stay bit-exact, at
-// 6 instead of 9 issue slots per pair test.
+// The tile holds point PAIRS (x0,x1,y0,y1 | z0,z1) so that the distance of one seed to two points comes
+// from one 16-byte and one 8-byte shared load; per component the arithmetic is the same IEEE operations in
+// the same order as torch_sqnorm (fma(dz,dz, fma(dy,dy, dx*dx)) on p - me), so counts stay bit-exact.
 __global__ void __launch_bounds__(kMsThreads) ms_density_kernel(MsArgs a) {
   __shared__ float4 s_xy[kMsDensTile / 2];   // (x0, x1, y0, y1)
   __shared__ float2 s_z[kMsDensTile / 2];    // (z0, z1)
@@ -202,10 +201,10 @@ __global__ void __launch_bounds__(kMsThreads) ms_density_kernel(MsArgs a) {
       const float4 xy = s_xy[j];
       const float2 z = s_z[j];
       // dis = torch.norm(Ar - Cr): diff = A_j - A_i   (meanshift_pytorch.py:46-48)
-      const float2 dx = __fadd2_rn(make_float2(xy.x, xy.y), nx);
-      const float2 dy = __fadd2_rn(make_float2(xy.z, xy.w), ny);
-      const float2 dz = __fadd2_rn(z, nz);
-      const float2 d2 = __ffma2_rn(dz, dz, __ffma2_rn(dy, dy, __fmul2_rn(dx, dx)));
+      const float2 dx = f2_add(make_float2(xy.x, xy.y), nx);
+      const float2 dy = f2_add(make_float2(xy.z, xy.w), ny);
+      const float2 dz = f2_add(z, nz);
+      const float2 d2 = f2_fma(dz, dz, f2_fma(dy, dy, f2_mul(dx, dx)));
       count += (d2.x < t2 ? 1 : 0) + (d2.y < t2 ? 1 : 0);
     }
   }
@@ -500,9 +499,7 @@ __device__ __forceinline__ int ms_phase_end(int p) {  // last iteration of phase
 // Shared-memory layout of a fit's points: point PAIRS, structure-of-arrays inside the pair
 //   s_pts[p] = (x0, x1, y0, y1)      s_pts[kMsPairs + p] = (z0, z1, w0, w1)       w = k |a'|^2
 // (two planes, so that a warp whose lanes read CONSECUTIVE pairs touches every bank once)
-// so that the sweep runs on the packed FP32 pipe (FFMA2 / FADD2: two points per instruction):
-// per point pair and seed 4 packed ops for the exponents, 2 MUFU.EX2, 4 packed ops to accumulate --
-// 5 issue slots per pair evaluation instead of 9.  An odd tail is padded with w = -inf (weight 0).
+// so that the sweep reads two points per pair of shared loads.  An odd tail is padded with w = -inf (weight 0).
 __device__ __forceinline__ void ms_stage_pairs(float4 *s_pts, const float4 *__restrict__ cpts, int n) {
   const int npairs = (n + 1) >> 1;
   for (int q = threadIdx.x; q < npairs; q += kMsThreads) {
@@ -530,12 +527,12 @@ __device__ __forceinline__ MsSeedQ ms_seed_q(float k, float cx, float cy, float 
 __device__ __forceinline__ void ms_pair_step(const float4 &A, const float4 &B, const MsSeedQ &q, MsSeedS &s) {
   const float2 x2 = make_float2(A.x, A.y), y2 = make_float2(A.z, A.w), z2 = make_float2(B.x, B.y),
                w2 = make_float2(B.z, B.w);
-  const float2 e = __ffma2_rn(x2, q.qx, __ffma2_rn(y2, q.qy, __ffma2_rn(z2, q.qz, __fadd2_rn(w2, q.qw))));
+  const float2 e = f2_fma(x2, q.qx, f2_fma(y2, q.qy, f2_fma(z2, q.qz, f2_add(w2, q.qw))));
   const float2 w = make_float2(ex2_approx(e.x), ex2_approx(e.y));
-  s.sw = __fadd2_rn(s.sw, w);
-  s.sx = __ffma2_rn(w, x2, s.sx);
-  s.sy = __ffma2_rn(w, y2, s.sy);
-  s.sz = __ffma2_rn(w, z2, s.sz);
+  s.sw = f2_add(s.sw, w);
+  s.sx = f2_fma(w, x2, s.sx);
+  s.sy = f2_fma(w, y2, s.sy);
+  s.sz = f2_fma(w, z2, s.sz);
 }
 
 template <int R>

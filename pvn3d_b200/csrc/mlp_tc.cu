@@ -1,6 +1,6 @@
-// mlp_tc.cu -- the shared-MLP contractions of set abstraction / feature propagation on the 5th-gen
-// tensor cores (tcgen05.mma kind::tf32, accumulators in TMEM), with the PointNet++ data movement fused
-// into the operand producer and the activation / max-pool fused into the epilogue.
+// mlp_tc.cu -- the shared-MLP contractions of set abstraction / feature propagation on the Hopper
+// tensor cores (wgmma.mma_async tf32, fp32 accumulators in registers), with the PointNet++ data movement
+// fused into the operand producer and the activation / max-pool fused into the epilogue.
 //
 // Replaces, per SharedMLP layer of the reference (pytorch_utils.py:25-50: Conv2d 1x1 (no bias) ->
 // BatchNorm2d -> ReLU, plus F.max_pool2d over nsample at pointnet2_modules.py:64-67): one cuDNN conv,
@@ -17,14 +17,15 @@
 //   FP_INTERP  row (b,j): [ sum_t w_t * known_feat_pm[b, idx_t, 0:C2] | skip[b, j, 0:C1] | 0 ... ]
 //              (three_interpolate + torch.cat of PointnetFPModule.forward, pointnet2_modules.py:188-199)
 // Operands are staged in shared memory in the canonical K-major SWIZZLE_128B layout (32 fp32 = 128 B
-// per row per stage; weights and pre-rounded activations arrive by cp.async), one elected thread of
-// warp 12 issues tcgen05.mma (M=128, N<=256, K=8 per instruction) into one of two TMEM accumulators
-// and releases stages with tcgen05.commit; the kernel is persistent (one CTA per SM, tiles strided),
-// so staging of tile j+1 and the epilogue of tile j-1 overlap the MMAs of tile j.  The epilogue warps
-// (0-3) read the accumulator with
-// tcgen05.ld (32x32b), add the folded-BN bias, apply ReLU and either store the point-major row or
-// reduce over the nsample rows of each centre with a transposing shuffle butterfly (max-pool) and
-// store one 128-byte line per centre.
+// per row per stage; weights arrive by TMA, pre-rounded activations by cp.async).  Two MMA warpgroups
+// (warps 12-19) each issue wgmma m64nNk8 (N = 16, 32, 64 or 128 columns per tile) for one 64-row half
+// of the tile, keep the accumulator in registers, release stages once wgmma.wait_group has retired the
+// MMAs that read them, and hand each finished tile to the epilogue through a swizzled shared-memory
+// accumulator tile; the kernel is persistent (one CTA per SM, tiles strided), so staging of tile j+1
+// and the epilogue of tile j-1 overlap the MMAs of tile j.  The epilogue warps (0-3) read the
+// accumulator tile one row per thread, add the folded-BN bias, apply ReLU and either store the
+// point-major row or reduce over the nsample rows of each centre with a transposing shuffle butterfly
+// (max-pool) and store one 128-byte line per centre.
 //
 // TF32: operands are rounded to nearest (cvt.rna.tf32.f32) when staged, accumulation is fp32 -- the
 // precision class of the reference's default cuDNN convolutions (torch.backends.cudnn.allow_tf32).
@@ -36,17 +37,19 @@ namespace pvn3d {
 namespace {
 
 constexpr int kMlpBM = 128;
-constexpr int kMlpEpiWarps = 4;  // warps 0-3: epilogue (warp w owns TMEM lanes 32w..32w+31)
+constexpr int kMlpEpiWarps = 4;  // warps 0-3: epilogue (warp w drains rows 32w..32w+31 of the accumulator tile)
 constexpr int kMlpProWarps = 8;  // warps 4-11: two producer groups of 128 threads, alternate K chunks
-constexpr int kMlpThreads = (kMlpEpiWarps + kMlpProWarps + 1) * 32;  // warp 12: TMEM owner + MMA issuer
+constexpr int kMlpMmaWarps = 8;  // warps 12-19: two MMA warpgroups, rows 0-63 / 64-127 of the tile
+constexpr int kMlpThreads = (kMlpEpiWarps + kMlpProWarps + kMlpMmaWarps) * 32;
 constexpr int kMlpMaxStages = 6;
+constexpr int kMlpSmemMax = 227 * 1024;  // dynamic shared memory a block may opt into on sm_90
 
 enum : int { PRO_DENSE = 0, PRO_SA_GATHER = 1, PRO_FP_INTERP = 2, PRO_SA_FACT = 3, PRO_FP_FACT = 4 };
 enum : int { EPI_STORE = 0, EPI_MAXPOOL = 1, EPI_SUMPOOL = 2, EPI_MAXPOOL_T = 3, EPI_STORE_T = 4 };
 
 struct MlpArgs {
   // W as a TMA tensor map ([n_pad][k_pad] fp32, box 32 columns x bn rows, SWIZZLE_128B): one
-  // cp.async.bulk.tensor.2d per K chunk lands the B operand in the UMMA layout (use_tma, else cp.async)
+  // cp.async.bulk.tensor.2d per K chunk lands the B operand in the wgmma layout (use_tma, else cp.async)
   alignas(64) CUtensorMap tmap;
   int use_tma;
   // GEMM
@@ -55,11 +58,9 @@ struct MlpArgs {
   long long rows;     // P
   int k_pad;          // multiple of 32
   int n_pad;          // multiple of 16
-  int bn;             // columns per tile (multiple of 16, <= 256)
+  int bn;             // columns per tile = wgmma N: 16, 32, 64 or 128 (the last tile of a row may be partial)
   int stages;
-  int tmem_cols;      // power of two >= max(32, bn); acc_bufs accumulators are allocated
-  int acc_bufs;       // 2: the epilogue of tile j overlaps the MMAs of tile j+1; 1: wide tiles (tmem_cols = 256) of two
-                      // co-resident CTAs -- the other CTA's MMAs fill the gap
+  int acc_ld;         // floats per row of the shared-memory accumulator tile: max(32, bn)
   // DENSE
   const float *a;
   int lda;
@@ -89,12 +90,6 @@ __device__ __forceinline__ void mbar_arrive(uint64_t *bar) {
 }
 __device__ __forceinline__ void fence_proxy_async_smem() {
   asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-}
-__device__ __forceinline__ void tc_fence_before() {
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-}
-__device__ __forceinline__ void tc_fence_after() {
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
 }
 __device__ __forceinline__ float to_tf32(float x) {
   uint32_t r;
@@ -137,71 +132,106 @@ __device__ __forceinline__ void tma_load_2d(uint32_t dst_smem, const CUtensorMap
       "l"(reinterpret_cast<uint64_t>(map)), "r"(x), "r"(y), "r"(smem_u32(bar))
       : "memory");
 }
-__device__ __forceinline__ void umma_tf32(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc,
-                                          uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t"
-      "}\n" ::"r"(tmem_d),
-      "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
+// ---- wgmma (warpgroup MMA) ----------------------------------------------------------------------------
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() {
+  asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory");
 }
-__device__ __forceinline__ void umma_commit(uint64_t *bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(
-                   smem_u32(bar))
-               : "memory");
+// keeps the compiler from moving accesses of the accumulator registers across an asynchronous MMA
+template <int R>
+__device__ __forceinline__ void acc_fence(float (&d)[R]) {
+#pragma unroll
+  for (int i = 0; i < R; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
-// 32 lanes x 32 columns of fp32: thread i of the warp gets row (lane base + i), columns c..c+31
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, float (&v)[32]) {
-  uint32_t r[32];
+// D[64 x N] (+)= A[64 x 8] . B[N x 8]^T, both operands K-major in shared memory, fp32 accumulate.
+// Accumulator fragment: thread (warp w of the warpgroup, lane l) holds in d[4j + e] the element
+// row 16w + l/4 + 8 (e >> 1), column 8j + 2 (l % 4) + (e & 1).
+template <int N>
+__device__ __forceinline__ void wgmma_tf32(float (&d)[N / 2], uint64_t adesc, uint64_t bdesc, uint32_t accumulate);
+template <>
+__device__ __forceinline__ void wgmma_tf32<16>(float (&d)[8], uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
   asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,"
-      "%26,%27,%28,%29,%30,%31}, [%32];\n"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-        "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]),
-        "=r"(r[15]), "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]),
-        "=r"(r[22]), "=r"(r[23]), "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]),
-        "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr));
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-#pragma unroll
-  for (int i = 0; i < 32; ++i) v[i] = __uint_as_float(r[i]);
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %10, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n16k8.f32.tf32.tf32 {%0,%1,%2,%3,%4,%5,%6,%7}, %8, %9, p, 1, 1;\n\t}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
+      : "l"(adesc), "l"(bdesc), "r"(accumulate));
 }
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, float (&v)[32]) {
-  uint32_t r[16];
+template <>
+__device__ __forceinline__ void wgmma_tf32<32>(float (&d)[16], uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
   asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-      "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];\n"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-        "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]),
-        "=r"(r[15])
-      : "r"(taddr));
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-#pragma unroll
-  for (int i = 0; i < 16; ++i) v[i] = __uint_as_float(r[i]);
-#pragma unroll
-  for (int i = 16; i < 32; ++i) v[i] = 0.f;
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %18, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n32k8.f32.tf32.tf32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, %16, %17, p, 1, 1;\n\t}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+      : "l"(adesc), "l"(bdesc), "r"(accumulate));
+}
+template <>
+__device__ __forceinline__ void wgmma_tf32<64>(float (&d)[32], uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n64k8.f32.tf32.tf32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, %32, %33, p, 1, 1;\n\t}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "l"(adesc), "l"(bdesc), "r"(accumulate));
+}
+template <>
+__device__ __forceinline__ void wgmma_tf32<128>(float (&d)[64], uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n128k8.f32.tf32.tf32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47,%48,%49,%50,%51,%52,%53,%54,%55,%56,%57,%58,%59,%60,%61,%62,%63}, %64, %65, p, 1, 1;\n\t}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "l"(adesc), "l"(bdesc), "r"(accumulate));
 }
 
-// K-major SWIZZLE_128B shared-memory matrix descriptor (cute::UMMA::SmemDescriptor): start >> 4,
-// LBO = 1 (unused for swizzled K-major), SBO = 1024 B (8 rows x 128 B), version 1, layout 2 (SW128).
+// K-major SWIZZLE_128B shared-memory matrix descriptor of wgmma: start >> 4, LBO = 1 (unused for
+// swizzled K-major), SBO = 1024 B (8 rows x 128 B), layout type 1 (128-byte swizzle) in bits 62-63.
 __device__ __forceinline__ uint64_t smem_desc_sw128(uint32_t saddr) {
   uint64_t d = 0;
   d |= static_cast<uint64_t>((saddr & 0x3FFFFu) >> 4);
   d |= static_cast<uint64_t>(1) << 16;
   d |= static_cast<uint64_t>(1024 >> 4) << 32;
-  d |= static_cast<uint64_t>(1) << 46;
-  d |= static_cast<uint64_t>(2) << 61;
+  d |= static_cast<uint64_t>(1) << 62;
   return d;
 }
-// cute::UMMA::InstrDescriptor for kind::tf32, fp32 accumulate, A and B K-major, M = 128
-__device__ __forceinline__ uint32_t instr_desc_tf32(int n) {
-  return (1u << 4) | (2u << 7) | (2u << 10) | (static_cast<uint32_t>(n >> 3) << 17) |
-         (static_cast<uint32_t>(kMlpBM >> 4) << 24);
+
+// ---- shared-memory accumulator tile: 128 rows x acc_ld floats (acc_ld a multiple of 32), the 16-byte
+// chunks of every 128-byte line XOR-swizzled by row & 7 so that a thread per row (epilogue), a thread
+// per column (transposed epilogues) and the wgmma fragment stores all run without bank conflicts
+__device__ __forceinline__ uint32_t acc_off(int r, int c, int ld) {
+  return static_cast<uint32_t>(r * ld * 4 + ((c >> 5) << 7) + ((((c >> 2) & 7) ^ (r & 7)) << 4) + (c & 3) * 4);
 }
+// the warpgroup's 64 x N fragment into rows 64 wg.. of the tile (frag_row = 64 wg + 16 (warp & 3) + lane / 4)
+template <int N>
+__device__ __forceinline__ void acc_store(uint32_t acc_s, int ld, int frag_row, unsigned lane, const float (&d)[N / 2]) {
+#pragma unroll
+  for (int j = 0; j < N / 8; ++j) {
+    const int c = 8 * j + 2 * static_cast<int>(lane & 3u);
+    asm volatile("st.shared.v2.f32 [%0], {%1,%2};" ::"r"(acc_s + acc_off(frag_row, c, ld)), "f"(d[4 * j]), "f"(d[4 * j + 1])
+                 : "memory");
+    asm volatile("st.shared.v2.f32 [%0], {%1,%2};" ::"r"(acc_s + acc_off(frag_row + 8, c, ld)), "f"(d[4 * j + 2]),
+                 "f"(d[4 * j + 3])
+                 : "memory");
+  }
+}
+// row r, columns c0..c0+31 (c0 % 32 == 0); cols = 16: columns c0..c0+15, the rest reads as zero
+__device__ __forceinline__ void acc_ld_row(uint32_t acc_s, int ld, int r, int c0, int cols, float (&v)[32]) {
+#pragma unroll
+  for (int q = 0; q < 8; ++q) {
+    float4 x = make_float4(0.f, 0.f, 0.f, 0.f);
+    if (q < 4 || cols == 32) x = lds128(acc_s + acc_off(r, c0 + 4 * q, ld));
+    v[4 * q + 0] = x.x; v[4 * q + 1] = x.y; v[4 * q + 2] = x.z; v[4 * q + 3] = x.w;
+  }
+}
+// column c, rows r0..r0+31
+__device__ __forceinline__ void acc_ld_col(uint32_t acc_s, int ld, int r0, int c, float (&v)[32]) {
+#pragma unroll
+  for (int i = 0; i < 32; ++i)
+    asm volatile("ld.shared.f32 %0, [%1];" : "=f"(v[i]) : "r"(acc_s + acc_off(r0 + i, c, ld)));
+}
+
+// wgmma N for `n_pad` columns: the narrowest of 16 / 32 / 64 / 128 that covers them (wider layers: 128-column tiles;
+// the MMA of a ragged last tile uses the N of its own width)
+__host__ __device__ constexpr int mma_n(int n_pad) { return n_pad <= 16 ? 16 : n_pad <= 32 ? 32 : n_pad <= 64 ? 64 : 128; }
 
 // byte offset of 16-byte chunk `c` (0..7) of row `r` inside a [rows x 128 B] SWIZZLE_128B tile
 __device__ __forceinline__ uint32_t sw128_off(int r, int c) {
@@ -506,32 +536,90 @@ __device__ __forceinline__ void warp_colmax_8(float (&v)[32], unsigned lane) {
 
 struct MlpSmemCtl {
   uint64_t full[kMlpMaxStages];   // 128 arrivals: every producer thread of the filling group
-  uint64_t empty[kMlpMaxStages];  // 1 arrival: tcgen05.commit of the MMAs that read the stage
-  uint64_t acc_full[2];           // 1 arrival: tcgen05.commit after a tile's last MMA
-  uint64_t acc_empty[2];          // 128 arrivals: the epilogue threads, once they have read it
-  uint32_t tmem_base;
+  uint64_t empty[kMlpMaxStages];  // 8 arrivals: one per MMA warp, once its MMAs that read the stage have retired
+  uint64_t acc_full;              // 256 arrivals: the MMA threads, once their fragments are in the accumulator tile
+  uint64_t acc_empty;             // 128 arrivals: the epilogue threads, once they have read it
 };
+
+// bytes of shared memory in front of the epilogue staging: 1024-byte alignment slack, the operand ring and the
+// accumulator tile (the kernels and their launchers compute the layout with the same function)
+static inline __host__ __device__ uint32_t mlp_smem_front(int stages, int bn, int acc_ld) {
+  return 1024u + static_cast<uint32_t>(stages) * (kMlpBM * 128u + ((static_cast<uint32_t>(bn) * 128u + 1023u) & ~1023u)) +
+         kMlpBM * static_cast<uint32_t>(acc_ld) * 4u;
+}
+
+// One tile of the MMA role for one of the two warpgroups: all K chunks of the ring into register accumulators
+// (chunk kc is released once wgmma.wait_group has retired it, while chunk kc+1 runs), then the 64 x N fragment
+// into the accumulator tile as soon as the epilogue has drained the previous tile.
+template <int N>
+__device__ __forceinline__ void mma_tile(uint32_t ring, uint32_t stage_bytes, int S, long long it_base, int kc_total,
+                                         uint64_t *full, uint64_t *empty, uint64_t *acc_full, uint64_t *acc_empty,
+                                         unsigned acc_parity, uint32_t acc_s, int acc_ld, unsigned wg, int frag_row,
+                                         unsigned lane) {
+  float d[N / 2];
+#pragma unroll
+  for (int i = 0; i < N / 2; ++i) d[i] = 0.f;
+  int prev = -1;
+  for (int kc = 0; kc < kc_total; ++kc) {
+    const long long it = it_base + kc;
+    const int s = static_cast<int>(it % S);
+    mbar_wait(&full[s], static_cast<unsigned>((it / S) & 1));
+    fence_proxy_async_smem();  // cp.async / st.shared (generic proxy) data of the stage -> async proxy
+    const uint32_t sa = ring + static_cast<uint32_t>(s) * stage_bytes;
+    // this warpgroup's 64 rows of A start 64 x 128 B = 8 KB into the stage (a multiple of the 1 KB swizzle atom)
+    const uint64_t adesc = smem_desc_sw128(sa + wg * 8192u), bdesc = smem_desc_sw128(sa + kMlpBM * 128u);
+    wgmma_fence();
+#pragma unroll
+    for (int k4 = 0; k4 < 4; ++k4)  // K = 8 tf32 = 32 bytes per instruction: +2 in 16-byte units
+      wgmma_tf32<N>(d, adesc + static_cast<uint64_t>(k4 * 2), bdesc + static_cast<uint64_t>(k4 * 2),
+                    (kc > 0 || k4 > 0) ? 1u : 0u);
+    wgmma_commit();
+    if (prev >= 0) {
+      wgmma_wait<1>();
+      if (lane == 0) mbar_arrive(&empty[prev]);
+    }
+    prev = s;
+  }
+  wgmma_wait<0>();
+  acc_fence(d);
+  if (prev >= 0 && lane == 0) mbar_arrive(&empty[prev]);
+  mbar_wait(acc_empty, acc_parity ^ 1u);
+  acc_store<N>(acc_s, acc_ld, frag_row, lane, d);
+  mbar_arrive(acc_full);
+}
+
+#define MLP_MMA_TILE(N)                                                                                            \
+  mma_tile<N>(ring, stage_bytes, S, it_base, kc_total, full, empty, acc_full, acc_empty, acc_parity, acc_s, acc_ld, wg, \
+              frag_row, lane)
+__device__ __forceinline__ void mma_tile_n(int n, uint32_t ring, uint32_t stage_bytes, int S, long long it_base,
+                                           int kc_total, uint64_t *full, uint64_t *empty, uint64_t *acc_full,
+                                           uint64_t *acc_empty, unsigned acc_parity, uint32_t acc_s, int acc_ld,
+                                           unsigned wg, int frag_row, unsigned lane) {
+  if (n == 16) MLP_MMA_TILE(16);
+  else if (n == 32) MLP_MMA_TILE(32);
+  else if (n == 64) MLP_MMA_TILE(64);
+  else MLP_MMA_TILE(128);
+}
+#undef MLP_MMA_TILE
 
 // Persistent, warp-specialised: CTA c works on tiles c, c+grid, ... (tile = 128 rows x bn columns).
 //   producers  fill a ring of K-chunk stages (A: 128 rows x 128 B, B: bn rows x 128 B), running ahead
 //              of the tensor core across tile boundaries;
-//   warp 12    issues the MMAs of tile j into accumulator j&1 of TMEM;
-//   epilogue   drains accumulator j&1 while the MMAs of tile j+1 fill the other one.
-// OCC = CTAs per SM the kernel is compiled for.  The layers are latency-bound (gathers through L2, TMEM
-// round trips) at 13 warps per SM; two co-resident CTAs (<= 78 registers per thread, half the operand ring,
-// two accumulators of <= 128 TMEM columns each) double the loads in flight for the narrow layers.
-template <int PRO, int EPI, int OCC>
-__global__ void __launch_bounds__(kMlpThreads, OCC) mlp_layer_kernel(const __grid_constant__ MlpArgs a) {
-  // dynamic shared memory only, 1024-byte aligned: [operand ring: stages x stage_bytes][epilogue staging 4 x 4 KB]
-  // [barriers].  No static block and no alignment slack: two CTAs with 96 KB rings each fit one SM's 228 KB.
-  extern __shared__ __align__(1024) unsigned char mlp_smem_al[];
-  const uint32_t ring = smem_u32(mlp_smem_al);   // SWIZZLE_128B atoms are 8 rows x 128 B
-  if (ring & 1023u) __trap();
+//   MMA        two warpgroups accumulate tile j in registers (64 rows each) while the epilogue drains tile j-1
+//              from the shared-memory accumulator tile;
+//   epilogue   bias / ReLU / pooling / stores of the tile in the accumulator tile.
+template <int PRO, int EPI>
+__global__ void __launch_bounds__(kMlpThreads, 1) mlp_layer_kernel(const __grid_constant__ MlpArgs a) {
+  // dynamic shared memory only: [operand ring: stages x stage_bytes, 1024-byte aligned][accumulator tile
+  // 128 x acc_ld floats][epilogue staging 4 x 4 KB][barriers]
+  extern __shared__ unsigned char mlp_smem_raw[];
+  const uint32_t raw = smem_u32(mlp_smem_raw);
+  const uint32_t ring = (raw + 1023u) & ~1023u;   // SWIZZLE_128B atoms are 8 rows x 128 B
   const uint32_t a_bytes = kMlpBM * 128u;
   const uint32_t stage_bytes = a_bytes + ((static_cast<uint32_t>(a.bn) * 128u + 1023u) & ~1023u);
-  MlpSmemCtl &ctl = *reinterpret_cast<MlpSmemCtl *>(mlp_smem_al + static_cast<size_t>(a.stages) * stage_bytes +
-                                                    kMlpEpiWarps * 4096);
-  const unsigned nbuf = static_cast<unsigned>(a.acc_bufs);
+  const uint32_t acc_s = ring + static_cast<uint32_t>(a.stages) * stage_bytes;
+  const uint32_t front = mlp_smem_front(a.stages, a.bn, a.acc_ld);
+  MlpSmemCtl &ctl = *reinterpret_cast<MlpSmemCtl *>(mlp_smem_raw + front + kMlpEpiWarps * 4096);
 
   const int t = threadIdx.x;
   const unsigned warp = t >> 5, lane = t & 31u;
@@ -541,29 +629,16 @@ __global__ void __launch_bounds__(kMlpThreads, OCC) mlp_layer_kernel(const __gri
   const int n_blocks = (a.n_pad + a.bn - 1) / a.bn;
   const long long total_tiles = row_tiles * n_blocks;
 
-  if (warp == kMlpEpiWarps + kMlpProWarps) {
-    if (lane == 0) {
-      for (int s = 0; s < S; ++s) {
-        mbar_init(&ctl.full[s], 128);
-        mbar_init(&ctl.empty[s], 1);
-      }
-      for (int b = 0; b < 2; ++b) {
-        mbar_init(&ctl.acc_full[b], 1);
-        mbar_init(&ctl.acc_empty[b], 128);
-      }
-      mbar_fence_init();
+  if (t == 0) {
+    for (int s = 0; s < S; ++s) {
+      mbar_init(&ctl.full[s], 128);
+      mbar_init(&ctl.empty[s], kMlpMmaWarps);
     }
-    __syncwarp();
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(
-                     smem_u32(&ctl.tmem_base)),
-                 "r"(nbuf * static_cast<uint32_t>(a.tmem_cols))
-                 : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
+    mbar_init(&ctl.acc_full, kMlpMmaWarps * 32);
+    mbar_init(&ctl.acc_empty, kMlpEpiWarps * 32);
+    mbar_fence_init();
   }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem = ctl.tmem_base;
 
   if (warp >= kMlpEpiWarps && warp < kMlpEpiWarps + kMlpProWarps) {
     // ================= producers ======================================================================
@@ -657,20 +732,17 @@ __global__ void __launch_bounds__(kMlpThreads, OCC) mlp_layer_kernel(const __gri
       mbar_arrive(&ctl.full[pend0]);
     }
   } else if (warp < kMlpEpiWarps) {
-    // ================= epilogue: warp w owns TMEM lanes 32w..32w+31 = rows p0+32w.. ==================
+    // ================= epilogue: warp w drains rows 32w..32w+31 = rows p0+32w.. of the accumulator tile ====
     long long j = 0;
+    const uint32_t stg = raw + front + warp * 4096u;  // after the accumulator tile
     for (long long tile = blockIdx.x; tile < total_tiles; tile += gridDim.x, ++j) {
       const long long rt = tile / n_blocks;
       const int nb = static_cast<int>(tile - rt * n_blocks);
       const long long p0 = rt * kMlpBM;
       const int n0 = nb * a.bn;
       const int bn = min(a.bn, a.n_pad - n0);
-      const unsigned buf = nbuf == 2 ? static_cast<unsigned>(j & 1) : 0u;
-      mbar_wait(&ctl.acc_full[buf], static_cast<unsigned>((nbuf == 2 ? (j >> 1) : j) & 1));
-      tc_fence_after();
+      mbar_wait(&ctl.acc_full, static_cast<unsigned>(j & 1));
       const long long prow = p0 + warp * 32 + lane;
-      const uint32_t stg = ring + static_cast<uint32_t>(S) * stage_bytes + warp * 4096u;  // after the ring
-      const uint32_t lane_addr = tmem + buf * static_cast<uint32_t>(a.tmem_cols) + ((warp * 32u) << 16);
       // per-frame bias (a 128-row tile never straddles batch elements: bias_npb % 128 == 0)
       const float *bias_t = a.bias + (a.bias_npb > 0 ? (p0 / a.bias_npb) * a.n_pad : 0);
       for (int c0 = 0; c0 < bn; c0 += 32) {
@@ -682,8 +754,10 @@ __global__ void __launch_bounds__(kMlpThreads, OCC) mlp_layer_kernel(const __gri
         if (EPI == EPI_STORE && col_on) bq = ldg128(bias_t + n0 + c0 + chunk * 4);
         float bch = 0.f;   // MAXPOOL_T: the lane's channel = n0 + 128 * (c0 / 128) + 32 * warp + lane
         if (EPI == EPI_MAXPOOL_T || EPI == EPI_STORE_T) bch = __ldg(bias_t + n0 + (c0 & ~127) + warp * 32 + lane);
-        if (cw == 32) tmem_ld32(lane_addr + c0, v);
-        else tmem_ld16(lane_addr + c0, v);
+        if (EPI == EPI_MAXPOOL_T || EPI == EPI_STORE_T)
+          acc_ld_col(acc_s, a.acc_ld, c0 & 127, (c0 & ~127) + static_cast<int>(warp * 32 + lane), v);   // v[i] = row c0+i
+        else
+          acc_ld_row(acc_s, a.acc_ld, static_cast<int>(warp * 32 + lane), c0, cw, v);
         if (EPI == EPI_SUMPOOL) {
           // sum over the 32 rows of the warp of relu(acc + bias): partial sums of a mean over points
           // (DenseFusion's AvgPool1d, pvn3d.py:165,178); rows past the end contribute 0
@@ -701,7 +775,7 @@ __global__ void __launch_bounds__(kMlpThreads, OCC) mlp_layer_kernel(const __gri
           if (col < cw && p0 + warp * 32 < a.rows)
             a.out[((p0 + warp * 32) / 32) * a.ldo + a.col0 + n0 + c0 + col] = v[0];
         } else if (EPI == EPI_STORE_T) {
-          // TRANSPOSED accumulator, stored channel-major: lane = channel, registers = 32 consecutive points of one
+          // TRANSPOSED read of the accumulator tile, stored channel-major: lane = channel, registers = 32 consecutive points of one
           // frame = 128 contiguous bytes of out[frame][channel][:] -- the [B, C, N] layout Pointnet2MSG.forward returns
           // (pvn3d.py:154) without a transposing pass over the [B*N, C] rows.  Bias / ReLU on the lane's channel, then
           // through the swizzled staging tile (row = channel) so that one STG.128 writes four full 128-byte lines
@@ -733,7 +807,7 @@ __global__ void __launch_bounds__(kMlpThreads, OCC) mlp_layer_kernel(const __gri
           }
           __syncwarp();
         } else if (EPI == EPI_MAXPOOL_T) {
-          // TRANSPOSED accumulator (the MMA ran as W . A^T): TMEM lane = output channel, column = row of the tile, so
+          // TRANSPOSED read of the accumulator tile: lane = output channel, register i = row c0 + i of the tile, so
           // the max over the `pool` consecutive rows of a centre is a max over REGISTERS of one thread -- no
           // shuffles -- and the 32 lanes of a warp store 32 consecutive channels of one pooled row (128 bytes).
           // Groups never straddle the end: rows % pool == 0 and 128 % pool == 0.
@@ -871,59 +945,17 @@ __global__ void __launch_bounds__(kMlpThreads, OCC) mlp_layer_kernel(const __gri
           }
         }
       }
-      tc_fence_before();
-      mbar_arrive(&ctl.acc_empty[buf]);  // accumulator `buf` may be overwritten
+      mbar_arrive(&ctl.acc_empty);  // the accumulator tile may be overwritten
     }
   } else {
-    // ================= warp 12: MMA issuer =============================================================
+    // ================= warps 12-19: MMA, warpgroup wg takes rows 64wg..64wg+63 of every tile ===========
+    const unsigned mw = warp - (kMlpEpiWarps + kMlpProWarps), wg = mw >> 2;
+    const int frag_row = static_cast<int>(64 * wg + 16 * (mw & 3) + (lane >> 2));
     long long it_base = 0, j = 0;
-    for (long long tile = blockIdx.x; tile < total_tiles; tile += gridDim.x, it_base += kc_total, ++j) {
-      const long long rt = tile / n_blocks;
-      const int nb = static_cast<int>(tile - rt * n_blocks);
-      const int bn = min(a.bn, a.n_pad - nb * a.bn);
-      const uint32_t idesc = instr_desc_tf32(bn);
-      const unsigned buf = nbuf == 2 ? static_cast<unsigned>(j & 1) : 0u;
-      mbar_wait(&ctl.acc_empty[buf], static_cast<unsigned>(((nbuf == 2 ? (j >> 1) : j) & 1) ^ 1));
-      tc_fence_after();
-      const uint32_t acc = tmem + buf * static_cast<uint32_t>(a.tmem_cols);
-      for (int kc = 0; kc < kc_total; ++kc) {
-        const long long it = it_base + kc;
-        const int s = static_cast<int>(it % S);
-        mbar_wait(&ctl.full[s], static_cast<unsigned>((it / S) & 1));
-        fence_proxy_async_smem();  // cp.async (generic proxy) data of the stage -> async proxy
-        tc_fence_after();
-        if (lane == 0) {
-          const uint32_t sa = ring + static_cast<uint32_t>(s) * stage_bytes;
-          const uint64_t adesc = smem_desc_sw128(sa), bdesc = smem_desc_sw128(sa + a_bytes);
-          if (EPI == EPI_MAXPOOL_T || EPI == EPI_STORE_T) {
-            // operands swapped: D^T[channel][row] = W . A^T, one M = 128 block of channels per accumulator of 128
-            // columns (the tile's rows); W's next 128 rows are 16 KB (>> 4 = 1024) further
-            const uint32_t idesc_t = instr_desc_tf32(kMlpBM);
-            for (int h = 0; h < bn / 128; ++h)
-#pragma unroll
-              for (int k4 = 0; k4 < 4; ++k4)
-                umma_tf32(acc + static_cast<uint32_t>(h * 128), bdesc + static_cast<uint64_t>(h * 1024 + k4 * 2),
-                          adesc + static_cast<uint64_t>(k4 * 2), idesc_t, (kc > 0 || k4 > 0) ? 1u : 0u);
-          } else {
-#pragma unroll
-            for (int k4 = 0; k4 < 4; ++k4)  // K = 8 tf32 = 32 bytes per instruction: +2 in 16-byte units
-              umma_tf32(acc, adesc + static_cast<uint64_t>(k4 * 2), bdesc + static_cast<uint64_t>(k4 * 2),
-                        idesc, (kc > 0 || k4 > 0) ? 1u : 0u);
-          }
-          umma_commit(&ctl.empty[s]);  // stage reusable once these MMAs have read it
-          if (kc == kc_total - 1) umma_commit(&ctl.acc_full[buf]);
-        }
-        __syncwarp();
-      }
-    }
-    tc_fence_before();
-  }
-  __syncthreads();
-  if (warp == kMlpEpiWarps + kMlpProWarps) {
-    tc_fence_after();
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem),
-                 "r"(nbuf * static_cast<uint32_t>(a.tmem_cols))
-                 : "memory");
+    for (long long tile = blockIdx.x; tile < total_tiles; tile += gridDim.x, it_base += kc_total, ++j)
+      mma_tile_n(mma_n(min(a.bn, a.n_pad - static_cast<int>(tile % n_blocks) * a.bn)), ring, stage_bytes, S, it_base,
+                 kc_total, ctl.full, ctl.empty, &ctl.acc_full, &ctl.acc_empty,
+                 static_cast<unsigned>(j & 1), acc_s, a.acc_ld, wg, frag_row, lane);
   }
 }
 
@@ -933,62 +965,22 @@ template <int PRO, int EPI>
 int launch_mlp(MlpArgs &a, cudaStream_t st) {
   if (a.rows <= 0) return PVN3D_OK;
   if (a.k_pad <= 0 || a.k_pad % 32 || a.n_pad <= 0 || a.n_pad % 16) return PVN3D_ERR_INVALID_ARG;
-  // columns per tile: <= 256, multiple of 16, as even a split as possible
-  const int nblk = ceil_div(a.n_pad, 256);
-  a.bn = ((ceil_div(a.n_pad, nblk) + 15) / 16) * 16;
-  int tc = 32;
-  while (tc < a.bn) tc <<= 1;
-  a.tmem_cols = tc;
+  a.bn = mma_n(a.n_pad);
+  a.acc_ld = std::max(32, a.bn);
   const size_t stage_bytes = kMlpBM * 128 + align_up(static_cast<size_t>(a.bn) * 128, 1024);
+  const size_t fixed = mlp_smem_front(0, a.bn, a.acc_ld) + kMlpEpiWarps * 4096 + sizeof(MlpSmemCtl);
+  int stages = static_cast<int>((kMlpSmemMax - fixed) / stage_bytes);
+  if (stages > kMlpMaxStages) stages = kMlpMaxStages;
+  // asynchronous producers (pre-rounded dense activations) keep two chunks in flight: >= 3 stages
+  if (stages < 3) return PVN3D_ERR_UNSUPPORTED;
+  a.stages = stages;
+  const size_t smem = mlp_smem_front(stages, a.bn, a.acc_ld) + kMlpEpiWarps * 4096 + sizeof(MlpSmemCtl);
+  a.use_tma = weight_tensor_map(&a.tmap, a.w, a.k_pad, a.n_pad, a.bn) ? 1 : 0;
   const int sms = std::max(1, sm_count() - a.reserve_sms);
   const long long tiles = ((a.rows + kMlpBM - 1) / kMlpBM) * ceil_div(a.n_pad, a.bn);
-  // two CTAs per SM when both fit: accumulators <= 512 TMEM columns in total (2 x 2 x <=128, or 2 x 1 x 256: wide
-  // tiles give up the second accumulator of the CTA, the co-resident CTA fills the gap), >= min_stages stages in
-  // half the shared memory, and enough tiles to feed twice the CTAs (PVN3D_MLP_OCC=1 forces one CTA per SM,
-  // PVN3D_MLP_ACC1=0 keeps wide tiles at one CTA per SM, PVN3D_MLP_OCC2_TILES = tiles-per-SM threshold)
-  static const int occ_env = [] { const char *e = getenv("PVN3D_MLP_OCC"); return e ? atoi(e) : 0; }();
-  static const int acc1_env = [] { const char *e = getenv("PVN3D_MLP_ACC1"); return e ? atoi(e) : 1; }();
-  static const int tiles_env = [] { const char *e = getenv("PVN3D_MLP_OCC2_TILES"); return e ? atoi(e) : 4; }();
-  static const int budget_env = [] { const char *e = getenv("PVN3D_MLP_OCC2_KB"); return e ? atoi(e) : 96; }();
-  const size_t budget2 = static_cast<size_t>(std::min(std::max(budget_env, 48), 96)) * 1024;   // ring of one of two co-resident CTAs
-  // asynchronous producers (pre-rounded dense activations) keep two chunks in flight: >= 3 stages
-  const size_t min_stages = ((PRO == PRO_DENSE || PRO == PRO_SA_GATHER) && a.a_tf32) ? 3 : 2;
-  // ... and at two CTAs per SM a ring of only three stages starves them unless a tile is a single chunk (measured:
-  // 96 -> 128 max-pool layer 154 us with 6 stages at one CTA per SM, 213 us with 3 stages at two)
-  const size_t min_stages2 = (min_stages == 3 && a.k_pad > 32) ? 4 : min_stages;
-  const bool fits2 = min_stages2 * stage_bytes <= budget2 && tiles >= static_cast<long long>(tiles_env) * sms;
-  bool occ2 = a.tmem_cols <= 128 && fits2;
-  a.acc_bufs = 2;
-  if (!occ2 && a.tmem_cols == 256 && fits2 && acc1_env) {
-    occ2 = true;
-    a.acc_bufs = 1;
-  }
-  if (occ_env == 1) {
-    occ2 = false;
-    a.acc_bufs = 2;
-  }
-  int stages = static_cast<int>((occ2 ? budget2 : size_t(208 * 1024)) / stage_bytes);
-  if (stages > kMlpMaxStages) stages = kMlpMaxStages;
-  if (stages < 2) stages = 2;
-  a.stages = stages;
-  const size_t smem = stages * stage_bytes + kMlpEpiWarps * 4096 + 256;  // ring + epilogue staging + barriers
-  static_assert(sizeof(MlpSmemCtl) <= 256, "barrier block");
-  a.use_tma = weight_tensor_map(&a.tmap, a.w, a.k_pad, a.n_pad, a.bn) ? 1 : 0;
-  if (occ2) {
-    auto kern = mlp_layer_kernel<PRO, EPI, 2>;
-    static PerDeviceOnce once2;
-    PVN3D_ONCE_PER_DEVICE(once2,
-                          (cudaFuncSetAttribute(kern, cudaFuncAttributePreferredSharedMemoryCarveout, 100),
-                           cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, 113 * 1024)),
-                          "mlp smem attr (2 CTAs/SM)");
-    const unsigned grid = static_cast<unsigned>(std::min<long long>(tiles, 2ll * sms));
-    kern<<<grid, kMlpThreads, smem, st>>>(a);
-    return check_launch("mlp_layer_kernel<2>");
-  }
-  auto kern = mlp_layer_kernel<PRO, EPI, 1>;
+  auto kern = mlp_layer_kernel<PRO, EPI>;
   static PerDeviceOnce once;
-  PVN3D_ONCE_PER_DEVICE(once,
-                        cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, 226 * 1024),
+  PVN3D_ONCE_PER_DEVICE(once, cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, kMlpSmemMax),
                         "mlp smem attr");
   const unsigned grid = static_cast<unsigned>(std::min<long long>(tiles, sms));
   kern<<<grid, kMlpThreads, smem, st>>>(a);
@@ -1007,8 +999,8 @@ int launch_mlp(MlpArgs &a, cudaStream_t st) {
 // waits on its own previous layer, a CTA works on TWO row tiles at a time ("slots"), in the order
 //     (A,L0) (B,L0) (A,L1) (B,L1) (A,L2) (B,L2) | next pair ...
 // Every (tile, layer, column block) is one ITEM; the three roles (producers / MMA issuer / epilogue) walk
-// the same item sequence, exactly like the per-layer kernel walks tiles: the operand ring and the two
-// TMEM accumulators are shared by all layers.  New dependency: the producers of (slot, l>0) wait on
+// the same item sequence, exactly like the per-layer kernel walks tiles: the operand ring and the
+// accumulator tile are shared by all layers.  New dependency: the producers of (slot, l>0) wait on
 // h_ready[slot], on which the 128 epilogue threads arrive after storing (slot, l-1).
 constexpr int kChainMaxSlots = 8;
 struct ChainLayer {
@@ -1017,10 +1009,10 @@ struct ChainLayer {
 };
 struct MlpChainArgs {
   // weight matrices as TMA tensor maps: [n_pad][k_pad] fp32, box = 32 columns (128 B) x bn rows,
-  // SWIZZLE_128B -- one cp.async.bulk.tensor.2d per K chunk lands the B operand in the UMMA layout
+  // SWIZZLE_128B -- one cp.async.bulk.tensor.2d per K chunk lands the B operand in the wgmma layout
   alignas(64) CUtensorMap tmap[3];
   int use_tma;
-  MlpArgs base;        // producer of layer 0 + final epilogue (rows, out, ldo, col0, pool)
+  MlpArgs base;        // producer of layer 0 + final epilogue (rows, out, ldo, col0, pool); bn = widest layer tile
   ChainLayer layer[3];
   int n_layers;
   float *scratch;      // [grid][n_slots][slot_floats]
@@ -1032,11 +1024,10 @@ struct MlpChainArgs {
 struct ChainSmemCtl {
   uint64_t full[kMlpMaxStages];
   uint64_t empty[kMlpMaxStages];
-  uint64_t acc_full[2];
-  uint64_t acc_empty[2];
+  uint64_t acc_full;
+  uint64_t acc_empty;
   uint64_t h_ready[kChainMaxSlots];   // 128 arrivals: epilogue threads, after storing a slot's intermediate tile
   uint64_t h_seen[kChainMaxSlots];    // 256 arrivals: every producer thread, once it has passed a h_ready phase
-  uint32_t tmem_base;
 };
 
 template <int PRO, int EPI>
@@ -1047,9 +1038,9 @@ __global__ void __launch_bounds__(kMlpThreads, 1) mlp_chain_kernel(const __grid_
   const uint32_t raw = smem_u32(mlp_smem_raw);
   const uint32_t ring = (raw + 1023u) & ~1023u;
   const uint32_t a_bytes = kMlpBM * 128u;
-  int bn_max = 0;
-  for (int l = 0; l < c.n_layers; ++l) bn_max = max(bn_max, c.layer[l].bn);
-  const uint32_t stage_bytes = a_bytes + ((static_cast<uint32_t>(bn_max) * 128u + 1023u) & ~1023u);
+  const uint32_t stage_bytes = a_bytes + ((static_cast<uint32_t>(a.bn) * 128u + 1023u) & ~1023u);
+  const uint32_t acc_s = ring + static_cast<uint32_t>(a.stages) * stage_bytes;
+  const uint32_t front = mlp_smem_front(a.stages, a.bn, a.acc_ld);
 
   const int t = threadIdx.x;
   const unsigned warp = t >> 5, lane = t & 31u;
@@ -1062,33 +1053,20 @@ __global__ void __launch_bounds__(kMlpThreads, 1) mlp_chain_kernel(const __grid_
   const long long n_pairs = (my_tiles + NS - 1) / NS;
   float *const scratch = c.scratch + static_cast<size_t>(blockIdx.x) * NS * c.slot_floats;
 
-  if (warp == kMlpEpiWarps + kMlpProWarps) {
-    if (lane == 0) {
-      for (int s = 0; s < S; ++s) {
-        mbar_init(&ctl.full[s], 128);
-        mbar_init(&ctl.empty[s], 1);
-      }
-      for (int b = 0; b < 2; ++b) {
-        mbar_init(&ctl.acc_full[b], 1);
-        mbar_init(&ctl.acc_empty[b], 128);
-      }
-      for (int b = 0; b < kChainMaxSlots; ++b) {
-        mbar_init(&ctl.h_ready[b], 128);
-        mbar_init(&ctl.h_seen[b], kMlpProWarps * 32);
-      }
-      mbar_fence_init();
+  if (t == 0) {
+    for (int s = 0; s < S; ++s) {
+      mbar_init(&ctl.full[s], 128);
+      mbar_init(&ctl.empty[s], kMlpMmaWarps);
     }
-    __syncwarp();
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(
-                     smem_u32(&ctl.tmem_base)),
-                 "r"(static_cast<uint32_t>(2 * a.tmem_cols))
-                 : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
+    mbar_init(&ctl.acc_full, kMlpMmaWarps * 32);
+    mbar_init(&ctl.acc_empty, kMlpEpiWarps * 32);
+    for (int b = 0; b < kChainMaxSlots; ++b) {
+      mbar_init(&ctl.h_ready[b], 128);
+      mbar_init(&ctl.h_seen[b], kMlpProWarps * 32);
+    }
+    mbar_fence_init();
   }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem = ctl.tmem_base;
 
   if (warp >= kMlpEpiWarps && warp < kMlpEpiWarps + kMlpProWarps) {
     // ================= producers ======================================================================
@@ -1211,7 +1189,7 @@ __global__ void __launch_bounds__(kMlpThreads, 1) mlp_chain_kernel(const __grid_
     // ================= epilogue =========================================================================
     long long j = 0;
     unsigned hsig_any = 0u, hsig_par = 0u;   // per slot: signalled before / parity of the last phase signalled
-    const uint32_t stg = ring + static_cast<uint32_t>(S) * stage_bytes + warp * 4096u;
+    const uint32_t stg = raw + front + warp * 4096u;
     for (long long pair = 0; pair < n_pairs; ++pair) {
       for (int l = 0; l < NL; ++l) {
         const ChainLayer &L = c.layer[l];
@@ -1225,16 +1203,12 @@ __global__ void __launch_bounds__(kMlpThreads, 1) mlp_chain_kernel(const __grid_
           for (int nb = 0; nb < L.n_blocks; ++nb, ++j) {
             const int n0 = nb * L.bn;
             const int bn = min(L.bn, L.n_pad - n0);
-            const unsigned buf = static_cast<unsigned>(j & 1);
-            mbar_wait(&ctl.acc_full[buf], static_cast<unsigned>((j >> 1) & 1));
-            tc_fence_after();
+            mbar_wait(&ctl.acc_full, static_cast<unsigned>(j & 1));
             const long long prow = p0 + warp * 32 + lane;
-            const uint32_t lane_addr = tmem + buf * static_cast<uint32_t>(a.tmem_cols) + ((warp * 32u) << 16);
             for (int c0 = 0; c0 < bn; c0 += 32) {
               float v[32];
               const int cw = min(32, bn - c0);
-              if (cw == 32) tmem_ld32(lane_addr + c0, v);
-              else tmem_ld16(lane_addr + c0, v);
+              acc_ld_row(acc_s, a.acc_ld, static_cast<int>(warp * 32 + lane), c0, cw, v);
               if (!last || EPI == EPI_STORE) {
                 // intermediate: bias + ReLU + TF32 rounding into the slot's scratch tile (row = local row);
                 // final STORE: bias + ReLU (+ rounding if asked) into out
@@ -1306,8 +1280,7 @@ __global__ void __launch_bounds__(kMlpThreads, 1) mlp_chain_kernel(const __grid_
                 }
               }
             }
-            tc_fence_before();
-            mbar_arrive(&ctl.acc_empty[buf]);
+            mbar_arrive(&ctl.acc_empty);
           }
           if (!last) {
             // the slot's tile of layer l is complete in global memory (L2): make it visible at GPU scope
@@ -1325,7 +1298,9 @@ __global__ void __launch_bounds__(kMlpThreads, 1) mlp_chain_kernel(const __grid_
       }
     }
   } else {
-    // ================= warp 12: MMA issuer =============================================================
+    // ================= warps 12-19: MMA, warpgroup wg takes rows 64wg..64wg+63 of every item ==========
+    const unsigned mw = warp - (kMlpEpiWarps + kMlpProWarps), wg = mw >> 2;
+    const int frag_row = static_cast<int>(64 * wg + 16 * (mw & 3) + (lane >> 2));
     long long it_base = 0, j = 0;
     for (long long pair = 0; pair < n_pairs; ++pair) {
       for (int l = 0; l < NL; ++l) {
@@ -1333,43 +1308,13 @@ __global__ void __launch_bounds__(kMlpThreads, 1) mlp_chain_kernel(const __grid_
         const int kc_total = L.k_pad / 32;
         for (int slot = 0; slot < NS; ++slot) {
           if (NS * pair + slot >= my_tiles) continue;
-          for (int nb = 0; nb < L.n_blocks; ++nb, ++j, it_base += kc_total) {
-            const int bn = min(L.bn, L.n_pad - nb * L.bn);
-            const uint32_t idesc = instr_desc_tf32(bn);
-            const unsigned buf = static_cast<unsigned>(j & 1);
-            mbar_wait(&ctl.acc_empty[buf], static_cast<unsigned>(((j >> 1) & 1) ^ 1));
-            tc_fence_after();
-            const uint32_t acc = tmem + buf * static_cast<uint32_t>(a.tmem_cols);
-            for (int kc = 0; kc < kc_total; ++kc) {
-              const long long it = it_base + kc;
-              const int s = static_cast<int>(it % S);
-              mbar_wait(&ctl.full[s], static_cast<unsigned>((it / S) & 1));
-              fence_proxy_async_smem();
-              tc_fence_after();
-              if (lane == 0) {
-                const uint32_t sa = ring + static_cast<uint32_t>(s) * stage_bytes;
-                const uint64_t adesc = smem_desc_sw128(sa), bdesc = smem_desc_sw128(sa + a_bytes);
-#pragma unroll
-                for (int k4 = 0; k4 < 4; ++k4)
-                  umma_tf32(acc, adesc + static_cast<uint64_t>(k4 * 2), bdesc + static_cast<uint64_t>(k4 * 2),
-                            idesc, (kc > 0 || k4 > 0) ? 1u : 0u);
-                umma_commit(&ctl.empty[s]);
-                if (kc == kc_total - 1) umma_commit(&ctl.acc_full[buf]);
-              }
-              __syncwarp();
-            }
-          }
+          for (int nb = 0; nb < L.n_blocks; ++nb, ++j, it_base += kc_total)
+            mma_tile_n(mma_n(min(L.bn, L.n_pad - nb * L.bn)), ring, stage_bytes, S, it_base, kc_total, ctl.full,
+                       ctl.empty, &ctl.acc_full, &ctl.acc_empty,
+                       static_cast<unsigned>(j & 1), acc_s, a.acc_ld, wg, frag_row, lane);
         }
       }
     }
-    tc_fence_before();
-  }
-  __syncthreads();
-  if (warp == kMlpEpiWarps + kMlpProWarps) {
-    tc_fence_after();
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem),
-                 "r"(static_cast<uint32_t>(2 * a.tmem_cols))
-                 : "memory");
   }
 }
 
@@ -1379,8 +1324,8 @@ int chain_plan(MlpChainArgs &c, const pvn3d_mlp_layer_t *layers, int n_layers) {
   for (int l = 0; l < n_layers; ++l) {
     ChainLayer &L = c.layer[l];
     L.w = layers[l].w; L.bias = layers[l].bias; L.k_pad = layers[l].k_pad; L.n_pad = layers[l].n_pad;
-    L.n_blocks = ceil_div(L.n_pad, 256);
-    L.bn = ((ceil_div(L.n_pad, L.n_blocks) + 15) / 16) * 16;
+    L.bn = mma_n(L.n_pad);
+    L.n_blocks = ceil_div(L.n_pad, L.bn);
     bn_max = std::max(bn_max, L.bn);
     if (l < n_layers - 1) {
       c.h_off[l] = off;
@@ -1389,10 +1334,8 @@ int chain_plan(MlpChainArgs &c, const pvn3d_mlp_layer_t *layers, int n_layers) {
   }
   c.n_layers = n_layers;
   c.slot_floats = off;
-  int tc = 32;
-  while (tc < bn_max) tc <<= 1;
-  c.base.tmem_cols = tc;
   c.base.bn = bn_max;
+  c.base.acc_ld = std::max(32, bn_max);
   return off;
 }
 
@@ -1449,14 +1392,14 @@ bool chain_layers_ok(const pvn3d_mlp_layer_t *layers, int n_layers, int k_first_
 }
 
 // row tiles a CTA keeps in flight: enough to cover the epilogue -> L2 -> producer latency of a layer
-// transition, as long as all scratch tiles of the grid stay well inside the 126 MB L2 (<= 48 MB)
+// transition, as long as all scratch tiles of the grid stay well inside the 50 MB L2 (<= 24 MB)
 int chain_slots(int slot_floats, long long row_tiles, unsigned grid) {
   int want = 4;
   if (const char *env = getenv("PVN3D_CHAIN_SLOTS")) want = atoi(env);
   want = std::max(2, std::min(kChainMaxSlots, want));
   const long long per_cta = (row_tiles + grid - 1) / std::max(1u, grid);
   while (want > 2 && want > per_cta) --want;
-  while (want > 2 && static_cast<size_t>(grid) * want * slot_floats * sizeof(float) > (48u << 20)) --want;
+  while (want > 2 && static_cast<size_t>(grid) * want * slot_floats * sizeof(float) > (24u << 20)) --want;
   return want;
 }
 
@@ -1464,16 +1407,19 @@ template <int PRO, int EPI>
 int launch_chain(MlpChainArgs &c, void *workspace, size_t workspace_bytes, cudaStream_t st) {
   MlpArgs &a = c.base;
   if (a.rows <= 0) return PVN3D_OK;
+  // the barrier block is static shared memory: the dynamic part stays below the block limit by one kilobyte
+  constexpr int kDynMax = kMlpSmemMax - 1024;
+  static_assert(sizeof(ChainSmemCtl) <= 1024, "barrier block");
   const size_t stage_bytes = kMlpBM * 128 + align_up(static_cast<size_t>(a.bn) * 128, 1024);
-  int stages = static_cast<int>((208 * 1024) / stage_bytes);
+  const size_t fixed = mlp_smem_front(0, a.bn, a.acc_ld) + kMlpEpiWarps * 4096;
+  int stages = static_cast<int>((kDynMax - fixed) / stage_bytes);
   if (stages > kMlpMaxStages) stages = kMlpMaxStages;
   if (stages < 3) return PVN3D_ERR_UNSUPPORTED;   // asynchronous producers keep two chunks in flight
   a.stages = stages;
-  const size_t smem = stages * stage_bytes + 1024 + kMlpEpiWarps * 4096;
+  const size_t smem = mlp_smem_front(stages, a.bn, a.acc_ld) + kMlpEpiWarps * 4096;
   auto kern = mlp_chain_kernel<PRO, EPI>;
   static PerDeviceOnce once;
-  PVN3D_ONCE_PER_DEVICE(once,
-                        cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, 226 * 1024),
+  PVN3D_ONCE_PER_DEVICE(once, cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, kDynMax),
                         "mlp chain smem attr");
   const int sms = std::max(1, sm_count() - a.reserve_sms);
   const long long row_tiles = (a.rows + kMlpBM - 1) / kMlpBM;
@@ -1492,10 +1438,9 @@ int dispatch(MlpArgs &a, int pro, int pool, cudaStream_t st) {
   if (pool) {
     if (pool != 8 && pool != 16 && pool != 32) return PVN3D_ERR_UNSUPPORTED;
     a.pool = pool;
-    // 128-channel pooled layers: transposed accumulator, register max instead of shuffles (79 -> 51 us and 154 -> 125 us
-    // on the SA2 scales).  Tiles of 256 channels work too (PVN3D_MLP_POOLT=2) but measured 5-25 % SLOWER: two
-    // M=128 x N=128 TF32 MMAs per K step read 128 B of shared memory per clock, the N=256 form 96.  PVN3D_MLP_POOLT=0:
-    // the shuffle epilogue everywhere.
+    // 128-channel pooled layers: transposed read of the accumulator tile, register max instead of shuffles.
+    // PVN3D_MLP_POOLT=2 takes every pooled layer of 128k channels that way, PVN3D_MLP_POOLT=0 the shuffle epilogue
+    // everywhere.
     static const int poolt_env = [] { const char *e = getenv("PVN3D_MLP_POOLT"); return e ? atoi(e) : 1; }();
     const bool t128 = a.n_pad == 128;
     const bool t256 = a.n_pad % 128 == 0 && (a.n_pad <= 256 || a.n_pad % 256 == 0);

@@ -1,10 +1,10 @@
-// pn2_ops.cu -- the element-wise / search ops of lib.pointnet2_utils._ext for sm_100a:
+// pn2_ops.cu -- the element-wise / search ops of lib.pointnet2_utils._ext for sm_90a:
 // gather_points(+grad), ball_query, group_points(+grad), three_nn, three_interpolate(+grad),
 // and the [B,C,N] <-> [B,N,C] staging transposes.
 //
 // The reference launches every one of these with grid = B (one CTA per cloud, e.g.
 // ball_query_gpu.cu:50, group_points_gpu.cu:35, interpolate_gpu.cu:64,107): at B = 16..32 that
-// leaves 3/4 of a 148-SM B200 idle.  Here each op is tiled so that the grid covers the chip, the
+// leaves most of the 132 SMs of an H100 idle.  Here each op is tiled so that the grid covers the chip, the
 // searched point set is staged through shared memory (bulk-copied by the TMA engine when
 // alignment allows) and read back as broadcasts, and global accesses are coalesced.
 #include "common.cuh"
@@ -204,8 +204,8 @@ __device__ __forceinline__ void best3_push(Best3 &b, float d, int k) {
 // scans known[0..m) of cloud b for the calling thread's query point (ux,uy,uz); all threads of the
 // CTA must call it (barriers inside).
 // The tile holds NEGATED known points as pairs, s_known[2p] = (-x0,-x1,-y0,-y1), s_known[2p+1] = (-z0,-z1,.,.):
-// u - q = u + (-q) exactly, so the distance of the query to two known points is three FADD2 + FMUL2 + two
-// FFMA2 on the packed fp32 pipe -- per lane the same IEEE operations in the same order as ref_sqdist
+// u - q = u + (-q) exactly, so the distance of the query to two known points is, per component, the same
+// IEEE operations in the same order as ref_sqdist
 // (fma(dz,dz, fma(dx,dx, dy*dy))), pushed in index order: results stay bit-exact.  An odd tail is a point
 // at infinity (d2 = inf never beats a finite or an initial inf candidate).
 __device__ __forceinline__ void three_nn_scan(const float *__restrict__ known_cloud, int m,
@@ -230,10 +230,10 @@ __device__ __forceinline__ void three_nn_scan(const float *__restrict__ known_cl
 #pragma unroll 4
     for (int k = 0; k < npairs; ++k) {
       const float4 a = s_known[2 * k], c = s_known[2 * k + 1];
-      const float2 dx = __fadd2_rn(make_float2(a.x, a.y), ux2);
-      const float2 dy = __fadd2_rn(make_float2(a.z, a.w), uy2);
-      const float2 dz = __fadd2_rn(make_float2(c.x, c.y), uz2);
-      const float2 d = __ffma2_rn(dz, dz, __ffma2_rn(dx, dx, __fmul2_rn(dy, dy)));
+      const float2 dx = f2_add(make_float2(a.x, a.y), ux2);
+      const float2 dy = f2_add(make_float2(a.z, a.w), uy2);
+      const float2 dz = f2_add(make_float2(c.x, c.y), uz2);
+      const float2 d = f2_fma(dz, dz, f2_fma(dx, dx, f2_mul(dy, dy)));
       best3_push(best, d.x, base + 2 * k);
       best3_push(best, d.y, base + 2 * k + 1);
     }
@@ -312,11 +312,10 @@ __device__ __forceinline__ void best3_push_lex(Best3 &b, float d, int k) {
 __global__ void __launch_bounds__(kNnThreads)
 three_nn_slab_kernel(const float *__restrict__ unknown, const float4 *__restrict__ sorted, int n, int m, int m_pad,
                      float *__restrict__ dist2, int *__restrict__ idx) {
-  extern __shared__ float4 s_k[];
+  // the walk reads the frame's sorted copy (<= 64 KB) through the read-only cache: staged in shared memory, the same
+  // walk lost the lower index of coincident known points on sm_90a (tests/test_pn2_gpu.py tie cases)
   const int b = blockIdx.y;
-  sorted += static_cast<size_t>(b) * m_pad;
-  for (int i = threadIdx.x; i < m; i += kNnThreads) s_k[i] = sorted[i];
-  __syncthreads();
+  const float4 *__restrict__ s_k = sorted + static_cast<size_t>(b) * m_pad;
   const int j = blockIdx.x * kNnThreads + threadIdx.x;
   if (j >= n) return;
   const float *u = unknown + (static_cast<size_t>(b) * n + j) * 3;
@@ -607,8 +606,6 @@ extern "C" int pvn3d_three_nn(const float *unknown, const float *known, int b, i
     if (once.pending()) {
       PVN3D_CUDA_TRY(cudaFuncSetAttribute(nn_sort_known_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                           kNnSlabMaxM * (int)sizeof(float4)), "nn sort smem attr");
-      PVN3D_CUDA_TRY(cudaFuncSetAttribute(three_nn_slab_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                          kNnSlabMaxM * (int)sizeof(float4)), "nn slab smem attr");
       once.mark();
     }
     int rc = keep_async_pool_warm();
@@ -619,7 +616,7 @@ extern "C" int pvn3d_three_nn(const float *unknown, const float *known, int b, i
     nn_sort_known_kernel<<<b, 512, smem, as_stream(stream)>>>(known, m, m_pad, sorted);
     rc = check_launch("nn_sort_known_kernel");
     if (rc == PVN3D_OK) {
-      three_nn_slab_kernel<<<grid, kNnThreads, static_cast<size_t>(m) * sizeof(float4), as_stream(stream)>>>(
+      three_nn_slab_kernel<<<grid, kNnThreads, 0, as_stream(stream)>>>(
           unknown, sorted, n, m, m_pad, dist2, idx);
       rc = check_launch("three_nn_slab_kernel");
     }

@@ -1,4 +1,4 @@
-// query_group.cu -- fused ball-query + grouping for sm_100a (the HBM-bound kernel of the path).
+// query_group.cu -- fused ball-query + grouping for sm_90a (the HBM-bound kernel of the path).
 //
 // Replaces the five launches + two copies the reference spends per scale in
 // QueryAndGroup.forward (pvn3d/lib/pointnet2_utils/pointnet2_utils.py:311-321):

@@ -7,7 +7,7 @@ convolutions -- 11x the PointNet++ shared MLPs -- and what `demo.py` waits on on
     heads = FusedHeads(model.rgbd_feat, model.SEG_layer, model.KpOF_layer, model.CtrOf_layer)
     pred_kp_of, pred_rgbd_seg, pred_ctr_of = heads(rgb_emb, pcld_emb)       # as PVN3D.forward returns them
 
-Everything runs point-major ([B*N, C] rows) through `pvn3d_mlp_dense*` (tcgen05 kind::tf32, weights by TMA):
+Everything runs point-major ([B*N, C] rows) through `pvn3d_mlp_dense*` (wgmma tf32, weights by TMA):
   * conv2_rgb, conv2_cld and conv3 read the same 256 columns [rgb | cld]: ONE launch with a block-structured
     [1024 x 256] weight writes feat_2 and conv3's output next to feat_1 in one activation table;
   * conv4 (512 -> 1024) is only ever averaged over the points (AvgPool1d, :165,178): its epilogue sums relu(.) over

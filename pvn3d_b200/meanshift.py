@@ -1,5 +1,5 @@
 """MeanShiftTorch -- drop-in for the reference class of the same name
-(pvn3d/lib/utils/meanshift_pytorch.py:18-51), running the batched sm_100a kernels of
+(pvn3d/lib/utils/meanshift_pytorch.py:18-51), running the batched sm_90a kernels of
 csrc/meanshift.cu through the C ABI.
 
     ms = MeanShiftTorch(bandwidth=0.08)

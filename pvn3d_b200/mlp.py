@@ -263,10 +263,9 @@ class FusedPointnet2MSG:
     def __init__(self, model: torch.nn.Module, device="cuda", chain: bool | None = None):
         self.dev = torch.device(device)
         #: chain=True: one launch per SharedMLP (inter-layer tiles stay in L2, DRAM traffic of the MLPs -95 %);
-        #: False (default): one launch per layer.  Same bits either way (tests/test_mlp_gpu.py).  Measured on B200
-        #: the chained kernel is 11 % SLOWER (5.25 vs 4.72 ms per 32-frame batch, DESIGN.md section 9): with 13 warps
-        #: per SM the layers are latency-bound, not HBM-bound, and the chain adds a dependency per layer.
-        #: PVN3D_MLP_CHAIN=1 selects it.
+        #: False (default): one launch per layer.  Same bits either way (tests/test_mlp_gpu.py).  The layers are
+        #: latency-bound rather than HBM-bound, and the chain adds a dependency per layer; its speed on the H100 is
+        #: not measured.  PVN3D_MLP_CHAIN=1 selects it.
         if chain is None:
             chain = os.environ.get("PVN3D_MLP_CHAIN", "0") == "1"
         self.chain = bool(chain)
@@ -367,7 +366,7 @@ class FusedPointnet2MSG:
     def sampling(self, pointcloud: torch.Tensor, fps_chunk: int = 0) -> "GeoPlan":
         """The four furthest-point samplings of Pointnet2MSG.forward and the sampled centres (reference
         pointnet2_modules.py:44-53): 3708 dependent arg-max iterations on ONE CTA per frame -- latency-bound
-        and narrow (B of the 148 SMs).  They depend on the coordinates only, so FramePipeline runs them for
+        and narrow (B of the SMs).  They depend on the coordinates only, so FramePipeline runs them for
         batch i+1 on a side stream under the shared MLPs of batch i.
         fps_chunk > 0: sample that many frames per launch, so that a caller who keeps only `fps_chunk` SMs free
         for this stream never has more sampling CTAs pending than free SMs."""

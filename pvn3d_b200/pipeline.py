@@ -32,7 +32,7 @@ class FramePipeline:
         self.dev = torch.device(device)
         self.shape, self.b, self.n, self.k = shape, int(batch), int(n_points), fixtures.N_KEYPOINTS
         self.model = (model if model is not None else seeded_pointnet2msg(0, 1)).to(self.dev).eval()
-        #: "fused"  = hot path A entirely on libpvn3d_b200 (tcgen05 shared MLPs, grouping/interpolation fused
+        #: "fused"  = hot path A entirely on libpvn3d_b200 (wgmma shared MLPs, grouping/interpolation fused
         #:            into the operand producers -- pvn3d_b200.mlp.FusedPointnet2MSG)
         #: "modules" = the Pointnet2MSG module graph on the library's `_ext` ops with cuDNN/cuBLAS MLPs
         self.engine = engine

@@ -14,6 +14,61 @@ SA_LEVELS = [(12288, 2048, (0.0175, 0.025), (16, 32)), (2048, 1024, (0.025, 0.05
              (1024, 512, (0.05, 0.1), (16, 32)), (512, 128, (0.1, 0.2), (16, 32))]
 
 
+# the point columns of the Pointnet2MSG features stored in tests/golden/dropin_ref.npz (a fixed sample of 12288)
+PN2MSG_POINTS = np.sort(np.random.default_rng(0).choice(12288, size=512, replace=False))[::2]
+
+
+# DenseFusion + heads cases of tests/test_heads_gpu.py and tests/golden/heads_ref.npz
+HEADS_CASES = [(2, 2048), (1, 12288), (2, 1000)]
+
+
+def heads_modules():
+    """DenseFusion + SEG / KpOF / CtrOf stacks in the reference's module layout, seeded, BN randomised (CPU)"""
+    from pvn3d_b200 import heads, testing
+
+    torch.manual_seed(3)
+    mods = [m.eval() for m in heads.reference_layout_modules(22, 8)]
+    for i, m in enumerate(mods):
+        testing.randomize_bn_(m, 10 + i)
+    return mods
+
+
+def heads_inputs(b, n):
+    """rgb_emb, cld_emb [b, 128, n] on the CPU (PointNet++ features are post-ReLU)"""
+    g = torch.Generator().manual_seed(n)
+    rgb_emb = torch.randn(b, 128, n, generator=g)
+    return rgb_emb, torch.randn(b, 128, n, generator=g).abs()
+
+
+def heads_points(n):
+    """the point columns of the head outputs stored in tests/golden/heads_ref.npz"""
+    return np.sort(np.random.default_rng(n).choice(n, size=min(n, 384), replace=False))
+
+
+def sa_module_and_inputs():
+    """the MSG set-abstraction module of the autograd drop-in test (this package's module, reference layout) and
+    its inputs xyz [2, 512, 3], features [2, 6, 512], all on the CPU"""
+    from pvn3d_b200.pointnet2 import PointnetSAModuleMSG
+
+    torch.manual_seed(1)
+    sa = PointnetSAModuleMSG(npoint=64, radii=[0.1, 0.2], nsamples=[8, 16], mlps=[[6, 16, 32], [6, 16, 32]]).eval()
+    g = torch.Generator().manual_seed(3)
+    return sa, torch.rand(2, 512, 3, generator=g), torch.rand(2, 6, 512, generator=g)
+
+
+def sa_feature_grad(sa, xyz, feat):
+    """d/dfeat of sum(out^2) through the module (fp32 cuDNN, TF32 off)"""
+    feat = feat.clone().requires_grad_(True)
+    prev = torch.backends.cudnn.allow_tf32
+    torch.backends.cudnn.allow_tf32 = False
+    try:
+        _, out = sa(xyz, feat)
+        out.square().sum().backward()
+    finally:
+        torch.backends.cudnn.allow_tf32 = prev
+    return feat.grad.detach()
+
+
 def load_ref_ext():
     """The UNMODIFIED reference op library built by oracle/build_ref_ext.sh, or None."""
     global _ref_ext, _ref_tried

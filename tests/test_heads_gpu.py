@@ -1,83 +1,56 @@
 """DenseFusion + SEG / KpOF / CtrOf heads (SURVEY section 8 f3) on the tensor-core layer kernel against the
-REFERENCE modules (pvn3d/lib/pvn3d.py:157-182,245-267,297-308), built from the reference's own classes staged under
-oracle/_ref/py and run in fp32 (TF32 off) on the GPU.
+REFERENCE modules (pvn3d/lib/pvn3d.py:157-182,245-267,297-308): tests/golden/heads_ref.npz holds what the reference's
+classes, with the weights of helpers.heads_modules, computed in fp32 (TF32 off) at a fixed sample of the points.
 
 Tolerance: TF32 operands through 6 stacked 1x1 convolutions with K up to 1024 -> mean error <= 3e-3 and max error <=
-3e-2 of the mean output magnitude per head (the class of the reference's default cuDNN TF32 path, measured alongside).
+3e-2 of the mean output magnitude per head (the class of the reference's default cuDNN TF32 path).
 """
+import os
+
 import numpy as np
 import pytest
 import torch
 
-from pvn3d_b200 import eval_utils, fixtures, heads, testing
+from pvn3d_b200 import eval_utils, fixtures, heads
 from pvn3d_b200.eval_utils import FramePoseSolver
 
-from helpers import load_reference_python
+from helpers import HEADS_CASES, heads_inputs, heads_modules, heads_points
 
 pytestmark = pytest.mark.gpu
 
 
 @pytest.fixture(scope="module")
 def ref_modules(cuda_dev):
-    ref = load_reference_python()
-    if ref is None:
-        pytest.skip("oracle/_ref/py not staged")
-    import lib.utils.etw_pytorch_utils as pt_utils
-    from torch import nn
-
-    torch.manual_seed(3)
-    n_cls, n_kps = 22, 8
-    fusion = ref.pvn3d.DenseFusion(2048)
-    # the three stacks exactly as PVN3D.__init__ builds them (pvn3d.py:245-267)
-    seg = (pt_utils.Seq(1792).conv1d(1024, bn=True, activation=nn.ReLU()).conv1d(512, bn=True, activation=nn.ReLU())
-           .conv1d(128, bn=True, activation=nn.ReLU()).conv1d(n_cls, activation=None))
-    kpof = (pt_utils.Seq(1792).conv1d(1024, bn=True, activation=nn.ReLU()).conv1d(512, bn=True, activation=nn.ReLU())
-            .conv1d(256, bn=True, activation=nn.ReLU()).conv1d(n_kps * 3, activation=None))
-    ctrof = (pt_utils.Seq(1792).conv1d(1024, bn=True, activation=nn.ReLU()).conv1d(512, bn=True, activation=nn.ReLU())
-             .conv1d(128, bn=True, activation=nn.ReLU()).conv1d(3, activation=None))
-    mods = [m.to(cuda_dev).eval() for m in (fusion, seg, kpof, ctrof)]
-    for i, m in enumerate(mods):
-        testing.randomize_bn_(m, 10 + i)
-    return mods
+    return [m.to(cuda_dev).eval() for m in heads_modules()]
 
 
-def _reference_forward(mods, rgb_emb, cld_emb, allow_tf32):
-    fusion, seg, kpof, ctrof = mods
-    bs, _, n = cld_emb.shape
-    fusion.ap1 = torch.nn.AvgPool1d(n)                      # DenseFusion(num_points) pools over all points (:165)
-    prev = torch.backends.cudnn.allow_tf32, torch.backends.cuda.matmul.allow_tf32
-    torch.backends.cudnn.allow_tf32 = torch.backends.cuda.matmul.allow_tf32 = allow_tf32
-    try:
-        with torch.no_grad():
-            f = fusion(rgb_emb, cld_emb)
-            pred_rgbd_seg = seg(f).transpose(1, 2).contiguous()                              # pvn3d.py:297
-            pred_kp_of = kpof(f).view(bs, 8, 3, n).permute(0, 1, 3, 2).contiguous()          # :298-302
-            pred_ctr_of = ctrof(f).view(bs, 1, 3, n).permute(0, 1, 3, 2).contiguous()        # :303-306
-    finally:
-        torch.backends.cudnn.allow_tf32, torch.backends.cuda.matmul.allow_tf32 = prev
-    return pred_kp_of, pred_rgbd_seg, pred_ctr_of
+@pytest.fixture(scope="module")
+def heads_golden(golden_dir):
+    return dict(np.load(os.path.join(golden_dir, "heads_ref.npz")))
 
 
-@pytest.mark.parametrize("b,n", [(2, 2048), (1, 12288), (2, 1000)])
-def test_fused_heads_match_reference_modules(cuda_dev, ref_modules, b, n):
-    g = torch.Generator().manual_seed(n)
-    rgb_emb = torch.randn(b, 128, n, generator=g).to(cuda_dev)
-    cld_emb = torch.randn(b, 128, n, generator=g).abs().to(cuda_dev)          # PointNet++ features are post-ReLU
-    want = _reference_forward(ref_modules, rgb_emb, cld_emb, allow_tf32=False)
-    want_tf32 = _reference_forward(ref_modules, rgb_emb, cld_emb, allow_tf32=True)
+@pytest.mark.parametrize("b,n", HEADS_CASES)
+def test_fused_heads_match_reference_modules(cuda_dev, ref_modules, heads_golden, b, n):
+    rgb_emb, cld_emb = (t.to(cuda_dev) for t in heads_inputs(b, n))
     eng = heads.FusedHeads(*ref_modules, device=cuda_dev)
     got = eng(rgb_emb, cld_emb)
-    for name, gt, w, wt in zip(("kp_of", "seg", "ctr_of"), got, want, want_tf32):
-        assert gt.shape == w.shape and gt.is_contiguous(), name
-        scale = float(w.abs().mean())
-        err, err_ref = (gt - w).abs(), (wt - w).abs()
-        print(f"{name} [{b}x{n}]: fused mean {float(err.mean()) / scale:.2e} max {float(err.max()) / scale:.2e} | "
-              f"cuDNN-TF32 reference: mean {float(err_ref.mean()) / scale:.2e} max {float(err_ref.max()) / scale:.2e}")
+    pts = torch.from_numpy(heads_points(n)).to(cuda_dev)
+    samples = (got[0][:, :, pts], got[1][:, pts], got[2][:, :, pts])
+    want = {}
+    for name, full, gt in zip(("kp_of", "seg", "ctr_of"), got, samples):
+        assert full.is_contiguous(), name
+        w = torch.from_numpy(heads_golden[f"{name}_{b}x{n}"]).to(cuda_dev)
+        want[name] = w
+        assert gt.shape == w.shape, name
+        scale = float(heads_golden[f"{name}_{b}x{n}_scale"])
+        err = (gt - w).abs()
+        print(f"{name} [{b}x{n}]: fused mean {float(err.mean()) / scale:.2e} max {float(err.max()) / scale:.2e}")
         assert float(err.mean()) <= 3e-3 * scale and float(err.max()) <= 3e-2 * scale, name
+    assert got[0].shape == (b, 8, n, 3) and got[1].shape == (b, n, 22) and got[2].shape == (b, 1, n, 3)
     # the predicted classes agree wherever the reference's own margin is not a rounding artefact
-    top2 = want[1].topk(2, dim=-1).values
-    clear = (top2[..., 0] - top2[..., 1]) > 1e-2 * float(want[1].abs().mean())
-    assert torch.equal(got[1].argmax(-1)[clear], want[1].argmax(-1)[clear])
+    top2 = want["seg"].topk(2, dim=-1).values
+    clear = (top2[..., 0] - top2[..., 1]) > 1e-2 * float(heads_golden[f"seg_{b}x{n}_scale"])
+    assert torch.equal(samples[1].argmax(-1)[clear], want["seg"].argmax(-1)[clear])
 
 
 def test_head_outputs_feed_the_pose_solver(cuda_dev, ref_modules):

@@ -110,26 +110,44 @@ def test_frame_shard_and_gather_gloo_world2(n_frames):
     assert all(ok for _, ok, _ in res) and all(mx == 2.0 for _, _, mx in res)
 
 
-@pytest.mark.skipif(not os.path.isdir("/root/reference/pvn3d"), reason="reference checkout not present")
-def test_unmodified_reference_binds_to_the_drop_in():
+def test_unmodified_reference_binds_to_the_drop_in(tmp_path):
     """`from lib.pointnet2_utils import _ext` (reference pointnet2_utils.py:19) resolves to this package's
-    module, and the post-processing names are rebound -- run in a subprocess to keep sys.modules clean."""
+    module, and the post-processing names are rebound.  This runs against a minimal stand-in of the reference
+    tree under tmp_path (lib/pointnet2_utils/pointnet2_utils.py importing _ext the way the reference does,
+    lib/utils/{meanshift_pytorch,pvn3d_eval_utils}.py defining the names demo.py calls), so it shows that
+    compat.install() rebinds those names, not that the real reference modules bind: that is covered only by
+    tests/test_reference_dropin_gpu.py where oracle/_ref/py is staged.  Run in a subprocess to keep sys.modules
+    clean."""
     import subprocess
+    files = {
+        "lib/__init__.py": "",
+        "lib/pointnet2_utils/__init__.py": "",
+        "lib/pointnet2_utils/pointnet2_utils.py": "from lib.pointnet2_utils import _ext\n",
+        "lib/utils/__init__.py": "",
+        "lib/utils/meanshift_pytorch.py": "class MeanShiftTorch:\n    pass\n",
+        "lib/utils/pvn3d_eval_utils.py": ("from lib.utils.meanshift_pytorch import MeanShiftTorch\n"
+                                          "def cal_frame_poses(*a):\n    raise AssertionError\n"
+                                          "def cal_frame_poses_lm(*a):\n    raise AssertionError\n"),
+    }
+    for rel, text in files.items():
+        f = tmp_path / rel
+        f.parent.mkdir(parents=True, exist_ok=True)
+        f.write_text(text)
     code = (
         "import sys; sys.path.insert(0, %r)\n"
         "from pvn3d_b200 import compat, _ext, meanshift\n"
-        "compat.install('/root/reference/pvn3d', patch_post=True)\n"
+        "compat.install(%r, patch_post=True)\n"
         "from lib.pointnet2_utils import pointnet2_utils as pu\n"
         "from lib.utils import pvn3d_eval_utils as ev, meanshift_pytorch as ms\n"
-        "from lib.pvn3d import Pointnet2MSG\n"
         "import torch\n"
         "assert pu._ext is _ext and ms.MeanShiftTorch is meanshift.MeanShiftTorch\n"
+        "assert ev.MeanShiftTorch is meanshift.MeanShiftTorch\n"
         "assert ev.cal_frame_poses.__module__ == 'pvn3d_b200.eval_utils'\n"
-        "m = Pointnet2MSG(input_channels=6)\n"
-        "try:\n    m(torch.zeros(1, 4096, 9)); raise SystemExit(3)\n"
+        "assert ev.cal_frame_poses_lm.__module__ == 'pvn3d_b200.eval_utils'\n"
+        "try:\n    pu._ext.furthest_point_sampling(torch.zeros(1, 4096, 3), 16); raise SystemExit(3)\n"
         "except RuntimeError as e:\n    assert 'CPU not supported' in str(e)\n"
-        "print('ok')\n") % os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-    r = subprocess.run([sys.executable, "-c", code], capture_output=True, text=True, cwd="/tmp")
+        "print('ok')\n") % (os.path.dirname(os.path.dirname(os.path.abspath(__file__))), str(tmp_path))
+    r = subprocess.run([sys.executable, "-c", code], capture_output=True, text=True, cwd=str(tmp_path))
     assert r.returncode == 0 and "ok" in r.stdout, r.stderr[-2000:]
 
 

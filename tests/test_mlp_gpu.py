@@ -1,4 +1,4 @@
-"""The tcgen05 shared-MLP layer kernel (csrc/mlp_tc.cu) against a float64 torch reference of the same
+"""The wgmma shared-MLP layer kernel (csrc/mlp_tc.cu) against a float64 torch reference of the same
 op on TF32-rounded operands, and the fused hot path A against features recorded from the REFERENCE
 Pointnet2MSG.  Tolerances: the kernel itself 2e-5 relative (fp32 accumulation order only); end to end
 the TF32 class of the reference's default cuDNN path (written at the assertion)."""
@@ -27,10 +27,10 @@ def ref_dense(a, w, b, relu, pool):
     (128, 32, 16, False, 0), (300, 64, 64, True, 0), (1000, 96, 128, True, 0), (512, 128, 196, True, 0),
     (512, 256, 384, True, 0), (640, 544, 256, True, 0), (2048, 384, 512, True, 32), (1024, 64, 32, True, 16),
     (256, 32, 16, False, 8), (131, 48, 80, True, 0),
-    # many tiles per persistent CTA (ring and both TMEM accumulators wrap), odd chunk counts, 2 column blocks
+    # many tiles per persistent CTA (ring and accumulator tile wrap), odd chunk counts, 2 column blocks
     (64000, 96, 128, True, 0), (70005, 32, 32, True, 0), (40960, 64, 64, True, 16), (9000, 544, 512, True, 0),
     (38400, 160, 272, True, 32),
-    # wide pooled layers: transposed accumulator (channel = TMEM lane), every pool size, ragged last tile, 1 / 2 / 4 column
+    # wide pooled layers: transposed accumulator read (channel = lane), every pool size, ragged last tile, 1 / 2 / 4 column
     # blocks, single-chunk K
     (8192, 96, 128, True, 32), (4144, 64, 128, True, 16), (8000, 224, 256, True, 8), (50016, 224, 256, True, 32),
     (2064, 256, 512, False, 16), (4096, 32, 1024, True, 32), (160, 384, 128, True, 16)])

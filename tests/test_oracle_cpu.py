@@ -156,7 +156,7 @@ def test_group_gather_interpolate_kat():
 
 def test_pn2_oracle_matches_reference_gpu_recording(golden_dir):
     """tests/golden/pn2_ref.npz = outputs of the UNMODIFIED reference op library (oracle/_ref/_ext.so) on a
-    B200 (tests/golden/make_golden_gpu.py).  This pins the C oracle to the reference bit for bit."""
+    GPU (tests/golden/make_golden_gpu.py).  This pins the C oracle to the reference bit for bit."""
     path = os.path.join(golden_dir, "pn2_ref.npz")
     if not os.path.exists(path):
         pytest.skip("pn2_ref.npz not recorded yet")

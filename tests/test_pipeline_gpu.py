@@ -1,4 +1,4 @@
-"""Hot path A end to end (Pointnet2MSG mirror on the sm_100a ops) against features recorded from the
+"""Hot path A end to end (Pointnet2MSG mirror on the sm_90a ops) against features recorded from the
 REFERENCE Pointnet2MSG (tests/golden/pn2msg.npz), and the FramePipeline on synthetic frames."""
 import os
 

@@ -1,4 +1,4 @@
-"""Parity of the sm_100a PointNet++ ops (through the C ABI) with the oracle and, when it loaded,
+"""Parity of the sm_90a PointNet++ ops (through the C ABI) with the oracle and, when it loaded,
 with the unmodified reference op library (oracle/_ref/_ext.so) on the same seeded inputs.
 
 Bar (BASELINE.json north_star): indices bit-exact; gathered / interpolated values bit-exact too

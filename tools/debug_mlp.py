@@ -1,4 +1,4 @@
-"""GPU-side diagnostics of the tcgen05 MLP layer kernel (prints, does not assert)."""
+"""GPU-side diagnostics of the wgmma MLP layer kernel (prints, does not assert)."""
 import sys, os
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import numpy as np

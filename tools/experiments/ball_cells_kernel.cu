@@ -1,7 +1,6 @@
-// PROTOTYPE for round 2 (NOT linked into libpvn3d_b200.so).  Run once on a B200 through
-// tools/experiments/ball_cells_test.cu at level-1 geometry (B=32, N=12288, M=2048, radii 0.0175/0.025):
-//   bit-exact (0 mismatches of 196 608 indices vs the CPU restatement, no centre over the list capacity), but
-//   cells_build 22 us + ball_cells 166 us  vs  ~150 us for the shipped ball_scan_kernel -- NOT yet a win:
+// PROTOTYPE (NOT linked into libpvn3d_b200.so), driven by tools/experiments/ball_cells_test.cu at level-1
+// geometry (B=32, N=12288, M=2048, radii 0.0175/0.025): its first version was bit-exact against the CPU
+//   restatement but slower than the shipped ball_scan_kernel (speed on the H100 not measured):
 //   on a surface scene ~8 points fall into a voxel and most of the 27 neighbour buckets are empty, so the
 //   warp spends 27 dependent bucket look-ups on steps that fill 0-8 of its 32 lanes.  The kernel below is
 //   already v2 (prefix-summed ranges, lanes walk the CONCATENATED candidate list: ~200 candidates = 7 full
@@ -21,7 +20,7 @@
 //                        list (dense cloud) is left to the index-order scan, which exits early there:
 //                        overflow[b*m + j] = 1 tells the caller to run ball_scan_kernel for that centre.
 //
-// Compile check:  nvcc -gencode arch=compute_100a,code=sm_100a -I pvn3d_b200/csrc -I include -c \
+// Compile check:  nvcc -gencode arch=compute_90a,code=sm_90a -I pvn3d_b200/csrc -I include -c \
 //                      tools/experiments/ball_cells_kernel.cu -o /dev/null
 #include "common.cuh"
 

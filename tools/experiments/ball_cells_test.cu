@@ -1,5 +1,5 @@
 // Stand-alone check + timing of the cell-list ball query draft (ball_cells_kernel.cu) on a GPU:
-//   nvcc -gencode arch=compute_100a,code=sm_100a -O3 -I pvn3d_b200/csrc -I include \
+//   nvcc -gencode arch=compute_90a,code=sm_90a -O3 -I pvn3d_b200/csrc -I include \
 //        tools/experiments/ball_cells_test.cu pvn3d_b200/csrc/runtime.cu -o tools/experiments/ball_cells_test
 // Scene: a raster-ordered depth image of a plane with boxes on it (like the bench clouds), level-1 geometry
 // (N = 12288, M = 2048 centres taken from the cloud, radii 0.0175 / 0.025, nsample 16 / 32).
@@ -84,7 +84,7 @@ int main() {
   cudaEventElapsedTime(&t_build, e0, e1);
   cudaEventElapsedTime(&t_query, e1, e2);
   printf("cuda status: %s\n", cudaGetErrorString(cudaGetLastError()));
-  printf("B=%d N=%d M=%d: cells_build %.1f us, ball_cells %.1f us (ball_scan_kernel of round 1: ~150 us)\n", B, N, M,
+  printf("B=%d N=%d M=%d: cells_build %.1f us, ball_cells %.1f us\n", B, N, M,
          t_build * 1e3, t_query * 1e3);
   std::vector<unsigned char> over(static_cast<size_t>(B) * M);
   cudaMemcpy(over.data(), a.overflow, over.size(), cudaMemcpyDeviceToHost);

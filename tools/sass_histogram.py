@@ -3,8 +3,7 @@
 
     python tools/sass_histogram.py r02
 
-Evidence for the claims DESIGN.md makes about the instruction mix (tcgen05 = UTCHMMA / UTCBAR / LDTM /
-UTCATOMSWS, TMA engine = UBLKCP / UTMALDG / UTMASTG, cp.async = LDGSTS, mbarrier = SYNCS, packed fp32 =
+Evidence for the claims DESIGN.md makes about the instruction mix (wgmma = HGMMA, TMA engine = UBLKCP / UTMALDG / UTMASTG, cp.async = LDGSTS, mbarrier = SYNCS, packed fp32 =
 FFMA2 / FADD2 / FMUL2, special function unit = MUFU.EX2, warp reductions = REDUX).  Runs on CPU
 (cuobjdump -sass of pvn3d_b200/_build/*.o); the objects are the ones linked into libpvn3d_b200.so.
 """
@@ -16,7 +15,7 @@ import sys
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 OBJ = os.path.join(ROOT, "pvn3d_b200", "_build")
-WATCH = ["UTCHMMA", "UTCQMMA", "UTCBAR", "UTCATOMSWS", "LDTM", "STTM", "UTMALDG", "UTMASTG", "UBLKCP", "UTMAPF", "LDGSTS",
+WATCH = ["HGMMA", "UTCHMMA", "UTCQMMA", "UTCBAR", "UTCATOMSWS", "LDTM", "STTM", "UTMALDG", "UTMASTG", "UBLKCP", "UTMAPF", "LDGSTS",
          "SYNCS", "HMMA", "MUFU.EX2", "MUFU.RSQ", "MUFU.RCP", "FFMA2", "FADD2", "FMUL2", "REDUX", "SHFL", "ATOMS", "ATOMG",
          "RED", "BAR.SYNC", "MEMBAR", "LDG", "STG", "LDS", "STS", "FFMA", "IMAD"]
 
@@ -64,8 +63,8 @@ def main():
                 if c:
                     counts[w] = c
             rows.append((f.replace(".o", ".cu"), d, total, counts))
-    lines = [f"# SASS opcode histogram, tag {tag}: `cuobjdump -sass pvn3d_b200/_build/*.o` (sm_100a, the objects linked into libpvn3d_b200.so)",
-             "", "Static instruction counts per kernel (not execution counts).  tcgen05: UTCHMMA (mma), UTCBAR (commit), LDTM (tcgen05.ld);",
+    lines = [f"# SASS opcode histogram, tag {tag}: `cuobjdump -sass pvn3d_b200/_build/*.o` (sm_90a, the objects linked into libpvn3d_b200.so)",
+             "", "Static instruction counts per kernel (not execution counts).  wgmma: HGMMA;",
              "TMA engine: UBLKCP (1-D bulk copy), UTMALDG/UTMASTG (tensor-map loads/stores); cp.async: LDGSTS; mbarrier: SYNCS.", "",
              "| source | kernel | SASS instr | watched opcodes |", "|---|---|---:|---|"]
     for src, d, total, counts in rows:
