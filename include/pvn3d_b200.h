@@ -242,6 +242,19 @@ int pvn3d_sa_centre_term(const float *centres, const float *wx, const float *bia
 int pvn3d_mlp_sa_fact(const float *u, const float *v, int ldu, int c_valid, const int *idx, int b, int n, int m,
                       int ns, const float *w, const float *bias, int k_pad, int n_pad, int flags, int pool,
                       float *out, int ldo, int col0, pvn3d_stream_t stream);
+/* Layers 2 AND 3 of a factored SA scale plus the max-pool over nsample, in one launch: the layer-2 activations
+ * stay in shared memory instead of going through HBM.  Same result, bit for bit, as
+ *   pvn3d_mlp_sa_fact(.., layer2, PVN3D_MLP_RELU | PVN3D_MLP_ROUND_OUT, pool = 0)  ->  h
+ *   pvn3d_mlp_dense(h, .., layer3, PVN3D_MLP_RELU [| PVN3D_MLP_ROUND_OUT], pool = ns) -> out
+ * pool must equal ns.  Both layers apply ReLU; flags: PVN3D_MLP_ROUND_OUT (pooled output) and
+ * PVN3D_MLP_RESERVE_SMS(n).  layer3->k_pad >= layer2->n_pad.  Any number of layer-2 K chunks.
+ * PVN3D_ERR_UNSUPPORTED (nothing launched) unless pvn3d_mlp_sa_fact2_supported(layer2, layer3, ns) is 1: ns 16 or 32,
+ * both n_pad <= 128, and both weight matrices, the layer-2 tile and two operand stages fit in a block's shared memory.
+ * The query is host-only and touches no device memory. */
+int pvn3d_mlp_sa_fact2(const float *u, const float *v, int ldu, int c_valid, const int *idx, int b, int n, int m,
+                       int ns, const pvn3d_mlp_layer_t *layer2, const pvn3d_mlp_layer_t *layer3, int flags, int pool,
+                       float *out, int ldo, int col0, pvn3d_stream_t stream);
+int pvn3d_mlp_sa_fact2_supported(const pvn3d_mlp_layer_t *layer2, const pvn3d_mlp_layer_t *layer3, int ns);
 /* FACTORED first layer of an FP module: three_interpolate commutes with the (linear) first layer, so
  *   P = W1k . known      once per KNOWN point   (pvn3d_mlp_dense without ReLU on the known table),
  *   S = W1s . skip + b1  over the skip columns  (pvn3d_mlp_dense without ReLU on the skip table),

@@ -988,6 +988,305 @@ int launch_mlp(MlpArgs &a, cudaStream_t st) {
 }
 
 // =====================================================================================================
+// Layers 2 and 3 of a FACTORED SA scale and the max-pool over nsample in ONE persistent kernel.
+//
+// As two launches (pvn3d_mlp_sa_fact with ROUND_OUT, then pvn3d_mlp_dense with pool = ns) the TF32-rounded
+// layer-2 activations H go to HBM and straight back: 67-400 MB per scale and 32-frame batch, far more than
+// L2 holds.  Here they never leave the SM.  Per 128-row tile (whole centres: 128 % ns == 0):
+//   producers (warps 0-7)  stage A1 = tf32(relu(U[idx] - V)) into a ring of K-chunk stages, exactly as the
+//                          PRO_SA_FACT producer of mlp_layer_kernel, running ahead across tiles;
+//   MMA       (warps 8-15) warpgroup wg accumulates rows 64wg..64wg+63 of layer 2 in registers (W2 resident in
+//                          shared memory), writes tf32(relu(acc + b2)) into ITS 64 rows of a K-major SWIZZLE_128B
+//                          H tile, runs layer 3 from that tile (W3 resident), and pools the layer-3 fragment in
+//                          registers: max over the 16 rows of a warp by a transposing shuffle butterfly (a
+//                          32-row centre combines two warps through shared memory), then + b3, ReLU, rounding
+//                          and the store into the column slice col0.. of the level table.
+// Same operands, the same wgmma N and K order per output element and the same epilogue arithmetic as the two
+// launches, so the results are bit-identical (max commutes with the bias add: rounding is monotone).
+constexpr int kSa2Threads = (kMlpProWarps + kMlpMmaWarps) * 32;
+constexpr int kSa2MaxStages = 8;
+constexpr uint32_t kSa2StageBytes = kMlpBM * 128u;   // one A chunk: 128 rows x 32 tf32
+
+struct Sa2Args {
+  MlpArgs a;            // PRO_SA_FACT producer fields, rows, out / ldo / col0 / round_out / pool; w, bias, k_pad, n_pad: layer 2
+  const float *w3, *bias3;
+  int k3_pad, n3_pad;   // k3_pad >= n_pad of layer 2; its columns past that are zero
+};
+
+struct Sa2SmemCtl {
+  uint64_t full[kSa2MaxStages];   // 128 arrivals: every producer thread of the filling group
+  uint64_t empty[kSa2MaxStages];  // 8 arrivals: one per MMA warp, once its layer-2 MMAs that read the stage have retired
+};
+
+// shared-memory layout behind the 1024-byte aligned base (kernel and launcher use the same function):
+// [W2: k2_pad/32 chunks of n2 x 128 B][W3: k3_pad/32 chunks of n3 x 128 B][H: k3_pad/32 chunks of 128 x 128 B]
+// [A ring: stages x 16 KB][pool exchange: 2 warpgroups x 2 warp pairs x max(n3, 32) floats][barriers]
+struct Sa2Smem {
+  uint32_t w2, w3, h, ring, xchg, ctl, bytes;   // offsets from the aligned base; bytes = dynamic size incl. alignment slack
+};
+static inline __host__ __device__ Sa2Smem sa2_smem(int k2_pad, int n2, int k3_pad, int n3, int stages) {
+  Sa2Smem s;
+  s.w2 = 0;
+  s.w3 = s.w2 + static_cast<uint32_t>(k2_pad / 32) * static_cast<uint32_t>(n2) * 128u;
+  s.h = s.w3 + static_cast<uint32_t>(k3_pad / 32) * static_cast<uint32_t>(n3) * 128u;
+  s.ring = s.h + static_cast<uint32_t>(k3_pad / 32) * kMlpBM * 128u;
+  s.xchg = s.ring + static_cast<uint32_t>(stages) * kSa2StageBytes;
+  s.ctl = s.xchg + 4u * static_cast<uint32_t>(n3 > 32 ? n3 : 32) * 4u;   // 32 lanes x max(1, n3 / 32) maxima per warp pair
+  s.bytes = 1024u + s.ctl + static_cast<uint32_t>(sizeof(Sa2SmemCtl));
+  return s;
+}
+
+__device__ __forceinline__ void named_bar_sync(int id, int threads) {
+  asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(threads) : "memory");
+}
+__device__ __forceinline__ void named_bar_arrive(int id, int threads) {
+  asm volatile("bar.arrive %0, %1;" ::"r"(id), "r"(threads) : "memory");
+}
+
+// `rows` rows x `k_pad` columns of a TF32-rounded weight matrix -> n rows of K-major SWIZZLE_128B chunks (rows >= rows zero)
+__device__ __forceinline__ void stage_weights(uint32_t dst, const float *w, int rows, int k_pad, int n) {
+  const int per_chunk = n * 8;
+  for (int i = threadIdx.x; i < (k_pad / 32) * per_chunk; i += blockDim.x) {
+    const int kc = i / per_chunk, r = (i - kc * per_chunk) >> 3, c = i & 7;
+    const float4 v = r < rows ? ldg128(w + static_cast<size_t>(r) * k_pad + kc * 32 + c * 4) : make_float4(0.f, 0.f, 0.f, 0.f);
+    sts128(dst + static_cast<uint32_t>(kc * per_chunk) * 16u + sw128_off(r, c), v.x, v.y, v.z, v.w);
+  }
+}
+
+// Layer 2 of one tile for warpgroup wg: K chunks of the ring x resident W2 into registers, then
+// H[row, c] = tf32(relu(acc + b2[c])) into the warpgroup's rows of the H tile (columns c < k3_pad; the rest of a
+// wgmma N wider than k3_pad is never read).  Stages are released once their MMAs have retired.
+template <int N2>
+__device__ __forceinline__ void sa2_layer2(const Sa2Args &g, uint32_t ring, uint32_t w2_s, uint32_t h_s, int S,
+                                           int it_base, int kc2, Sa2SmemCtl &ctl, unsigned wg, int frag_row,
+                                           unsigned lane) {
+  float d[N2 / 2];
+#pragma unroll
+  for (int i = 0; i < N2 / 2; ++i) d[i] = 0.f;
+  // chunk kc-1 is released as soon as its MMAs have retired (while chunk kc runs), so a tile may have more K
+  // chunks than the ring has stages
+  int prev = -1;
+  for (int kc = 0; kc < kc2; ++kc) {
+    const int it = it_base + kc;
+    const int s = it % S;
+    mbar_wait(&ctl.full[s], static_cast<unsigned>((it / S) & 1));
+    fence_proxy_async_smem();
+    const uint64_t adesc = smem_desc_sw128(ring + static_cast<uint32_t>(s) * kSa2StageBytes + wg * 8192u);
+    const uint64_t bdesc = smem_desc_sw128(w2_s + static_cast<uint32_t>(kc * N2) * 128u);
+    wgmma_fence();
+#pragma unroll
+    for (int k4 = 0; k4 < 4; ++k4)
+      wgmma_tf32<N2>(d, adesc + static_cast<uint64_t>(k4 * 2), bdesc + static_cast<uint64_t>(k4 * 2), (kc > 0 || k4 > 0) ? 1u : 0u);
+    wgmma_commit();
+    if (prev >= 0) {
+      wgmma_wait<1>();
+      if (lane == 0) mbar_arrive(&ctl.empty[prev]);
+    }
+    prev = s;
+  }
+  wgmma_wait<0>();
+  acc_fence(d);
+  if (lane == 0) mbar_arrive(&ctl.empty[prev]);
+  // every warp of the warpgroup has finished the previous tile's layer 3 (its reads of H and of the pool exchange)
+  named_bar_sync(1 + static_cast<int>(wg), 128);
+  const int n2 = g.a.n_pad;
+#pragma unroll
+  for (int j = 0; j < N2 / 8; ++j) {
+    if (8 * j >= g.k3_pad) break;
+    const int c = 8 * j + 2 * static_cast<int>(lane & 3u);
+    const float b0 = c < n2 ? __ldg(g.a.bias + c) : 0.f, b1 = c + 1 < n2 ? __ldg(g.a.bias + c + 1) : 0.f;
+    const uint32_t off = static_cast<uint32_t>(c >> 5) * (kMlpBM * 128u) + static_cast<uint32_t>(frag_row) * 128u +
+                         ((static_cast<uint32_t>(((c & 31) >> 2) ^ (frag_row & 7))) << 4) + (c & 3) * 4u;
+    asm volatile("st.shared.v2.f32 [%0], {%1,%2};" ::"r"(h_s + off), "f"(to_tf32(fmaxf(d[4 * j] + b0, 0.f))),
+                 "f"(to_tf32(fmaxf(d[4 * j + 1] + b1, 0.f)))
+                 : "memory");
+    asm volatile("st.shared.v2.f32 [%0], {%1,%2};" ::"r"(h_s + off + 8u * 128u), "f"(to_tf32(fmaxf(d[4 * j + 2] + b0, 0.f))),
+                 "f"(to_tf32(fmaxf(d[4 * j + 3] + b1, 0.f)))
+                 : "memory");
+  }
+  fence_proxy_async_smem();   // generic-proxy stores of H -> visible to the tensor core
+  named_bar_sync(1 + static_cast<int>(wg), 128);
+}
+
+// one level of a max over lanes that differ in bit O: lanes keep the lower (bit clear) or upper (bit set) HALF of
+// their values, combined with the partner's; HALF == 0: plain reduction of p[0]
+template <int HALF, int O, int NV>
+__device__ __forceinline__ void rowmax_level(float (&p)[NV], unsigned lane) {
+  if constexpr (HALF >= 1) {
+    const bool hi = (lane & static_cast<unsigned>(O)) != 0;
+#pragma unroll
+    for (int i = 0; i < HALF; ++i) {
+      const float keep = hi ? p[i + HALF] : p[i];
+      const float send = hi ? p[i] : p[i + HALF];
+      p[i] = fmaxf(keep, __shfl_xor_sync(0xffffffffu, send, O));
+    }
+  } else {
+    p[0] = fmaxf(p[0], __shfl_xor_sync(0xffffffffu, p[0], O));
+  }
+}
+
+template <int N3>
+__global__ void __launch_bounds__(kSa2Threads, 1) mlp_sa_fact2_kernel(const __grid_constant__ Sa2Args g) {
+  const MlpArgs &a = g.a;
+  extern __shared__ unsigned char mlp_smem_raw[];
+  const uint32_t raw = smem_u32(mlp_smem_raw);
+  const uint32_t base = (raw + 1023u) & ~1023u;   // SWIZZLE_128B atoms are 8 rows x 128 B
+  const int n2_mma = mma_n(a.n_pad);
+  const int kc2 = a.k_pad / 32, kc3 = g.k3_pad / 32;
+  const int S = a.stages;   // what the launcher's budget left (it computes the layout with the same function)
+  const Sa2Smem L = sa2_smem(a.k_pad, n2_mma, g.k3_pad, N3, S);
+  Sa2SmemCtl &ctl = *reinterpret_cast<Sa2SmemCtl *>(mlp_smem_raw + (base - raw) + L.ctl);
+  const int t = threadIdx.x;
+  const unsigned warp = t >> 5, lane = t & 31u;
+  const int tiles = static_cast<int>((a.rows + kMlpBM - 1) / kMlpBM);   // the launcher checks tiles * kc2 < 2^31
+
+  stage_weights(base + L.w2, a.w, a.n_pad, a.k_pad, n2_mma);
+  stage_weights(base + L.w3, g.w3, g.n3_pad, g.k3_pad, N3);
+  // H columns past the layer-2 MMA width are K padding of layer 3: zero once, never written again
+  for (uint32_t i = t; i < static_cast<uint32_t>(kc3) * kMlpBM * 8u; i += kSa2Threads) sts128(base + L.h + i * 16u, 0.f, 0.f, 0.f, 0.f);
+  if (t == 0) {
+    for (int s = 0; s < S; ++s) {
+      mbar_init(&ctl.full[s], 128);
+      mbar_init(&ctl.empty[s], kMlpMmaWarps);
+    }
+    mbar_fence_init();
+  }
+  fence_proxy_async_smem();   // resident weights / zeroed H (generic stores) -> tensor-core proxy
+  __syncthreads();
+
+  if (warp < kMlpProWarps) {
+    // ================= producers: group grp stages the chunks it & 1 == grp (whole tiles when K is one chunk) ====
+    const int pt = t & 127;
+    const unsigned grp = warp >> 2;
+    const int pw = pt >> 5, sub = static_cast<int>(lane & 7u), rg = static_cast<int>(lane >> 3);
+    const int r_first = 32 * pw + rg;
+    int it_base = 0;
+    for (int tile = blockIdx.x; tile < tiles; tile += gridDim.x, it_base += kc2) {
+      if (kc2 == 1 && static_cast<unsigned>(it_base & 1) != grp) continue;
+      const long long p_first = static_cast<long long>(tile) * kMlpBM + r_first;
+      RowState rs;
+      rows_setup<PRO_SA_FACT>(a, p_first, rs);
+      for (int kc = 0; kc < kc2; ++kc) {
+        const int it = it_base + kc;
+        if (static_cast<unsigned>(it & 1) != grp) continue;
+        const int s = static_cast<int>(it % S);
+        mbar_wait(&ctl.empty[s], static_cast<unsigned>(((it / S) & 1) ^ 1));
+        stage_a_chunk<PRO_SA_FACT>(a, rs, p_first, r_first, sub, kc * 32, base + L.ring + static_cast<uint32_t>(s) * kSa2StageBytes,
+                                   true);
+        fence_proxy_async_smem();
+        mbar_arrive(&ctl.full[s]);
+      }
+    }
+  } else {
+    // ================= MMA + epilogue: warpgroup wg, warp w4 of it holds rows 64wg + 16w4 .. +15 of the tile ======
+    const unsigned mw = warp - kMlpProWarps, wg = mw >> 2, w4 = mw & 3u;
+    const int frag_row = static_cast<int>(64 * wg + 16 * w4 + (lane >> 2));
+    const uint32_t h_wg = base + L.h + wg * 8192u;
+    const uint32_t xchg = base + L.xchg + (wg * 2u + (w4 >> 1)) * ((N3 > 32 ? N3 : 32) * 4u);
+    constexpr int NV = N3 / 4;                 // values per lane after the max over its two rows
+    constexpr int NF = NV >= 8 ? NV / 8 : 1;   // ... and after the max over the 8 lane groups
+    int it_base = 0;
+    for (int tile = blockIdx.x; tile < tiles; tile += gridDim.x, it_base += kc2) {
+      const long long p0 = static_cast<long long>(tile) * kMlpBM;
+      if (n2_mma == 16) sa2_layer2<16>(g, base + L.ring, base + L.w2, base + L.h, S, it_base, kc2, ctl, wg, frag_row, lane);
+      else if (n2_mma == 32) sa2_layer2<32>(g, base + L.ring, base + L.w2, base + L.h, S, it_base, kc2, ctl, wg, frag_row, lane);
+      else if (n2_mma == 64) sa2_layer2<64>(g, base + L.ring, base + L.w2, base + L.h, S, it_base, kc2, ctl, wg, frag_row, lane);
+      else sa2_layer2<128>(g, base + L.ring, base + L.w2, base + L.h, S, it_base, kc2, ctl, wg, frag_row, lane);
+      // ---- layer 3: A = this warpgroup's 64 rows of H, B = resident W3, same K order as the per-layer kernel
+      float d[N3 / 2];
+#pragma unroll
+      for (int i = 0; i < N3 / 2; ++i) d[i] = 0.f;
+      wgmma_fence();
+      for (int kc = 0; kc < kc3; ++kc) {
+        const uint64_t adesc = smem_desc_sw128(h_wg + static_cast<uint32_t>(kc) * (kMlpBM * 128u));
+        const uint64_t bdesc = smem_desc_sw128(base + L.w3 + static_cast<uint32_t>(kc * N3) * 128u);
+#pragma unroll
+        for (int k4 = 0; k4 < 4; ++k4)
+          wgmma_tf32<N3>(d, adesc + static_cast<uint64_t>(k4 * 2), bdesc + static_cast<uint64_t>(k4 * 2), (kc > 0 || k4 > 0) ? 1u : 0u);
+      }
+      wgmma_commit();
+      wgmma_wait<0>();
+      acc_fence(d);
+      // ---- max over the warp's 16 rows: the lane's two rows, then a transposing butterfly over lane bits 4, 3, 2
+      // (lanes that differ there hold the same columns); p[2j + e] is column 8j + 2 (lane & 3) + e
+      float p[NV];
+#pragma unroll
+      for (int j = 0; j < N3 / 8; ++j) {
+        p[2 * j] = fmaxf(d[4 * j], d[4 * j + 2]);
+        p[2 * j + 1] = fmaxf(d[4 * j + 1], d[4 * j + 3]);
+      }
+      rowmax_level<NV / 2, 16>(p, lane);
+      rowmax_level<NV / 4, 8>(p, lane);
+      rowmax_level<NV / 8, 4>(p, lane);
+      // a 32-row centre: the odd warp of each pair hands its 16-row maxima to the even one
+      bool owner = true;
+      long long grow = (p0 + 64 * wg + 16 * w4) / 16;
+      if (a.pool == 32) {
+        if (w4 & 1u) {
+#pragma unroll
+          for (int i = 0; i < NF; ++i)
+            asm volatile("st.shared.f32 [%0], %1;" ::"r"(xchg + (lane * NF + i) * 4u), "f"(p[i]) : "memory");
+          named_bar_arrive(3 + static_cast<int>(wg * 2 + (w4 >> 1)), 64);
+          owner = false;
+        } else {
+          named_bar_sync(3 + static_cast<int>(wg * 2 + (w4 >> 1)), 64);
+#pragma unroll
+          for (int i = 0; i < NF; ++i) {
+            float q;
+            asm volatile("ld.shared.f32 %0, [%1];" : "=f"(q) : "r"(xchg + (lane * NF + i) * 4u) : "memory");
+            p[i] = fmaxf(p[i], q);
+          }
+        }
+        grow = (p0 + 64 * wg + 32 * (w4 >> 1)) / 32;
+      }
+      // the group's rows exist entirely or not at all (rows % pool == 0); NV < 8 leaves duplicates in lane bit 2
+      if (owner && grow * a.pool < a.rows && (NV >= 8 || !(lane & 4u))) {
+        const unsigned b4 = (lane >> 4) & 1u, b3 = (lane >> 3) & 1u, b2 = (lane >> 2) & 1u;
+        float *o = a.out + grow * a.ldo + a.col0;
+#pragma unroll
+        for (int i = 0; i < NF; ++i) {
+          const int io = i + (b4 ? NV / 2 : 0) + (b3 && NV >= 4 ? NV / 4 : 0) + (b2 && NV >= 8 ? NV / 8 : 0);
+          const int col = 8 * (io >> 1) + 2 * static_cast<int>(lane & 3u) + (io & 1);
+          if (col < g.n3_pad) {
+            float r = fmaxf(p[i] + __ldg(g.bias3 + col), 0.f);
+            if (a.round_out) r = to_tf32(r);
+            o[col] = r;
+          }
+        }
+      }
+    }
+  }
+}
+
+// ring stages pvn3d_mlp_sa_fact2 runs a scale with; 0: the scale is not covered (nsample other than 16 / 32, a layer
+// wider than 128 columns, or resident weights + H tile + two stages beyond the shared memory of a block)
+int sa2_stages(int k2_pad, int n2_pad, int k3_pad, int n3_pad, int ns) {
+  if ((ns != 16 && ns != 32) || n2_pad > 128 || n3_pad > 128) return 0;
+  const uint32_t fixed = sa2_smem(k2_pad, mma_n(n2_pad), k3_pad, mma_n(n3_pad), 0).bytes;
+  if (fixed >= static_cast<uint32_t>(kMlpSmemMax)) return 0;
+  const int stages = std::min<int>(kSa2MaxStages, static_cast<int>((kMlpSmemMax - fixed) / kSa2StageBytes));
+  return stages >= 2 ? stages : 0;   // the two producer groups alternate stages
+}
+
+template <int N3>
+int launch_sa_fact2(Sa2Args &g, int stages, cudaStream_t st) {
+  MlpArgs &a = g.a;
+  if (a.rows <= 0) return PVN3D_OK;
+  a.stages = stages;
+  const size_t smem = sa2_smem(a.k_pad, mma_n(a.n_pad), g.k3_pad, N3, stages).bytes;
+  const int sms = std::max(1, sm_count() - a.reserve_sms);
+  const long long tiles = (a.rows + kMlpBM - 1) / kMlpBM;
+  if (tiles * (a.k_pad / 32) > 0x7fffffffll) return PVN3D_ERR_UNSUPPORTED;   // the kernel counts K chunks in 32 bits
+  auto kern = mlp_sa_fact2_kernel<N3>;
+  static PerDeviceOnce once;
+  PVN3D_ONCE_PER_DEVICE(once, cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, kMlpSmemMax),
+                        "mlp sa_fact2 smem attr");
+  const unsigned grid = static_cast<unsigned>(std::min<long long>(tiles, sms));
+  kern<<<grid, kSa2Threads, smem, st>>>(g);
+  return check_launch("mlp_sa_fact2_kernel");
+}
+
+// =====================================================================================================
 // The whole SharedMLP of one SA scale (3 layers) / FP module (2 layers) in ONE persistent kernel.
 //
 // One launch per layer sends every inter-layer activation through HBM twice (write + read: 7.0 of the
@@ -1689,6 +1988,47 @@ extern "C" int pvn3d_mlp_sa_fact(const float *u, const float *v, int ldu, int c_
   a.relu = flags & PVN3D_MLP_RELU; a.round_out = (flags & PVN3D_MLP_ROUND_OUT) ? 1 : 0;
   a.reserve_sms = (flags >> 8) & 0xff;
   return dispatch(a, PRO_SA_FACT, pool, as_stream(stream));
+}
+
+extern "C" int pvn3d_mlp_sa_fact2(const float *u, const float *v, int ldu, int c_valid, const int *idx, int b, int n,
+                                  int m, int ns, const pvn3d_mlp_layer_t *layer2, const pvn3d_mlp_layer_t *layer3,
+                                  int flags, int pool, float *out, int ldo, int col0, pvn3d_stream_t stream) {
+  if (!u || !v || !idx || !layer2 || !layer3 || !layer2->w || !layer2->bias || !layer3->w || !layer3->bias || !out ||
+      b < 0 || n <= 0 || m < 0 || ns <= 0 || c_valid <= 0 || c_valid % 4 || ldu < c_valid || ldu % 4 ||
+      layer2->k_pad < c_valid || layer2->k_pad <= 0 || layer2->k_pad % 32 || layer2->n_pad <= 0 || layer2->n_pad % 16 ||
+      layer3->k_pad < layer2->n_pad || layer3->k_pad % 32 || layer3->n_pad <= 0 || layer3->n_pad % 16 || ldo % 4 ||
+      col0 % 4 || (reinterpret_cast<uintptr_t>(u) & 15u) || (reinterpret_cast<uintptr_t>(v) & 15u) ||
+      (reinterpret_cast<uintptr_t>(layer2->w) & 15u) || (reinterpret_cast<uintptr_t>(layer3->w) & 15u))
+    return PVN3D_ERR_INVALID_ARG;
+  if (pool != ns) return PVN3D_ERR_INVALID_ARG;
+  const int stages = sa2_stages(layer2->k_pad, layer2->n_pad, layer3->k_pad, layer3->n_pad, ns);
+  if (!stages) return PVN3D_ERR_UNSUPPORTED;
+  if (static_cast<long long>(m) * ns > 0x3fffffffll || static_cast<long long>(b) * n > 0x7fffffffll ||
+      static_cast<long long>(b) * m > 0x7fffffffll)
+    return PVN3D_ERR_UNSUPPORTED;
+  Sa2Args g{};
+  MlpArgs &a = g.a;
+  a.w = layer2->w; a.bias = layer2->bias; a.k_pad = layer2->k_pad; a.n_pad = layer2->n_pad;
+  a.rows = static_cast<long long>(b) * m * ns;
+  a.feat = u; a.new_xyz = v; a.ldf = ldu; a.c_feat = c_valid; a.idx = idx;
+  a.n = n; a.m = m; a.ns = ns; a.pool = pool;
+  a.out = out; a.ldo = ldo; a.col0 = col0; a.relu = 1;
+  a.round_out = (flags & PVN3D_MLP_ROUND_OUT) ? 1 : 0;
+  a.reserve_sms = (flags >> 8) & 0xff;
+  g.w3 = layer3->w; g.bias3 = layer3->bias; g.k3_pad = layer3->k_pad; g.n3_pad = layer3->n_pad;
+  switch (mma_n(layer3->n_pad)) {
+    case 16: return launch_sa_fact2<16>(g, stages, as_stream(stream));
+    case 32: return launch_sa_fact2<32>(g, stages, as_stream(stream));
+    case 64: return launch_sa_fact2<64>(g, stages, as_stream(stream));
+    default: return launch_sa_fact2<128>(g, stages, as_stream(stream));
+  }
+}
+
+extern "C" int pvn3d_mlp_sa_fact2_supported(const pvn3d_mlp_layer_t *layer2, const pvn3d_mlp_layer_t *layer3, int ns) {
+  if (!layer2 || !layer3 || layer2->k_pad <= 0 || layer2->k_pad % 32 || layer2->n_pad <= 0 || layer2->n_pad % 16 ||
+      layer3->k_pad < layer2->n_pad || layer3->k_pad % 32 || layer3->n_pad <= 0 || layer3->n_pad % 16)
+    return 0;
+  return sa2_stages(layer2->k_pad, layer2->n_pad, layer3->k_pad, layer3->n_pad, ns) ? 1 : 0;
 }
 
 extern "C" int pvn3d_mlp_fp_fact(const float *p, const float *s, int ld, int c_valid, const int *nn_idx,

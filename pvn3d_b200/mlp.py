@@ -162,6 +162,34 @@ def mlp_sa_fact(u: torch.Tensor, v: torch.Tensor, idx: torch.Tensor, n: int, lay
     return out
 
 
+def _layer_struct(layer: PackedLayer) -> _lib.MlpLayer:
+    return _lib.MlpLayer(layer.w.data_ptr(), layer.bias.data_ptr(), layer.k_pad, layer.n_pad)
+
+
+def sa_fact2_fits(layer2: PackedLayer, layer3: PackedLayer, ns: int) -> bool:
+    """whether pvn3d_mlp_sa_fact2 takes the scale (the library's own rule: nsample 16 or 32, both layers at most 128
+    columns, weights + layer-2 tile within shared memory -- SA1 and SA2)"""
+    l2, l3 = _layer_struct(layer2), _layer_struct(layer3)
+    return bool(_lib.load().pvn3d_mlp_sa_fact2_supported(ctypes.addressof(l2), ctypes.addressof(l3), ns))
+
+
+def mlp_sa_fact2(u: torch.Tensor, v: torch.Tensor, idx: torch.Tensor, n: int, layer2: PackedLayer, layer3: PackedLayer,
+                 out=None, col0=0, round_out=False, reserve=0):
+    """layers 2 and 3 of a factored SA scale + max-pool over nsample in one launch (pvn3d_mlp_sa_fact2): the same bits
+    as mlp_sa_fact(.., layer2, round_out=True) -> mlp_dense(.., layer3, pool=ns, a_tf32=True)"""
+    lib = _lib.load()
+    b, m, ns = idx.shape
+    if out is None:
+        out = torch.empty((b * m, layer3.n_pad), dtype=torch.float32, device=u.device)
+    l2, l3 = _layer_struct(layer2), _layer_struct(layer3)
+    with torch.cuda.device(u.device):
+        rc = lib.pvn3d_mlp_sa_fact2(ptr(u), ptr(v), u.size(-1), u.size(-1), ptr(idx), b, n, m, ns, ctypes.addressof(l2),
+                                    ctypes.addressof(l3), _flags(True, round_out, reserve=reserve), ns, ptr(out), out.size(-1),
+                                    col0, _stream(u.device))
+    check(rc, "pvn3d_mlp_sa_fact2")
+    return out
+
+
 def mlp_fp_fact(p: torch.Tensor, s_: torch.Tensor, nn_idx: torch.Tensor, nn_w: torch.Tensor, m_known: int,
                 layer: PackedLayer, relu=True, round_out=False, reserve=0, out_cn=False):
     """second layer of a factored FP module: rows relu(sum_t w_t P[idx_t] + S) -> layer (pvn3d_mlp_fp_fact).
@@ -446,6 +474,12 @@ class FusedPointnet2MSG:
                     u = mlp_dense(table, first, relu=False, a_tf32=True, reserve=rs)        # once per point
                     v = sa_centre_term(new_xyz, wx, b1)                                     # once per centre
                     last2 = len(layers) == 2
+                    if len(layers) == 3 and sa_fact2_fits(layers[1], layers[2], ns):
+                        # SA1 / SA2: layer 2 stays on chip (DESIGN.md section 4)
+                        mlp_sa_fact2(u, v, idx, x.size(1), layers[1], layers[2], out=out_l.view(b * npoint, -1), col0=col,
+                                     round_out=self.round_tables and li < 3, reserve=rs)
+                        col += layers[-1].n
+                        continue
                     h = mlp_sa_fact(u, v, idx, x.size(1), layers[1], pool=ns if last2 else 0, round_out=not last2 or
                                     (self.round_tables and li < 3), reserve=rs,
                                     out=out_l.view(b * npoint, -1) if last2 else None, col0=col if last2 else 0)
