@@ -255,6 +255,17 @@ int pvn3d_mlp_sa_fact2(const float *u, const float *v, int ldu, int c_valid, con
                        int ns, const pvn3d_mlp_layer_t *layer2, const pvn3d_mlp_layer_t *layer3, int flags, int pool,
                        float *out, int ldo, int col0, pvn3d_stream_t stream);
 int pvn3d_mlp_sa_fact2_supported(const pvn3d_mlp_layer_t *layer2, const pvn3d_mlp_layer_t *layer3, int ns);
+/* The same for a WIDE last layer (layer3->n_pad > 128: SA3, SA4), where the weights cannot stay resident: 64-row
+ * tiles, both layers in 128-column blocks, W2 and W3 streamed from L2 by TMA once per tile, the layer-2 activations
+ * in shared memory.  Same arguments, same bit-identical result as the two launches above.
+ * PVN3D_ERR_UNSUPPORTED (nothing launched) unless pvn3d_mlp_sa_fact2w_supported(layer2, layer3, ns) is 1: ns 16 or
+ * 32, layer3->n_pad > 128, layer2->k_pad <= 256, layer3->k_pad within the 128-column blocks of layer 2, the A and H
+ * tiles and three weight stages within a block's shared memory, and weight loads by TMA (not PVN3D_MLP_TMA=0).
+ * The query is host-only and touches no device memory. */
+int pvn3d_mlp_sa_fact2w(const float *u, const float *v, int ldu, int c_valid, const int *idx, int b, int n, int m,
+                        int ns, const pvn3d_mlp_layer_t *layer2, const pvn3d_mlp_layer_t *layer3, int flags, int pool,
+                        float *out, int ldo, int col0, pvn3d_stream_t stream);
+int pvn3d_mlp_sa_fact2w_supported(const pvn3d_mlp_layer_t *layer2, const pvn3d_mlp_layer_t *layer3, int ns);
 /* FACTORED first layer of an FP module: three_interpolate commutes with the (linear) first layer, so
  *   P = W1k . known      once per KNOWN point   (pvn3d_mlp_dense without ReLU on the known table),
  *   S = W1s . skip + b1  over the skip columns  (pvn3d_mlp_dense without ReLU on the skip table),

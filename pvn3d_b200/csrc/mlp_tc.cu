@@ -1287,6 +1287,313 @@ int launch_sa_fact2(Sa2Args &g, int stages, cudaStream_t st) {
 }
 
 // =====================================================================================================
+// Layers 2 and 3 of a factored SA scale with a WIDE last layer (n3_pad > 128: SA3, SA4) and the max-pool, in ONE
+// persistent kernel.  mlp_sa_fact2_kernel keeps both weight matrices resident and a whole layer-3 row in registers;
+// for 256 / 512 output columns neither fits (W3 of SA3 alone is 229 KB).  Here the weights STREAM and both layers
+// run in 128-column blocks, so a thread never holds more than one 64 x 128 fragment.  Per 64-row tile (whole
+// centres: 64 % ns == 0):
+//   producers (warps 0-3)   stage A = tf32(relu(U[idx] - V)) ONCE into a resident A tile (all layer-2 K chunks),
+//                           with the PRO_SA_FACT producer of the per-layer kernel;
+//   loader    (warp 12)     streams 32-column K chunks of W2 and W3 (128 output columns each) by TMA through a ring,
+//                           in the order the warpgroups consume them;
+//   MMA       (warps 4-11)  both warpgroups work on the same 64 rows; warpgroup wg takes the column blocks
+//                           nb % 2 == wg of each layer.  Layer 2: wgmma N = 128 over the K chunks of the A tile,
+//                           then tf32(relu(acc + b2)) into the block's columns of a K-major SWIZZLE_128B H tile;
+//                           layer 3: the same from the H tile, max-pooled in registers (shuffle butterfly; a
+//                           32-row centre combines two warps through shared memory), + b3, ReLU, rounding, store.
+// The chunks of the two blocks a warpgroup pair works on are interleaved in the ring, so both warpgroups draw
+// from it at once.  Every output column keeps the per-layer kernel's operands, wgmma N (128) and K order, so the
+// results are bit-identical to pvn3d_mlp_sa_fact + pvn3d_mlp_dense(pool = ns).
+constexpr int kSa2wBM = 64;
+constexpr int kSa2wProWarps = 4;
+constexpr int kSa2wLoaderWarp = kSa2wProWarps + kMlpMmaWarps;   // warp 12
+constexpr int kSa2wThreads = (kSa2wLoaderWarp + 1) * 32;
+constexpr int kSa2wMaxStages = 8;
+constexpr int kSa2wMaxKc2 = 8;                             // layer-2 K chunks of the resident A tile (K <= 256)
+constexpr uint32_t kSa2wChunk = kSa2wBM * 128u;            // one K chunk of the A or H tile: 64 rows x 32 tf32
+constexpr uint32_t kSa2wStageBytes = 128u * 128u;          // one weight chunk: 128 output columns x 32 tf32
+
+struct Sa2wArgs {
+  MlpArgs a;            // PRO_SA_FACT producer fields, rows, out / ldo / col0 / round_out / pool; tmap, w, bias, k_pad, n_pad: layer 2
+  alignas(64) CUtensorMap tmap3;
+  const float *w3, *bias3;
+  int k3_pad, n3_pad;   // k3_pad >= n_pad of layer 2; its columns past that are zero
+};
+
+struct Sa2wSmemCtl {
+  uint64_t full[kSa2wMaxStages];   // the loader's arrive.expect_tx + the TMA bytes of the weight chunk
+  uint64_t empty[kSa2wMaxStages];  // 4 arrivals: the warps of the warpgroup that consumed the chunk
+  uint64_t a_full[kSa2wMaxKc2];    // 64 arrivals: the producer threads of K chunk kc of the A tile
+  uint64_t a_empty;                // 8 arrivals: every MMA warp, once its layer-2 MMAs of the tile have retired
+};
+
+// shared-memory layout behind the 1024-byte aligned base (kernel and launcher use the same function):
+// [A: k2_pad/32 chunks of 64 x 128 B][H: k3_pad/32 chunks of 64 x 128 B][weight ring: stages x 16 KB][barriers]
+struct Sa2wSmem {
+  uint32_t a, h, ring, ctl, bytes;   // offsets from the aligned base; bytes = dynamic size incl. alignment slack
+};
+static inline __host__ __device__ Sa2wSmem sa2w_smem(int k2_pad, int k3_pad, int stages) {
+  Sa2wSmem s;
+  s.a = 0;
+  s.h = s.a + static_cast<uint32_t>(k2_pad / 32) * kSa2wChunk;
+  s.ring = s.h + static_cast<uint32_t>(k3_pad / 32) * kSa2wChunk;
+  s.ctl = s.ring + static_cast<uint32_t>(stages) * kSa2wStageBytes;
+  s.bytes = 1024u + s.ctl + static_cast<uint32_t>(sizeof(Sa2wSmemCtl));
+  return s;
+}
+
+// The weight chunks of one layer in ring order: the column blocks in pairs (2p, 2p+1), K chunks of the pair
+// interleaved -- (2p, 0) (2p+1, 0) (2p, 1) (2p+1, 1) ..; chunk kc of block 2p + q is item kc * cnt + q of the pair.
+__device__ __forceinline__ int sa2w_pair_blocks(int nb, int pp) { return nb - pp < 2 ? nb - pp : 2; }
+
+// One 64 x 128 block of a layer for the calling warpgroup: K chunks of `a_tile` (64 rows each) x the weight chunks
+// of the ring into registers, each ring stage released once the MMAs that read it have retired -- except the last
+// one with `keep_last`, which the caller releases (returned).  With `a_bars`, K chunk kc of the A tile is waited for
+// first (layer 2; parity `a_par`).
+__device__ __forceinline__ int sa2w_block(float (&d)[64], uint32_t a_tile, uint32_t ring, int S, int it0, int step, int kcs,
+                                          Sa2wSmemCtl &ctl, uint64_t *a_bars, unsigned a_par, bool keep_last, unsigned lane) {
+#pragma unroll
+  for (int i = 0; i < 64; ++i) d[i] = 0.f;
+  int prev = -1;
+  for (int kc = 0; kc < kcs; ++kc) {
+    const int it = it0 + kc * step;
+    const int s = it % S;
+    if (a_bars) mbar_wait(&a_bars[kc], a_par);
+    mbar_wait(&ctl.full[s], static_cast<unsigned>((it / S) & 1));
+    fence_proxy_async_smem();
+    const uint64_t adesc = smem_desc_sw128(a_tile + static_cast<uint32_t>(kc) * kSa2wChunk);
+    const uint64_t bdesc = smem_desc_sw128(ring + static_cast<uint32_t>(s) * kSa2wStageBytes);
+    wgmma_fence();
+#pragma unroll
+    for (int k4 = 0; k4 < 4; ++k4)
+      wgmma_tf32<128>(d, adesc + static_cast<uint64_t>(k4 * 2), bdesc + static_cast<uint64_t>(k4 * 2), (kc > 0 || k4 > 0) ? 1u : 0u);
+    wgmma_commit();
+    if (prev >= 0) {
+      wgmma_wait<1>();
+      if (lane == 0) mbar_arrive(&ctl.empty[prev]);
+    }
+    prev = s;
+  }
+  wgmma_wait<0>();
+  acc_fence(d);
+  if (lane == 0 && !keep_last) mbar_arrive(&ctl.empty[prev]);
+  return prev;
+}
+
+__global__ void __launch_bounds__(kSa2wThreads, 1) mlp_sa_fact2w_kernel(const __grid_constant__ Sa2wArgs g) {
+  const MlpArgs &a = g.a;
+  extern __shared__ unsigned char mlp_smem_raw[];
+  const uint32_t raw = smem_u32(mlp_smem_raw);
+  const uint32_t base = (raw + 1023u) & ~1023u;   // SWIZZLE_128B atoms are 8 rows x 128 B
+  const int kc2 = a.k_pad / 32, kc3 = g.k3_pad / 32;
+  const int nb2 = (a.n_pad + 127) / 128, nb3 = (g.n3_pad + 127) / 128;
+  const int S = a.stages;   // what the launcher's budget left (it computes the layout with the same function)
+  const Sa2wSmem L = sa2w_smem(a.k_pad, g.k3_pad, S);
+  Sa2wSmemCtl &ctl = *reinterpret_cast<Sa2wSmemCtl *>(mlp_smem_raw + (base - raw) + L.ctl);
+  const int t = threadIdx.x;
+  const unsigned warp = t >> 5, lane = t & 31u;
+  const int tiles = static_cast<int>((a.rows + kSa2wBM - 1) / kSa2wBM);   // the launcher checks the 32-bit counts
+
+  if (t == 0) {
+    for (int s = 0; s < S; ++s) {
+      mbar_init(&ctl.full[s], 1);
+      mbar_init(&ctl.empty[s], 4);
+    }
+    for (int kc = 0; kc < kc2; ++kc) mbar_init(&ctl.a_full[kc], 64);
+    mbar_init(&ctl.a_empty, kMlpMmaWarps);
+    mbar_fence_init();
+  }
+  __syncthreads();
+
+  if (warp < kSa2wProWarps) {
+    // ================= producers: warp w stages rows 32 (w & 1).. of the K chunks kc % 2 == w >> 1 ============
+    const int rb = static_cast<int>(warp & 1u), kc_first = static_cast<int>(warp >> 1);
+    const int sub = static_cast<int>(lane & 7u), r_first = 32 * rb + static_cast<int>(lane >> 3);
+    int j = 0;
+    for (int tile = blockIdx.x; tile < tiles; tile += gridDim.x, ++j) {
+      const long long p_first = static_cast<long long>(tile) * kSa2wBM + r_first;
+      RowState rs;
+      rows_setup<PRO_SA_FACT>(a, p_first, rs);
+      mbar_wait(&ctl.a_empty, static_cast<unsigned>((j & 1) ^ 1));   // the previous tile's layer 2 is done
+      for (int kc = kc_first; kc < kc2; kc += 2) {
+        stage_a_chunk<PRO_SA_FACT>(a, rs, p_first, r_first, sub, kc * 32, base + L.a + static_cast<uint32_t>(kc) * kSa2wChunk,
+                                   true);
+        fence_proxy_async_smem();
+        mbar_arrive(&ctl.a_full[kc]);
+      }
+    }
+  } else if (warp == kSa2wLoaderWarp) {
+    // ================= loader: every weight chunk of every tile, in ring order ===============================
+    if (lane == 0) {
+      int it = 0;
+      for (int tile = blockIdx.x; tile < tiles; tile += gridDim.x) {
+        for (int layer = 0; layer < 2; ++layer) {
+          const CUtensorMap *map = layer ? &g.tmap3 : &a.tmap;
+          const int nb = layer ? nb3 : nb2, kcs = layer ? kc3 : kc2;
+          for (int pp = 0; pp < nb; pp += 2) {
+            const int cnt = sa2w_pair_blocks(nb, pp);
+            for (int kc = 0; kc < kcs; ++kc)
+              for (int q = 0; q < cnt; ++q, ++it) {
+                const int s = it % S;
+                mbar_wait(&ctl.empty[s], static_cast<unsigned>(((it / S) & 1) ^ 1));
+                mbar_expect_tx(&ctl.full[s], kSa2wStageBytes);   // rows past n_pad arrive as zeros and count too
+                tma_load_2d(base + L.ring + static_cast<uint32_t>(s) * kSa2wStageBytes, map, kc * 32, (pp + q) * 128,
+                            &ctl.full[s]);
+              }
+          }
+        }
+      }
+    }
+  } else {
+    // ================= MMA + epilogue: warpgroup wg, warp w4 of it holds rows 16 w4 .. +15 of the tile ======
+    const unsigned mw = warp - kSa2wProWarps, wg = mw >> 2, w4 = mw & 3u;
+    const int frag_row = static_cast<int>(16 * w4 + (lane >> 2));
+    const int pair_bar = 2 + static_cast<int>(wg * 2 + (w4 >> 1));
+    const int n2 = a.n_pad;
+    int it_base = 0;
+    float d[64];
+    int j = 0;
+    for (int tile = blockIdx.x; tile < tiles; tile += gridDim.x, ++j) {
+      const long long p0 = static_cast<long long>(tile) * kSa2wBM;
+      // ---- layer 2 -> H tile
+      bool synced = false;
+      for (int pp = 0; pp < nb2; pp += 2) {
+        const int cnt = sa2w_pair_blocks(nb2, pp);
+        if (static_cast<int>(wg) < cnt) {
+          const int nb = pp + static_cast<int>(wg);
+          sa2w_block(d, base + L.a, base + L.ring, S, it_base + static_cast<int>(wg), cnt, kc2, ctl, ctl.a_full,
+                     static_cast<unsigned>(j & 1), false, lane);
+          // both warpgroups have finished the previous tile's layer 3 (its reads of H)
+          if (!synced) named_bar_sync(1, 2 * 128);
+          synced = true;
+          // H[row, c] = tf32(relu(acc + b2[c])) for the block's columns c < k3_pad; columns n2.. are layer 3's K padding
+#pragma unroll
+          for (int jj = 0; jj < 16; ++jj) {
+            const int c = 128 * nb + 8 * jj + 2 * static_cast<int>(lane & 3u);
+            if (c >= g.k3_pad) break;
+            const bool on0 = c < n2, on1 = c + 1 < n2;
+            const float b0 = on0 ? __ldg(a.bias + c) : 0.f, b1 = on1 ? __ldg(a.bias + c + 1) : 0.f;
+            const uint32_t off = static_cast<uint32_t>(c >> 5) * kSa2wChunk + static_cast<uint32_t>(frag_row) * 128u +
+                                 ((static_cast<uint32_t>(((c & 31) >> 2) ^ (frag_row & 7))) << 4) + (c & 3) * 4u;
+            asm volatile("st.shared.v2.f32 [%0], {%1,%2};" ::"r"(base + L.h + off),
+                         "f"(on0 ? to_tf32(fmaxf(d[4 * jj] + b0, 0.f)) : 0.f), "f"(on1 ? to_tf32(fmaxf(d[4 * jj + 1] + b1, 0.f)) : 0.f)
+                         : "memory");
+            asm volatile("st.shared.v2.f32 [%0], {%1,%2};" ::"r"(base + L.h + off + 8u * 128u),
+                         "f"(on0 ? to_tf32(fmaxf(d[4 * jj + 2] + b0, 0.f)) : 0.f),
+                         "f"(on1 ? to_tf32(fmaxf(d[4 * jj + 3] + b1, 0.f)) : 0.f)
+                         : "memory");
+          }
+        }
+        it_base += kc2 * cnt;
+      }
+      if (lane == 0) mbar_arrive(&ctl.a_empty);   // this warp's layer-2 MMAs have retired: the A tile may be refilled
+      if (!synced) named_bar_sync(1, 2 * 128);
+      fence_proxy_async_smem();   // generic-proxy stores of H -> visible to the tensor core
+      named_bar_sync(1, 2 * 128); // every block of H is written
+      // ---- layer 3 from the H tile, pooled over the centres of the tile
+      for (int pp = 0; pp < nb3; pp += 2) {
+        const int cnt = sa2w_pair_blocks(nb3, pp);
+        if (static_cast<int>(wg) < cnt) {
+          const int nb = pp + static_cast<int>(wg);
+          const int last = sa2w_block(d, base + L.h, base + L.ring, S, it_base + static_cast<int>(wg), cnt, kc3, ctl, nullptr, 0u,
+                                      true, lane);
+          // max over the warp's 16 rows: the lane's two rows, then a transposing butterfly over lane bits 4, 3, 2
+          // (lanes that differ there hold the same columns); p[2j + e] is column 8j + 2 (lane & 3) + e
+          float p[32];
+#pragma unroll
+          for (int jj = 0; jj < 16; ++jj) {
+            p[2 * jj] = fmaxf(d[4 * jj], d[4 * jj + 2]);
+            p[2 * jj + 1] = fmaxf(d[4 * jj + 1], d[4 * jj + 3]);
+          }
+          rowmax_level<16, 16>(p, lane);
+          rowmax_level<8, 8>(p, lane);
+          rowmax_level<4, 4>(p, lane);
+          // a 32-row centre: the odd warp of each pair hands its 16-row maxima to the even one through the block's
+          // last weight stage -- only this warpgroup read it, its MMAs have retired, and the loader refills it only
+          // after all four warps have released it below
+          bool owner = true;
+          long long grow = (p0 + 16 * w4) / 16;
+          if (a.pool == 32) {
+            const uint32_t xc = base + L.ring + static_cast<uint32_t>(last) * kSa2wStageBytes + (w4 >> 1) * 512u;
+            if (w4 & 1u) {
+#pragma unroll
+              for (int i = 0; i < 4; ++i)
+                asm volatile("st.shared.f32 [%0], %1;" ::"r"(xc + (lane * 4 + i) * 4u), "f"(p[i]) : "memory");
+              fence_proxy_async_smem();   // these generic stores before the stage's next TMA write
+              named_bar_sync(pair_bar, 64);
+              owner = false;
+            } else {
+              named_bar_sync(pair_bar, 64);
+#pragma unroll
+              for (int i = 0; i < 4; ++i) {
+                float q;
+                asm volatile("ld.shared.f32 %0, [%1];" : "=f"(q) : "r"(xc + (lane * 4 + i) * 4u) : "memory");
+                p[i] = fmaxf(p[i], q);
+              }
+            }
+            grow = (p0 + 32 * (w4 >> 1)) / 32;
+          }
+          __syncwarp();   // every lane's exchange loads / stores before the release
+          if (lane == 0) mbar_arrive(&ctl.empty[last]);
+          // the group's rows exist entirely or not at all (rows % pool == 0)
+          if (owner && grow * a.pool < a.rows) {
+            const unsigned b4 = (lane >> 4) & 1u, b3 = (lane >> 3) & 1u, b2 = (lane >> 2) & 1u;
+            float *o = a.out + grow * a.ldo + a.col0;
+#pragma unroll
+            for (int i = 0; i < 4; ++i) {
+              const int io = i + (b4 ? 16 : 0) + (b3 ? 8 : 0) + (b2 ? 4 : 0);
+              const int col = 128 * nb + 8 * (io >> 1) + 2 * static_cast<int>(lane & 3u) + (io & 1);
+              if (col < g.n3_pad) {
+                float r = fmaxf(p[i] + __ldg(g.bias3 + col), 0.f);
+                if (a.round_out) r = to_tf32(r);
+                o[col] = r;
+              }
+            }
+          }
+        }
+        it_base += kc3 * cnt;
+      }
+    }
+  }
+}
+
+// ring stages pvn3d_mlp_sa_fact2w runs a scale with; 0: the scale is not covered (nsample other than 16 / 32, a last
+// layer of at most 128 columns -- pvn3d_mlp_sa_fact2's -- more than 8 layer-2 K chunks, a layer-3 K beyond the
+// 128-column blocks of layer 2, A + H tiles + three weight
+// stages beyond the shared memory of a block, or weight streaming by TMA switched off with PVN3D_MLP_TMA=0)
+int sa2w_stages(int k2_pad, int n2_pad, int k3_pad, int n3_pad, int ns) {
+  // every H column layer 3 reads is written by a layer-2 block each tile: k3_pad within the 128-column blocks of layer 2
+  if ((ns != 16 && ns != 32) || n3_pad <= 128 || k2_pad / 32 > kSa2wMaxKc2 || k3_pad > 128 * ceil_div(n2_pad, 128)) return 0;
+  if (const char *env = getenv("PVN3D_MLP_TMA"))
+    if (env[0] == '0') return 0;
+  const uint32_t fixed = sa2w_smem(k2_pad, k3_pad, 0).bytes;
+  if (fixed >= static_cast<uint32_t>(kMlpSmemMax)) return 0;
+  const int stages = std::min<int>(kSa2wMaxStages, static_cast<int>((kMlpSmemMax - fixed) / kSa2wStageBytes));
+  return stages >= 3 ? stages : 0;   // one stage per warpgroup in use and one in flight
+}
+
+int launch_sa_fact2w(Sa2wArgs &g, int stages, cudaStream_t st) {
+  MlpArgs &a = g.a;
+  if (a.rows <= 0) return PVN3D_OK;
+  a.stages = stages;
+  const size_t smem = sa2w_smem(a.k_pad, g.k3_pad, stages).bytes;
+  const int sms = std::max(1, sm_count() - a.reserve_sms);
+  const long long tiles = (a.rows + kSa2wBM - 1) / kSa2wBM;
+  const long long chunks = static_cast<long long>(ceil_div(a.n_pad, 128)) * (a.k_pad / 32) +
+                           static_cast<long long>(ceil_div(g.n3_pad, 128)) * (g.k3_pad / 32);
+  if (tiles * chunks > 0x7fffffffll) return PVN3D_ERR_UNSUPPORTED;   // the kernel counts weight chunks in 32 bits
+  if (!weight_tensor_map(&a.tmap, a.w, a.k_pad, a.n_pad, 128) || !weight_tensor_map(&g.tmap3, g.w3, g.k3_pad, g.n3_pad, 128))
+    return PVN3D_ERR_UNSUPPORTED;
+  auto kern = mlp_sa_fact2w_kernel;
+  static PerDeviceOnce once;
+  PVN3D_ONCE_PER_DEVICE(once, cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, kMlpSmemMax),
+                        "mlp sa_fact2w smem attr");
+  const unsigned grid = static_cast<unsigned>(std::min<long long>(tiles, sms));
+  kern<<<grid, kSa2wThreads, smem, st>>>(g);
+  return check_launch("mlp_sa_fact2w_kernel");
+}
+
+// =====================================================================================================
 // The whole SharedMLP of one SA scale (3 layers) / FP module (2 layers) in ONE persistent kernel.
 //
 // One launch per layer sends every inter-layer activation through HBM twice (write + read: 7.0 of the
@@ -2029,6 +2336,42 @@ extern "C" int pvn3d_mlp_sa_fact2_supported(const pvn3d_mlp_layer_t *layer2, con
       layer3->k_pad < layer2->n_pad || layer3->k_pad % 32 || layer3->n_pad <= 0 || layer3->n_pad % 16)
     return 0;
   return sa2_stages(layer2->k_pad, layer2->n_pad, layer3->k_pad, layer3->n_pad, ns) ? 1 : 0;
+}
+
+extern "C" int pvn3d_mlp_sa_fact2w(const float *u, const float *v, int ldu, int c_valid, const int *idx, int b, int n,
+                                   int m, int ns, const pvn3d_mlp_layer_t *layer2, const pvn3d_mlp_layer_t *layer3,
+                                   int flags, int pool, float *out, int ldo, int col0, pvn3d_stream_t stream) {
+  if (!u || !v || !idx || !layer2 || !layer3 || !layer2->w || !layer2->bias || !layer3->w || !layer3->bias || !out ||
+      b < 0 || n <= 0 || m < 0 || ns <= 0 || c_valid <= 0 || c_valid % 4 || ldu < c_valid || ldu % 4 ||
+      layer2->k_pad < c_valid || layer2->k_pad <= 0 || layer2->k_pad % 32 || layer2->n_pad <= 0 || layer2->n_pad % 16 ||
+      layer3->k_pad < layer2->n_pad || layer3->k_pad % 32 || layer3->n_pad <= 0 || layer3->n_pad % 16 || ldo % 4 ||
+      col0 % 4 || (reinterpret_cast<uintptr_t>(u) & 15u) || (reinterpret_cast<uintptr_t>(v) & 15u) ||
+      (reinterpret_cast<uintptr_t>(layer2->w) & 15u) || (reinterpret_cast<uintptr_t>(layer3->w) & 15u))
+    return PVN3D_ERR_INVALID_ARG;
+  if (pool != ns) return PVN3D_ERR_INVALID_ARG;
+  const int stages = sa2w_stages(layer2->k_pad, layer2->n_pad, layer3->k_pad, layer3->n_pad, ns);
+  if (!stages) return PVN3D_ERR_UNSUPPORTED;
+  if (static_cast<long long>(m) * ns > 0x3fffffffll || static_cast<long long>(b) * n > 0x7fffffffll ||
+      static_cast<long long>(b) * m > 0x7fffffffll)
+    return PVN3D_ERR_UNSUPPORTED;
+  Sa2wArgs g{};
+  MlpArgs &a = g.a;
+  a.w = layer2->w; a.bias = layer2->bias; a.k_pad = layer2->k_pad; a.n_pad = layer2->n_pad;
+  a.rows = static_cast<long long>(b) * m * ns;
+  a.feat = u; a.new_xyz = v; a.ldf = ldu; a.c_feat = c_valid; a.idx = idx;
+  a.n = n; a.m = m; a.ns = ns; a.pool = pool;
+  a.out = out; a.ldo = ldo; a.col0 = col0; a.relu = 1;
+  a.round_out = (flags & PVN3D_MLP_ROUND_OUT) ? 1 : 0;
+  a.reserve_sms = (flags >> 8) & 0xff;
+  g.w3 = layer3->w; g.bias3 = layer3->bias; g.k3_pad = layer3->k_pad; g.n3_pad = layer3->n_pad;
+  return launch_sa_fact2w(g, stages, as_stream(stream));
+}
+
+extern "C" int pvn3d_mlp_sa_fact2w_supported(const pvn3d_mlp_layer_t *layer2, const pvn3d_mlp_layer_t *layer3, int ns) {
+  if (!layer2 || !layer3 || layer2->k_pad <= 0 || layer2->k_pad % 32 || layer2->n_pad <= 0 || layer2->n_pad % 16 ||
+      layer3->k_pad < layer2->n_pad || layer3->k_pad % 32 || layer3->n_pad <= 0 || layer3->n_pad % 16)
+    return 0;
+  return sa2w_stages(layer2->k_pad, layer2->n_pad, layer3->k_pad, layer3->n_pad, ns) ? 1 : 0;
 }
 
 extern "C" int pvn3d_mlp_fp_fact(const float *p, const float *s, int ld, int c_valid, const int *nn_idx,

@@ -190,6 +190,30 @@ def mlp_sa_fact2(u: torch.Tensor, v: torch.Tensor, idx: torch.Tensor, n: int, la
     return out
 
 
+def sa_fact2w_fits(layer2: PackedLayer, layer3: PackedLayer, ns: int) -> bool:
+    """whether pvn3d_mlp_sa_fact2w takes the scale (the library's own rule: nsample 16 or 32, a last layer wider than
+    128 columns, layer-2 K at most 256, A + H tiles + three weight stages within shared memory -- SA3 and SA4)"""
+    l2, l3 = _layer_struct(layer2), _layer_struct(layer3)
+    return bool(_lib.load().pvn3d_mlp_sa_fact2w_supported(ctypes.addressof(l2), ctypes.addressof(l3), ns))
+
+
+def mlp_sa_fact2w(u: torch.Tensor, v: torch.Tensor, idx: torch.Tensor, n: int, layer2: PackedLayer, layer3: PackedLayer,
+                  out=None, col0=0, round_out=False, reserve=0):
+    """mlp_sa_fact2 for a wide last layer (pvn3d_mlp_sa_fact2w: weights streamed, both layers in 128-column blocks):
+    the same bits as mlp_sa_fact(.., layer2, round_out=True) -> mlp_dense(.., layer3, pool=ns, a_tf32=True)"""
+    lib = _lib.load()
+    b, m, ns = idx.shape
+    if out is None:
+        out = torch.empty((b * m, layer3.n_pad), dtype=torch.float32, device=u.device)
+    l2, l3 = _layer_struct(layer2), _layer_struct(layer3)
+    with torch.cuda.device(u.device):
+        rc = lib.pvn3d_mlp_sa_fact2w(ptr(u), ptr(v), u.size(-1), u.size(-1), ptr(idx), b, n, m, ns, ctypes.addressof(l2),
+                                     ctypes.addressof(l3), _flags(True, round_out, reserve=reserve), ns, ptr(out), out.size(-1),
+                                     col0, _stream(u.device))
+    check(rc, "pvn3d_mlp_sa_fact2w")
+    return out
+
+
 def mlp_fp_fact(p: torch.Tensor, s_: torch.Tensor, nn_idx: torch.Tensor, nn_w: torch.Tensor, m_known: int,
                 layer: PackedLayer, relu=True, round_out=False, reserve=0, out_cn=False):
     """second layer of a factored FP module: rows relu(sum_t w_t P[idx_t] + S) -> layer (pvn3d_mlp_fp_fact).
@@ -453,6 +477,8 @@ class FusedPointnet2MSG:
         if not plan.ball:
             self.queries(plan)
         # level-0 descriptors are columns 3.. of the input rows themselves (point-major already)
+        # PVN3D_MLP_SA_WIDE=0: SA3 / SA4 scales as two launches (layer 2, then layer 3 + max-pool) -- for A/B runs
+        wide_on = os.environ.get("PVN3D_MLP_SA_WIDE", "1") != "0"
         feats: List[Tuple[int, int, int]] = [(pointcloud.data_ptr() + 12, width, c0)]   # (address, ld, channels)
         keep = [pointcloud]
         l_xyz = plan.l_xyz
@@ -474,10 +500,14 @@ class FusedPointnet2MSG:
                     u = mlp_dense(table, first, relu=False, a_tf32=True, reserve=rs)        # once per point
                     v = sa_centre_term(new_xyz, wx, b1)                                     # once per centre
                     last2 = len(layers) == 2
+                    fused = None
                     if len(layers) == 3 and sa_fact2_fits(layers[1], layers[2], ns):
-                        # SA1 / SA2: layer 2 stays on chip (DESIGN.md section 4)
-                        mlp_sa_fact2(u, v, idx, x.size(1), layers[1], layers[2], out=out_l.view(b * npoint, -1), col0=col,
-                                     round_out=self.round_tables and li < 3, reserve=rs)
+                        fused = mlp_sa_fact2        # SA1 / SA2: layer 2 stays on chip (DESIGN.md section 4)
+                    elif len(layers) == 3 and wide_on and sa_fact2w_fits(layers[1], layers[2], ns):
+                        fused = mlp_sa_fact2w       # SA3 / SA4: the same, weights streamed
+                    if fused is not None:
+                        fused(u, v, idx, x.size(1), layers[1], layers[2], out=out_l.view(b * npoint, -1), col0=col,
+                              round_out=self.round_tables and li < 3, reserve=rs)
                         col += layers[-1].n
                         continue
                     h = mlp_sa_fact(u, v, idx, x.size(1), layers[1], pool=ns if last2 else 0, round_out=not last2 or
