@@ -361,6 +361,49 @@ int pvn3d_frame_poses_batch(const float *pcld, const int *mask, const float *ctr
                             uint8_t *present, float *cls_kps, int *new_mask, void *workspace,
                             size_t workspace_bytes, pvn3d_stream_t stream);
 
+/* ICP pose refinement: my_icp(A, B, init_pose, max_iterations, tolerance) of the reference
+ * (lib/utils/icp/icp.py:141-192) as pvn3d/eval_icp.py:94-185 applies it per object, in float64.
+ *
+ * Model set: object-frame points of n_models models, pts [total_pts,3] f32, model m owning rows
+ * [model_off[m], model_off[m+1]) (model_off [n_models+1] i32, device; an empty range = no model).
+ * pvn3d_icp_build_models builds, on device, the exact nearest-neighbour structure every fit
+ * searches into `buf` (pvn3d_icp_models_bytes(n_models, total_pts) bytes, 256-B aligned).  Its
+ * layout is private to the library; `pts` may be freed once the build has run.
+ *
+ * Fit semantics, per fit with scene set B [n,3] and init pose P_0 (3x4, rigid):
+ *   for i in 0..max_iter-1: d_j, idx_j = nearest model point of every scene point under P_i
+ *     (exact: equal to a float64 brute-force scan, lowest model index on exact ties);
+ *     P_{i+1} = Kabsch(A[idx], B) (float64, reflection-fixed);
+ *     stop when |prev - mean(d)| < tol, prev starting at 0.
+ *   result: P_{i+1}, the distances d of iteration i, and i (max_iter-1 when it never stopped).
+ * The per-iteration sums run in a fixed order: results are reproducible bit for bit.
+ * The first 8 bytes of the workspace count (u64) the model points the call's searches tested. */
+size_t pvn3d_icp_models_bytes(int n_models, int total_pts);
+int pvn3d_icp_build_models(const float *pts, const int *model_off, int n_models, int total_pts,
+                           void *buf, size_t bytes, pvn3d_stream_t stream);
+/* workspace of pvn3d_icp_refine_batch(b, n, n_cls, max_pts); (1, n, 1, n) also sizes pvn3d_icp_fit */
+size_t pvn3d_icp_workspace_bytes(int b, int n, int n_cls, int max_pts);
+/* One fit per (frame b, class c), c in 1..n_cls-1, model c of the set (n_cls <= 64):
+ *   pcld [B,N,3] f32, mask [B,N] i32 (class per point), init_poses [B,n_cls,3,4] f32 (promoted to
+ *   f64), present [B,n_cls] u8 -- the outputs of pvn3d_frame_poses_batch.
+ *   Scene set: the class's points in ascending index; with cnt > max_pts of them, the points at
+ *   positions floor(j*cnt/max_pts), j < max_pts.  Skipped (pose = init, iters = 0, err = 0,
+ *   refined = 0): c == 0, present == 0, cnt < min_pts, cnt == 0, or no model for c.
+ * outputs: poses_out [B,n_cls,3,4] f64, iters_out [B,n_cls] i32 (the loop index i),
+ *   err_out [B,n_cls] f64 (mean of the last iteration's distances), refined_out [B,n_cls] u8.
+ * max_iter >= 1, tol >= 0. */
+int pvn3d_icp_refine_batch(const void *models, const float *pcld, const int *mask, int b, int n,
+                           int n_cls, const float *init_poses, const uint8_t *present, int max_pts,
+                           int min_pts, int max_iter, double tol, double *poses_out, int *iters_out,
+                           double *err_out, uint8_t *refined_out, void *workspace,
+                           size_t workspace_bytes, pvn3d_stream_t stream);
+/* One fit of an explicit scene set scene [n,3] f32 against model `model`, init_pose [3,4] f64
+ * (same kernel as the batch): pose_out [3,4] f64, dist_out [n] f64 (NULL to skip), iter_out [1]
+ * i32, err_out [1] f64.  A missing or empty model leaves pose = init and iter = -1. */
+int pvn3d_icp_fit(const void *models, int model, const float *scene, int n, const double *init_pose,
+                  int max_iter, double tol, double *pose_out, double *dist_out, int *iter_out,
+                  double *err_out, void *workspace, size_t workspace_bytes, pvn3d_stream_t stream);
+
 /* ------------------------------------------------------------------------------------------
  * Callers either side of the path (SURVEY section 8 f4)
  * ---------------------------------------------------------------------------------------- */

@@ -97,6 +97,12 @@ _SIGNATURES = {
     "pvn3d_frame_poses_workspace_bytes": (c_size_t, [c_int, c_int, c_int, c_int, c_int]),
     "pvn3d_frame_poses_ms_workspace_offset": (c_size_t, [c_int, c_int, c_int, c_int, c_int]),
     "pvn3d_frame_poses_batch": (c_int, [_P, _P, _P, _P, c_int, c_int, c_int, c_int, _P, _P, c_int, c_double, c_int, c_uint, _P, _P, _P, _P, _P, c_size_t, _P]),
+    "pvn3d_icp_models_bytes": (c_size_t, [c_int, c_int]),
+    "pvn3d_icp_build_models": (c_int, [_P, _P, c_int, c_int, _P, c_size_t, _P]),
+    "pvn3d_icp_workspace_bytes": (c_size_t, [c_int, c_int, c_int, c_int]),
+    "pvn3d_icp_refine_batch": (c_int, [_P, _P, _P, c_int, c_int, c_int, _P, _P, c_int, c_int, c_int, c_double, _P, _P, _P, _P,
+                                       _P, c_size_t, _P]),
+    "pvn3d_icp_fit": (c_int, [_P, c_int, _P, c_int, _P, c_int, c_double, _P, _P, _P, _P, _P, c_size_t, _P]),
 }
 EXPORTED_SYMBOLS = tuple(_SIGNATURES)
 

@@ -168,3 +168,101 @@ def stack(frames: List[Frame]):
         "ctr_of": np.stack([f.ctr_of[0] for f in frames]),
         "kp_of": np.stack([f.kp_of for f in frames]),
     }
+
+
+# --------------------------------------------------------------------------------------------------
+# ICP refinement inputs: box-like object models, visible surfaces under random poses
+# --------------------------------------------------------------------------------------------------
+_BOX_NORMALS = np.array([[1, 0, 0], [-1, 0, 0], [0, 1, 0], [0, -1, 0], [0, 0, 1], [0, 0, -1]], np.float64)
+
+
+def box_surface(extents, n: int, rng) -> np.ndarray:
+    """n points uniformly on the surface of a box of the given extents centred at the origin -> [n,3] f32"""
+    e = np.asarray(extents, np.float64)
+    area = np.array([e[1] * e[2]] * 2 + [e[0] * e[2]] * 2 + [e[0] * e[1]] * 2)
+    face = rng.choice(6, size=n, p=area / area.sum())
+    pts = rng.uniform(-0.5, 0.5, size=(n, 3)) * e
+    ax = np.abs(_BOX_NORMALS[face]).argmax(1)
+    pts[np.arange(n), ax] = 0.5 * e[ax] * _BOX_NORMALS[face, ax]
+    return pts.astype(np.float32)
+
+
+def visible_box_points(extents, R, t, n: int, noise: float, rng, faces=None) -> np.ndarray:
+    """n camera-frame points of the faces of the box (pose R, t) that face a camera at the origin
+    (or of the listed face indices), with N(0, noise) per coordinate -> [n,3] f64"""
+    e = np.asarray(extents, np.float64)
+    if faces is None:
+        centres = (0.5 * e * _BOX_NORMALS) @ R.T + t
+        faces = [f for f in range(6) if (R @ _BOX_NORMALS[f]) @ centres[f] < 0]
+    faces = np.asarray(faces)
+    area = np.array([e[1] * e[2]] * 2 + [e[0] * e[2]] * 2 + [e[0] * e[1]] * 2)[faces]
+    face = faces[rng.choice(len(faces), size=n, p=area / area.sum())]
+    pts = rng.uniform(-0.5, 0.5, size=(n, 3)) * e
+    ax = np.abs(_BOX_NORMALS[face]).argmax(1)
+    pts[np.arange(n), ax] = 0.5 * e[ax] * _BOX_NORMALS[face, ax]
+    return pts @ R.T + t + rng.normal(0.0, noise, size=(n, 3))
+
+
+def perturb_pose(R, t, angle_deg: float, offset: float, rng):
+    """(R', t'): R rotated by angle_deg about a random axis (through the object origin), t moved by
+    `offset` metres in a random direction"""
+    axis = rng.normal(size=3)
+    axis /= np.linalg.norm(axis)
+    a = np.deg2rad(angle_deg)
+    K = np.array([[0, -axis[2], axis[1]], [axis[2], 0, -axis[0]], [-axis[1], axis[0], 0]])
+    dR = np.eye(3) + np.sin(a) * K + (1 - np.cos(a)) * K @ K
+    d = rng.normal(size=3)
+    return dR @ R, t + offset * d / np.linalg.norm(d)
+
+
+def make_icp_batch(batch: int, n_obj: int, pts_per_obj: int, seed: int = 0, n_cls: int = fixtures.YCB_N_CLASSES,
+                   model_pts: int = 3000, noise: float = 0.001, outlier_frac: float = 0.0, n_bg: int = 2000,
+                   angle_deg: float = 5.0, offset: float = 0.01) -> dict:
+    """A batch for IcpRefiner: per-class box-like models (distinct extents, 3-12 cm), and per frame
+    n_obj distinct classes, each seen as pts_per_obj points of its camera-facing faces under a random
+    pose (z in 0.6-1.0 m) with N(0, noise) noise, `outlier_frac` of them replaced by uniform points in
+    the object's bounding box, plus n_bg background-plane points (label 0) at z = 1.2 m; points are
+    shuffled.  Returns dict(models: list[n_cls] of [P,3] f32 (None for class 0), extents [n_cls,3],
+    pcld [B,N,3] f32, mask [B,N] i32, gt [B,n_cls,3,4] f64, init [B,n_cls,3,4] f32 (gt perturbed by
+    angle_deg / offset; identity for absent classes), present [B,n_cls] u8)."""
+    rng = np.random.default_rng(seed)
+    extents = np.zeros((n_cls, 3))
+    models = [None] * n_cls
+    for c in range(1, n_cls):
+        extents[c] = np.sort(rng.uniform(0.03, 0.12, size=3))[::-1]
+        models[c] = box_surface(extents[c], model_pts, rng)
+    n = n_obj * pts_per_obj + n_bg
+    pcld = np.zeros((batch, n, 3), np.float32)
+    mask = np.zeros((batch, n), np.int32)
+    gt = np.zeros((batch, n_cls, 3, 4))
+    init = np.zeros((batch, n_cls, 3, 4), np.float32)
+    init[:, :, :3, :3] = np.eye(3, dtype=np.float32)
+    gt[:, :, :3, :3] = np.eye(3)
+    present = np.zeros((batch, n_cls), np.uint8)
+    grid = [(-0.15, -0.1), (0.0, -0.1), (0.15, -0.1), (-0.15, 0.1), (0.0, 0.1), (0.15, 0.1),
+            (-0.3, 0.0), (0.3, 0.0)]
+    for b in range(batch):
+        cls = np.sort(rng.choice(np.arange(1, n_cls), size=n_obj, replace=False))
+        pts, lab = [], []
+        for k, c in enumerate(cls):
+            R = _haar_rotation(rng)
+            gx, gy = grid[k % len(grid)]
+            t = np.array([gx, gy, rng.uniform(0.6, 1.0)])
+            p = visible_box_points(extents[c], R, t, pts_per_obj, noise, rng)
+            n_out = int(round(outlier_frac * pts_per_obj))
+            if n_out:
+                lo, hi = p.min(0), p.max(0)
+                p[rng.choice(pts_per_obj, size=n_out, replace=False)] = rng.uniform(lo, hi, size=(n_out, 3))
+            pts.append(p)
+            lab.append(np.full(pts_per_obj, c, np.int32))
+            gt[b, c, :, :3], gt[b, c, :, 3] = R, t
+            Ri, ti = perturb_pose(R, t, angle_deg, offset, rng)
+            init[b, c, :, :3], init[b, c, :, 3] = Ri, ti
+            present[b, c] = 1
+        bg = np.column_stack([rng.uniform(-0.5, 0.5, n_bg), rng.uniform(-0.4, 0.4, n_bg), np.full(n_bg, 1.2)])
+        pts.append(bg + rng.normal(0.0, noise, size=(n_bg, 3)))
+        lab.append(np.zeros(n_bg, np.int32))
+        order = rng.permutation(n)
+        pcld[b] = np.concatenate(pts, 0)[order]
+        mask[b] = np.concatenate(lab, 0)[order]
+    return dict(models=models, extents=extents, pcld=pcld, mask=mask, gt=gt, init=init, present=present)
