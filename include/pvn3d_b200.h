@@ -197,31 +197,12 @@ int pvn3d_mlp_fp_first(const float *known_feat_pm, int c2, const int *nn_idx, co
                        const float *skip_pm, int lds, int c1, int b, int n_unknown, int m_known,
                        const float *w, const float *bias, int k_pad, int n_pad, int flags, float *out,
                        int ldo, int col0, pvn3d_stream_t stream);
-/* A whole SharedMLP in ONE launch: every layer is Conv1x1+BN(folded)+ReLU (pytorch_utils.py:25-50), the
- * 128-row tiles of the inter-layer activations stay in a per-SM scratch tile (L2) instead of crossing HBM.
- *   layers[l]: w [n_pad][k_pad] TF32-rounded, bias [n_pad]; k_pad(l) >= n_pad(l-1); 1 <= n_layers <= 3
- *   pvn3d_mlp_sa_chain: SA scale = QueryAndGroup producer (as pvn3d_mlp_sa_first) -> layers -> max-pool over
- *                       nsample when pool == ns (pointnet2_modules.py:58-69), else the point-major rows
- *   pvn3d_mlp_fp_chain: FP module = three_interpolate + concat producer (as pvn3d_mlp_fp_first) -> layers
- *   flags: only PVN3D_MLP_RESERVE_SMS(n) (every layer applies ReLU)
- *   workspace: pvn3d_mlp_chain_workspace_bytes(layers, n_layers) bytes, 16-byte aligned, private to the
- *              launch until it completes.
- * Results are identical to running the per-layer entry points above with PVN3D_MLP_ROUND_OUT between the
- * layers (same operands, same MMA order per output element). */
+/* one folded layer: w [n_pad][k_pad] TF32-rounded, bias [n_pad] */
 typedef struct {
   const float *w;
   const float *bias;
   int k_pad, n_pad;
 } pvn3d_mlp_layer_t;
-size_t pvn3d_mlp_chain_workspace_bytes(const pvn3d_mlp_layer_t *layers, int n_layers);
-int pvn3d_mlp_sa_chain(const float *xyz, const float *new_xyz, const float *feat_pm, int ldf, int c_feat,
-                       const int *idx, int b, int n, int m, int ns, const pvn3d_mlp_layer_t *layers,
-                       int n_layers, int flags, int pool, float *out, int ldo, int col0, void *workspace,
-                       size_t workspace_bytes, pvn3d_stream_t stream);
-int pvn3d_mlp_fp_chain(const float *known_feat_pm, int c2, const int *nn_idx, const float *nn_w,
-                       const float *skip_pm, int lds, int c1, int b, int n_unknown, int m_known,
-                       const pvn3d_mlp_layer_t *layers, int n_layers, int flags, float *out, int ldo,
-                       int col0, void *workspace, size_t workspace_bytes, pvn3d_stream_t stream);
 /* FACTORED first layer of an SA scale.  Conv1x1 + BN is linear before its ReLU, and QueryAndGroup's row is
  * [f_j | x_j - c_i] (pointnet2_utils.py:311-321), so  W1.[f_j | x_j - c_i] + b1 = U_j - V_i  with
  *   U_j = W1f.f_j + W1x.x_j   once per POINT    (pvn3d_sa_factor_table + pvn3d_mlp_dense without ReLU), and

@@ -959,7 +959,40 @@ __global__ void __launch_bounds__(kMlpThreads, 1) mlp_layer_kernel(const __grid_
   }
 }
 
-bool weight_tensor_map(CUtensorMap *map, const float *w, int k_pad, int n_pad, int bn);   // below
+// cuTensorMapEncodeTiled lives in libcuda; the library links only the runtime, so the entry point is
+// fetched once through cudaGetDriverEntryPoint
+typedef CUresult (*EncodeTiledFn)(CUtensorMap *, CUtensorMapDataType, cuuint32_t, void *, const cuuint64_t *,
+                                  const cuuint64_t *, const cuuint32_t *, const cuuint32_t *,
+                                  CUtensorMapInterleave, CUtensorMapSwizzle, CUtensorMapL2promotion,
+                                  CUtensorMapFloatOOBfill);
+EncodeTiledFn encode_tiled_fn() {
+  static EncodeTiledFn fn = nullptr;
+  static bool tried = false;
+  if (!tried) {
+    void *p = nullptr;
+    cudaDriverEntryPointQueryResult q;
+    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &q) == cudaSuccess &&
+        q == cudaDriverEntryPointSuccess)
+      fn = reinterpret_cast<EncodeTiledFn>(p);
+    tried = true;
+  }
+  return fn;
+}
+
+// tensor map of one weight matrix; false -> the kernel falls back to per-thread cp.async
+bool weight_tensor_map(CUtensorMap *map, const float *w, int k_pad, int n_pad, int bn) {
+  const char *env = getenv("PVN3D_MLP_TMA");
+  if (env && env[0] == '0') return false;
+  EncodeTiledFn enc = encode_tiled_fn();
+  if (!enc || (reinterpret_cast<uintptr_t>(w) & 15u)) return false;
+  const cuuint64_t dims[2] = {static_cast<cuuint64_t>(k_pad), static_cast<cuuint64_t>(n_pad)};
+  const cuuint64_t strides[1] = {static_cast<cuuint64_t>(k_pad) * sizeof(float)};
+  const cuuint32_t box[2] = {32u, static_cast<cuuint32_t>(bn)};
+  const cuuint32_t estr[2] = {1u, 1u};
+  return enc(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, const_cast<float *>(w), dims, strides, box, estr,
+             CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+             CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
+}
 
 template <int PRO, int EPI>
 int launch_mlp(MlpArgs &a, cudaStream_t st) {
@@ -1593,453 +1626,6 @@ int launch_sa_fact2w(Sa2wArgs &g, int stages, cudaStream_t st) {
   return check_launch("mlp_sa_fact2w_kernel");
 }
 
-// =====================================================================================================
-// The whole SharedMLP of one SA scale (3 layers) / FP module (2 layers) in ONE persistent kernel.
-//
-// One launch per layer sends every inter-layer activation through HBM twice (write + read: 7.0 of the
-// 10.4 GB a 32-frame batch moves, 6.8 GB measured by ncu in round 1).  Rows of a shared MLP are
-// independent, so a CTA can take a 128-row tile through ALL layers: layer l's epilogue stores its
-// TF32-rounded tile into a CTA-private scratch tile (128 x n_pad floats, re-used for every row tile of the
-// CTA: it lives in L2 and is overwritten before it is ever evicted), and the producers of layer l+1 pull
-// it back with cp.async.  To keep the tensor core, the producers and the epilogue busy while one tile
-// waits on its own previous layer, a CTA works on TWO row tiles at a time ("slots"), in the order
-//     (A,L0) (B,L0) (A,L1) (B,L1) (A,L2) (B,L2) | next pair ...
-// Every (tile, layer, column block) is one ITEM; the three roles (producers / MMA issuer / epilogue) walk
-// the same item sequence, exactly like the per-layer kernel walks tiles: the operand ring and the
-// accumulator tile are shared by all layers.  New dependency: the producers of (slot, l>0) wait on
-// h_ready[slot], on which the 128 epilogue threads arrive after storing (slot, l-1).
-constexpr int kChainMaxSlots = 8;
-struct ChainLayer {
-  const float *w, *bias;
-  int k_pad, n_pad, bn, n_blocks;
-};
-struct MlpChainArgs {
-  // weight matrices as TMA tensor maps: [n_pad][k_pad] fp32, box = 32 columns (128 B) x bn rows,
-  // SWIZZLE_128B -- one cp.async.bulk.tensor.2d per K chunk lands the B operand in the wgmma layout
-  alignas(64) CUtensorMap tmap[3];
-  int use_tma;
-  MlpArgs base;        // producer of layer 0 + final epilogue (rows, out, ldo, col0, pool); bn = widest layer tile
-  ChainLayer layer[3];
-  int n_layers;
-  float *scratch;      // [grid][n_slots][slot_floats]
-  int h_off[2];        // float offset of layer l's output tile inside a slot (l < n_layers - 1)
-  int slot_floats;
-  int n_slots;         // row tiles a CTA keeps in flight (2..kChainMaxSlots)
-};
-
-struct ChainSmemCtl {
-  uint64_t full[kMlpMaxStages];
-  uint64_t empty[kMlpMaxStages];
-  uint64_t acc_full;
-  uint64_t acc_empty;
-  uint64_t h_ready[kChainMaxSlots];   // 128 arrivals: epilogue threads, after storing a slot's intermediate tile
-  uint64_t h_seen[kChainMaxSlots];    // 256 arrivals: every producer thread, once it has passed a h_ready phase
-};
-
-template <int PRO, int EPI>
-__global__ void __launch_bounds__(kMlpThreads, 1) mlp_chain_kernel(const __grid_constant__ MlpChainArgs c) {
-  extern __shared__ unsigned char mlp_smem_raw[];
-  __shared__ ChainSmemCtl ctl;
-  const MlpArgs &a = c.base;
-  const uint32_t raw = smem_u32(mlp_smem_raw);
-  const uint32_t ring = (raw + 1023u) & ~1023u;
-  const uint32_t a_bytes = kMlpBM * 128u;
-  const uint32_t stage_bytes = a_bytes + ((static_cast<uint32_t>(a.bn) * 128u + 1023u) & ~1023u);
-  const uint32_t acc_s = ring + static_cast<uint32_t>(a.stages) * stage_bytes;
-  const uint32_t front = mlp_smem_front(a.stages, a.bn, a.acc_ld);
-
-  const int t = threadIdx.x;
-  const unsigned warp = t >> 5, lane = t & 31u;
-  const int S = a.stages;
-  const int NL = c.n_layers;
-  const long long row_tiles = (a.rows + kMlpBM - 1) / kMlpBM;
-  // row tiles of this CTA: blockIdx.x, +grid, ...; handled NS at a time
-  const int NS = c.n_slots;
-  const long long my_tiles = row_tiles > blockIdx.x ? (row_tiles - blockIdx.x + gridDim.x - 1) / gridDim.x : 0;
-  const long long n_pairs = (my_tiles + NS - 1) / NS;
-  float *const scratch = c.scratch + static_cast<size_t>(blockIdx.x) * NS * c.slot_floats;
-
-  if (t == 0) {
-    for (int s = 0; s < S; ++s) {
-      mbar_init(&ctl.full[s], 128);
-      mbar_init(&ctl.empty[s], kMlpMmaWarps);
-    }
-    mbar_init(&ctl.acc_full, kMlpMmaWarps * 32);
-    mbar_init(&ctl.acc_empty, kMlpEpiWarps * 32);
-    for (int b = 0; b < kChainMaxSlots; ++b) {
-      mbar_init(&ctl.h_ready[b], 128);
-      mbar_init(&ctl.h_seen[b], kMlpProWarps * 32);
-    }
-    mbar_fence_init();
-  }
-  __syncthreads();
-
-  if (warp >= kMlpEpiWarps && warp < kMlpEpiWarps + kMlpProWarps) {
-    // ================= producers ======================================================================
-    const int pt = (t - kMlpEpiWarps * 32) & 127;
-    const unsigned grp = (warp - kMlpEpiWarps) >> 2;
-    const int pw = pt >> 5, sub = static_cast<int>(lane & 7u), rg = static_cast<int>(lane >> 3);
-    const int r_first = 32 * pw + rg;
-    bool vec_ok = true;
-    if (PRO == PRO_DENSE) vec_ok = (a.lda % 4 == 0) && ((reinterpret_cast<uintptr_t>(a.a) & 15u) == 0);
-    if (PRO == PRO_SA_GATHER)
-      vec_ok = a.c_feat > 0 && (a.ldf % 4 == 0) && ((reinterpret_cast<uintptr_t>(a.feat) & 15u) == 0);
-    if (PRO == PRO_FP_INTERP)
-      vec_ok = (a.c2 % 4 == 0) && ((reinterpret_cast<uintptr_t>(a.known_feat) & 15u) == 0);
-    int pend0 = 0, pend1 = 0, npend = 0;
-    unsigned hwaits = 0u;   // bit `slot`: parity of the next h_ready phase this thread waits for
-    long long it_base = 0;
-    for (long long pair = 0; pair < n_pairs; ++pair) {
-      for (int l = 0; l < NL; ++l) {
-        const ChainLayer &L = c.layer[l];
-        const int kc_total = L.k_pad / 32;
-        for (int slot = 0; slot < NS; ++slot) {
-          const long long local = NS * pair + slot;
-          if (local >= my_tiles) continue;
-          const long long rt = blockIdx.x + local * gridDim.x;
-          const long long p_first = rt * kMlpBM + r_first;
-          RowState rs;
-          int a_cols_l = 0;
-          if (l == 0) {
-            rows_setup<PRO>(a, p_first, rs);
-          } else {
-            // input = this slot's intermediate tile of layer l-1 (all 128 rows exist, TF32-rounded).
-            // Nothing of this thread may stay unpublished while it blocks: the MMA warp consumes chunks in
-            // order, and the tile awaited here is produced behind every chunk staged so far.
-            if (npend > 0) {
-              cp_async_wait<0>();
-              fence_proxy_async_smem();
-              mbar_arrive(&ctl.full[pend0]);
-              if (npend == 2) mbar_arrive(&ctl.full[pend1]);
-              npend = 0;
-            }
-            mbar_wait(&ctl.h_ready[slot], (hwaits >> slot) & 1u);
-            hwaits ^= 1u << slot;
-            mbar_arrive(&ctl.h_seen[slot]);   // this phase has been observed: the epilogue may open the next one
-            const float *h = scratch + static_cast<size_t>(slot) * c.slot_floats + c.h_off[l - 1];
-            const int ld = c.layer[l - 1].n_pad;
-            rs.live = 0xffu;
-#pragma unroll
-            for (int j = 0; j < 8; ++j) rs.row[j] = h + static_cast<size_t>(r_first + 4 * j) * ld;
-            a_cols_l = ld;
-          }
-          for (int nb = 0; nb < L.n_blocks; ++nb) {
-            const int n0 = nb * L.bn;
-            const int bn = min(L.bn, L.n_pad - n0);
-            for (int kc = 0; kc < kc_total; ++kc) {
-              const long long it = it_base + kc;
-              if (static_cast<unsigned>(it & 1) != grp) continue;
-              const int s = static_cast<int>(it % S);
-              if (npend == 2 || (l == 0 && npend > 0)) {
-                // publish the older asynchronous chunk(s) before this thread can block on a free stage
-                // (layer 0 stages synchronously: everything still pending is flushed first)
-                if (npend == 2 && l != 0) {
-                  cp_async_wait<1>();
-                  fence_proxy_async_smem();
-                  mbar_arrive(&ctl.full[pend0]);
-                  pend0 = pend1;
-                  npend = 1;
-                } else {
-                  cp_async_wait<0>();
-                  fence_proxy_async_smem();
-                  mbar_arrive(&ctl.full[pend0]);
-                  if (npend == 2) mbar_arrive(&ctl.full[pend1]);
-                  npend = 0;
-                }
-              }
-              mbar_wait(&ctl.empty[s], static_cast<unsigned>(((it / S) & 1) ^ 1));
-              const uint32_t sa = ring + static_cast<uint32_t>(s) * stage_bytes;
-              const uint32_t sb = sa + a_bytes;
-              if (c.use_tma) {
-                // B operand by the TMA engine: rows n0..n0+L.bn of W, columns kc*32..+32, swizzled on the fly;
-                // completes on the stage's `full` barrier (transaction bytes registered first)
-                if (pt == 0) {
-                  mbar_expect_tx_only(&ctl.full[s], static_cast<unsigned>(L.bn) * 128u);
-                  tma_load_2d(sb, &c.tmap[l], kc * 32, n0, &ctl.full[s]);
-                }
-              } else {
-                for (int i = pt; i < bn * 8; i += 128) {
-                  const int n = i >> 3, cc = i & 7;
-                  cp_async16(sb + sw128_off(n, cc), L.w + static_cast<size_t>(n0 + n) * L.k_pad + kc * 32 + cc * 4);
-                }
-              }
-              if (l > 0) {
-                const int k = kc * 32 + 4 * sub;
-#pragma unroll
-                for (int j = 0; j < 8; ++j)
-                  cp_async16(sa + sw128_off(r_first + 4 * j, sub), rs.row[j] + (k < a_cols_l ? k : 0),
-                             k < a_cols_l ? 16u : 0u);
-                cp_async_commit();
-                if (npend == 0) pend0 = s; else pend1 = s;
-                ++npend;
-              } else {
-                cp_async_commit();
-                stage_a_chunk<PRO>(a, rs, p_first, r_first, sub, kc * 32, sa, vec_ok);
-                cp_async_wait<0>();
-                fence_proxy_async_smem();
-                mbar_arrive(&ctl.full[s]);
-              }
-            }
-            it_base += kc_total;
-          }
-        }
-      }
-    }
-    if (npend > 0) {
-      cp_async_wait<0>();
-      fence_proxy_async_smem();
-      mbar_arrive(&ctl.full[pend0]);
-      if (npend == 2) mbar_arrive(&ctl.full[pend1]);
-    }
-  } else if (warp < kMlpEpiWarps) {
-    // ================= epilogue =========================================================================
-    long long j = 0;
-    unsigned hsig_any = 0u, hsig_par = 0u;   // per slot: signalled before / parity of the last phase signalled
-    const uint32_t stg = raw + front + warp * 4096u;
-    for (long long pair = 0; pair < n_pairs; ++pair) {
-      for (int l = 0; l < NL; ++l) {
-        const ChainLayer &L = c.layer[l];
-        const bool last = l == NL - 1;
-        for (int slot = 0; slot < NS; ++slot) {
-          const long long local = NS * pair + slot;
-          if (local >= my_tiles) continue;
-          const long long rt = blockIdx.x + local * gridDim.x;
-          const long long p0 = rt * kMlpBM;
-          float *const h = scratch + static_cast<size_t>(slot) * c.slot_floats + (last ? 0 : c.h_off[l]);
-          for (int nb = 0; nb < L.n_blocks; ++nb, ++j) {
-            const int n0 = nb * L.bn;
-            const int bn = min(L.bn, L.n_pad - n0);
-            mbar_wait(&ctl.acc_full, static_cast<unsigned>(j & 1));
-            const long long prow = p0 + warp * 32 + lane;
-            for (int c0 = 0; c0 < bn; c0 += 32) {
-              float v[32];
-              const int cw = min(32, bn - c0);
-              acc_ld_row(acc_s, a.acc_ld, static_cast<int>(warp * 32 + lane), c0, cw, v);
-              if (!last || EPI == EPI_STORE) {
-                // intermediate: bias + ReLU + TF32 rounding into the slot's scratch tile (row = local row);
-                // final STORE: bias + ReLU (+ rounding if asked) into out
-                const bool rnd = !last || a.round_out;
-#pragma unroll
-                for (int q = 0; q < 8; ++q) {
-                  if (q * 4 < cw) {
-                    const float4 bq = ldg128(L.bias + n0 + c0 + q * 4);
-                    float4 r;
-                    r.x = fmaxf(v[q * 4 + 0] + bq.x, 0.f);
-                    r.y = fmaxf(v[q * 4 + 1] + bq.y, 0.f);
-                    r.z = fmaxf(v[q * 4 + 2] + bq.z, 0.f);
-                    r.w = fmaxf(v[q * 4 + 3] + bq.w, 0.f);
-                    if (rnd) {
-                      r.x = to_tf32(r.x); r.y = to_tf32(r.y); r.z = to_tf32(r.z); r.w = to_tf32(r.w);
-                    }
-                    sts128(stg + lane * 128u + ((static_cast<uint32_t>(q) ^ (lane & 7u)) << 4), r.x, r.y, r.z, r.w);
-                  }
-                }
-                __syncwarp();
-                const unsigned chunk = lane & 7u;
-                if (static_cast<int>(chunk) * 4 < cw) {
-#pragma unroll
-                  for (int i = 0; i < 8; ++i) {
-                    const unsigned row = 4u * i + (lane >> 3);
-                    const float4 r = lds128(stg + row * 128u + ((chunk ^ (row & 7u)) << 4));
-                    if (!last) {
-                      *reinterpret_cast<float4 *>(h + static_cast<size_t>(warp * 32 + row) * L.n_pad + n0 + c0 + chunk * 4) = r;
-                    } else {
-                      const long long pr = p0 + warp * 32 + row;
-                      if (pr < a.rows)
-                        *reinterpret_cast<float4 *>(a.out + pr * a.ldo + a.col0 + n0 + c0 + chunk * 4) = r;
-                    }
-                  }
-                }
-                __syncwarp();
-              } else {
-                // final layer of an SA scale: ReLU(max over the `pool` rows of each centre + bias)
-                if (prow >= a.rows) {
-#pragma unroll
-                  for (int i = 0; i < 32; ++i) v[i] = -__int_as_float(0x7f800000);
-                }
-                const long long grow0 = (p0 + warp * 32) / a.pool;
-                if (a.pool == 32) {
-                  warp_colmax_32(v, lane);
-                  const int col = static_cast<int>(lane);
-                  if (col < cw && p0 + warp * 32 < a.rows)
-                    a.out[grow0 * a.ldo + a.col0 + n0 + c0 + col] = fmaxf(v[0] + __ldg(L.bias + n0 + c0 + col), 0.f);
-                } else if (a.pool == 16) {
-                  warp_colmax_16(v, lane);
-                  const int g = lane >> 4, col = static_cast<int>(lane & 15u) * 2;
-                  if (col < cw && p0 + warp * 32 + g * 16 < a.rows) {
-                    float2 r;
-                    r.x = fmaxf(v[0] + __ldg(L.bias + n0 + c0 + col), 0.f);
-                    r.y = fmaxf(v[1] + __ldg(L.bias + n0 + c0 + col + 1), 0.f);
-                    *reinterpret_cast<float2 *>(a.out + (grow0 + g) * a.ldo + a.col0 + n0 + c0 + col) = r;
-                  }
-                } else {  // pool == 8
-                  warp_colmax_8(v, lane);
-                  const int g = lane >> 3, col = static_cast<int>(lane & 7u) * 4;
-                  if (col < cw && p0 + warp * 32 + g * 8 < a.rows) {
-                    float4 r;
-                    r.x = fmaxf(v[0] + __ldg(L.bias + n0 + c0 + col), 0.f);
-                    r.y = fmaxf(v[1] + __ldg(L.bias + n0 + c0 + col + 1), 0.f);
-                    r.z = fmaxf(v[2] + __ldg(L.bias + n0 + c0 + col + 2), 0.f);
-                    r.w = fmaxf(v[3] + __ldg(L.bias + n0 + c0 + col + 3), 0.f);
-                    *reinterpret_cast<float4 *>(a.out + (grow0 + g) * a.ldo + a.col0 + n0 + c0 + col) = r;
-                  }
-                }
-              }
-            }
-            mbar_arrive(&ctl.acc_empty);
-          }
-          if (!last) {
-            // the slot's tile of layer l is complete in global memory (L2): make it visible at GPU scope
-            // (the producers read it back with cp.async.cg, which goes to L2) and release the next layer
-            __threadfence();
-            // phase k of h_ready[slot] may only complete once every producer thread has observed phase k-1
-            // (a parity wait cannot tell phase k-1 from phase k+1)
-            if ((hsig_any >> slot) & 1u) mbar_wait(&ctl.h_seen[slot], (hsig_par >> slot) & 1u);
-            else hsig_par |= 1u << slot;       // first signal: the next wait is for phase 0 -> parity 0 after the toggle
-            hsig_any |= 1u << slot;
-            hsig_par ^= 1u << slot;
-            mbar_arrive(&ctl.h_ready[slot]);
-          }
-        }
-      }
-    }
-  } else {
-    // ================= warps 12-19: MMA, warpgroup wg takes rows 64wg..64wg+63 of every item ==========
-    const unsigned mw = warp - (kMlpEpiWarps + kMlpProWarps), wg = mw >> 2;
-    const int frag_row = static_cast<int>(64 * wg + 16 * (mw & 3) + (lane >> 2));
-    long long it_base = 0, j = 0;
-    for (long long pair = 0; pair < n_pairs; ++pair) {
-      for (int l = 0; l < NL; ++l) {
-        const ChainLayer &L = c.layer[l];
-        const int kc_total = L.k_pad / 32;
-        for (int slot = 0; slot < NS; ++slot) {
-          if (NS * pair + slot >= my_tiles) continue;
-          for (int nb = 0; nb < L.n_blocks; ++nb, ++j, it_base += kc_total)
-            mma_tile_n(mma_n(min(L.bn, L.n_pad - nb * L.bn)), ring, stage_bytes, S, it_base, kc_total, ctl.full,
-                       ctl.empty, &ctl.acc_full, &ctl.acc_empty,
-                       static_cast<unsigned>(j & 1), acc_s, a.acc_ld, wg, frag_row, lane);
-        }
-      }
-    }
-  }
-}
-
-// per-layer tile geometry of a chain; returns the scratch floats one slot needs
-int chain_plan(MlpChainArgs &c, const pvn3d_mlp_layer_t *layers, int n_layers) {
-  int bn_max = 0, off = 0;
-  for (int l = 0; l < n_layers; ++l) {
-    ChainLayer &L = c.layer[l];
-    L.w = layers[l].w; L.bias = layers[l].bias; L.k_pad = layers[l].k_pad; L.n_pad = layers[l].n_pad;
-    L.bn = mma_n(L.n_pad);
-    L.n_blocks = ceil_div(L.n_pad, L.bn);
-    bn_max = std::max(bn_max, L.bn);
-    if (l < n_layers - 1) {
-      c.h_off[l] = off;
-      off += kMlpBM * L.n_pad;
-    }
-  }
-  c.n_layers = n_layers;
-  c.slot_floats = off;
-  c.base.bn = bn_max;
-  c.base.acc_ld = std::max(32, bn_max);
-  return off;
-}
-
-// cuTensorMapEncodeTiled lives in libcuda; the library links only the runtime, so the entry point is
-// fetched once through cudaGetDriverEntryPoint
-typedef CUresult (*EncodeTiledFn)(CUtensorMap *, CUtensorMapDataType, cuuint32_t, void *, const cuuint64_t *,
-                                  const cuuint64_t *, const cuuint32_t *, const cuuint32_t *,
-                                  CUtensorMapInterleave, CUtensorMapSwizzle, CUtensorMapL2promotion,
-                                  CUtensorMapFloatOOBfill);
-EncodeTiledFn encode_tiled_fn() {
-  static EncodeTiledFn fn = nullptr;
-  static bool tried = false;
-  if (!tried) {
-    void *p = nullptr;
-    cudaDriverEntryPointQueryResult q;
-    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &q) == cudaSuccess &&
-        q == cudaDriverEntryPointSuccess)
-      fn = reinterpret_cast<EncodeTiledFn>(p);
-    tried = true;
-  }
-  return fn;
-}
-
-// tensor map of one weight matrix; false -> the kernel falls back to per-thread cp.async
-bool weight_tensor_map(CUtensorMap *map, const float *w, int k_pad, int n_pad, int bn) {
-  const char *env = getenv("PVN3D_MLP_TMA");
-  if (env && env[0] == '0') return false;
-  EncodeTiledFn enc = encode_tiled_fn();
-  if (!enc || (reinterpret_cast<uintptr_t>(w) & 15u)) return false;
-  const cuuint64_t dims[2] = {static_cast<cuuint64_t>(k_pad), static_cast<cuuint64_t>(n_pad)};
-  const cuuint64_t strides[1] = {static_cast<cuuint64_t>(k_pad) * sizeof(float)};
-  const cuuint32_t box[2] = {32u, static_cast<cuuint32_t>(bn)};
-  const cuuint32_t estr[2] = {1u, 1u};
-  return enc(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, const_cast<float *>(w), dims, strides, box, estr,
-             CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-             CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
-}
-bool chain_tensor_maps(MlpChainArgs &c) {
-  for (int l = 0; l < c.n_layers; ++l)
-    if (!weight_tensor_map(&c.tmap[l], c.layer[l].w, c.layer[l].k_pad, c.layer[l].n_pad, c.layer[l].bn)) return false;
-  return true;
-}
-
-bool chain_layers_ok(const pvn3d_mlp_layer_t *layers, int n_layers, int k_first_min) {
-  if (!layers || n_layers < 1 || n_layers > 3) return false;
-  for (int l = 0; l < n_layers; ++l) {
-    if (!layers[l].w || !layers[l].bias || layers[l].k_pad <= 0 || layers[l].k_pad % 32 ||
-        layers[l].n_pad <= 0 || layers[l].n_pad % 16)
-      return false;
-    // layer l reads the n_pad(l-1) columns of the previous tile: its K must cover them
-    if (l > 0 && layers[l].k_pad < layers[l - 1].n_pad) return false;
-  }
-  return layers[0].k_pad >= k_first_min;
-}
-
-// row tiles a CTA keeps in flight: enough to cover the epilogue -> L2 -> producer latency of a layer
-// transition, as long as all scratch tiles of the grid stay well inside the 50 MB L2 (<= 24 MB)
-int chain_slots(int slot_floats, long long row_tiles, unsigned grid) {
-  int want = 4;
-  if (const char *env = getenv("PVN3D_CHAIN_SLOTS")) want = atoi(env);
-  want = std::max(2, std::min(kChainMaxSlots, want));
-  const long long per_cta = (row_tiles + grid - 1) / std::max(1u, grid);
-  while (want > 2 && want > per_cta) --want;
-  while (want > 2 && static_cast<size_t>(grid) * want * slot_floats * sizeof(float) > (24u << 20)) --want;
-  return want;
-}
-
-template <int PRO, int EPI>
-int launch_chain(MlpChainArgs &c, void *workspace, size_t workspace_bytes, cudaStream_t st) {
-  MlpArgs &a = c.base;
-  if (a.rows <= 0) return PVN3D_OK;
-  // the barrier block is static shared memory: the dynamic part stays below the block limit by one kilobyte
-  constexpr int kDynMax = kMlpSmemMax - 1024;
-  static_assert(sizeof(ChainSmemCtl) <= 1024, "barrier block");
-  const size_t stage_bytes = kMlpBM * 128 + align_up(static_cast<size_t>(a.bn) * 128, 1024);
-  const size_t fixed = mlp_smem_front(0, a.bn, a.acc_ld) + kMlpEpiWarps * 4096;
-  int stages = static_cast<int>((kDynMax - fixed) / stage_bytes);
-  if (stages > kMlpMaxStages) stages = kMlpMaxStages;
-  if (stages < 3) return PVN3D_ERR_UNSUPPORTED;   // asynchronous producers keep two chunks in flight
-  a.stages = stages;
-  const size_t smem = mlp_smem_front(stages, a.bn, a.acc_ld) + kMlpEpiWarps * 4096;
-  auto kern = mlp_chain_kernel<PRO, EPI>;
-  static PerDeviceOnce once;
-  PVN3D_ONCE_PER_DEVICE(once, cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, kDynMax),
-                        "mlp chain smem attr");
-  const int sms = std::max(1, sm_count() - a.reserve_sms);
-  const long long row_tiles = (a.rows + kMlpBM - 1) / kMlpBM;
-  const unsigned grid = static_cast<unsigned>(std::min<long long>(row_tiles, sms));
-  c.n_slots = chain_slots(c.slot_floats, row_tiles, grid);
-  const size_t need = static_cast<size_t>(grid) * c.n_slots * c.slot_floats * sizeof(float);
-  if (c.n_layers > 1 && (!workspace || workspace_bytes < need || (reinterpret_cast<uintptr_t>(workspace) & 15u)))
-    return PVN3D_ERR_WORKSPACE;
-  c.scratch = static_cast<float *>(workspace);
-  c.use_tma = chain_tensor_maps(c) ? 1 : 0;
-  kern<<<grid, kMlpThreads, smem, st>>>(c);
-  return check_launch("mlp_chain_kernel");
-}
-
 int dispatch(MlpArgs &a, int pro, int pool, cudaStream_t st) {
   if (pool) {
     if (pool != 8 && pool != 16 && pool != 32) return PVN3D_ERR_UNSUPPORTED;
@@ -2194,63 +1780,6 @@ extern "C" int pvn3d_three_nn_weights(const float *dist2, long long rows, float 
   nn_weights_kernel<<<static_cast<unsigned>((rows + 255) / 256), 256, 0, as_stream(stream)>>>(
       dist2, rows, weight);
   return check_launch("nn_weights_kernel");
-}
-
-extern "C" size_t pvn3d_mlp_chain_workspace_bytes(const pvn3d_mlp_layer_t *layers, int n_layers) {
-  if (!layers || n_layers < 1 || n_layers > 3) return 0;
-  size_t floats = 0;
-  for (int l = 0; l + 1 < n_layers; ++l) floats += static_cast<size_t>(kMlpBM) * layers[l].n_pad;
-  return static_cast<size_t>(std::max(1, sm_count())) * kChainMaxSlots * floats * sizeof(float) + 256;
-}
-
-extern "C" int pvn3d_mlp_sa_chain(const float *xyz, const float *new_xyz, const float *feat_pm, int ldf,
-                                  int c_feat, const int *idx, int b, int n, int m, int ns,
-                                  const pvn3d_mlp_layer_t *layers, int n_layers, int flags, int pool,
-                                  float *out, int ldo, int col0, void *workspace, size_t workspace_bytes,
-                                  pvn3d_stream_t stream) {
-  if (!xyz || !new_xyz || !idx || !out || b < 0 || n <= 0 || m < 0 || ns <= 0 || c_feat < 0 ||
-      (c_feat > 0 && (!feat_pm || ldf < c_feat)) || ldo % 4 || col0 % 4 ||
-      !chain_layers_ok(layers, n_layers, c_feat + 3))
-    return PVN3D_ERR_INVALID_ARG;
-  if (pool && pool != ns) return PVN3D_ERR_INVALID_ARG;
-  if (pool && pool != 8 && pool != 16 && pool != 32) return PVN3D_ERR_UNSUPPORTED;
-  if (static_cast<long long>(m) * ns > 0x3fffffffll || static_cast<long long>(b) * n > 0x7fffffffll ||
-      static_cast<long long>(b) * m > 0x7fffffffll)
-    return PVN3D_ERR_UNSUPPORTED;
-  MlpChainArgs c{};
-  MlpArgs &a = c.base;
-  a.rows = static_cast<long long>(b) * m * ns;
-  a.xyz = xyz; a.new_xyz = new_xyz; a.feat = feat_pm; a.ldf = ldf; a.c_feat = c_feat; a.idx = idx;
-  a.n = n; a.m = m; a.ns = ns;
-  a.out = out; a.ldo = ldo; a.col0 = col0; a.relu = 1; a.round_out = 0; a.pool = pool;
-  a.reserve_sms = (flags >> 8) & 0xff;
-  a.k_pad = layers[0].k_pad;
-  chain_plan(c, layers, n_layers);
-  if (pool) return launch_chain<PRO_SA_GATHER, EPI_MAXPOOL>(c, workspace, workspace_bytes, as_stream(stream));
-  return launch_chain<PRO_SA_GATHER, EPI_STORE>(c, workspace, workspace_bytes, as_stream(stream));
-}
-
-extern "C" int pvn3d_mlp_fp_chain(const float *known_feat_pm, int c2, const int *nn_idx, const float *nn_w,
-                                  const float *skip_pm, int lds, int c1, int b, int n_unknown,
-                                  int m_known, const pvn3d_mlp_layer_t *layers, int n_layers, int flags,
-                                  float *out, int ldo, int col0, void *workspace, size_t workspace_bytes,
-                                  pvn3d_stream_t stream) {
-  if (!known_feat_pm || !nn_idx || !nn_w || !out || b < 0 || n_unknown < 0 || m_known <= 0 || c2 <= 0 ||
-      c1 < 0 || (c1 > 0 && (!skip_pm || lds < c1)) || ldo % 4 || col0 % 4 ||
-      !chain_layers_ok(layers, n_layers, c2 + c1))
-    return PVN3D_ERR_INVALID_ARG;
-  if (static_cast<long long>(b) * m_known > 0x7fffffffll || n_unknown > 0x3fffffff)
-    return PVN3D_ERR_UNSUPPORTED;
-  MlpChainArgs c{};
-  MlpArgs &a = c.base;
-  a.rows = static_cast<long long>(b) * n_unknown;
-  a.known_feat = known_feat_pm; a.c2 = c2; a.nn_idx = nn_idx; a.nn_w = nn_w; a.skip = skip_pm;
-  a.lds = lds; a.c1 = c1; a.n_unknown = n_unknown; a.m_known = m_known;
-  a.out = out; a.ldo = ldo; a.col0 = col0; a.relu = 1; a.round_out = 0; a.pool = 0;
-  a.reserve_sms = (flags >> 8) & 0xff;
-  a.k_pad = layers[0].k_pad;
-  chain_plan(c, layers, n_layers);
-  return launch_chain<PRO_FP_INTERP, EPI_STORE>(c, workspace, workspace_bytes, as_stream(stream));
 }
 
 extern "C" int pvn3d_sa_factor_table(const float *xyz, const float *feat_pm, int ldf, int c_feat, long long rows,

@@ -4,13 +4,22 @@ Takes a Pointnet2MSG module (this package's mirror or the reference's -- same st
 folds every Conv2d(1x1, no bias) + BatchNorm2d (eval) pair into a TF32-rounded, zero-padded weight
 matrix + bias, and runs `Pointnet2MSG.forward` (reference pvn3d/lib/pvn3d.py:126-154) as:
 
-  per SA level : furthest_point_sampling -> (per scale) ball_query -> first SharedMLP layer with the
-                 grouping fused into the tensor-core operand producer (pvn3d_mlp_sa_first) -> middle
-                 layer (pvn3d_mlp_dense) -> last layer with ReLU + max-pool over nsample fused into the
-                 epilogue, written straight into the level's point-major feature table
-  per FP level : three_nn -> inverse-distance weights -> first layer with three_interpolate + concat
-                 fused into the producer (pvn3d_mlp_fp_first) -> second layer
-  last         : [B,N,128] -> [B,128,N] (the layout the reference returns)
+  per SA level : furthest_point_sampling -> ball_query of both radii -> factored first SharedMLP layer:
+                 U = W1 . [f | x] once per point (pvn3d_sa_factor_table, shared by both scales, then
+                 pvn3d_mlp_dense) and V = W1x . c - b1 once per centre (pvn3d_sa_centre_term) -> layers 2
+                 and 3 on relu(U[idx] - V) with ReLU + max-pool over nsample in ONE launch
+                 (pvn3d_mlp_sa_fact2 for SA1 / SA2, pvn3d_mlp_sa_fact2w for SA3 / SA4), written straight
+                 into the level's point-major feature table
+  per FP level : three_nn -> inverse-distance weights ->
+                 FP2-4: first layer with three_interpolate + concat fused into the tensor-core operand
+                        producer (pvn3d_mlp_fp_first) -> second layer (pvn3d_mlp_dense)
+                 FP1  : factored first layer (P = W1k . known, S = W1s . skip + b1 by pvn3d_mlp_dense) ->
+                        second layer on relu(interpolated P + S) (pvn3d_mlp_fp_fact), stored channel-major
+                        [B,128,N], the layout the reference returns (when N % 32 == 0; else a transpose follows)
+
+PVN3D_MLP_FACTOR=0 (or `factor = False`) runs the unfactored layers instead: the first SA layer with the
+grouping fused into the producer (pvn3d_mlp_sa_first) -> pvn3d_mlp_dense -> pvn3d_mlp_dense with the
+max-pool, and FP1 as FP2-4, followed by a [B,N,128] -> [B,128,N] transpose.
 
 The grouped tensors [B,3+C,M,S] and the interpolated tensors [B,C,n] are never materialised; no
 cuDNN / cuBLAS / ATen kernel runs in this path.
@@ -232,57 +241,6 @@ def mlp_fp_fact(p: torch.Tensor, s_: torch.Tensor, nn_idx: torch.Tensor, nn_w: t
     return out
 
 
-class LayerChain:
-    """the layers of one SharedMLP as the pvn3d_mlp_layer_t array pvn3d_mlp_{sa,fp}_chain take, plus the
-    scratch the chained kernel needs (inter-layer tiles of the CTAs, L2-resident)"""
-
-    def __init__(self, layers: List[PackedLayer]):
-        self.layers = layers
-        self.arr = (_lib.MlpLayer * len(layers))()
-        for i, pl in enumerate(layers):
-            self.arr[i].w, self.arr[i].bias = pl.w.data_ptr(), pl.bias.data_ptr()
-            self.arr[i].k_pad, self.arr[i].n_pad = pl.k_pad, pl.n_pad
-        self.n = len(layers)
-        self.ws_bytes = int(_lib.load().pvn3d_mlp_chain_workspace_bytes(ctypes.addressof(self.arr), self.n))
-        self.ws = torch.empty((self.ws_bytes + 16,), dtype=torch.uint8, device=layers[0].w.device)
-        self.ws_ptr = (self.ws.data_ptr() + 15) // 16 * 16
-
-    @property
-    def ptr(self) -> int:
-        return ctypes.addressof(self.arr)
-
-
-def mlp_sa_chain(xyz, new_xyz, feat_pm, ldf, c_feat, idx, chain: LayerChain, pool=0, out=None, col0=0, reserve=0):
-    """a whole SA-scale SharedMLP (QueryAndGroup producer -> layers -> max-pool) in one launch"""
-    lib = _lib.load()
-    b, n = xyz.shape[0], xyz.shape[1]
-    m, ns = idx.shape[1], idx.shape[2]
-    rows = b * m * ns
-    if out is None:
-        out = torch.empty((rows // pool if pool else rows, chain.layers[-1].n_pad), dtype=torch.float32, device=xyz.device)
-    with torch.cuda.device(xyz.device):
-        rc = lib.pvn3d_mlp_sa_chain(ptr(xyz), ptr(new_xyz), feat_pm, ldf, c_feat, ptr(idx), b, n, m, ns, chain.ptr, chain.n,
-                                    _flags(True, reserve=reserve), pool, ptr(out), out.size(-1), col0, chain.ws_ptr,
-                                    chain.ws_bytes, _stream(xyz.device))
-    check(rc, "pvn3d_mlp_sa_chain")
-    return out
-
-
-def mlp_fp_chain(known_feat_pm, nn_idx, nn_w, skip_ptr, lds, c1, chain: LayerChain, out=None, reserve=0):
-    """a whole FP-module SharedMLP (three_interpolate + concat producer -> layers) in one launch"""
-    lib = _lib.load()
-    b, m_known, c2 = known_feat_pm.shape
-    n_unknown = nn_idx.shape[1]
-    if out is None:
-        out = torch.empty((b * n_unknown, chain.layers[-1].n_pad), dtype=torch.float32, device=known_feat_pm.device)
-    with torch.cuda.device(known_feat_pm.device):
-        rc = lib.pvn3d_mlp_fp_chain(ptr(known_feat_pm), c2, ptr(nn_idx), ptr(nn_w), skip_ptr, lds, c1, b, n_unknown, m_known,
-                                    chain.ptr, chain.n, _flags(True, reserve=reserve), ptr(out), out.size(-1), 0, chain.ws_ptr,
-                                    chain.ws_bytes, _stream(known_feat_pm.device))
-    check(rc, "pvn3d_mlp_fp_chain")
-    return out
-
-
 def three_nn_weights(dist2: torch.Tensor) -> torch.Tensor:
     lib = _lib.load()
     w = torch.empty_like(dist2)
@@ -312,15 +270,8 @@ class GeoPlan:
 class FusedPointnet2MSG:
     """Inference engine for Pointnet2MSG on libpvn3d_b200 only (see module docstring)."""
 
-    def __init__(self, model: torch.nn.Module, device="cuda", chain: bool | None = None):
+    def __init__(self, model: torch.nn.Module, device="cuda"):
         self.dev = torch.device(device)
-        #: chain=True: one launch per SharedMLP (inter-layer tiles stay in L2, DRAM traffic of the MLPs -95 %);
-        #: False (default): one launch per layer.  Same bits either way (tests/test_mlp_gpu.py).  The layers are
-        #: latency-bound rather than HBM-bound, and the chain adds a dependency per layer; its speed on the H100 is
-        #: not measured.  PVN3D_MLP_CHAIN=1 selects it.
-        if chain is None:
-            chain = os.environ.get("PVN3D_MLP_CHAIN", "0") == "1"
-        self.chain = bool(chain)
         model = model.to(self.dev).eval()
         self.sa: List[List[List[PackedLayer]]] = []
         self.sa_out: List[int] = []
@@ -351,10 +302,10 @@ class FusedPointnet2MSG:
             self.fp.append(layers)
         #: store the level tables of SA1-3 TF32-rounded so that the next level gathers them with cp.async
         #: (identical features: every reader of those tables rounds on staging; PVN3D_MLP_ROUND_TABLES=0 disables)
-        self.round_tables = (not self.chain) and os.environ.get("PVN3D_MLP_ROUND_TABLES", "1") != "0"
+        self.round_tables = os.environ.get("PVN3D_MLP_ROUND_TABLES", "1") != "0"
         #: evaluate the first layer of every SA scale once per POINT instead of once per (centre, neighbour) pair
         #: (it is linear before its ReLU; DESIGN.md section 4).  PVN3D_MLP_FACTOR=0 keeps the gather-first layers.
-        self.factor = (not self.chain) and os.environ.get("PVN3D_MLP_FACTOR", "1") != "0"
+        self.factor = os.environ.get("PVN3D_MLP_FACTOR", "1") != "0"
         self.sa_fact = []
         for li, sa in enumerate(model.SA_modules):
             per_scale = []
@@ -381,8 +332,6 @@ class FusedPointnet2MSG:
             if i == 0:     # the skip of FP1 is the raw cloud (ld 9): read it through the level-0 factor table [f | hi x | lo x]
                 ws = torch.cat([ws, torch.zeros((w.size(0), 6), dtype=ws.dtype, device=ws.device)], dim=1)
             self.fp_fact.append((lk, PackedLayer(ws.contiguous(), bias), c2))
-        self.sa_chain = [[LayerChain(layers) for layers in scales] for scales in self.sa] if self.chain else None
-        self.fp_chain = [LayerChain(layers) for layers in self.fp] if self.chain else None
         self._marks = None
 
     def _m(self, family: str) -> None:
@@ -520,11 +469,6 @@ class FusedPointnet2MSG:
                                   round_out=self.round_tables and li < 3)
                     col += layers[-1].n
                     continue
-                if self.chain:
-                    mlp_sa_chain(x, new_xyz, fptr, ldf, c_feat, idx, self.sa_chain[li][si], pool=ns,
-                                 out=out_l.view(b * npoint, -1), col0=col, reserve=rs)
-                    col += layers[-1].n
-                    continue
                 # intermediates are stored TF32-rounded (what the next layer's operand is anyway); so are the
                 # level tables of SA1-3, whose only readers round them anyway (SA gather producers, FP skip
                 # columns): their rows then go global -> shared by cp.async (SA4's table feeds the fp32
@@ -565,8 +509,6 @@ class FusedPointnet2MSG:
                 if cn:
                     self._m("mlp")
                     return h
-            elif self.chain:
-                h = mlp_fp_chain(known_feat, nn_idx, nn_w, sptr, lds, c1, self.fp_chain[i], reserve=rs)
             else:
                 h = mlp_fp_first(known_feat, nn_idx, nn_w, sptr, lds, c1, layers[0], round_out=True, reserve=rs)
                 for li2, lyr in enumerate(layers[1:]):

@@ -168,93 +168,16 @@ def test_fused_pointnet2msg_matches_reference_features(cuda_dev, golden_dir):
     assert err.mean() <= 3e-3 * scale and err.max() <= 5e-2 * scale
 
 
-# --------------------------------------------------------------------------------------------------
-# chained SharedMLP kernel (one launch per SA scale / FP module, inter-layer tiles through L2)
-# --------------------------------------------------------------------------------------------------
-def _sa_case(cuda_dev, b, n, m, ns, c_feat, widths, seed):
-    rng = np.random.default_rng(seed)
-    xyz = torch.from_numpy(rng.uniform(0, 1, (b, n, 3)).astype(np.float32)).to(cuda_dev)
-    new_xyz = xyz[:, :m].contiguous()
-    idx = torch.from_numpy(rng.integers(0, n, (b, m, ns)).astype(np.int32)).to(cuda_dev)
-    feat = torch.from_numpy(rng.normal(size=(b, n, max(c_feat, 4))).astype(np.float32)).to(cuda_dev)
-    g = torch.Generator().manual_seed(seed)
-    layers, prev, k = [], None, c_feat + 3
-    for w_out in widths:
-        w = torch.randn(w_out, k, generator=g) / np.sqrt(k)
-        bias = torch.randn(w_out, generator=g) * 0.1
-        pl = mlp.PackedLayer(w.to(cuda_dev), bias.to(cuda_dev), prev)
-        prev, k = pl.n_pad, w_out
-        layers.append(pl)
-    return xyz, new_xyz, idx, feat, layers
-
-
-@pytest.mark.parametrize("b,n,m,ns,c_feat,widths", [
-    (2, 4096, 1024, 16, 6, (16, 16, 32)),       # SA1 scale 0: every layer is ONE K chunk (producer groups alternate items)
-    (2, 4096, 1024, 32, 6, (32, 32, 64)),       # SA1 scale 1
-    (3, 2048, 777, 16, 96, (64, 64, 128)),      # ragged row count, odd number of row tiles
-    (2, 1024, 512, 32, 96, (64, 96, 128)),      # n_pad 96: K of the last layer not a multiple of its input tile
-    (2, 1024, 300, 16, 256, (128, 196, 256)),   # 196 -> n_pad 208, k_pad 224
-    (2, 512, 128, 32, 512, (256, 384, 512)),    # two column blocks in the last layer, few row tiles per CTA
-    (1, 512, 40, 8, 64, (32, 48)),              # two layers, pool 8, fewer row tiles than CTAs
-    (32, 2048, 1024, 32, 6, (32, 32, 64)),      # many row-tile pairs per CTA: ring, accumulators and slots wrap
-])
-def test_sa_chain_equals_per_layer_launches(cuda_dev, b, n, m, ns, c_feat, widths):
-    """pvn3d_mlp_sa_chain == pvn3d_mlp_sa_first -> pvn3d_mlp_dense -> pvn3d_mlp_dense(pool), bit for bit
-    (same operands, same MMA order per output element)"""
-    xyz, new_xyz, idx, feat, layers = _sa_case(cuda_dev, b, n, m, ns, c_feat, widths, seed=b + m + ns)
-    fptr, ldf = feat.data_ptr(), feat.size(-1)
-    h = mlp.mlp_sa_first(xyz, new_xyz, fptr, ldf, c_feat, idx, layers[0], round_out=True)
-    for mid in layers[1:-1]:
-        h = mlp.mlp_dense(h, mid, round_out=True, a_tf32=True)
-    want = mlp.mlp_dense(h, layers[-1], pool=ns, a_tf32=True)
-    chain = mlp.LayerChain(layers)
-    got = mlp.mlp_sa_chain(xyz, new_xyz, fptr, ldf, c_feat, idx, chain, pool=ns)
-    assert got.shape == want.shape == (b * m, layers[-1].n_pad)
-    assert torch.equal(got, want), float((got - want).abs().max())
-    # un-pooled rows (EPI_STORE as the final epilogue)
-    want_rows = mlp.mlp_dense(h, layers[-1], a_tf32=True)
-    got_rows = mlp.mlp_sa_chain(xyz, new_xyz, fptr, ldf, c_feat, idx, chain, pool=0)
-    assert torch.equal(got_rows, want_rows)
-
-
-@pytest.mark.parametrize("b,n_u,m_k,c2,c1,widths", [(2, 512, 128, 1024, 512, (512, 512)), (2, 4096, 1024, 256, 6, (128, 128)),
-                                                   (3, 1000, 333, 512, 96, (256, 256)), (1, 100, 20, 64, 0, (32, 16))])
-def test_fp_chain_equals_per_layer_launches(cuda_dev, b, n_u, m_k, c2, c1, widths):
-    rng = np.random.default_rng(n_u)
-    unk = rng.uniform(0, 1, (b, n_u, 3)).astype(np.float32)
-    kn = rng.uniform(0, 1, (b, m_k, 3)).astype(np.float32)
-    d2, nn = pn2.three_nn(unk, kn)
-    kf = torch.from_numpy(rng.normal(size=(b, m_k, c2)).astype(np.float32)).to(cuda_dev)
-    sk = torch.from_numpy(rng.normal(size=(b, n_u, max(c1, 4))).astype(np.float32)).to(cuda_dev)
-    nw = mlp.three_nn_weights(torch.from_numpy(d2).to(cuda_dev))
-    nn_d = torch.from_numpy(nn).to(cuda_dev)
-    g = torch.Generator().manual_seed(c2)
-    layers, prev, k = [], None, c2 + c1
-    for w_out in widths:
-        pl = mlp.PackedLayer((torch.randn(w_out, k, generator=g) / np.sqrt(k)).to(cuda_dev),
-                             (torch.randn(w_out, generator=g) * 0.1).to(cuda_dev), prev)
-        prev, k = pl.n_pad, w_out
-        layers.append(pl)
-    h = mlp.mlp_fp_first(kf, nn_d, nw, sk.data_ptr(), sk.size(-1), c1, layers[0], round_out=True)
-    want = mlp.mlp_dense(h, layers[1], a_tf32=True)
-    got = mlp.mlp_fp_chain(kf, nn_d, nw, sk.data_ptr(), sk.size(-1), c1, mlp.LayerChain(layers))
-    assert torch.equal(got, want), float((got - want).abs().max())
-
-
-def test_chain_engine_equals_layer_engine_and_is_deterministic(cuda_dev):
-    """whole hot path A: chained engine == per-layer engine bit for bit, and 200 repetitions of the
-    chained forward give identical bits (stress for the warp-specialised mbarrier pipeline)."""
+def test_fused_engine_is_deterministic(cuda_dev):
+    """whole hot path A on the default engine: 200 repetitions of one forward give identical bits (stress for the
+    warp-specialised mbarrier pipelines of the per-layer and fused SA kernels)."""
     from pvn3d_b200 import synth
 
     model = testing.seeded_pointnet2msg(0, 1)
     frames = synth.make_batch("ycb", 2, n_points=12288, config_id=13)
     x = torch.from_numpy(np.stack([f.cld_rgb_nrm for f in frames])).to(cuda_dev)
-    layer_eng = mlp.FusedPointnet2MSG(model, cuda_dev, chain=False)
-    layer_eng.factor = False          # the chained kernel runs the unfactored first layer: same operands, same bits
-    y_layer = layer_eng(x)
-    eng = mlp.FusedPointnet2MSG(model, cuda_dev, chain=True)
+    eng = mlp.FusedPointnet2MSG(model, cuda_dev)
     y0 = eng(x).clone()
-    assert torch.equal(y0, y_layer), float((y0 - y_layer).abs().max())
     for i in range(200):
         assert torch.equal(eng(x), y0), f"run {i} differs"
 
@@ -267,7 +190,7 @@ def test_rounded_level_tables_do_not_change_the_features(cuda_dev):
     model = testing.seeded_pointnet2msg(0, 1)
     frames = synth.make_batch("linemod", 2, n_points=12288, config_id=14)
     x = torch.from_numpy(np.stack([f.cld_rgb_nrm for f in frames])).to(cuda_dev)
-    eng = mlp.FusedPointnet2MSG(model, cuda_dev, chain=False)
+    eng = mlp.FusedPointnet2MSG(model, cuda_dev)
     assert eng.round_tables
     y_async = eng(x).clone()
     eng.round_tables = False
@@ -284,7 +207,7 @@ def test_factored_first_layer_matches_unfactored_engine(cuda_dev, golden_dir):
     z = np.load(os.path.join(golden_dir, "pn2msg_big.npz"))
     model = testing.seeded_pointnet2msg(0, 1)
     x = torch.from_numpy(z["cld_rgb_nrm"])[None].to(cuda_dev)
-    eng = mlp.FusedPointnet2MSG(model, cuda_dev, chain=False)
+    eng = mlp.FusedPointnet2MSG(model, cuda_dev)
     assert eng.factor
     y_fact = eng(x).clone()
     eng.factor = False

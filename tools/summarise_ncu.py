@@ -77,7 +77,7 @@ if __name__ == "__main__":
     tag = sys.argv[1] if len(sys.argv) > 1 else "r01"
     os.makedirs(OUT, exist_ok=True)
     launches(tag)
-    for name in ("qg", "ms", "mlp", "msdens", "mswit", "fps", "nn", "ball", "chain", "glue"):
+    for name in ("qg", "ms", "mlp", "msdens", "mswit", "fps", "nn", "ball", "glue"):
         gz = os.path.join(ROOT, "gpurun_out", f"prof_{name}_{tag}.ncu-rep.gz")
         if os.path.exists(gz) and not os.path.exists(gz[:-3]):
             subprocess.run(["gunzip", "-kf", gz])

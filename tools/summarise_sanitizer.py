@@ -15,8 +15,8 @@ for f in sorted(glob.glob(os.path.join(ROOT, "gpurun_out", f"sanitizer_*_{tag}.l
     rows.append((m.group(1), m.group(2), tests[-1] if tests else "?", summ[-1] if summ else "?"))
 out = [f"# compute-sanitizer, tag {tag} (`tools/sanitizer_r02.sh` on the GPU)", "",
        "Small-shape selections of the GPU parity tests (the tools slow kernels down 10-100x): MLP = per-layer kernel",
-       "(dense / SA-gather / FP-interp producers, store and max-pool epilogues, 1 and 2 CTAs per SM, TMA weights) and the",
-       "chained kernel; ms = mean-shift in all four modes (witness + fallback + cooperative sweep), cal_frame_poses_lm,",
+       "(dense / SA-gather / FP-interp producers, store and max-pool epilogues, 1 and 2 CTAs per SM, TMA weights);",
+       "ms = mean-shift in all four modes (witness + fallback + cooperative sweep), cal_frame_poses_lm,",
        "Kabsch, ADD/ADD-S, seg argmax; pn2 = three_nn, ball_query, FPS, gathers.", "",
        "| tool | suite | pytest | sanitizer summary |", "|---|---|---|---|"]
 for r in rows:
