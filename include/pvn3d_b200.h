@@ -385,6 +385,49 @@ int pvn3d_icp_fit(const void *models, int model, const float *scene, int n, cons
                   int max_iter, double tol, double *pose_out, double *dist_out, int *iter_out,
                   double *err_out, void *workspace, size_t workspace_bytes, pvn3d_stream_t stream);
 
+/* Flat-kernel mean shift: sklearn's MeanShift(bandwidth, bin_seeding=True).fit(X) with min_bin_freq=1
+ * and cluster_all=True, as pvn3d/eval_icp.py:56-64 (get_cld_bigest_clus) runs it on float64 points.
+ * One CTA per fit; at most PVN3D_FLAT_MS_MAX_PTS points per fit.
+ *   1. bin keys rint(x / bw) per coordinate (float64 division, round-half-even), bins in order of first
+ *      occurrence, seed = float32(key) * float32(bw) in float32; the points themselves when every point
+ *      has its own bin.
+ *   2. per seed: members d2 <= bw*bw, d2 = (dx*dx + dy*dy) + dz*dz without FMA; no member -> the seed
+ *      is dropped; mean = float64 sum of the members in ascending index order / count; stop when
+ *      sqrt((ddx*ddx + ddy*ddy) + ddz*ddz) <= 1e-3*bw or after max_iter completed iterations.
+ *   3. equal centres (==) collapse into the first seed's centre with the last seed's count.
+ *   4. order by (count, x, y, z) descending; 5. a kept centre removes every later one with
+ *      d2 <= bw*bw; 6. label = nearest kept centre by the same d2, the lower index on ties.
+ * Results are bit-identical run to run.  (sklearn itself sums the members in its neighbour search's
+ * order, so it agrees to rounding.) */
+#define PVN3D_FLAT_MS_MAX_PTS 4096
+/* Fit f clusters X [fit_off[f], fit_off[f+1]) (X [total,3] f64, fit_off [n_fits+1] i32, device).
+ *   max_fit_pts  an upper bound on every fit's point count (sizes shared memory): above
+ *                PVN3D_FLAT_MS_MAX_PTS the call returns PVN3D_ERR_UNSUPPORTED and launches nothing;
+ *                a fit larger than it is not clustered (labels -1, n_clusters -1).
+ * outputs, rows indexed like X: labels_out [total] i32; centres_out [total,3] f64 (fit f's K kept
+ *   centres at rows fit_off[f]..fit_off[f]+K-1, the rest untouched); counts_out [total] i32 (their
+ *   member counts; NULL to skip); per fit n_clusters_out [n_fits] i32 (K; 0 when no seed had a member,
+ *   labels then -1) and n_iter_out [n_fits] i32 (max completed iterations over the seeds).
+ * bandwidth > 0, max_iter >= 0. */
+int pvn3d_flat_ms_fit_batch(const double *X, const int *fit_off, int n_fits, int max_fit_pts,
+                            double bandwidth, int max_iter, int *labels_out, double *centres_out,
+                            int *counts_out, int *n_clusters_out, int *n_iter_out, pvn3d_stream_t stream);
+/* pvn3d_icp_refine_batch with eval_icp's pre-filter: each fit's scene set (the strided selection, after
+ * the skip rules) is clustered as above with cluster_bw / cluster_max_iter, and the fit uses only the
+ * points labelled 0, in ascending order.  cluster_pts_out [B,n_cls] i32: points the fit used (0 when
+ * skipped; a fit whose filter keeps nothing is skipped).  max_pts <= PVN3D_FLAT_MS_MAX_PTS.
+ * Workspace: pvn3d_icp_clustered_workspace_bytes(b, n, n_cls, max_pts) (0 when unsupported).  From byte
+ * pvn3d_icp_workspace_bytes(b, n, n_cls, max_pts) of it, int32 [B,N]: in row b, fit (b, c)'s
+ * cluster_pts_out[b,c] frame point indices (into pcld[b]) that the fit used, ascending, start at position
+ * (number of points of frame b with class id in 1..c-1). */
+size_t pvn3d_icp_clustered_workspace_bytes(int b, int n, int n_cls, int max_pts);
+int pvn3d_icp_refine_batch_clustered(const void *models, const float *pcld, const int *mask, int b, int n,
+                                     int n_cls, const float *init_poses, const uint8_t *present,
+                                     int max_pts, int min_pts, int max_iter, double tol, double cluster_bw,
+                                     int cluster_max_iter, double *poses_out, int *iters_out,
+                                     double *err_out, uint8_t *refined_out, int *cluster_pts_out,
+                                     void *workspace, size_t workspace_bytes, pvn3d_stream_t stream);
+
 /* ------------------------------------------------------------------------------------------
  * Callers either side of the path (SURVEY section 8 f4)
  * ---------------------------------------------------------------------------------------- */

@@ -20,7 +20,7 @@ CSRC = os.path.join(HERE, "csrc")
 OBJ = os.path.join(HERE, "_build")
 LIB = os.path.join(HERE, "libpvn3d_b200.so")
 SOURCES = ["runtime.cu", "fps.cu", "pn2_ops.cu", "query_group.cu", "meanshift.cu", "poses.cu", "mlp_tc.cu", "metrics.cu",
-           "icp.cu"]
+           "icp.cu", "flat_meanshift.cu"]
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a",

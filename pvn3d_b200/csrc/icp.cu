@@ -30,6 +30,7 @@
 #include <cmath>
 
 #include "common.cuh"
+#include "flat_meanshift.cuh"
 #include "kabsch.cuh"
 
 namespace pvn3d {
@@ -426,6 +427,10 @@ struct FitParams {
   double *dist_out;
   int *match;  // [fits][match_stride] sorted model positions of the current matches
   int match_stride;
+  // the clustered refiner (batched selection only): keep_cnt[f] is the number of points the flat
+  // mean-shift pre-filter kept, and `perm` holds their frame point indices, ascending, at the start of
+  // the fit's class run (cls_off) in place of the class's points
+  const int *keep_cnt;
   unsigned long long *tests_out;
 };
 
@@ -490,6 +495,9 @@ __device__ __forceinline__ void block_sum(double (&v)[K], double (*s_red)[9]) {
     }
 }
 
+// kKeep: the clustered refiner -- the fit takes the keep_cnt[f] kept points from the start of its run of
+// p.perm (scene_pt's stride is then the identity); the plain instantiation is the kernel without it
+template <bool kKeep>
 __global__ void __launch_bounds__(kFitThreads, 1) icp_fit_kernel(const FitParams p) {
   const ModelsView mv = models_view(p.models);
   const int f = blockIdx.x, t = threadIdx.x;
@@ -516,6 +524,10 @@ __global__ void __launch_bounds__(kFitThreads, 1) icp_fit_kernel(const FitParams
       skip = model < 0 || model >= mv.n_models;
     }
     skip = skip || cnt < 1 || mv.hdr[model].n_pts < 1;
+    if (kKeep && !skip) {
+      cnt = p.keep_cnt[f];
+      skip = cnt < 1;
+    }
     s_cnt = cnt;
     s_nsel = p.pcld ? min(cnt, p.max_pts) : cnt;
     s_start = start;
@@ -706,6 +718,47 @@ __global__ void __launch_bounds__(kFitThreads, 1) icp_fit_kernel(const FitParams
   }
 }
 
+// ------------------------------------------------------------------------------------------------
+// eval_icp's pre-filter: the biggest flat mean-shift cluster of each fit's strided selection
+// (flat_meanshift.cuh), one CTA per (frame, class), with the fit kernel's skip rules applied first
+// ------------------------------------------------------------------------------------------------
+__global__ void __launch_bounds__(kFlatMsThreads, 1)
+icp_cluster_kernel(const FitParams p, double bw, int max_iter, int *keep_out, int *keep_cnt_out) {
+  extern __shared__ __align__(16) unsigned char smem[];
+  const ModelsView mv = models_view(p.models);
+  const int f = blockIdx.x, t = threadIdx.x;
+  const int b = f / p.n_cls, c = f % p.n_cls;
+  const int *off = p.cls_off + static_cast<size_t>(b) * (p.n_cls + 1);
+  const int cnt = c > 0 ? off[c + 1] - off[c] : 0;
+  if (c == 0 || !p.present[f] || cnt < p.min_pts || c >= mv.n_models || cnt < 1 || mv.hdr[c].n_pts < 1) {
+    if (t == 0) keep_cnt_out[f] = 0;
+    return;
+  }
+  const int nstr = min(cnt, p.max_pts);
+  const FlatMsSmem s = flat_ms_smem(smem, p.max_pts);
+  for (int j = t; j < nstr; j += kFlatMsThreads) {  // icp_fit_kernel's scene_pt, promoted to float64
+    const int qpos = static_cast<int>(static_cast<long long>(j) * cnt / nstr);
+    const int i = p.perm[static_cast<size_t>(b) * p.n + off[c] + qpos];
+    const float *src = p.pcld + (static_cast<size_t>(b) * p.n + i) * 3;
+    s.x[j] = src[0];
+    s.y[j] = src[1];
+    s.z[j] = src[2];
+  }
+  __syncthreads();
+  int *keep = keep_out + static_cast<size_t>(b) * p.n + off[c];  // the class's run, in a copy of perm
+  FlatMsOut o{};
+  o.kept = keep;
+  o.n_kept = keep_cnt_out + f;
+  flat_ms_cta(s, nstr, bw, max_iter, o);
+  __syncthreads();
+  // selection positions -> point indices of the frame, as icp_fit_kernel reads them
+  const int nk = keep_cnt_out[f];
+  for (int k = t; k < nk; k += kFlatMsThreads) {
+    const int qpos = static_cast<int>(static_cast<long long>(keep[k]) * cnt / nstr);
+    keep[k] = p.perm[static_cast<size_t>(b) * p.n + off[c] + qpos];
+  }
+}
+
 struct IcpWsLayout {
   size_t stats, perm, cls_off, match, total;
 };
@@ -759,25 +812,33 @@ extern "C" size_t pvn3d_icp_workspace_bytes(int b, int n, int n_cls, int max_pts
   return icp_ws_layout(b, n, n_cls, max_pts).total;
 }
 
-extern "C" int pvn3d_icp_refine_batch(const void *models, const float *pcld, const int *mask, int b,
-                                      int n, int n_cls, const float *init_poses, const uint8_t *present,
-                                      int max_pts, int min_pts, int max_iter, double tol,
-                                      double *poses_out, int *iters_out, double *err_out,
-                                      uint8_t *refined_out, void *workspace, size_t workspace_bytes,
-                                      pvn3d_stream_t stream) {
+namespace pvn3d {
+namespace {
+
+// the batched refinement; cluster_bw > 0 runs the pre-filter first and fits only the kept points
+int refine_batch(const void *models, const float *pcld, const int *mask, int b, int n, int n_cls,
+                 const float *init_poses, const uint8_t *present, int max_pts, int min_pts, int max_iter,
+                 double tol, double cluster_bw, int cluster_max_iter, double *poses_out, int *iters_out,
+                 double *err_out, uint8_t *refined_out, int *cluster_pts_out, void *workspace,
+                 size_t workspace_bytes, cudaStream_t st) {
   if (!models_ok(models) || !pcld || !mask || !init_poses || !present || !poses_out || !iters_out ||
       !err_out || !refined_out || !workspace || b < 0 || n < 1 || n_cls < 2 || max_pts < 1 ||
       min_pts < 0 || max_iter < 1 || !(tol >= 0.0))
     return PVN3D_ERR_INVALID_ARG;
+  const bool clustered = cluster_pts_out != nullptr;
+  if (clustered && (!(cluster_bw > 0.0) || !(cluster_bw < INFINITY) || cluster_max_iter < 0))
+    return PVN3D_ERR_INVALID_ARG;
+  if (clustered && max_pts > kFlatMsMaxPts) return PVN3D_ERR_UNSUPPORTED;
   if (b == 0) return PVN3D_OK;
   if (n_cls > kMaxIcpCls) return PVN3D_ERR_UNSUPPORTED;
   if (static_cast<long long>(b) * n_cls * max_pts > 0x7fffffffll || static_cast<long long>(b) * n > 0x7fffffffll)
     return PVN3D_ERR_UNSUPPORTED;
   const IcpWsLayout L = icp_ws_layout(b, n, n_cls, max_pts);
-  if (workspace_bytes < L.total) return PVN3D_ERR_WORKSPACE;
+  const size_t keep_at = L.total;  // the clustered form's kept-point perm [B,N] follows the plain workspace
+  const size_t need = clustered ? keep_at + align_up(static_cast<size_t>(b) * n * 4, 256) : L.total;
+  if (workspace_bytes < need) return PVN3D_ERR_WORKSPACE;
   if (reinterpret_cast<uintptr_t>(workspace) & 255u) return PVN3D_ERR_INVALID_ARG;
   unsigned char *ws = static_cast<unsigned char *>(workspace);
-  cudaStream_t st = as_stream(stream);
   PVN3D_CUDA_TRY(cudaMemsetAsync(ws + L.stats, 0, 8, st), "icp stats reset");
   int *perm = reinterpret_cast<int *>(ws + L.perm), *cls_off = reinterpret_cast<int *>(ws + L.cls_off);
   int rc = class_compact_launch(mask, b, n, n_cls, perm, cls_off, nullptr, st);
@@ -802,8 +863,58 @@ extern "C" int pvn3d_icp_refine_batch(const void *models, const float *pcld, con
   p.match = reinterpret_cast<int *>(ws + L.match);
   p.match_stride = max_pts;
   p.tests_out = reinterpret_cast<unsigned long long *>(ws + L.stats);
-  icp_fit_kernel<<<b * n_cls, kFitThreads, 0, st>>>(p);
+  if (clustered) {
+    static PerDeviceOnce once;
+    PVN3D_ONCE_PER_DEVICE(once,
+                          cudaFuncSetAttribute(icp_cluster_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                               static_cast<int>(flat_ms_smem_bytes(kFlatMsMaxPts))),
+                          "icp_cluster_kernel smem");
+    int *keep = reinterpret_cast<int *>(ws + keep_at);
+    icp_cluster_kernel<<<b * n_cls, kFlatMsThreads, flat_ms_smem_bytes(max_pts), st>>>(
+        p, cluster_bw, cluster_max_iter, keep, cluster_pts_out);
+    rc = check_launch("icp_cluster_kernel");
+    if (rc != PVN3D_OK) return rc;
+    p.perm = keep;
+    p.keep_cnt = cluster_pts_out;
+  }
+  if (clustered)
+    icp_fit_kernel<true><<<b * n_cls, kFitThreads, 0, st>>>(p);
+  else
+    icp_fit_kernel<false><<<b * n_cls, kFitThreads, 0, st>>>(p);
   return check_launch("icp_fit_kernel");
+}
+
+}  // namespace
+}  // namespace pvn3d
+
+extern "C" int pvn3d_icp_refine_batch(const void *models, const float *pcld, const int *mask, int b,
+                                      int n, int n_cls, const float *init_poses, const uint8_t *present,
+                                      int max_pts, int min_pts, int max_iter, double tol,
+                                      double *poses_out, int *iters_out, double *err_out,
+                                      uint8_t *refined_out, void *workspace, size_t workspace_bytes,
+                                      pvn3d_stream_t stream) {
+  return refine_batch(models, pcld, mask, b, n, n_cls, init_poses, present, max_pts, min_pts, max_iter, tol, 0.0,
+                      0, poses_out, iters_out, err_out, refined_out, nullptr, workspace, workspace_bytes,
+                      as_stream(stream));
+}
+
+extern "C" size_t pvn3d_icp_clustered_workspace_bytes(int b, int n, int n_cls, int max_pts) {
+  if (max_pts > kFlatMsMaxPts) return 0;
+  const size_t plain = pvn3d_icp_workspace_bytes(b, n, n_cls, max_pts);
+  return plain ? plain + align_up(static_cast<size_t>(b) * n * 4, 256) : 0;
+}
+
+extern "C" int pvn3d_icp_refine_batch_clustered(const void *models, const float *pcld, const int *mask, int b,
+                                                int n, int n_cls, const float *init_poses, const uint8_t *present,
+                                                int max_pts, int min_pts, int max_iter, double tol,
+                                                double cluster_bw, int cluster_max_iter, double *poses_out,
+                                                int *iters_out, double *err_out, uint8_t *refined_out,
+                                                int *cluster_pts_out, void *workspace, size_t workspace_bytes,
+                                                pvn3d_stream_t stream) {
+  if (!cluster_pts_out) return PVN3D_ERR_INVALID_ARG;
+  return refine_batch(models, pcld, mask, b, n, n_cls, init_poses, present, max_pts, min_pts, max_iter, tol,
+                      cluster_bw, cluster_max_iter, poses_out, iters_out, err_out, refined_out, cluster_pts_out,
+                      workspace, workspace_bytes, as_stream(stream));
 }
 
 extern "C" int pvn3d_icp_fit(const void *models, int model, const float *scene, int n,
@@ -834,6 +945,6 @@ extern "C" int pvn3d_icp_fit(const void *models, int model, const float *scene, 
   p.match = reinterpret_cast<int *>(ws + L.match);
   p.match_stride = n;
   p.tests_out = reinterpret_cast<unsigned long long *>(ws + L.stats);
-  icp_fit_kernel<<<1, kFitThreads, 0, st>>>(p);
+  icp_fit_kernel<false><<<1, kFitThreads, 0, st>>>(p);
   return check_launch("icp_fit_kernel");
 }

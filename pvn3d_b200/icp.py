@@ -4,6 +4,8 @@ float64 by csrc/icp.cu.
     T, distances, i = my_icp(A, B, init_pose, max_iterations=500, tolerance=1e-9)   # drop-in, one object
     ref = IcpRefiner(models, n_cls, batch, n_pts, max_pts=..., min_pts=..., device="cuda")
     poses64, iters, err, refined = ref.refine(pcld, mask, poses, present)          # batched, sync-free
+    p3ds = get_cld_bigest_clus(p3ds, radius=0.06)    # eval_icp's biggest flat mean-shift cluster
+    ref = IcpRefiner(..., cluster_bandwidth=0.06)    # the same filter before every batched fit
 
 The batched form takes FramePoseSolver.solve()'s poses and present flags as they come out and runs
 one fit per (frame, class) on the current stream, as pvn3d/eval_icp.py:94-185 does per object.
@@ -106,10 +108,16 @@ class IcpRefiner:
     depth masks; a network cloud of 12288 points holds only about 1000-1300 points per YCB-sized
     object, so those values would skip every fit there: choose them for the cloud at hand.
     max_iter, tol  eval_icp's 500 and 1e-9 (my_icp's own defaults are 20 and 1e-3).
+    cluster_bandwidth  None (default): fit every selected point.  A bandwidth (eval_icp uses 0.06): first
+             keep only the biggest cluster of sklearn's flat MeanShift(bandwidth, bin_seeding=True,
+             max_iter=cluster_max_iter) of each fit's selection, as eval_icp's get_cld_bigest_clus does,
+             and fit those points; `cluster_pts` [B,n_cls] i32 then holds how many each fit used
+             (0 when skipped).  Needs max_pts <= 4096.
     """
 
     def __init__(self, models, n_cls: int, batch: int, n_pts: int, *, max_pts: int, min_pts: int,
-                 max_iter: int = 500, tol: float = 1e-9, device="cuda"):
+                 max_iter: int = 500, tol: float = 1e-9, cluster_bandwidth=None, cluster_max_iter: int = 300,
+                 device="cuda"):
         self.dev = _cuda_device(device, "IcpRefiner")
         self.n_cls, self.b, self.n = int(n_cls), int(batch), int(n_pts)
         self.max_pts, self.min_pts = int(max_pts), int(min_pts)
@@ -122,10 +130,21 @@ class IcpRefiner:
             raise ValueError(f"max_pts={max_pts} must be >= 1 and min_pts={min_pts} >= 0")
         if self.max_iter < 1 or not self.tol >= 0.0:
             raise ValueError(f"max_iter={max_iter} must be >= 1 and tol={tol} >= 0")
+        self.cluster_bw = None if cluster_bandwidth is None else float(cluster_bandwidth)
+        self.cluster_max_iter = int(cluster_max_iter)
+        if self.cluster_bw is not None:
+            if not 0.0 < self.cluster_bw < float("inf") or self.cluster_max_iter < 0:
+                raise ValueError(f"cluster_bandwidth={cluster_bandwidth} must be > 0 and finite, "
+                                 f"cluster_max_iter={cluster_max_iter} >= 0")
+            if self.max_pts > _lib.FLAT_MS_MAX_PTS:
+                raise ValueError(f"max_pts={max_pts}: the cluster filter takes at most {_lib.FLAT_MS_MAX_PTS} "
+                                 "points per fit")
         pts, off = model_table(models, self.n_cls)
         self.lib = _lib.load()
         self.models = IcpModels(pts, off, self.dev)
-        self.ws_bytes = int(self.lib.pvn3d_icp_workspace_bytes(self.b, self.n, self.n_cls, self.max_pts))
+        ws_query = (self.lib.pvn3d_icp_workspace_bytes if self.cluster_bw is None
+                    else self.lib.pvn3d_icp_clustered_workspace_bytes)
+        self.ws_bytes = int(ws_query(self.b, self.n, self.n_cls, self.max_pts))
         if self.ws_bytes == 0:
             raise ValueError("IcpRefiner: problem too large for 32-bit indexing")
         self._ws, self._ws_ptr = _aligned(self.ws_bytes, self.dev)
@@ -134,11 +153,24 @@ class IcpRefiner:
         self.iters = torch.empty(shape, dtype=torch.int32, device=self.dev)
         self.err = torch.empty(shape, dtype=torch.float64, device=self.dev)
         self.refined = torch.empty(shape, dtype=torch.uint8, device=self.dev)
+        #: points each fit of the last refine() used after the cluster filter (cluster_bandwidth set only)
+        self.cluster_pts = None if self.cluster_bw is None else torch.empty(shape, dtype=torch.int32, device=self.dev)
 
     def pair_tests(self) -> int:
         """diagnostics (synchronises): model points the last refine()'s searches tested"""
         off = self._ws_ptr - self._ws.data_ptr()
         return int(self._ws[off:off + 8].view(torch.int64).item())
+
+    def kept_points(self) -> torch.Tensor:
+        """cluster filter only: [B,N] int32 device view of the workspace.  After refine(), row b holds,
+        for each refined class c, the cluster_pts[b, c] frame point indices (into pcld[b]) that fit (b, c)
+        used, ascending, starting at position (number of points of frame b with class id in 1..c-1); the
+        rest is unspecified.  Valid until the next refine() on the same stream."""
+        if self.cluster_bw is None:
+            raise RuntimeError("IcpRefiner.kept_points: the refiner has no cluster filter")
+        off = self._ws_ptr - self._ws.data_ptr() + int(self.lib.pvn3d_icp_workspace_bytes(self.b, self.n, self.n_cls,
+                                                                                          self.max_pts))
+        return self._ws[off:off + 4 * self.b * self.n].view(torch.int32).view(self.b, self.n)
 
     def refine(self, pcld: torch.Tensor, mask: torch.Tensor, poses: torch.Tensor, present: torch.Tensor):
         """pcld [B,N,3] f32, mask [B,N] i32 (the solver's new_mask for YCB, the network mask for LineMOD),
@@ -155,12 +187,19 @@ class IcpRefiner:
         with torch.cuda.device(self.dev):
             cur = torch.cuda.current_stream(self.dev)
             cur.wait_event(self.models.ready)                 # the model build may have run on another stream
-            rc = self.lib.pvn3d_icp_refine_batch(
-                self.models.ptr, ptr(pcld), ptr(mask), b, self.n, self.n_cls, ptr(poses), ptr(present),
-                self.max_pts, self.min_pts, self.max_iter, self.tol, ptr(self.poses), ptr(self.iters),
-                ptr(self.err), ptr(self.refined), self._ws_ptr, self.ws_bytes,
-                cur.cuda_stream)
-        check(rc, "pvn3d_icp_refine_batch")
+            if self.cluster_bw is None:
+                rc = self.lib.pvn3d_icp_refine_batch(
+                    self.models.ptr, ptr(pcld), ptr(mask), b, self.n, self.n_cls, ptr(poses), ptr(present),
+                    self.max_pts, self.min_pts, self.max_iter, self.tol, ptr(self.poses), ptr(self.iters),
+                    ptr(self.err), ptr(self.refined), self._ws_ptr, self.ws_bytes,
+                    cur.cuda_stream)
+            else:
+                rc = self.lib.pvn3d_icp_refine_batch_clustered(
+                    self.models.ptr, ptr(pcld), ptr(mask), b, self.n, self.n_cls, ptr(poses), ptr(present),
+                    self.max_pts, self.min_pts, self.max_iter, self.tol, self.cluster_bw, self.cluster_max_iter,
+                    ptr(self.poses), ptr(self.iters), ptr(self.err), ptr(self.refined), ptr(self.cluster_pts),
+                    self._ws_ptr, self.ws_bytes, cur.cuda_stream)
+        check(rc, "pvn3d_icp_refine_batch" + ("" if self.cluster_bw is None else "_clustered"))
         return self.poses[:b], self.iters[:b], self.err[:b], self.refined[:b]
 
 
@@ -201,3 +240,18 @@ def my_icp(A, B, init_pose=None, max_iterations=20, tolerance=0.001, device="cud
     T = np.eye(4)
     T[:3] = pose.cpu().numpy()
     return T, dist.cpu().numpy(), int(it.cpu()[0])
+
+
+def get_cld_bigest_clus(p3ds, radius: float = 0.06, device="cuda"):
+    """pvn3d/eval_icp.py:56-64: p3ds[labels == 0] for the labels of sklearn's MeanShift(bandwidth=radius,
+    bin_seeding=True) -- the biggest flat mean-shift cluster -- in input order.  p3ds [n,3], n <= 4096, is
+    clustered as float64 on the GPU; the result keeps p3ds's type and dtype (an array or a tensor on its
+    own device), as the reference's indexing does.  CUDA only."""
+    from .meanshift import flat_mean_shift
+
+    a = p3ds.detach().cpu().numpy() if torch.is_tensor(p3ds) else np.asarray(p3ds)
+    _, labels, _ = flat_mean_shift(a, radius, device=device)
+    keep = np.where(labels == 0)[0]
+    if torch.is_tensor(p3ds):
+        return p3ds[torch.from_numpy(keep).to(p3ds.device), :]
+    return a[keep, :]

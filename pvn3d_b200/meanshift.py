@@ -115,3 +115,73 @@ class MeanShiftTorch:
         cap, nf = self._last_cap_nf
         o = off + int(_lib.load().pvn3d_meanshift_workspace_counts_offset(cap, nf, int(self.max_iter)))
         return ws[o:o + 4 * cap].view(torch.int32)
+
+
+# --------------------------------------------------------------------------------------------------
+# Flat-kernel mean shift (sklearn's MeanShift(bandwidth, bin_seeding=True)), csrc/flat_meanshift.cu
+# --------------------------------------------------------------------------------------------------
+def flat_mean_shift_batch(X: torch.Tensor, fit_off, bandwidth: float, max_iter: int = 300):
+    """Cluster every segment X[fit_off[f]:fit_off[f+1]] in one launch on the current stream.
+    X [total,3] float64 contiguous on a CUDA device; fit_off: the F+1 non-decreasing segment offsets on the
+    host (a sequence, array or CPU tensor), each segment at most _lib.FLAT_MS_MAX_PTS points -- checked
+    here, before anything is launched.  Returns device tensors (labels [total] i32, centres [total,3] f64,
+    counts [total] i32, n_clusters [F] i32, n_iter [F] i32): fit f's K = n_clusters[f] centres and their
+    member counts are rows fit_off[f] .. fit_off[f]+K-1 (the other rows are unspecified)."""
+    import numpy as np
+
+    if not (X.is_cuda and X.dtype == torch.float64 and X.is_contiguous() and X.dim() == 2 and X.size(1) == 3):
+        raise ValueError("flat_mean_shift_batch: X must be a contiguous [total,3] float64 CUDA tensor")
+    off = fit_off.numpy() if torch.is_tensor(fit_off) else np.asarray(fit_off)
+    if off.ndim != 1 or len(off) < 1 or not np.issubdtype(off.dtype, np.integer):
+        raise ValueError("flat_mean_shift_batch: fit_off must be F+1 integer offsets")
+    sizes = np.diff(off)
+    if off[0] < 0 or off[-1] > X.size(0) or (sizes < 0).any():
+        raise ValueError(f"flat_mean_shift_batch: fit_off must be non-decreasing within [0, {X.size(0)}]")
+    max_fit_pts = int(sizes.max()) if len(sizes) else 0
+    if max_fit_pts > _lib.FLAT_MS_MAX_PTS:
+        raise ValueError(f"flat_mean_shift_batch: a segment of {max_fit_pts} points, at most "
+                         f"{_lib.FLAT_MS_MAX_PTS} per fit")
+    if not float(bandwidth) > 0.0:
+        raise ValueError(f"bandwidth={bandwidth} must be > 0")
+    if int(max_iter) < 0:
+        raise ValueError(f"max_iter={max_iter} must be >= 0")
+    fit_off = torch.from_numpy(np.ascontiguousarray(off, dtype=np.int32)).to(X.device)
+    lib = _lib.load()
+    total, n_fits = X.size(0), fit_off.numel() - 1
+    labels = torch.empty((total,), dtype=torch.int32, device=X.device)
+    centres = torch.empty((total, 3), dtype=torch.float64, device=X.device)
+    counts = torch.empty((total,), dtype=torch.int32, device=X.device)
+    n_clusters = torch.empty((n_fits,), dtype=torch.int32, device=X.device)
+    n_iter = torch.empty((n_fits,), dtype=torch.int32, device=X.device)
+    with torch.cuda.device(X.device):
+        rc = lib.pvn3d_flat_ms_fit_batch(ptr(X), ptr(fit_off), n_fits, int(max_fit_pts), float(bandwidth),
+                                         int(max_iter), ptr(labels), ptr(centres), ptr(counts), ptr(n_clusters),
+                                         ptr(n_iter), torch.cuda.current_stream(X.device).cuda_stream)
+    check(rc, "pvn3d_flat_ms_fit_batch")
+    return labels, centres, counts, n_clusters, n_iter
+
+
+def flat_mean_shift(X, bandwidth: float, max_iter: int = 300, device="cuda"):
+    """sklearn.cluster.mean_shift(X, bandwidth=bandwidth, bin_seeding=True, max_iter=max_iter) on the GPU:
+    X [n,3] (array or tensor, used as float64, n <= _lib.FLAT_MS_MAX_PTS) -> (cluster_centers [K,3] f64,
+    labels [n] int64, n_iter) as NumPy arrays and an int.  The members of each seed are summed in index
+    order, so the result is bit-identical run to run and agrees with sklearn to rounding.  Raises
+    ValueError when no point lies within bandwidth of any seed (as sklearn does)."""
+    import numpy as np
+
+    a = X.detach().cpu().numpy() if torch.is_tensor(X) else np.asarray(X)
+    a = np.ascontiguousarray(a, dtype=np.float64)
+    if a.ndim != 2 or a.shape[1] != 3 or len(a) == 0:
+        raise ValueError(f"flat_mean_shift: expected non-empty [n,3] points, got shape {a.shape}")
+    dev = torch.device(device)
+    if dev.type != "cuda":
+        raise RuntimeError("flat_mean_shift: CUDA only -- no CPU fallback")
+    n = len(a)
+    if n > _lib.FLAT_MS_MAX_PTS:
+        raise ValueError(f"flat_mean_shift: {n} points, at most {_lib.FLAT_MS_MAX_PTS} per call")
+    d_x = torch.from_numpy(a).to(dev)
+    labels, centres, _, n_clusters, n_iter = flat_mean_shift_batch(d_x, [0, n], bandwidth, max_iter)
+    k = int(n_clusters.cpu()[0])
+    if k == 0:
+        raise ValueError(f"flat_mean_shift: no point within bandwidth={bandwidth} of any seed")
+    return centres[:k].cpu().numpy(), labels.cpu().numpy().astype(np.int64), int(n_iter.cpu()[0])

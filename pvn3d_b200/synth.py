@@ -217,12 +217,15 @@ def perturb_pose(R, t, angle_deg: float, offset: float, rng):
 
 def make_icp_batch(batch: int, n_obj: int, pts_per_obj: int, seed: int = 0, n_cls: int = fixtures.YCB_N_CLASSES,
                    model_pts: int = 3000, noise: float = 0.001, outlier_frac: float = 0.0, n_bg: int = 2000,
-                   angle_deg: float = 5.0, offset: float = 0.01) -> dict:
+                   angle_deg: float = 5.0, offset: float = 0.01, n_stray: int = 0) -> dict:
     """A batch for IcpRefiner: per-class box-like models (distinct extents, 3-12 cm), and per frame
     n_obj distinct classes, each seen as pts_per_obj points of its camera-facing faces under a random
     pose (z in 0.6-1.0 m) with N(0, noise) noise, `outlier_frac` of them replaced by uniform points in
     the object's bounding box, plus n_bg background-plane points (label 0) at z = 1.2 m; points are
-    shuffled.  Returns dict(models: list[n_cls] of [P,3] f32 (None for class 0), extents [n_cls,3],
+    shuffled.  n_stray > 0 adds, per object, that many points carrying the object's label in a blob
+    (N(0, 5 mm)) whose centre lies 0.2 m beyond the box's half-diagonal from the object's centre, in a
+    random direction -- a fragment of something else that the segmentation gave the object's label.
+    The RNG is drawn from for it only when n_stray > 0, so other batches do not change.  Returns dict(models: list[n_cls] of [P,3] f32 (None for class 0), extents [n_cls,3],
     pcld [B,N,3] f32, mask [B,N] i32, gt [B,n_cls,3,4] f64, init [B,n_cls,3,4] f32 (gt perturbed by
     angle_deg / offset; identity for absent classes), present [B,n_cls] u8)."""
     rng = np.random.default_rng(seed)
@@ -231,7 +234,7 @@ def make_icp_batch(batch: int, n_obj: int, pts_per_obj: int, seed: int = 0, n_cl
     for c in range(1, n_cls):
         extents[c] = np.sort(rng.uniform(0.03, 0.12, size=3))[::-1]
         models[c] = box_surface(extents[c], model_pts, rng)
-    n = n_obj * pts_per_obj + n_bg
+    n = n_obj * (pts_per_obj + n_stray) + n_bg
     pcld = np.zeros((batch, n, 3), np.float32)
     mask = np.zeros((batch, n), np.int32)
     gt = np.zeros((batch, n_cls, 3, 4))
@@ -253,8 +256,12 @@ def make_icp_batch(batch: int, n_obj: int, pts_per_obj: int, seed: int = 0, n_cl
             if n_out:
                 lo, hi = p.min(0), p.max(0)
                 p[rng.choice(pts_per_obj, size=n_out, replace=False)] = rng.uniform(lo, hi, size=(n_out, 3))
+            if n_stray > 0:
+                d = rng.normal(size=3)
+                ctr = t + d / np.linalg.norm(d) * (0.5 * np.linalg.norm(extents[c]) + 0.2)
+                p = np.concatenate([p, ctr + rng.normal(0.0, 0.005, size=(n_stray, 3))])
             pts.append(p)
-            lab.append(np.full(pts_per_obj, c, np.int32))
+            lab.append(np.full(len(p), c, np.int32))
             gt[b, c, :, :3], gt[b, c, :, 3] = R, t
             Ri, ti = perturb_pose(R, t, angle_deg, offset, rng)
             init[b, c, :, :3], init[b, c, :, 3] = Ri, ti
