@@ -148,12 +148,13 @@ int pvn3d_three_nn_interpolate(const float *unknown, const float *known, const f
  * max-pool over nsample of pointnet2_modules.py:64-67).  One call = one layer:
  *      out[p, col0 + 0:n_pad] = act( A[p, 0:k_pad] . W^T + bias ),   optionally max over `pool` rows
  *   w    [n_pad, k_pad] f32, BN folded into rows, values rounded to TF32, zero padded
- *        (k_pad multiple of 32, n_pad multiple of 16); bias [n_pad] (folded BN shift, 0 in the pad)
+ *        (k_pad multiple of 32, n_pad multiple of 16), 16-byte aligned (else PVN3D_ERR_INVALID_ARG: it is
+ *        read 16 bytes at a time); bias [n_pad] (folded BN shift, 0 in the pad)
  *   out  point-major rows of length ldo (ldo, col0 multiples of 4); pool in {0, 8, 16, 32}
  * Arithmetic: TF32 operands (round-to-nearest), fp32 accumulation.
  * flags: PVN3D_MLP_RELU       apply ReLU (flags = 1 / 0 is the plain relu switch)
  *        PVN3D_MLP_ROUND_OUT  store the activations (pooled or not) already rounded to TF32
- *        PVN3D_MLP_A_TF32     (mlp_dense) `a` / (mlp_sa_first) `feat_pm` was produced with ROUND_OUT and is
+ *        PVN3D_MLP_A_TF32     (mlp_dense) `a` was produced with ROUND_OUT and is
  *                             16-byte aligned with a leading dimension % 4 == 0: its rows are copied global ->
  *                             shared asynchronously, without the rounding pass (unrounded values would be
  *                             TRUNCATED by the tensor core)
@@ -183,14 +184,6 @@ int pvn3d_mlp_dense_frame_bias(const float *a, int lda, int a_cols, long long ro
  * Summation order is fixed (reproducible). */
 int pvn3d_mlp_dense_sum32(const float *a, int lda, int a_cols, long long rows, const float *w, const float *bias,
                           int k_pad, int n_pad, int flags, float *out, int ldo, int col0, pvn3d_stream_t stream);
-/* First layer of one SA scale with QueryAndGroup fused into the operand producer: row (b,j,s) =
- * [ feat_pm[b, idx[b,j,s], 0:c_feat] | xyz[b,idx] - new_xyz[b,j] | 0.. ]  -- NOTE the column order:
- * the reference concatenates xyz FIRST (pointnet2_utils.py:319-321); W must have its three xyz
- * columns moved behind the c_feat descriptor columns.  rows = B*M*S in idx order. */
-int pvn3d_mlp_sa_first(const float *xyz, const float *new_xyz, const float *feat_pm, int ldf,
-                       int c_feat, const int *idx, int b, int n, int m, int ns, const float *w,
-                       const float *bias, int k_pad, int n_pad, int flags, int pool, float *out,
-                       int ldo, int col0, pvn3d_stream_t stream);
 /* First layer of an FP module with three_interpolate + concat fused: row (b,j) =
  * [ sum_t nn_w[b,j,t] * known_feat_pm[b, nn_idx[b,j,t], 0:c2] | skip_pm[b, j, 0:c1] | 0.. ] */
 int pvn3d_mlp_fp_first(const float *known_feat_pm, int c2, const int *nn_idx, const float *nn_w,
@@ -210,8 +203,8 @@ typedef struct {
  * instead of one GEMM row per (centre, neighbour) pair: 5-16x fewer rows.  The second layer then takes
  * relu(U[idx] - V) as its operand (pvn3d_mlp_sa_fact).  The table carries x as hi + lo TF32 parts (columns
  * [c_feat, c_feat+3) and [c_feat+3, c_feat+6)), to be multiplied by [W1f | W1x | W1x]: the coordinate term is
- * evaluated to ~2^-21, MORE accurately than rounding the difference x_j - c_i to TF32 as the unfactored producer
- * (and cuDNN's TF32 path) does.
+ * evaluated to ~2^-21, MORE accurately than rounding the difference x_j - c_i to TF32 as cuDNN's TF32 path
+ * does.
  *   pvn3d_sa_factor_table: xyz [rows,3], feat_pm [rows, ldf] (c_feat columns) -> out [rows, k_pad] TF32-rounded
  *   pvn3d_sa_centre_term : centres [rows,3], wx [n_pad,3] (TF32-rounded), bias [n_pad] -> out [rows, n_pad]
  *   pvn3d_mlp_sa_fact    : u [B*n, ldu], v [B*m, ldu] (c_valid columns), idx [B,m,ns] -> layer (w, bias) as
@@ -241,7 +234,7 @@ int pvn3d_mlp_sa_fact2_supported(const pvn3d_mlp_layer_t *layer2, const pvn3d_ml
  * in shared memory.  Same arguments, same bit-identical result as the two launches above.
  * PVN3D_ERR_UNSUPPORTED (nothing launched) unless pvn3d_mlp_sa_fact2w_supported(layer2, layer3, ns) is 1: ns 16 or
  * 32, layer3->n_pad > 128, layer2->k_pad <= 256, layer3->k_pad within the 128-column blocks of layer 2, the A and H
- * tiles and three weight stages within a block's shared memory, and weight loads by TMA (not PVN3D_MLP_TMA=0).
+ * tiles and three weight stages within a block's shared memory.
  * The query is host-only and touches no device memory. */
 int pvn3d_mlp_sa_fact2w(const float *u, const float *v, int ldu, int c_valid, const int *idx, int b, int n, int m,
                         int ns, const pvn3d_mlp_layer_t *layer2, const pvn3d_mlp_layer_t *layer3, int flags, int pool,

@@ -67,7 +67,6 @@ _SIGNATURES = {
     "pvn3d_mlp_dense": (c_int, [_P, c_int, c_int, ctypes.c_longlong, _P, _P, c_int, c_int, c_int, c_int, _P, c_int, c_int, _P]),
     "pvn3d_mlp_dense_frame_bias": (c_int, [_P, c_int, c_int, ctypes.c_longlong, c_int, _P, _P, c_int, c_int, c_int, _P, c_int, c_int, _P]),
     "pvn3d_mlp_dense_sum32": (c_int, [_P, c_int, c_int, ctypes.c_longlong, _P, _P, c_int, c_int, c_int, _P, c_int, c_int, _P]),
-    "pvn3d_mlp_sa_first": (c_int, [_P, _P, _P, c_int, c_int, _P, c_int, c_int, c_int, c_int, _P, _P, c_int, c_int, c_int, c_int, _P, c_int, c_int, _P]),
     "pvn3d_mlp_fp_first": (c_int, [_P, c_int, _P, _P, _P, c_int, c_int, c_int, c_int, c_int, _P, _P, c_int, c_int, c_int, _P, c_int, c_int, _P]),
     "pvn3d_sa_factor_table": (c_int, [_P, _P, c_int, c_int, ctypes.c_longlong, c_int, _P, _P]),
     "pvn3d_sa_centre_term": (c_int, [_P, _P, _P, ctypes.c_longlong, c_int, _P, _P]),

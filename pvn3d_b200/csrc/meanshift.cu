@@ -1353,8 +1353,7 @@ int meanshift_launch(const float4 *pts, const int *fit_start, const int *fit_cou
     if ((rc = check_launch("ms_setup_kernel")) != PVN3D_OK) return rc;
     // upper bound on density tiles: every fit wastes < 1 tile
     const int tiles = ceil_div(cap, kMsThreads) + nf;
-    static const bool prune_env = [] { const char *e = getenv("PVN3D_MS_PRUNED_DENSITY"); return !(e && e[0] == '0'); }();
-    a.dens_pruned = (prune_env && !(flags & PVN3D_MS_BRUTE_DENSITY)) ? 1 : 0;
+    a.dens_pruned = (flags & PVN3D_MS_BRUTE_DENSITY) ? 0 : 1;
     a.bwf = bwf;
     if (a.dens_pruned) {
       static PerDeviceOnce once_pr;

@@ -11,11 +11,11 @@
 //
 // A-operand producers (warps 4-11, eight lanes per row of the 128-row tile):
 //   DENSE      rows of a point-major activation matrix [P, lda]
-//   SA_GATHER  row (b,j,s): [ feat_pm[b, idx[b,j,s], 0:C] | xyz[b,idx] - new_xyz[b,j] | 0 ... ]
-//              (QueryAndGroup.forward, pointnet2_utils.py:311-321, never materialised; the weight
-//              matrix has its xyz columns moved behind the feature columns to keep rows 16-B aligned)
+//   SA_FACT    row (b,i,s): relu(U[b, idx[b,i,s], :] - V[b, i, :]) -- the second layer of a factored SA scale
+//              (QueryAndGroup.forward, pointnet2_utils.py:311-321, and the first layer never materialised)
 //   FP_INTERP  row (b,j): [ sum_t w_t * known_feat_pm[b, idx_t, 0:C2] | skip[b, j, 0:C1] | 0 ... ]
 //              (three_interpolate + torch.cat of PointnetFPModule.forward, pointnet2_modules.py:188-199)
+//   FP_FACT    row (b,j): relu(sum_t w_t * P[b, idx_t, :] + S[b, j, :]) -- the second layer of a factored FP module
 // Operands are staged in shared memory in the canonical K-major SWIZZLE_128B layout (32 fp32 = 128 B
 // per row per stage; weights arrive by TMA, pre-rounded activations by cp.async).  Two MMA warpgroups
 // (warps 12-19) each issue wgmma m64nNk8 (N = 16, 32, 64 or 128 columns per tile) for one 64-row half
@@ -44,7 +44,7 @@ constexpr int kMlpThreads = (kMlpEpiWarps + kMlpProWarps + kMlpMmaWarps) * 32;
 constexpr int kMlpMaxStages = 6;
 constexpr int kMlpSmemMax = 227 * 1024;  // dynamic shared memory a block may opt into on sm_90
 
-enum : int { PRO_DENSE = 0, PRO_SA_GATHER = 1, PRO_FP_INTERP = 2, PRO_SA_FACT = 3, PRO_FP_FACT = 4 };
+enum : int { PRO_DENSE = 0, PRO_FP_INTERP = 2, PRO_SA_FACT = 3, PRO_FP_FACT = 4 };
 enum : int { EPI_STORE = 0, EPI_MAXPOOL = 1, EPI_SUMPOOL = 2, EPI_MAXPOOL_T = 3, EPI_STORE_T = 4 };
 
 struct MlpArgs {
@@ -66,8 +66,8 @@ struct MlpArgs {
   int lda;
   int a_cols;  // valid columns of a (multiple of 4); the rest of k_pad reads as zero
   int a_tf32;  // a is already TF32-rounded and 16-byte aligned: copied with cp.async, no registers
-  // SA_GATHER
-  const float *xyz, *new_xyz, *feat;
+  // SA_FACT: feat = U [B*n, ldf], new_xyz = V [B*m, ldf], c_feat valid columns
+  const float *new_xyz, *feat;
   const int *idx;
   int ldf, c_feat, n, m, ns;
   // FP_INTERP
@@ -246,8 +246,8 @@ __device__ __forceinline__ uint32_t sw128_off(int r, int c) {
 // loads are all in flight before the first store.
 struct RowState {
   unsigned live;        // bit j: row of pass j exists (p < rows)
-  const float *row[8];  // DENSE: a + p*lda;  SA: feature row of the grouped point
-  int qrow[8], crow[8];        // SA: row of the grouped point in xyz (b*n + idx), of its centre (b*m + j)
+  const float *row[8];  // DENSE: a + p*lda;  SA: U row of the grouped point (b*n + idx)
+  int crow[8];                 // SA: row of its centre in V (b*m + j)
   int g1[8], g2[8], g3[8];     // FP: rows of the three neighbours in known_feat (b*m_known + idx)
   float w1[8], w2[8], w3[8];   // FP: their weights
 };
@@ -256,7 +256,7 @@ struct RowState {
 template <int PRO>
 __device__ __forceinline__ void rows_setup(const MlpArgs &a, long long p_first, RowState &s) {
   s.live = 0u;
-  const unsigned per_b = (PRO == PRO_SA_GATHER || PRO == PRO_SA_FACT)
+  const unsigned per_b = PRO == PRO_SA_FACT
                              ? static_cast<unsigned>(a.m) * static_cast<unsigned>(a.ns)
                              : static_cast<unsigned>(a.n_unknown);
   unsigned b0 = 0, rem0 = 0;
@@ -282,11 +282,10 @@ __device__ __forceinline__ void rows_setup(const MlpArgs &a, long long p_first, 
     }
     if (PRO == PRO_DENSE) {
       s.row[j] = a.a + pc * a.lda;
-    } else if (PRO == PRO_SA_GATHER || PRO == PRO_SA_FACT) {
+    } else if (PRO == PRO_SA_FACT) {
       const int q = __ldg(a.idx + pc);
-      s.qrow[j] = static_cast<int>(b) * a.n + q;
       s.crow[j] = static_cast<int>(b) * a.m + static_cast<int>(rem / static_cast<unsigned>(a.ns));
-      s.row[j] = a.feat + static_cast<size_t>(s.qrow[j]) * a.ldf;  // never read when c_feat == 0
+      s.row[j] = a.feat + static_cast<size_t>(static_cast<int>(b) * a.n + q) * a.ldf;
     } else {
       const int base = static_cast<int>(b) * a.m_known;
       s.g1[j] = base + __ldg(a.nn_idx + pc * 3 + 0);
@@ -373,10 +372,8 @@ __device__ __forceinline__ void stage_a_chunk(const MlpArgs &a, const RowState &
     }
     return;
   }
-  if (PRO == PRO_DENSE || PRO == PRO_SA_GATHER) {
-    const int seg = PRO == PRO_DENSE ? a.a_cols : a.c_feat;        // vector-loadable prefix of the row
-    const int end = PRO == PRO_DENSE ? a.a_cols : a.c_feat + 3;    // logical row length
-    if (vec_ok && k + 4 <= seg) {
+  if (PRO == PRO_DENSE) {
+    if (vec_ok && k + 4 <= a.a_cols) {
       float4 v[8];
 #pragma unroll
       for (int j = 0; j < 8; ++j) v[j] = (s.live >> j) & 1u ? ldg128(s.row[j] + k) : zero;
@@ -384,7 +381,7 @@ __device__ __forceinline__ void stage_a_chunk(const MlpArgs &a, const RowState &
       for (int j = 0; j < 8; ++j) sts_tf32(sa + sw128_off(r_first + 4 * j, sub), v[j]);
       return;
     }
-    if (k >= end) {
+    if (k >= a.a_cols) {
 #pragma unroll
       for (int j = 0; j < 8; ++j) sts128(sa + sw128_off(r_first + 4 * j, sub), 0.f, 0.f, 0.f, 0.f);
       return;
@@ -449,15 +446,6 @@ __device__ __forceinline__ void stage_a_chunk(const MlpArgs &a, const RowState &
       if (PRO == PRO_DENSE) {
         const bool on = live && kk < a.a_cols;
         v = on ? __ldg(s.row[j] + (on ? kk : 0)) : 0.f;
-      } else if (PRO == PRO_SA_GATHER) {
-        const bool isf = live && kk < a.c_feat;
-        const int d = kk - a.c_feat;
-        const bool isx = live && d >= 0 && d <= 2;
-        const float f = isf ? __ldg(s.row[j] + (isf ? kk : 0)) : 0.f;
-        // grouped_xyz -= new_xyz (pointnet2_utils.py:314)
-        const float px = isx ? __ldg(a.xyz + static_cast<size_t>(s.qrow[j]) * 3 + (isx ? d : 0)) : 0.f;
-        const float pc = isx ? __ldg(a.new_xyz + static_cast<size_t>(s.crow[j]) * 3 + (isx ? d : 0)) : 0.f;
-        v = isf ? f : px - pc;
       } else {
         const bool isk = live && kk < a.c2;
         const int d = kk - a.c2;
@@ -648,15 +636,11 @@ __global__ void __launch_bounds__(kMlpThreads, 1) mlp_layer_kernel(const __grid_
     const int r_first = 32 * pw + rg;
     bool vec_ok = true;
     if (PRO == PRO_DENSE) vec_ok = (a.lda % 4 == 0) && ((reinterpret_cast<uintptr_t>(a.a) & 15u) == 0);
-    if (PRO == PRO_SA_GATHER)
-      vec_ok = a.c_feat > 0 && (a.ldf % 4 == 0) && ((reinterpret_cast<uintptr_t>(a.feat) & 15u) == 0);
     if (PRO == PRO_FP_INTERP)
       vec_ok = (a.c2 % 4 == 0) && ((reinterpret_cast<uintptr_t>(a.known_feat) & 15u) == 0);
-    // pre-rounded rows are copied global -> shared asynchronously: DENSE activations of a ROUND_OUT layer, and
-    // the descriptor columns of SA_GATHER rows when the level table was stored rounded (PVN3D_MLP_A_TF32);
-    // the xyz / padding chunk of a gathered row and everything else is staged through registers
-    const bool a_async = (PRO == PRO_DENSE || PRO == PRO_SA_GATHER) && a.a_tf32 && vec_ok;
-    const int async_cols = PRO == PRO_DENSE ? a.k_pad : (a.c_feat / 32) * 32;   // chunks [0, async_cols) are asynchronous
+    // pre-rounded rows are copied global -> shared asynchronously: DENSE activations of a ROUND_OUT layer
+    // (PVN3D_MLP_A_TF32); everything else is staged through registers
+    const bool a_async = PRO == PRO_DENSE && a.a_tf32 && vec_ok;
     int pend0 = 0, pend1 = 0, npend = 0;  // stages whose copies are committed but not yet published
     long long it_base = 0;  // number of K chunks staged before this tile (same in every role)
     for (long long tile = blockIdx.x; tile < total_tiles; tile += gridDim.x, it_base += kc_total) {
@@ -697,13 +681,12 @@ __global__ void __launch_bounds__(kMlpThreads, 1) mlp_layer_kernel(const __grid_
             cp_async16(sb + sw128_off(n, c), a.w + static_cast<size_t>(n0 + n) * a.k_pad + kc * 32 + c * 4);
           }
         }
-        if (a_async && kc * 32 < async_cols) {
+        if (a_async) {
           const int k = kc * 32 + 4 * sub;
-          const int valid = PRO == PRO_DENSE ? a.a_cols : a.c_feat;
 #pragma unroll
           for (int j = 0; j < 8; ++j)
-            cp_async16(sa + sw128_off(r_first + 4 * j, sub), rs.row[j] + (k < valid ? k : 0),
-                       (((rs.live >> j) & 1u) && k < valid) ? 16u : 0u);
+            cp_async16(sa + sw128_off(r_first + 4 * j, sub), rs.row[j] + (k < a.a_cols ? k : 0),
+                       (((rs.live >> j) & 1u) && k < a.a_cols) ? 16u : 0u);
           cp_async_commit();
           if (npend == 0) pend0 = s; else pend1 = s;
           ++npend;
@@ -979,10 +962,9 @@ EncodeTiledFn encode_tiled_fn() {
   return fn;
 }
 
-// tensor map of one weight matrix; false -> the kernel falls back to per-thread cp.async
+// tensor map of one weight matrix; false: the driver cannot encode it (mlp_layer_kernel then loads the weights with
+// per-thread cp.async -- the same bytes, 16-byte aligned as launch_mlp requires -- and pvn3d_mlp_sa_fact2w refuses)
 bool weight_tensor_map(CUtensorMap *map, const float *w, int k_pad, int n_pad, int bn) {
-  const char *env = getenv("PVN3D_MLP_TMA");
-  if (env && env[0] == '0') return false;
   EncodeTiledFn enc = encode_tiled_fn();
   if (!enc || (reinterpret_cast<uintptr_t>(w) & 15u)) return false;
   const cuuint64_t dims[2] = {static_cast<cuuint64_t>(k_pad), static_cast<cuuint64_t>(n_pad)};
@@ -997,7 +979,8 @@ bool weight_tensor_map(CUtensorMap *map, const float *w, int k_pad, int n_pad, i
 template <int PRO, int EPI>
 int launch_mlp(MlpArgs &a, cudaStream_t st) {
   if (a.rows <= 0) return PVN3D_OK;
-  if (a.k_pad <= 0 || a.k_pad % 32 || a.n_pad <= 0 || a.n_pad % 16) return PVN3D_ERR_INVALID_ARG;
+  if (a.k_pad <= 0 || a.k_pad % 32 || a.n_pad <= 0 || a.n_pad % 16 || (reinterpret_cast<uintptr_t>(a.w) & 15u))
+    return PVN3D_ERR_INVALID_ARG;   // the weights are read 16 bytes at a time, by TMA or cp.async
   a.bn = mma_n(a.n_pad);
   a.acc_ld = std::max(32, a.bn);
   const size_t stage_bytes = kMlpBM * 128 + align_up(static_cast<size_t>(a.bn) * 128, 1024);
@@ -1592,13 +1575,10 @@ __global__ void __launch_bounds__(kSa2wThreads, 1) mlp_sa_fact2w_kernel(const __
 
 // ring stages pvn3d_mlp_sa_fact2w runs a scale with; 0: the scale is not covered (nsample other than 16 / 32, a last
 // layer of at most 128 columns -- pvn3d_mlp_sa_fact2's -- more than 8 layer-2 K chunks, a layer-3 K beyond the
-// 128-column blocks of layer 2, A + H tiles + three weight
-// stages beyond the shared memory of a block, or weight streaming by TMA switched off with PVN3D_MLP_TMA=0)
+// 128-column blocks of layer 2, or A + H tiles + three weight stages beyond the shared memory of a block)
 int sa2w_stages(int k2_pad, int n2_pad, int k3_pad, int n3_pad, int ns) {
   // every H column layer 3 reads is written by a layer-2 block each tile: k3_pad within the 128-column blocks of layer 2
   if ((ns != 16 && ns != 32) || n3_pad <= 128 || k2_pad / 32 > kSa2wMaxKc2 || k3_pad > 128 * ceil_div(n2_pad, 128)) return 0;
-  if (const char *env = getenv("PVN3D_MLP_TMA"))
-    if (env[0] == '0') return 0;
   const uint32_t fixed = sa2w_smem(k2_pad, k3_pad, 0).bytes;
   if (fixed >= static_cast<uint32_t>(kMlpSmemMax)) return 0;
   const int stages = std::min<int>(kSa2wMaxStages, static_cast<int>((kMlpSmemMax - fixed) / kSa2wStageBytes));
@@ -1630,16 +1610,9 @@ int dispatch(MlpArgs &a, int pro, int pool, cudaStream_t st) {
   if (pool) {
     if (pool != 8 && pool != 16 && pool != 32) return PVN3D_ERR_UNSUPPORTED;
     a.pool = pool;
-    // 128-channel pooled layers: transposed read of the accumulator tile, register max instead of shuffles.
-    // PVN3D_MLP_POOLT=2 takes every pooled layer of 128k channels that way, PVN3D_MLP_POOLT=0 the shuffle epilogue
-    // everywhere.
-    static const int poolt_env = [] { const char *e = getenv("PVN3D_MLP_POOLT"); return e ? atoi(e) : 1; }();
-    const bool t128 = a.n_pad == 128;
-    const bool t256 = a.n_pad % 128 == 0 && (a.n_pad <= 256 || a.n_pad % 256 == 0);
-    if (pro == PRO_DENSE && ((poolt_env == 1 && t128) || (poolt_env == 2 && t256)))
-      return launch_mlp<PRO_DENSE, EPI_MAXPOOL_T>(a, st);
+    // 128-channel pooled layers: transposed read of the accumulator tile, register max instead of shuffles
+    if (pro == PRO_DENSE && a.n_pad == 128) return launch_mlp<PRO_DENSE, EPI_MAXPOOL_T>(a, st);
     if (pro == PRO_DENSE) return launch_mlp<PRO_DENSE, EPI_MAXPOOL>(a, st);
-    if (pro == PRO_SA_GATHER) return launch_mlp<PRO_SA_GATHER, EPI_MAXPOOL>(a, st);
     if (pro == PRO_SA_FACT) return launch_mlp<PRO_SA_FACT, EPI_MAXPOOL>(a, st);
     return PVN3D_ERR_INVALID_ARG;
   }
@@ -1647,7 +1620,6 @@ int dispatch(MlpArgs &a, int pro, int pool, cudaStream_t st) {
   if (pro == PRO_DENSE) return launch_mlp<PRO_DENSE, EPI_STORE>(a, st);
   if (pro == PRO_SA_FACT) return launch_mlp<PRO_SA_FACT, EPI_STORE>(a, st);
   if (pro == PRO_FP_FACT) return launch_mlp<PRO_FP_FACT, EPI_STORE>(a, st);
-  if (pro == PRO_SA_GATHER) return launch_mlp<PRO_SA_GATHER, EPI_STORE>(a, st);
   return launch_mlp<PRO_FP_INTERP, EPI_STORE>(a, st);
 }
 
@@ -1727,29 +1699,6 @@ extern "C" int pvn3d_mlp_dense(const float *a, int lda, int a_cols, long long ro
   m.a_tf32 = (flags & PVN3D_MLP_A_TF32) ? 1 : 0;
   m.reserve_sms = (flags >> 8) & 0xff;
   return dispatch(m, PRO_DENSE, pool, as_stream(stream));
-}
-
-extern "C" int pvn3d_mlp_sa_first(const float *xyz, const float *new_xyz, const float *feat_pm,
-                                  int ldf, int c_feat, const int *idx, int b, int n, int m, int ns,
-                                  const float *w, const float *bias, int k_pad, int n_pad, int flags,
-                                  int pool, float *out, int ldo, int col0, pvn3d_stream_t stream) {
-  if (!xyz || !new_xyz || !idx || !w || !bias || !out || b < 0 || n <= 0 || m < 0 || ns <= 0 ||
-      c_feat < 0 || (c_feat > 0 && (!feat_pm || ldf < c_feat)) || k_pad < c_feat + 3 || ldo % 4 ||
-      col0 % 4)
-    return PVN3D_ERR_INVALID_ARG;
-  if (pool && pool != ns) return PVN3D_ERR_INVALID_ARG;
-  if (static_cast<long long>(m) * ns > 0x3fffffffll || static_cast<long long>(b) * n > 0x7fffffffll ||
-      static_cast<long long>(b) * m > 0x7fffffffll)
-    return PVN3D_ERR_UNSUPPORTED;
-  MlpArgs a{};
-  a.w = w; a.bias = bias; a.rows = static_cast<long long>(b) * m * ns; a.k_pad = k_pad; a.n_pad = n_pad;
-  a.xyz = xyz; a.new_xyz = new_xyz; a.feat = feat_pm; a.ldf = ldf; a.c_feat = c_feat; a.idx = idx;
-  a.n = n; a.m = m; a.ns = ns;
-  a.out = out; a.ldo = ldo; a.col0 = col0;
-  a.relu = flags & PVN3D_MLP_RELU; a.round_out = (flags & PVN3D_MLP_ROUND_OUT) ? 1 : 0;
-  a.a_tf32 = (flags & PVN3D_MLP_A_TF32) ? 1 : 0;   // feat_pm rows are TF32-rounded: asynchronous copies
-  a.reserve_sms = (flags >> 8) & 0xff;
-  return dispatch(a, PRO_SA_GATHER, pool, as_stream(stream));
 }
 
 extern "C" int pvn3d_mlp_fp_first(const float *known_feat_pm, int c2, const int *nn_idx,

@@ -596,8 +596,7 @@ extern "C" int pvn3d_three_nn(const float *unknown, const float *known, int b, i
   if (b == 0 || n == 0) return PVN3D_OK;
   if (b > 65535) return PVN3D_ERR_UNSUPPORTED;
   dim3 grid(ceil_div(n, kNnThreads), b);
-  static const bool slab_env = [] { const char *e = getenv("PVN3D_NN_SLAB"); return !(e && e[0] == '0'); }();
-  if (slab_env && m >= 512 && m <= kNnSlabMaxM && n >= 2 * m) {
+  if (m >= 512 && m <= kNnSlabMaxM && n >= 2 * m) {
     // x-sorted copy of the known set (stream-ordered scratch), then the outward walk
     int m_pad = 1;
     while (m_pad < m) m_pad <<= 1;

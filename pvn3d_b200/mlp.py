@@ -17,18 +17,13 @@ matrix + bias, and runs `Pointnet2MSG.forward` (reference pvn3d/lib/pvn3d.py:126
                         second layer on relu(interpolated P + S) (pvn3d_mlp_fp_fact), stored channel-major
                         [B,128,N], the layout the reference returns (when N % 32 == 0; else a transpose follows)
 
-PVN3D_MLP_FACTOR=0 (or `factor = False`) runs the unfactored layers instead: the first SA layer with the
-grouping fused into the producer (pvn3d_mlp_sa_first) -> pvn3d_mlp_dense -> pvn3d_mlp_dense with the
-max-pool, and FP1 as FP2-4, followed by a [B,N,128] -> [B,128,N] transpose.
-
 The grouped tensors [B,3+C,M,S] and the interpolated tensors [B,C,n] are never materialised; no
 cuDNN / cuBLAS / ATen kernel runs in this path.
 """
 from __future__ import annotations
 
 import ctypes
-import os
-from typing import Dict, List, Tuple
+from typing import Callable, Dict, List, Tuple
 
 import torch
 
@@ -98,22 +93,6 @@ def mlp_dense(a2d: torch.Tensor, layer: PackedLayer, relu=True, pool=0, out=None
         rc = lib.pvn3d_mlp_dense(ptr(a2d), lda, lda, rows, ptr(layer.w), ptr(layer.bias), layer.k_pad, layer.n_pad,
                                  _flags(relu, round_out, a_tf32, reserve), pool, ptr(out), out.size(-1), col0, _stream(a2d.device))
     check(rc, "pvn3d_mlp_dense")
-    return out
-
-
-def mlp_sa_first(xyz, new_xyz, feat_pm, ldf, c_feat, idx, layer: PackedLayer, relu=True, pool=0, out=None, col0=0,
-                 round_out=False, reserve=0, feat_tf32=False):
-    lib = _lib.load()
-    b, n = xyz.shape[0], xyz.shape[1]
-    m, ns = idx.shape[1], idx.shape[2]
-    rows = b * m * ns
-    if out is None:
-        out = torch.empty((rows // pool if pool else rows, layer.n_pad), dtype=torch.float32, device=xyz.device)
-    with torch.cuda.device(xyz.device):
-        rc = lib.pvn3d_mlp_sa_first(ptr(xyz), ptr(new_xyz), feat_pm, ldf, c_feat, ptr(idx), b, n, m, ns, ptr(layer.w),
-                                    ptr(layer.bias), layer.k_pad, layer.n_pad, _flags(relu, round_out, feat_tf32, reserve), pool, ptr(out),
-                                    out.size(-1), col0, _stream(xyz.device))
-    check(rc, "pvn3d_mlp_sa_first")
     return out
 
 
@@ -273,65 +252,59 @@ class FusedPointnet2MSG:
     def __init__(self, model: torch.nn.Module, device="cuda"):
         self.dev = torch.device(device)
         model = model.to(self.dev).eval()
-        self.sa: List[List[List[PackedLayer]]] = []
+        # SA scales: the first layer is evaluated once per POINT instead of once per (centre, neighbour) pair (it is
+        # linear before its ReLU; DESIGN.md section 4), layers 2 and 3 + the max-pool run as one launch
+        #: per level, per scale: (first layer [W_f | W_x | W_x] with its bias moved into V, Wx [n_pad,3], b1 [n_pad])
+        self.sa_fact: List[List[Tuple[PackedLayer, torch.Tensor, torch.Tensor]]] = []
+        #: per level, per scale: (layer 2, layer 3, the kernel that runs both and the max-pool)
+        self.sa: List[List[Tuple[PackedLayer, PackedLayer, Callable]]] = []
         self.sa_out: List[int] = []
-        for li, sa in enumerate(model.SA_modules):
-            scales = []
-            for mlp in sa.mlps:
-                layers = []
-                prev_pad = None
-                for k, layer in enumerate(mlp):
-                    w, bias = fold_conv_bn(layer)
-                    if k == 0:   # reference column order is [xyz(3) | features]; the producer emits [features | xyz]
-                        w = torch.cat([w[:, 3:], w[:, :3]], dim=1)
-                    pl = PackedLayer(w, bias, prev_pad)
-                    prev_pad = pl.n_pad
-                    layers.append(pl)
-                scales.append(layers)
-            self.sa.append(scales)
-            self.sa_out.append(sum(s[-1].n for s in scales))
-            assert all(s[-1].n % 4 == 0 for s in scales)
-        self.fp: List[List[PackedLayer]] = []
-        for fp in model.FP_modules:
-            layers, prev_pad = [], None
-            for layer in fp.mlp:
-                w, bias = fold_conv_bn(layer)
-                pl = PackedLayer(w, bias, prev_pad)
-                prev_pad = pl.n_pad
-                layers.append(pl)
-            self.fp.append(layers)
-        #: store the level tables of SA1-3 TF32-rounded so that the next level gathers them with cp.async
-        #: (identical features: every reader of those tables rounds on staging; PVN3D_MLP_ROUND_TABLES=0 disables)
-        self.round_tables = os.environ.get("PVN3D_MLP_ROUND_TABLES", "1") != "0"
-        #: evaluate the first layer of every SA scale once per POINT instead of once per (centre, neighbour) pair
-        #: (it is linear before its ReLU; DESIGN.md section 4).  PVN3D_MLP_FACTOR=0 keeps the gather-first layers.
-        self.factor = os.environ.get("PVN3D_MLP_FACTOR", "1") != "0"
-        self.sa_fact = []
-        for li, sa in enumerate(model.SA_modules):
-            per_scale = []
-            for si, mlp in enumerate(sa.mlps):
+        for li, (sa, (_, _, nsamples, _)) in enumerate(zip(model.SA_modules, SA_SPEC)):
+            facts, scales = [], []
+            for si, (mlp, ns) in enumerate(zip(sa.mlps, nsamples)):
                 w, bias = fold_conv_bn(mlp[0])                    # reference column order [xyz(3) | features]
                 wf, wxyz = w[:, 3:], w[:, :3]
-                first = PackedLayer(torch.cat([wf, wxyz, wxyz], dim=1), torch.zeros_like(bias))   # [W_f | W_x | W_x], bias in V
+                first = PackedLayer(torch.cat([wf, wxyz, wxyz], dim=1), torch.zeros_like(bias))
                 n_pad = first.n_pad
                 wx = torch.zeros((n_pad, 3), dtype=torch.float32, device=self.dev)
                 wx[: w.size(0)] = tf32_round(wxyz.to(self.dev))
                 b1 = torch.zeros((n_pad,), dtype=torch.float32, device=self.dev)
                 b1[: w.size(0)] = bias.to(self.dev)
-                per_scale.append((first, wx.contiguous(), b1))
-            self.sa_fact.append(per_scale)
-        # factored FP first layers: W1 = [W_k (known columns) | W_s (skip columns)]
-        self.fp_fact = []
-        skip_c = [model.SA_modules[0].mlps[0][0].conv.weight.size(1) - 3] + self.sa_out[:3]     # skip widths of FP1..FP4
+                facts.append((first, wx.contiguous(), b1))
+                l2 = PackedLayer(*fold_conv_bn(mlp[1]), n_pad)
+                l3 = PackedLayer(*fold_conv_bn(mlp[2]), l2.n_pad)
+                if sa_fact2_fits(l2, l3, ns):
+                    fused = mlp_sa_fact2        # SA1 / SA2: weights resident, layer 2 stays on chip
+                elif sa_fact2w_fits(l2, l3, ns):
+                    fused = mlp_sa_fact2w       # SA3 / SA4: the same, weights streamed
+                else:
+                    raise ValueError(f"SA{li + 1} scale {si}: no fused kernel takes layers 2 and 3 "
+                                     f"({l2.n} -> {l3.n} channels) at nsample {ns}")
+                scales.append((l2, l3, fused))
+            self.sa_fact.append(facts)
+            self.sa.append(scales)
+            self.sa_out.append(sum(l3.n for _, l3, _ in scales))
+            assert all(l3.n % 4 == 0 for _, l3, _ in scales)
+        #: FP2-FP4 (keys 1-3): first layer with the interpolation fused into its producer, then the second layer
+        self.fp: Dict[int, List[PackedLayer]] = {}
         for i, fp in enumerate(model.FP_modules):
-            w, bias = fold_conv_bn(fp.mlp[0])
-            c1 = skip_c[i]
-            c2 = w.size(1) - c1
-            lk = PackedLayer(w[:, :c2].contiguous(), torch.zeros_like(bias))
-            ws = w[:, c2:]
-            if i == 0:     # the skip of FP1 is the raw cloud (ld 9): read it through the level-0 factor table [f | hi x | lo x]
-                ws = torch.cat([ws, torch.zeros((w.size(0), 6), dtype=ws.dtype, device=ws.device)], dim=1)
-            self.fp_fact.append((lk, PackedLayer(ws.contiguous(), bias), c2))
+            if i == 0:
+                continue
+            layers, prev_pad = [], None
+            for layer in fp.mlp:
+                pl = PackedLayer(*fold_conv_bn(layer), prev_pad)
+                prev_pad = pl.n_pad
+                layers.append(pl)
+            self.fp[i] = layers
+        #: FP1, factored: W1 = [W_k (known columns) | W_s (skip columns)] as (P layer W_k, S layer W_s + b1, layer 2).
+        #: The skip of FP1 is the raw cloud: W_s reads it through the level-0 factor table [f | hi x | lo x].
+        fp1 = model.FP_modules[0].mlp
+        w, bias = fold_conv_bn(fp1[0])
+        c2 = w.size(1) - (model.SA_modules[0].mlps[0][0].conv.weight.size(1) - 3)
+        lk = PackedLayer(w[:, :c2].contiguous(), torch.zeros_like(bias))
+        ws = torch.cat([w[:, c2:], torch.zeros((w.size(0), 6), dtype=w.dtype, device=w.device)], dim=1)
+        ls = PackedLayer(ws.contiguous(), bias)
+        self.fp1 = (lk, ls, PackedLayer(*fold_conv_bn(fp1[1]), lk.n_pad))
         self._marks = None
 
     def _m(self, family: str) -> None:
@@ -422,14 +395,11 @@ class FusedPointnet2MSG:
         b, n0, width = pointcloud.shape
         c0 = width - 3
         rs_all = int(reserve_sms)
-        rs = rs_all if reserve_levels > 0 else 0
         if not plan.ball:
             self.queries(plan)
         # level-0 descriptors are columns 3.. of the input rows themselves (point-major already)
-        # PVN3D_MLP_SA_WIDE=0: SA3 / SA4 scales as two launches (layer 2, then layer 3 + max-pool) -- for A/B runs
-        wide_on = os.environ.get("PVN3D_MLP_SA_WIDE", "1") != "0"
         feats: List[Tuple[int, int, int]] = [(pointcloud.data_ptr() + 12, width, c0)]   # (address, ld, channels)
-        keep = [pointcloud]
+        l_feat = [pointcloud]          # l_feat[i]: tensor owning level i's descriptors (point-major)
         l_xyz = plan.l_xyz
         table0 = None
         for li, (npoint, radii, nsamples, _) in enumerate(SA_SPEC):
@@ -437,90 +407,51 @@ class FusedPointnet2MSG:
             x, new_xyz = l_xyz[li], l_xyz[li + 1]
             fptr, ldf, c_feat = feats[-1]
             out_l = torch.empty((b, npoint, self.sa_out[li]), dtype=torch.float32, device=self.dev)
+            table = sa_factor_table(x, fptr, ldf, c_feat, self.sa_fact[li][0][0].k_pad)   # shared by both scales
+            if li == 0:
+                table0 = table                                                          # FP1's skip columns
             col = 0
-            table = None
-            if self.factor and len(self.sa[li][0]) >= 2:
-                table = sa_factor_table(x, fptr, ldf, c_feat, self.sa_fact[li][0][0].k_pad)   # shared by both scales
-                if li == 0:
-                    table0 = table
-            for si, (idx, ns, layers) in enumerate(zip(plan.ball[li], nsamples, self.sa[li])):
-                if table is not None:
-                    first, wx, b1 = self.sa_fact[li][si]
-                    u = mlp_dense(table, first, relu=False, a_tf32=True, reserve=rs)        # once per point
-                    v = sa_centre_term(new_xyz, wx, b1)                                     # once per centre
-                    last2 = len(layers) == 2
-                    fused = None
-                    if len(layers) == 3 and sa_fact2_fits(layers[1], layers[2], ns):
-                        fused = mlp_sa_fact2        # SA1 / SA2: layer 2 stays on chip (DESIGN.md section 4)
-                    elif len(layers) == 3 and wide_on and sa_fact2w_fits(layers[1], layers[2], ns):
-                        fused = mlp_sa_fact2w       # SA3 / SA4: the same, weights streamed
-                    if fused is not None:
-                        fused(u, v, idx, x.size(1), layers[1], layers[2], out=out_l.view(b * npoint, -1), col0=col,
-                              round_out=self.round_tables and li < 3, reserve=rs)
-                        col += layers[-1].n
-                        continue
-                    h = mlp_sa_fact(u, v, idx, x.size(1), layers[1], pool=ns if last2 else 0, round_out=not last2 or
-                                    (self.round_tables and li < 3), reserve=rs,
-                                    out=out_l.view(b * npoint, -1) if last2 else None, col0=col if last2 else 0)
-                    if not last2:
-                        for mid in layers[2:-1]:
-                            h = mlp_dense(h, mid, round_out=True, a_tf32=True, reserve=rs)
-                        mlp_dense(h, layers[-1], pool=ns, out=out_l.view(b * npoint, -1), col0=col, a_tf32=True, reserve=rs,
-                                  round_out=self.round_tables and li < 3)
-                    col += layers[-1].n
-                    continue
-                # intermediates are stored TF32-rounded (what the next layer's operand is anyway); so are the
-                # level tables of SA1-3, whose only readers round them anyway (SA gather producers, FP skip
-                # columns): their rows then go global -> shared by cp.async (SA4's table feeds the fp32
-                # interpolation of FP4 and stays unrounded)
-                h = mlp_sa_first(x, new_xyz, fptr, ldf, c_feat, idx, layers[0], round_out=True, reserve=rs,
-                                 feat_tf32=self.round_tables and li >= 1)
-                for mid in layers[1:-1]:
-                    h = mlp_dense(h, mid, round_out=True, a_tf32=True, reserve=rs)
-                mlp_dense(h, layers[-1], pool=ns, out=out_l.view(b * npoint, -1), col0=col, a_tf32=True, reserve=rs,
-                          round_out=self.round_tables and li < 3)
-                col += layers[-1].n
+            for idx, (first, wx, b1), (l2, l3, fused) in zip(plan.ball[li], self.sa_fact[li], self.sa[li]):
+                u = mlp_dense(table, first, relu=False, a_tf32=True, reserve=rs)        # once per point
+                v = sa_centre_term(new_xyz, wx, b1)                                     # once per centre
+                # the level tables of SA1-3 are stored TF32-rounded, as their readers (the next level's factor table,
+                # the skip columns of FP2-4) round them anyway; SA4's feeds the fp32 interpolation of FP4
+                fused(u, v, idx, x.size(1), l2, l3, out=out_l.view(b * npoint, -1), col0=col, round_out=li < 3,
+                      reserve=rs)
+                col += l3.n
             self._m("mlp")
             feats.append((out_l.data_ptr(), out_l.size(-1), out_l.size(-1)))
-            keep.append(out_l)
+            l_feat.append(out_l)
         # feature propagation, deepest first (pvn3d.py:149-152)
-        l_feat = list(keep)            # l_feat[i]: tensor owning level i's descriptors (point-major)
         rs = rs_all if reserve_levels >= 5 else 0
-        for i in range(3, -1, -1):
+        for i in range(3, 0, -1):
             unknown, known = l_xyz[i], l_xyz[i + 1]
             nn_idx, nn_w = plan.nn[i]
-            known_feat = l_feat[i + 1]
-            if known_feat.dim() == 2:
-                known_feat = known_feat.view(b, known.size(1), -1)
             sptr, lds, c1 = feats[i]
             layers = self.fp[i]
-            # FP factoring pays only where the known descriptors are much wider than the layer and the skip is narrow:
-            # FP1 (256 + 6 -> 128 at 12288 points): 382 vs 420 us; FP2-4 measured 10-40 % SLOWER (DESIGN.md section 9)
-            if self.factor and len(layers) == 2 and i == 0 and table0 is not None:
-                lk, ls, c2 = self.fp_fact[i]
-                kf2d = known_feat.reshape(-1, known_feat.size(-1))
-                assert kf2d.size(-1) == c2
-                pk = mlp_dense(kf2d, lk, relu=False, reserve=rs)                                   # once per known point
-                skip2d = table0 if i == 0 else keep[i].view(-1, keep[i].size(-1))
-                sk = mlp_dense(skip2d, ls, relu=False, reserve=rs, a_tf32=(i == 0) or self.round_tables)
-                # the module's output IS the network's: written channel-major ([B,128,N]) straight from the accumulator
-                cn = layers[1].n_pad in (128, 256) and layers[1].n == layers[1].n_pad and unknown.size(1) % 32 == 0
-                h = mlp_fp_fact(pk, sk, nn_idx, nn_w, known.size(1), layers[1], round_out=False, reserve=rs, out_cn=cn)
-                if cn:
-                    self._m("mlp")
-                    return h
-            else:
-                h = mlp_fp_first(known_feat, nn_idx, nn_w, sptr, lds, c1, layers[0], round_out=True, reserve=rs)
-                for li2, lyr in enumerate(layers[1:]):
-                    last = li2 == len(layers) - 2        # level tables stay full fp32
-                    h = mlp_dense(h, lyr, round_out=not last, a_tf32=True, reserve=rs)
+            h = mlp_fp_first(l_feat[i + 1], nn_idx, nn_w, sptr, lds, c1, layers[0], round_out=True, reserve=rs)
+            for li2, lyr in enumerate(layers[1:]):
+                last = li2 == len(layers) - 2        # level tables stay full fp32
+                h = mlp_dense(h, lyr, round_out=not last, a_tf32=True, reserve=rs)
             l_feat[i] = h.view(b, unknown.size(1), -1)
-            feats[i] = (h.data_ptr(), h.size(-1), h.size(-1))
             self._m("mlp")
-        out_pm = l_feat[0]
-        n_out = self.fp[0][-1].n
-        if out_pm.size(-1) != n_out:
-            out_pm = out_pm[..., :n_out].contiguous()
+        # FP1, factored -- it pays only where the known descriptors are much wider than the layer and the skip is
+        # narrow: 256 + 6 -> 128 at 12288 points, 382 vs 420 us; FP2-4 measured 10-40 % SLOWER (DESIGN.md section 9)
+        lk, ls, l2 = self.fp1
+        nn_idx, nn_w = plan.nn[0]
+        kf2d = l_feat[1].reshape(-1, l_feat[1].size(-1))
+        assert kf2d.size(-1) == lk.k
+        pk = mlp_dense(kf2d, lk, relu=False, reserve=rs)                                   # once per known point
+        sk = mlp_dense(table0, ls, relu=False, reserve=rs, a_tf32=True)
+        # the module's output IS the network's: written channel-major ([B,128,N]) straight from the accumulator
+        cn = l2.n_pad in (128, 256) and l2.n == l2.n_pad and n0 % 32 == 0
+        h = mlp_fp_fact(pk, sk, nn_idx, nn_w, l_xyz[1].size(1), l2, round_out=False, reserve=rs, out_cn=cn)
+        self._m("mlp")
+        if cn:
+            return h
+        out_pm = h.view(b, n0, -1)
+        if out_pm.size(-1) != l2.n:
+            out_pm = out_pm[..., :l2.n].contiguous()
         out = _ext.transpose_nc_to_cn(out_pm)
         self._m("glue")
         return out

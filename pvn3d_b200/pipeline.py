@@ -12,8 +12,6 @@ from __future__ import annotations
 
 from typing import Dict, Optional
 
-import os
-
 import numpy as np
 import torch
 
@@ -75,13 +73,12 @@ class FramePipeline:
         #: over by then and the later, larger half of the MLPs takes the whole machine.  (Round 2 first used 16-frame
         #: chunks under all layers: 2 x 2 ms of sampling -- hidden while the MLPs took 3.4 ms, the critical path once
         #: they took 2.8.)
-        fps_chunk = int(os.environ.get("PVN3D_LA_CHUNK", fps_chunk))
         # 32 x 12288: the MLPs (2.7 ms) outlast the sampling (2.1 ms) -> reserve under SA1-2 only (3.93 vs 4.38 ms per step
         # with all levels reserving).  Smaller batches / larger clouds: the sampling is the critical path and a sampling
         # kernel that finds every SM taken by a full-width layer waits for it -> reserve under every layer
         if reserve_levels is None:
             reserve_levels = 2 if (self.b >= 24 and self.n <= 16384) else 5
-        self.reserve_levels = int(os.environ.get("PVN3D_LA_LEVELS", reserve_levels))
+        self.reserve_levels = int(reserve_levels)
         self.fps_chunk = max(1, min(fps_chunk if fps_chunk > 0 else self.b, self.b))
         # high priority: a sampling CTA needs a whole SM (512 threads, ~56 K registers, 147 KB shared memory); when
         # an SM drains, it must win it before the thousands of small CTAs of hot path B refill it
@@ -148,7 +145,7 @@ class FramePipeline:
                     nplan.done = torch.cuda.Event()
                     nplan.done.record(g)
                 self._plan = nplan
-                reserve = int(os.environ.get("PVN3D_LA_RESERVE", min(self.fps_chunk, nc.size(0))))
+                reserve = min(self.fps_chunk, nc.size(0))
             self.features = self.fused.features(cld_rgb_nrm, plan, reserve_sms=reserve,
                                                 reserve_levels=self.reserve_levels)        # hot path A: [B,128,N]
         else:

@@ -154,8 +154,7 @@ def test_unmodified_reference_binds_to_the_drop_in(tmp_path):
 def test_mlp_packing_folds_batchnorm_and_rounds_to_tf32():
     """Host half of the tensor-core MLP path (pvn3d_b200/mlp.py): Conv2d(1x1)+BatchNorm2d(eval) folded into one
     matrix + bias reproduces the module (pytorch_utils.py:25-50), weights are TF32 values (10-bit mantissa, ties
-    away = cvt.rna) zero-padded to the kernel's k_pad % 32 / n_pad % 16 grid, and the first SA layer's xyz
-    columns are moved behind the descriptor columns (the order pvn3d_mlp_sa_first's producer emits)."""
+    away = cvt.rna) zero-padded to the kernel's k_pad % 32 / n_pad % 16 grid."""
     from pvn3d_b200 import mlp
     x = torch.tensor([1.0, 1.0 + 2 ** -11, 1.0 + 2 ** -10, -3.0000002, 65504.5, 0.0, 1e-30])
     r = mlp.tf32_round(x)
@@ -180,8 +179,6 @@ def test_mlp_packing_folds_batchnorm_and_rounds_to_tf32():
     nxt = mlp.PackedLayer(torch.randn(40, w.shape[0], generator=g), torch.zeros(40), pk.n_pad)
     assert nxt.k_pad >= pk.n_pad                               # consumes the padded activations of `pk`
 
-    eng_cols = torch.cat([w[:, 3:], w[:, :3]], dim=1)          # [xyz | feat] -> [feat | xyz]
-    assert torch.equal(eng_cols[:, -3:], w[:, :3]) and torch.equal(eng_cols[:, :-3], w[:, 3:])
     assert mlp.MLP_RELU == 1 and mlp.MLP_ROUND_OUT == 2 and mlp.MLP_A_TF32 == 4          # include/pvn3d_b200.h
     hdr = open(os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "include", "pvn3d_b200.h")).read()
     for name, val in (("PVN3D_MLP_RELU", 1), ("PVN3D_MLP_ROUND_OUT", 2), ("PVN3D_MLP_A_TF32", 4)):

@@ -94,28 +94,6 @@ def test_chained_layers_take_tf32_activations_asynchronously(cuda_dev, rows, k, 
     assert (out.cpu()[:, :n2] - want).abs().max() <= 2e-5 * max(1.0, want.abs().max())
 
 
-def test_sa_first_layer_fuses_query_and_group(cuda_dev):
-    rng = np.random.default_rng(1)
-    b_, n_, m_, c_, ns_ = 2, 1024, 128, 96, 16
-    xyz = rng.uniform(0, 1, (b_, n_, 3)).astype(np.float32)
-    fidx = pn2.furthest_point_sampling(xyz, m_)
-    new = np.take_along_axis(xyz, fidx[..., None].astype(np.int64).repeat(3, -1), 1)
-    feats = rng.normal(size=(b_, c_, n_)).astype(np.float32)
-    grouped, idx = pn2.query_and_group(xyz, new, feats, float(np.float32(0.15)), ns_)      # [B,3+C,M,S] oracle
-    w = torch.from_numpy((rng.normal(size=(64, 3 + c_)) / 10).astype(np.float32))
-    bias = torch.from_numpy(rng.normal(size=64).astype(np.float32))
-    X = torch.from_numpy(grouped).permute(0, 2, 3, 1).reshape(-1, 3 + c_)
-    want = ref_dense(mlp.tf32_round(X), mlp.tf32_round(w), bias, True, 0)
-    layer = mlp.PackedLayer(torch.cat([w[:, 3:], w[:, :3]], 1).to(cuda_dev), bias.to(cuda_dev))
-    feat_pm = torch.from_numpy(feats).permute(0, 2, 1).contiguous().to(cuda_dev)
-    args = (torch.from_numpy(xyz).to(cuda_dev), torch.from_numpy(new).to(cuda_dev), feat_pm.data_ptr(), c_, c_,
-            torch.from_numpy(idx).to(cuda_dev), layer)
-    out = mlp.mlp_sa_first(*args).cpu()
-    assert (out[:, :64] - want).abs().max() <= 2e-5 * want.abs().max()
-    pooled = mlp.mlp_sa_first(*args, pool=ns_).cpu()
-    assert (pooled[:, :64] - want.view(-1, ns_, 64).max(1).values).abs().max() <= 2e-5 * want.abs().max()
-
-
 def test_fp_first_layer_fuses_interpolation(cuda_dev):
     rng = np.random.default_rng(2)
     b_, n_u, m_k, c2, c1 = 2, 512, 128, 256, 96
@@ -180,47 +158,6 @@ def test_fused_engine_is_deterministic(cuda_dev):
     y0 = eng(x).clone()
     for i in range(200):
         assert torch.equal(eng(x), y0), f"run {i} differs"
-
-
-def test_rounded_level_tables_do_not_change_the_features(cuda_dev):
-    """SA1-3 level tables stored TF32-rounded (so that the next level gathers them with cp.async) vs stored in
-    fp32 and rounded while staging: identical features, bit for bit"""
-    from pvn3d_b200 import synth
-
-    model = testing.seeded_pointnet2msg(0, 1)
-    frames = synth.make_batch("linemod", 2, n_points=12288, config_id=14)
-    x = torch.from_numpy(np.stack([f.cld_rgb_nrm for f in frames])).to(cuda_dev)
-    eng = mlp.FusedPointnet2MSG(model, cuda_dev)
-    assert eng.round_tables
-    y_async = eng(x).clone()
-    eng.round_tables = False
-    y_sync = eng(x)
-    assert torch.equal(y_async, y_sync), float((y_async - y_sync).abs().max())
-
-
-def test_factored_first_layer_matches_unfactored_engine(cuda_dev, golden_dir):
-    """first SA layer evaluated once per point (U_j - V_i, coordinate term split hi + lo) vs once per grouped row with
-    the difference x_j - c_i rounded to TF32: same function, different rounding points -> TF32-class agreement; and the
-    factored engine is at least as close to the reference's fp32 features as the unfactored one"""
-    from pvn3d_b200 import synth
-
-    z = np.load(os.path.join(golden_dir, "pn2msg_big.npz"))
-    model = testing.seeded_pointnet2msg(0, 1)
-    x = torch.from_numpy(z["cld_rgb_nrm"])[None].to(cuda_dev)
-    eng = mlp.FusedPointnet2MSG(model, cuda_dev)
-    assert eng.factor
-    y_fact = eng(x).clone()
-    eng.factor = False
-    y_plain = eng(x)
-    scale = float(y_plain.abs().mean())
-    d = (y_fact - y_plain).abs()
-    assert float(d.mean()) <= 3e-3 * scale and float(d.max()) <= 5e-2 * scale, (float(d.mean()) / scale, float(d.max()) / scale)
-    cols = torch.from_numpy(z["cols"]).long().to(cuda_dev)
-    ref = torch.from_numpy(z["feats"]).to(cuda_dev)
-    e_fact = float((y_fact[0][:, cols] - ref).abs().mean())
-    e_plain = float((y_plain[0][:, cols] - ref).abs().mean())
-    print(f"mean |err| vs reference fp32 features: factored {e_fact / scale:.2e}, unfactored {e_plain / scale:.2e}")
-    assert e_fact <= 1.2 * e_plain + 1e-6
 
 
 @pytest.mark.parametrize("b,n,m,ns,c_feat,n1,n2", [(2, 1024, 300, 16, 96, 64, 96), (1, 512, 100, 32, 6, 32, 32),

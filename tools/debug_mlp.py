@@ -65,34 +65,10 @@ print("identity probe max err", (out - want).abs().max().item())
 if (out - want).abs().max().item() > 1e-3:
     print(out[:8, :8])
 
-# SA first layer vs composed ops
+# FP first layer
 from oracle import pn2
 rng = np.random.default_rng(1)
-b_, n_, m_, c_, ns_ = 2, 1024, 128, 96, 16
-xyz = rng.uniform(0, 1, (b_, n_, 3)).astype(np.float32)
-fidx = pn2.furthest_point_sampling(xyz, m_)
-new = np.take_along_axis(xyz, fidx[..., None].astype(np.int64).repeat(3, -1), 1)
-feats = rng.normal(size=(b_, c_, n_)).astype(np.float32)
-grouped, idx = pn2.query_and_group(xyz, new, feats, float(np.float32(0.15)), ns_)     # [B,3+C,M,S]
-w = (rng.normal(size=(64, 3 + c_)) / 10).astype(np.float32)
-bias = rng.normal(size=64).astype(np.float32)
-X = torch.from_numpy(grouped).permute(0, 2, 3, 1).reshape(-1, 3 + c_)                  # rows (b,j,s), cols [xyz|feat]
-want = ref_dense(mlp.tf32_round(X), mlp.tf32_round(torch.from_numpy(w)), torch.from_numpy(bias), True, 0).to(dev)
-wperm = torch.cat([torch.from_numpy(w)[:, 3:], torch.from_numpy(w)[:, :3]], 1)
-layer = mlp.PackedLayer(wperm.to(dev), torch.from_numpy(bias).to(dev))
-feat_pm = torch.from_numpy(feats).permute(0, 2, 1).contiguous().to(dev)
-out = mlp.mlp_sa_first(torch.from_numpy(xyz).to(dev), torch.from_numpy(new).to(dev), feat_pm.data_ptr(), c_, c_,
-                       torch.from_numpy(idx).to(dev), layer)
-torch.cuda.synchronize()
-check("sa_first C=96 ns=16", out[:, :64], want)
-want_p = want.view(-1, ns_, 64).max(1).values
-outp = mlp.mlp_sa_first(torch.from_numpy(xyz).to(dev), torch.from_numpy(new).to(dev), feat_pm.data_ptr(), c_, c_,
-                        torch.from_numpy(idx).to(dev), layer, pool=ns_)
-torch.cuda.synchronize()
-check("sa_first + pool16", outp[:, :64], want_p)
-
-# FP first layer
-n_u, m_k, c2, c1 = 512, 128, 256, 96
+b_, n_u, m_k, c2, c1 = 2, 512, 128, 256, 96
 unk = rng.uniform(0, 1, (b_, n_u, 3)).astype(np.float32)
 kn = rng.uniform(0, 1, (b_, m_k, 3)).astype(np.float32)
 d2, nn = pn2.three_nn(unk, kn)

@@ -1,5 +1,5 @@
-"""shared-MLP time of one 32-frame batch (FusedPointnet2MSG.features on a fixed geometry plan) under the
-environment's PVN3D_MLP_* settings: total ms per call, output checksum, per-launch durations (CUPTI)"""
+"""shared-MLP time of one 32-frame batch (FusedPointnet2MSG.features on a fixed geometry plan): total ms per call,
+output checksum, per-launch durations (CUPTI) -- run it on two trees to compare them"""
 import os, sys, hashlib
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import numpy as np, torch
@@ -22,8 +22,7 @@ for _ in range(n):
     out = eng.features(cloud, plan)
 e1.record()
 torch.cuda.synchronize()
-tag = " ".join(f"{k[10:]}={v}" for k, v in sorted(os.environ.items()) if k.startswith("PVN3D_MLP_"))
-print(f"[{tag or 'default'}] features: {e0.elapsed_time(e1) / n:.3f} ms  sha {hashlib.sha1(out.cpu().numpy().tobytes()).hexdigest()[:12]}")
+print(f"features: {e0.elapsed_time(e1) / n:.3f} ms  sha {hashlib.sha1(out.cpu().numpy().tobytes()).hexdigest()[:12]}")
 if os.environ.get("AB_LAUNCHES", "1") == "1":
     from torch.profiler import profile, ProfilerActivity
     with profile(activities=[ProfilerActivity.CUDA]) as prof:
