@@ -240,6 +240,21 @@ int pvn3d_mlp_sa_fact2w(const float *u, const float *v, int ldu, int c_valid, co
                         int ns, const pvn3d_mlp_layer_t *layer2, const pvn3d_mlp_layer_t *layer3, int flags, int pool,
                         float *out, int ldo, int col0, pvn3d_stream_t stream);
 int pvn3d_mlp_sa_fact2w_supported(const pvn3d_mlp_layer_t *layer2, const pvn3d_mlp_layer_t *layer3, int ns);
+/* Both layers of an FP module with a two-layer MLP (FP2-FP4), in one launch: the interpolated first-layer operand is
+ * produced once per pair of 128-column blocks instead of once per block, and the layer-1 activations stay in shared
+ * memory instead of going through HBM.  Same result, bit for bit, as
+ *   pvn3d_mlp_fp_first(.., layer1, PVN3D_MLP_RELU | PVN3D_MLP_ROUND_OUT) -> h [b*n_unknown, layer1->n_pad]
+ *   pvn3d_mlp_dense(h, .., layer2, PVN3D_MLP_RELU [| PVN3D_MLP_ROUND_OUT] | PVN3D_MLP_A_TF32) -> out
+ * Arguments as pvn3d_mlp_fp_first; out rows = b * n_unknown, columns col0 .. col0 + layer2->n_pad of rows ldo apart.
+ * Both layers apply ReLU; flags: PVN3D_MLP_ROUND_OUT (output) and PVN3D_MLP_RESERVE_SMS(n).  Weight pointers must be
+ * 16-byte aligned (else PVN3D_ERR_INVALID_ARG, before any CUDA call).
+ * PVN3D_ERR_UNSUPPORTED (nothing launched) unless pvn3d_mlp_fp2_supported(layer1, layer2) is 1: layer1->n_pad 256 or
+ * 512, layer2->k_pad == layer1->n_pad, layer2->n_pad a multiple of 128, and the layer-1 tile, four operand stages and
+ * three weight stages within a block's shared memory.  The query is host-only and touches no device memory. */
+int pvn3d_mlp_fp2(const float *known_feat_pm, int c2, const int *nn_idx, const float *nn_w, const float *skip_pm, int lds,
+                  int c1, int b, int n_unknown, int m_known, const pvn3d_mlp_layer_t *layer1, const pvn3d_mlp_layer_t *layer2,
+                  int flags, float *out, int ldo, int col0, pvn3d_stream_t stream);
+int pvn3d_mlp_fp2_supported(const pvn3d_mlp_layer_t *layer1, const pvn3d_mlp_layer_t *layer2);
 /* FACTORED first layer of an FP module: three_interpolate commutes with the (linear) first layer, so
  *   P = W1k . known      once per KNOWN point   (pvn3d_mlp_dense without ReLU on the known table),
  *   S = W1s . skip + b1  over the skip columns  (pvn3d_mlp_dense without ReLU on the skip table),

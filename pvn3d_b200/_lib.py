@@ -78,6 +78,8 @@ _SIGNATURES = {
     "pvn3d_mlp_sa_fact2w": (c_int, [_P, _P, c_int, c_int, _P, c_int, c_int, c_int, c_int, _P, _P, c_int, c_int, _P, c_int,
                                     c_int, _P]),
     "pvn3d_mlp_sa_fact2w_supported": (c_int, [_P, _P, c_int]),
+    "pvn3d_mlp_fp2": (c_int, [_P, c_int, _P, _P, _P, c_int, c_int, c_int, c_int, c_int, _P, _P, c_int, _P, c_int, c_int, _P]),
+    "pvn3d_mlp_fp2_supported": (c_int, [_P, _P]),
     "pvn3d_mlp_fp_fact": (c_int, [_P, _P, c_int, c_int, _P, _P, c_int, c_int, c_int, _P, _P, c_int, c_int, c_int, _P, c_int, c_int,
                                   _P]),
     "pvn3d_three_nn_weights": (c_int, [_P, ctypes.c_longlong, _P, _P]),

@@ -1367,7 +1367,8 @@ __device__ __forceinline__ int sa2w_pair_blocks(int nb, int pp) { return nb - pp
 // one with `keep_last`, which the caller releases (returned).  With `a_bars`, K chunk kc of the A tile is waited for
 // first (layer 2; parity `a_par`).
 __device__ __forceinline__ int sa2w_block(float (&d)[64], uint32_t a_tile, uint32_t ring, int S, int it0, int step, int kcs,
-                                          Sa2wSmemCtl &ctl, uint64_t *a_bars, unsigned a_par, bool keep_last, unsigned lane) {
+                                          uint64_t *full, uint64_t *empty, uint64_t *a_bars, unsigned a_par, bool keep_last,
+                                          unsigned lane) {
 #pragma unroll
   for (int i = 0; i < 64; ++i) d[i] = 0.f;
   int prev = -1;
@@ -1375,7 +1376,7 @@ __device__ __forceinline__ int sa2w_block(float (&d)[64], uint32_t a_tile, uint3
     const int it = it0 + kc * step;
     const int s = it % S;
     if (a_bars) mbar_wait(&a_bars[kc], a_par);
-    mbar_wait(&ctl.full[s], static_cast<unsigned>((it / S) & 1));
+    mbar_wait(&full[s], static_cast<unsigned>((it / S) & 1));
     fence_proxy_async_smem();
     const uint64_t adesc = smem_desc_sw128(a_tile + static_cast<uint32_t>(kc) * kSa2wChunk);
     const uint64_t bdesc = smem_desc_sw128(ring + static_cast<uint32_t>(s) * kSa2wStageBytes);
@@ -1386,13 +1387,13 @@ __device__ __forceinline__ int sa2w_block(float (&d)[64], uint32_t a_tile, uint3
     wgmma_commit();
     if (prev >= 0) {
       wgmma_wait<1>();
-      if (lane == 0) mbar_arrive(&ctl.empty[prev]);
+      if (lane == 0) mbar_arrive(&empty[prev]);
     }
     prev = s;
   }
   wgmma_wait<0>();
   acc_fence(d);
-  if (lane == 0 && !keep_last) mbar_arrive(&ctl.empty[prev]);
+  if (lane == 0 && !keep_last) mbar_arrive(&empty[prev]);
   return prev;
 }
 
@@ -1477,7 +1478,7 @@ __global__ void __launch_bounds__(kSa2wThreads, 1) mlp_sa_fact2w_kernel(const __
         const int cnt = sa2w_pair_blocks(nb2, pp);
         if (static_cast<int>(wg) < cnt) {
           const int nb = pp + static_cast<int>(wg);
-          sa2w_block(d, base + L.a, base + L.ring, S, it_base + static_cast<int>(wg), cnt, kc2, ctl, ctl.a_full,
+          sa2w_block(d, base + L.a, base + L.ring, S, it_base + static_cast<int>(wg), cnt, kc2, ctl.full, ctl.empty, ctl.a_full,
                      static_cast<unsigned>(j & 1), false, lane);
           // both warpgroups have finished the previous tile's layer 3 (its reads of H)
           if (!synced) named_bar_sync(1, 2 * 128);
@@ -1511,7 +1512,7 @@ __global__ void __launch_bounds__(kSa2wThreads, 1) mlp_sa_fact2w_kernel(const __
         const int cnt = sa2w_pair_blocks(nb3, pp);
         if (static_cast<int>(wg) < cnt) {
           const int nb = pp + static_cast<int>(wg);
-          const int last = sa2w_block(d, base + L.h, base + L.ring, S, it_base + static_cast<int>(wg), cnt, kc3, ctl, nullptr, 0u,
+          const int last = sa2w_block(d, base + L.h, base + L.ring, S, it_base + static_cast<int>(wg), cnt, kc3, ctl.full, ctl.empty, nullptr, 0u,
                                       true, lane);
           // max over the warp's 16 rows: the lane's two rows, then a transposing butterfly over lane bits 4, 3, 2
           // (lanes that differ there hold the same columns); p[2j + e] is column 8j + 2 (lane & 3) + e
@@ -1604,6 +1605,374 @@ int launch_sa_fact2w(Sa2wArgs &g, int stages, cudaStream_t st) {
   const unsigned grid = static_cast<unsigned>(std::min<long long>(tiles, sms));
   kern<<<grid, kSa2wThreads, smem, st>>>(g);
   return check_launch("mlp_sa_fact2w_kernel");
+}
+
+// =====================================================================================================
+// Both layers of an FP module whose first layer reads the interpolated known descriptors and the skip columns (FP2-FP4),
+// in ONE persistent kernel.
+//
+// As two launches (pvn3d_mlp_fp_first with ROUND_OUT, then pvn3d_mlp_dense) every interpolated operand element is
+// produced once per 128-column block of layer 1 (4 times for 512 columns), and the TF32-rounded layer-1 activations H
+// go to HBM and come back once per layer-2 column block (33-67 MB per module and 32-frame batch).  Per 64-row tile:
+//   producers (warps 0-3)   stage A = [tf32(sum_t w_t known[idx_t]) | tf32(skip) | 0] in 64 x 32 K chunks through a ring,
+//                           as the PRO_FP_INTERP producer of the per-layer kernel does (its per-row neighbour indices
+//                           and weights kept in shared memory, not 48 registers); each chunk is read by BOTH
+//                           warpgroups, so A is produced once per pair of layer-1 column blocks (once for 256 columns,
+//                           twice for 512), running ahead across passes and tiles;
+//   loader    (warp 12)     streams 32-column K chunks of W1 and W2 (128 output columns each) by TMA through a second
+//                           ring, in the order the warpgroups consume them;
+//   MMA       (warps 4-11)  both warpgroups work on the same 64 rows; warpgroup wg takes the column blocks nb % 2 == wg
+//                           of each layer.  Layer 1: wgmma N = 128 over the A chunks, then tf32(relu(acc + b1)) into
+//                           the block's columns of a K-major SWIZZLE_128B H tile; layer 2: the same from the H tile,
+//                           relu(acc + b2) [rounded with ROUND_OUT] stored point-major, 32-byte row segments per quad.
+// A thread never holds more than one 64 x 128 fragment.  Every output element keeps the per-layer kernels' operands,
+// wgmma N (128), K order and epilogue arithmetic, so the results are bit-identical to the two launches.
+constexpr int kFp2BM = 64;
+constexpr int kFp2ProWarps = 4;   // two pairs, a pair stages one 64-row A chunk (more warps: under 128 registers, spills)
+constexpr int kFp2Pairs = kFp2ProWarps / 2;
+constexpr int kFp2LoaderWarp = kFp2ProWarps + kMlpMmaWarps;      // warp 12
+constexpr int kFp2Threads = (kFp2LoaderWarp + 1) * 32;
+constexpr int kFp2MaxStages = 8;
+constexpr uint32_t kFp2AStageBytes = kFp2BM * 128u;              // one A chunk, and one K chunk of the H tile: 64 rows x 32 tf32
+constexpr uint32_t kFp2WStageBytes = 128u * 128u;                // one weight chunk: 128 output columns x 32 tf32
+
+struct Fp2Args {
+  MlpArgs a;            // PRO_FP_INTERP producer fields, rows, out / ldo / col0 / round_out; tmap, w, bias, k_pad, n_pad: layer 1
+  alignas(64) CUtensorMap tmap2;
+  const float *w2, *bias2;
+  int k2_pad, n2_pad;   // k2_pad == n_pad of layer 1
+  int a_stages, w_stages;
+};
+
+struct Fp2SmemCtl {
+  uint64_t a_full[kFp2MaxStages];   // 64 arrivals: the producer threads of the pair that staged the chunk
+  uint64_t a_empty[kFp2MaxStages];  // 8 arrivals: every MMA warp, once its MMAs that read the chunk have retired
+  uint64_t w_full[kFp2MaxStages];   // the loader's arrive.expect_tx + the TMA bytes of the weight chunk
+  uint64_t w_empty[kFp2MaxStages];  // 4 arrivals: the warps of the warpgroup that consumed the chunk
+};
+
+// shared-memory layout behind the 1024-byte aligned base (kernel, launcher and pvn3d_mlp_fp2_supported use the same
+// function): [H: k2_pad/32 chunks of 64 x 128 B][A ring: a_stages x 8 KB][weight ring: w_stages x 16 KB]
+// [row states: 32 B per row of each producer warp][barriers]
+struct Fp2Smem {
+  uint32_t h, aring, wring, rows, ctl, bytes;   // offsets from the aligned base; bytes = dynamic size incl. alignment slack
+};
+static inline __host__ __device__ Fp2Smem fp2_smem(int k2_pad, int a_stages, int w_stages) {
+  Fp2Smem s;
+  s.h = 0;
+  s.aring = s.h + static_cast<uint32_t>(k2_pad / 32) * kFp2AStageBytes;
+  s.wring = s.aring + static_cast<uint32_t>(a_stages) * kFp2AStageBytes;
+  s.rows = s.wring + static_cast<uint32_t>(w_stages) * kFp2WStageBytes;
+  s.ctl = s.rows + kFp2ProWarps * 32u * 32u;
+  s.bytes = 1024u + s.ctl + static_cast<uint32_t>(sizeof(Fp2SmemCtl));
+  return s;
+}
+
+// Row state of a producer thread's 8 rows (rows_setup<PRO_FP_INTERP>) in shared memory instead of 48 registers, 32 B
+// per row: {g1, g2, g3, -} {w1, w2, w3, live}.  Row j of the thread is at `rst` + 128 j (its warp's rows rg + 4 j).
+__device__ __forceinline__ void fp2_rows_store(const RowState &rs, uint32_t rst, unsigned sub) {
+  if (sub != 0) return;   // the 8 lanes of a row hold the same state
+#pragma unroll
+  for (int j = 0; j < 8; ++j) {
+    asm volatile("st.shared.v4.s32 [%0], {%1,%2,%3,%4};" ::"r"(rst + 128u * j), "r"(rs.g1[j]), "r"(rs.g2[j]), "r"(rs.g3[j]), "r"(0)
+                 : "memory");
+    sts128(rst + 128u * j + 16u, rs.w1[j], rs.w2[j], rs.w3[j], ((rs.live >> j) & 1u) ? 1.f : 0.f);
+  }
+}
+__device__ __forceinline__ int4 lds128i(uint32_t addr) {
+  int4 v;
+  asm volatile("ld.shared.v4.s32 {%0,%1,%2,%3}, [%4];" : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w) : "r"(addr));
+  return v;
+}
+
+// stage_a_chunk<PRO_FP_INTERP> with the row state read from shared memory (fp2_rows_store): the same loads, the same
+// contraction fma(p3,w3, fma(p1,w1, p2*w2)), the same TF32 rounding and zeros -- the same bits in the A chunk
+__device__ __forceinline__ void fp2_stage_chunk(const MlpArgs &a, uint32_t rst, long long p_first, int r_first, int sub,
+                                                int k0, uint32_t sa, bool vec_ok) {
+  const int k = k0 + 4 * sub;
+  const float4 zero = make_float4(0.f, 0.f, 0.f, 0.f);
+  if (vec_ok && k + 4 <= a.c2) {
+    const float *kf = a.known_feat + k;
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {  // two halves: 12 LDG.128 in flight each
+      float4 p1[4], p2[4], p3[4];
+#pragma unroll
+      for (int jj = 0; jj < 4; ++jj) {
+        const int4 gi = lds128i(rst + 128u * (h * 4 + jj));
+        p1[jj] = ldg128(kf + static_cast<size_t>(gi.x) * a.c2);
+        p2[jj] = ldg128(kf + static_cast<size_t>(gi.y) * a.c2);
+        p3[jj] = ldg128(kf + static_cast<size_t>(gi.z) * a.c2);
+      }
+#pragma unroll
+      for (int jj = 0; jj < 4; ++jj) {
+        const int j = h * 4 + jj;
+        const float4 w = lds128(rst + 128u * j + 16u);
+        float4 v;
+        v.x = __fmaf_rn(p3[jj].x, w.z, __fmaf_rn(p1[jj].x, w.x, __fmul_rn(p2[jj].x, w.y)));
+        v.y = __fmaf_rn(p3[jj].y, w.z, __fmaf_rn(p1[jj].y, w.x, __fmul_rn(p2[jj].y, w.y)));
+        v.z = __fmaf_rn(p3[jj].z, w.z, __fmaf_rn(p1[jj].z, w.x, __fmul_rn(p2[jj].z, w.y)));
+        v.w = __fmaf_rn(p3[jj].w, w.z, __fmaf_rn(p1[jj].w, w.x, __fmul_rn(p2[jj].w, w.y)));
+        if (w.w == 0.f) v = zero;
+        sts_tf32(sa + sw128_off(r_first + 4 * j, sub), v);
+      }
+    }
+    return;
+  }
+  const bool skip_vec = (a.c2 % 4 == 0) && (a.lds % 4 == 0) && ((reinterpret_cast<uintptr_t>(a.skip) & 15u) == 0);
+  if (skip_vec && k >= a.c2 && k - a.c2 + 4 <= a.c1) {
+    float4 v[8];
+#pragma unroll
+    for (int j = 0; j < 8; ++j)
+      v[j] = lds128(rst + 128u * j + 16u).w != 0.f ? ldg128(a.skip + (p_first + 4 * j) * a.lds + (k - a.c2)) : zero;
+#pragma unroll
+    for (int j = 0; j < 8; ++j) sts_tf32(sa + sw128_off(r_first + 4 * j, sub), v[j]);
+    return;
+  }
+  if (k >= a.c2 + a.c1) {
+#pragma unroll
+    for (int j = 0; j < 8; ++j) sts128(sa + sw128_off(r_first + 4 * j, sub), 0.f, 0.f, 0.f, 0.f);
+    return;
+  }
+  // generic path (a chunk that straddles the interpolated / skip / padding boundary, unaligned rows): per element
+#pragma unroll
+  for (int j = 0; j < 8; ++j) {
+    const int4 gi = lds128i(rst + 128u * j);
+    const float4 w = lds128(rst + 128u * j + 16u);
+    const bool live = w.w != 0.f;
+    const long long p = p_first + 4 * j;
+    float vv[4];
+#pragma unroll
+    for (int e = 0; e < 4; ++e) {
+      const int kk = k + e;
+      const bool isk = live && kk < a.c2;
+      const int d = kk - a.c2;
+      const bool iss = live && d >= 0 && d < a.c1;
+      const float *kf = a.known_feat + (isk ? kk : 0);
+      const float p1 = isk ? __ldg(kf + static_cast<size_t>(gi.x) * a.c2) : 0.f;
+      const float p2 = isk ? __ldg(kf + static_cast<size_t>(gi.y) * a.c2) : 0.f;
+      const float p3 = isk ? __ldg(kf + static_cast<size_t>(gi.z) * a.c2) : 0.f;
+      const float sk = iss ? __ldg(a.skip + p * a.lds + (iss ? d : 0)) : 0.f;
+      vv[e] = isk ? __fmaf_rn(p3, w.z, __fmaf_rn(p1, w.x, __fmul_rn(p2, w.y))) : sk;
+    }
+    sts_tf32(sa + sw128_off(r_first + 4 * j, sub), make_float4(vv[0], vv[1], vv[2], vv[3]));
+  }
+}
+
+// One 64 x 128 block of layer 1 for the calling warpgroup: the kc1 A chunks of the ring (items ita0..) x its weight
+// chunks (items itw0, itw0 + 2, ..) into registers; each stage is released once the MMAs that read it have retired.
+__device__ __forceinline__ void fp2_layer1_block(float (&d)[64], uint32_t aring, uint32_t wring, int SA, int SW, int ita0,
+                                                 int itw0, int kc1, Fp2SmemCtl &ctl, unsigned lane) {
+#pragma unroll
+  for (int i = 0; i < 64; ++i) d[i] = 0.f;
+  int pa = -1, pw = -1;
+  for (int kc = 0; kc < kc1; ++kc) {
+    const int ita = ita0 + kc, itw = itw0 + 2 * kc;
+    const int sa = ita % SA, sw = itw % SW;
+    mbar_wait(&ctl.a_full[sa], static_cast<unsigned>((ita / SA) & 1));
+    mbar_wait(&ctl.w_full[sw], static_cast<unsigned>((itw / SW) & 1));
+    fence_proxy_async_smem();
+    const uint64_t adesc = smem_desc_sw128(aring + static_cast<uint32_t>(sa) * kFp2AStageBytes);
+    const uint64_t bdesc = smem_desc_sw128(wring + static_cast<uint32_t>(sw) * kFp2WStageBytes);
+    wgmma_fence();
+#pragma unroll
+    for (int k4 = 0; k4 < 4; ++k4)
+      wgmma_tf32<128>(d, adesc + static_cast<uint64_t>(k4 * 2), bdesc + static_cast<uint64_t>(k4 * 2), (kc > 0 || k4 > 0) ? 1u : 0u);
+    wgmma_commit();
+    if (pa >= 0) {
+      wgmma_wait<1>();
+      if (lane == 0) {
+        mbar_arrive(&ctl.a_empty[pa]);
+        mbar_arrive(&ctl.w_empty[pw]);
+      }
+    }
+    pa = sa;
+    pw = sw;
+  }
+  wgmma_wait<0>();
+  acc_fence(d);
+  if (lane == 0) {
+    mbar_arrive(&ctl.a_empty[pa]);
+    mbar_arrive(&ctl.w_empty[pw]);
+  }
+}
+
+__global__ void __launch_bounds__(kFp2Threads, 1) mlp_fp2_kernel(const __grid_constant__ Fp2Args g) {
+  const MlpArgs &a = g.a;
+  extern __shared__ unsigned char mlp_smem_raw[];
+  const uint32_t raw = smem_u32(mlp_smem_raw);
+  const uint32_t base = (raw + 1023u) & ~1023u;   // SWIZZLE_128B atoms are 8 rows x 128 B
+  const int kc1 = a.k_pad / 32, kc2 = g.k2_pad / 32;
+  const int nb1 = a.n_pad / 128, nb2 = g.n2_pad / 128;   // nb1 = 2 or 4: every layer-1 pass has a block per warpgroup
+  const int SA = g.a_stages, SW = g.w_stages;
+  const Fp2Smem L = fp2_smem(g.k2_pad, SA, SW);
+  Fp2SmemCtl &ctl = *reinterpret_cast<Fp2SmemCtl *>(mlp_smem_raw + (base - raw) + L.ctl);
+  const int t = threadIdx.x;
+  const unsigned warp = t >> 5, lane = t & 31u;
+  const int tiles = static_cast<int>((a.rows + kFp2BM - 1) / kFp2BM);   // the launcher checks the 32-bit counts
+
+  if (t == 0) {
+    for (int s = 0; s < SA; ++s) {
+      mbar_init(&ctl.a_full[s], 64);
+      mbar_init(&ctl.a_empty[s], kMlpMmaWarps);
+    }
+    for (int s = 0; s < SW; ++s) {
+      mbar_init(&ctl.w_full[s], 1);
+      mbar_init(&ctl.w_empty[s], 4);
+    }
+    mbar_fence_init();
+  }
+  __syncthreads();
+
+  if (warp < kFp2ProWarps) {
+    // ================= producers: pair q = warp / 2 stages the A items it % 2 == q, warp w rows 32 (w & 1).. ======
+    const unsigned pair = warp >> 1;
+    const int sub = static_cast<int>(lane & 7u), r_first = 32 * static_cast<int>(warp & 1u) + static_cast<int>(lane >> 3);
+    const bool vec_ok = (a.c2 % 4 == 0) && ((reinterpret_cast<uintptr_t>(a.known_feat) & 15u) == 0);
+    const int per_tile = (nb1 / 2) * kc1;   // A items per tile: one pass over K per pair of layer-1 blocks
+    const uint32_t rst = base + L.rows + warp * 1024u + (lane >> 3) * 32u;
+    int it = 0;
+    for (int tile = blockIdx.x; tile < tiles; tile += gridDim.x) {
+      const long long p_first = static_cast<long long>(tile) * kFp2BM + r_first;
+      {
+        RowState rs;
+        rows_setup<PRO_FP_INTERP>(a, p_first, rs);
+        __syncwarp();   // every lane is done with the previous tile's row state
+        fp2_rows_store(rs, rst, static_cast<unsigned>(sub));
+        __syncwarp();
+      }
+      for (int i = 0; i < per_tile; ++i, ++it) {
+        if (static_cast<unsigned>(it % kFp2Pairs) != pair) continue;
+        const int s = it % SA;
+        mbar_wait(&ctl.a_empty[s], static_cast<unsigned>(((it / SA) & 1) ^ 1));
+        const int kc = i % kc1;
+        fp2_stage_chunk(a, rst, p_first, r_first, sub, kc * 32, base + L.aring + static_cast<uint32_t>(s) * kFp2AStageBytes, vec_ok);
+        fence_proxy_async_smem();
+        mbar_arrive(&ctl.a_full[s]);
+      }
+    }
+  } else if (warp == kFp2LoaderWarp) {
+    // ================= loader: every weight chunk of every tile, in ring order ===============================
+    if (lane == 0) {
+      int it = 0;
+      for (int tile = blockIdx.x; tile < tiles; tile += gridDim.x) {
+        for (int layer = 0; layer < 2; ++layer) {
+          const CUtensorMap *map = layer ? &g.tmap2 : &a.tmap;
+          const int nb = layer ? nb2 : nb1, kcs = layer ? kc2 : kc1;
+          for (int pp = 0; pp < nb; pp += 2) {
+            const int cnt = sa2w_pair_blocks(nb, pp);
+            for (int kc = 0; kc < kcs; ++kc)
+              for (int q = 0; q < cnt; ++q, ++it) {
+                const int s = it % SW;
+                mbar_wait(&ctl.w_empty[s], static_cast<unsigned>(((it / SW) & 1) ^ 1));
+                mbar_expect_tx(&ctl.w_full[s], kFp2WStageBytes);
+                tma_load_2d(base + L.wring + static_cast<uint32_t>(s) * kFp2WStageBytes, map, kc * 32, (pp + q) * 128,
+                            &ctl.w_full[s]);
+              }
+          }
+        }
+      }
+    }
+  } else {
+    // ================= MMA + epilogues: warpgroup wg, warp w4 of it holds rows 16 w4 .. +15 of the tile ======
+    const unsigned mw = warp - kFp2ProWarps, wg = mw >> 2, w4 = mw & 3u;
+    const int frag_row = static_cast<int>(16 * w4 + (lane >> 2));
+    const uint32_t h_s = base + L.h;
+    int ita = 0, itw = 0;
+    float d[64];
+    for (int tile = blockIdx.x; tile < tiles; tile += gridDim.x) {
+      const long long p0 = static_cast<long long>(tile) * kFp2BM;
+      // ---- layer 1 -> H tile, one pass over the A chunks per pair of column blocks
+      for (int pp = 0; pp < nb1; pp += 2) {
+        const int nb = pp + static_cast<int>(wg);
+        fp2_layer1_block(d, base + L.aring, base + L.wring, SA, SW, ita, itw + static_cast<int>(wg), kc1, ctl, lane);
+        ita += kc1;
+        itw += 2 * kc1;
+        // both warpgroups have finished the previous tile's layer 2 (its reads of H)
+        if (pp == 0) named_bar_sync(1, 2 * 128);
+        // H[row, c] = tf32(relu(acc + b1[c])): the epilogue of pvn3d_mlp_fp_first with RELU | ROUND_OUT
+#pragma unroll
+        for (int jj = 0; jj < 16; ++jj) {
+          const int c = 128 * nb + 8 * jj + 2 * static_cast<int>(lane & 3u);
+          const float b0 = __ldg(a.bias + c), b1 = __ldg(a.bias + c + 1);
+          const uint32_t off = static_cast<uint32_t>(c >> 5) * kFp2AStageBytes + static_cast<uint32_t>(frag_row) * 128u +
+                               ((static_cast<uint32_t>(((c & 31) >> 2) ^ (frag_row & 7))) << 4) + (c & 3) * 4u;
+          asm volatile("st.shared.v2.f32 [%0], {%1,%2};" ::"r"(h_s + off), "f"(to_tf32(fmaxf(d[4 * jj] + b0, 0.f))),
+                       "f"(to_tf32(fmaxf(d[4 * jj + 1] + b1, 0.f)))
+                       : "memory");
+          asm volatile("st.shared.v2.f32 [%0], {%1,%2};" ::"r"(h_s + off + 8u * 128u), "f"(to_tf32(fmaxf(d[4 * jj + 2] + b0, 0.f))),
+                       "f"(to_tf32(fmaxf(d[4 * jj + 3] + b1, 0.f)))
+                       : "memory");
+        }
+      }
+      fence_proxy_async_smem();   // generic-proxy stores of H -> visible to the tensor core
+      named_bar_sync(1, 2 * 128); // every block of H is written
+      // ---- layer 2 from the H tile: out = relu(acc + b2) [tf32], the epilogue of pvn3d_mlp_dense with RELU
+      const long long r0 = p0 + frag_row;
+      for (int pp = 0; pp < nb2; pp += 2) {
+        const int cnt = sa2w_pair_blocks(nb2, pp);
+        if (static_cast<int>(wg) < cnt) {
+          const int nb = pp + static_cast<int>(wg);
+          sa2w_block(d, h_s, base + L.wring, SW, itw + static_cast<int>(wg), cnt, kc2, ctl.w_full, ctl.w_empty, nullptr, 0u,
+                     false, lane);
+          // a quad of lanes writes 32 contiguous bytes of a row: whole sectors
+          float *o = a.out + r0 * a.ldo + a.col0 + 128 * nb + 2 * static_cast<int>(lane & 3u);
+          const bool on0 = r0 < a.rows, on1 = r0 + 8 < a.rows;
+#pragma unroll
+          for (int jj = 0; jj < 16; ++jj) {
+            const int c = 128 * nb + 8 * jj + 2 * static_cast<int>(lane & 3u);
+            const float b0 = __ldg(g.bias2 + c), b1 = __ldg(g.bias2 + c + 1);
+            float2 v0 = make_float2(fmaxf(d[4 * jj] + b0, 0.f), fmaxf(d[4 * jj + 1] + b1, 0.f));
+            float2 v1 = make_float2(fmaxf(d[4 * jj + 2] + b0, 0.f), fmaxf(d[4 * jj + 3] + b1, 0.f));
+            if (a.round_out) {
+              v0.x = to_tf32(v0.x); v0.y = to_tf32(v0.y); v1.x = to_tf32(v1.x); v1.y = to_tf32(v1.y);
+            }
+            if (on0) *reinterpret_cast<float2 *>(o + 8 * jj) = v0;
+            if (on1) *reinterpret_cast<float2 *>(o + 8 * static_cast<size_t>(a.ldo) + 8 * jj) = v1;
+          }
+        }
+        itw += kc2 * cnt;
+      }
+    }
+  }
+}
+
+// pvn3d_mlp_fp2's ring stages for a module (A ring, weight ring); false: the module is not covered -- a first layer of
+// other than 256 or 512 columns, a second layer not a multiple of 128 columns, a layer-2 K other than the layer-1
+// width, or H + four A stages + three weight stages beyond the shared memory of a block
+bool fp2_stages(int k1_pad, int n1_pad, int k2_pad, int n2_pad, int *a_stages, int *w_stages) {
+  if ((n1_pad != 256 && n1_pad != 512) || n2_pad <= 0 || n2_pad % 128 || k2_pad != n1_pad || k1_pad <= 0 || k1_pad % 32)
+    return false;
+  const uint32_t fixed = fp2_smem(k2_pad, 0, 0).bytes;
+  const uint32_t least = 4u * kFp2AStageBytes + 3u * kFp2WStageBytes;
+  if (fixed + least > static_cast<uint32_t>(kMlpSmemMax)) return false;
+  // the A ring first (the gathering producers are the slower side), at least three weight stages
+  const uint32_t avail = static_cast<uint32_t>(kMlpSmemMax) - fixed;
+  const int sa = std::min<int>(kFp2MaxStages, static_cast<int>((avail - 3u * kFp2WStageBytes) / kFp2AStageBytes));
+  const int sw = std::min<int>(kFp2MaxStages, static_cast<int>((avail - static_cast<uint32_t>(sa) * kFp2AStageBytes) / kFp2WStageBytes));
+  *a_stages = sa;
+  *w_stages = sw;
+  return true;
+}
+
+int launch_fp2(Fp2Args &g, cudaStream_t st) {
+  MlpArgs &a = g.a;
+  if (a.rows <= 0) return PVN3D_OK;
+  const size_t smem = fp2_smem(g.k2_pad, g.a_stages, g.w_stages).bytes;
+  const long long tiles = (a.rows + kFp2BM - 1) / kFp2BM;
+  const long long a_items = static_cast<long long>(a.n_pad / 256) * (a.k_pad / 32);
+  const long long w_items = 2 * a_items + static_cast<long long>(g.n2_pad / 128) * (g.k2_pad / 32);
+  if (tiles * w_items > 0x7fffffffll || tiles * a_items > 0x7fffffffll)
+    return PVN3D_ERR_UNSUPPORTED;   // the kernel counts ring items in 32 bits
+  if (!weight_tensor_map(&a.tmap, a.w, a.k_pad, a.n_pad, 128) || !weight_tensor_map(&g.tmap2, g.w2, g.k2_pad, g.n2_pad, 128))
+    return PVN3D_ERR_UNSUPPORTED;
+  const int sms = std::max(1, sm_count() - a.reserve_sms);
+  auto kern = mlp_fp2_kernel;
+  static PerDeviceOnce once;
+  PVN3D_ONCE_PER_DEVICE(once, cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, kMlpSmemMax),
+                        "mlp fp2 smem attr");
+  const unsigned grid = static_cast<unsigned>(std::min<long long>(tiles, sms));
+  kern<<<grid, kFp2Threads, smem, st>>>(g);
+  return check_launch("mlp_fp2_kernel");
 }
 
 int dispatch(MlpArgs &a, int pro, int pool, cudaStream_t st) {
@@ -1850,6 +2219,40 @@ extern "C" int pvn3d_mlp_sa_fact2w_supported(const pvn3d_mlp_layer_t *layer2, co
       layer3->k_pad < layer2->n_pad || layer3->k_pad % 32 || layer3->n_pad <= 0 || layer3->n_pad % 16)
     return 0;
   return sa2w_stages(layer2->k_pad, layer2->n_pad, layer3->k_pad, layer3->n_pad, ns) ? 1 : 0;
+}
+
+extern "C" int pvn3d_mlp_fp2(const float *known_feat_pm, int c2, const int *nn_idx, const float *nn_w, const float *skip_pm,
+                             int lds, int c1, int b, int n_unknown, int m_known, const pvn3d_mlp_layer_t *layer1,
+                             const pvn3d_mlp_layer_t *layer2, int flags, float *out, int ldo, int col0, pvn3d_stream_t stream) {
+  if (!known_feat_pm || !nn_idx || !nn_w || !layer1 || !layer2 || !layer1->w || !layer1->bias || !layer2->w || !layer2->bias ||
+      !out || b < 0 || n_unknown < 0 || m_known <= 0 || c2 <= 0 || c1 < 0 || (c1 > 0 && (!skip_pm || lds < c1)) ||
+      layer1->k_pad < c2 + c1 || layer1->k_pad % 32 || layer1->n_pad <= 0 || layer1->n_pad % 16 || layer2->k_pad < layer1->n_pad ||
+      layer2->k_pad % 32 || layer2->n_pad <= 0 || layer2->n_pad % 16 || ldo % 4 || col0 % 4 ||
+      (reinterpret_cast<uintptr_t>(layer1->w) & 15u) || (reinterpret_cast<uintptr_t>(layer2->w) & 15u))
+    return PVN3D_ERR_INVALID_ARG;
+  int a_stages = 0, w_stages = 0;
+  if (!fp2_stages(layer1->k_pad, layer1->n_pad, layer2->k_pad, layer2->n_pad, &a_stages, &w_stages)) return PVN3D_ERR_UNSUPPORTED;
+  if (static_cast<long long>(b) * m_known > 0x7fffffffll || n_unknown > 0x3fffffff) return PVN3D_ERR_UNSUPPORTED;
+  Fp2Args g{};
+  MlpArgs &a = g.a;
+  a.w = layer1->w; a.bias = layer1->bias; a.k_pad = layer1->k_pad; a.n_pad = layer1->n_pad;
+  a.rows = static_cast<long long>(b) * n_unknown;
+  a.known_feat = known_feat_pm; a.c2 = c2; a.nn_idx = nn_idx; a.nn_w = nn_w; a.skip = skip_pm;
+  a.lds = lds; a.c1 = c1; a.n_unknown = n_unknown; a.m_known = m_known;
+  a.out = out; a.ldo = ldo; a.col0 = col0; a.relu = 1;
+  a.round_out = (flags & PVN3D_MLP_ROUND_OUT) ? 1 : 0;
+  a.reserve_sms = (flags >> 8) & 0xff;
+  g.w2 = layer2->w; g.bias2 = layer2->bias; g.k2_pad = layer2->k_pad; g.n2_pad = layer2->n_pad;
+  g.a_stages = a_stages; g.w_stages = w_stages;
+  return launch_fp2(g, as_stream(stream));
+}
+
+extern "C" int pvn3d_mlp_fp2_supported(const pvn3d_mlp_layer_t *layer1, const pvn3d_mlp_layer_t *layer2) {
+  if (!layer1 || !layer2 || layer1->k_pad <= 0 || layer1->k_pad % 32 || layer1->n_pad <= 0 || layer1->n_pad % 16 ||
+      layer2->k_pad < layer1->n_pad || layer2->k_pad % 32 || layer2->n_pad <= 0 || layer2->n_pad % 16)
+    return 0;
+  int a_stages = 0, w_stages = 0;
+  return fp2_stages(layer1->k_pad, layer1->n_pad, layer2->k_pad, layer2->n_pad, &a_stages, &w_stages) ? 1 : 0;
 }
 
 extern "C" int pvn3d_mlp_fp_fact(const float *p, const float *s, int ld, int c_valid, const int *nn_idx,

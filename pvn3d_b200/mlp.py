@@ -11,8 +11,8 @@ matrix + bias, and runs `Pointnet2MSG.forward` (reference pvn3d/lib/pvn3d.py:126
                  (pvn3d_mlp_sa_fact2 for SA1 / SA2, pvn3d_mlp_sa_fact2w for SA3 / SA4), written straight
                  into the level's point-major feature table
   per FP level : three_nn -> inverse-distance weights ->
-                 FP2-4: first layer with three_interpolate + concat fused into the tensor-core operand
-                        producer (pvn3d_mlp_fp_first) -> second layer (pvn3d_mlp_dense)
+                 FP2-4: both layers in ONE launch (pvn3d_mlp_fp2): three_interpolate + concat fused into the
+                        tensor-core operand producer, the layer-1 activations kept in shared memory
                  FP1  : factored first layer (P = W1k . known, S = W1s . skip + b1 by pvn3d_mlp_dense) ->
                         second layer on relu(interpolated P + S) (pvn3d_mlp_fp_fact), stored channel-major
                         [B,128,N], the layout the reference returns (when N % 32 == 0; else a transpose follows)
@@ -107,6 +107,31 @@ def mlp_fp_first(known_feat_pm, nn_idx, nn_w, skip_ptr, lds, c1, layer: PackedLa
                                     _flags(relu, round_out, reserve=reserve), ptr(out), out.size(-1), 0,
                                     _stream(known_feat_pm.device))
     check(rc, "pvn3d_mlp_fp_first")
+    return out
+
+
+def fp2_fits(layer1: PackedLayer, layer2: PackedLayer) -> bool:
+    """whether pvn3d_mlp_fp2 takes a two-layer FP module (the library's own rule: a first layer of 256 or 512 columns, a
+    second layer of a multiple of 128 columns over exactly those, tiles and stages within shared memory -- FP2-FP4)"""
+    l1, l2 = _layer_struct(layer1), _layer_struct(layer2)
+    return bool(_lib.load().pvn3d_mlp_fp2_supported(ctypes.addressof(l1), ctypes.addressof(l2)))
+
+
+def mlp_fp2(known_feat_pm, nn_idx, nn_w, skip_ptr, lds, c1, layer1: PackedLayer, layer2: PackedLayer, out=None, col0=0,
+            round_out=False, reserve=0):
+    """both layers of an FP module in one launch (pvn3d_mlp_fp2): the same bits as
+    mlp_fp_first(.., layer1, round_out=True) -> mlp_dense(.., layer2, a_tf32=True, round_out=round_out)"""
+    lib = _lib.load()
+    b, m_known, c2 = known_feat_pm.shape
+    n_unknown = nn_idx.shape[1]
+    if out is None:
+        out = torch.empty((b * n_unknown, layer2.n_pad), dtype=torch.float32, device=known_feat_pm.device)
+    l1, l2 = _layer_struct(layer1), _layer_struct(layer2)
+    with torch.cuda.device(known_feat_pm.device):
+        rc = lib.pvn3d_mlp_fp2(ptr(known_feat_pm), c2, ptr(nn_idx), ptr(nn_w), skip_ptr, lds, c1, b, n_unknown, m_known,
+                               ctypes.addressof(l1), ctypes.addressof(l2), _flags(True, round_out, reserve=reserve), ptr(out),
+                               out.size(-1), col0, _stream(known_feat_pm.device))
+    check(rc, "pvn3d_mlp_fp2")
     return out
 
 
@@ -285,8 +310,9 @@ class FusedPointnet2MSG:
             self.sa.append(scales)
             self.sa_out.append(sum(l3.n for _, l3, _ in scales))
             assert all(l3.n % 4 == 0 for _, l3, _ in scales)
-        #: FP2-FP4 (keys 1-3): first layer with the interpolation fused into its producer, then the second layer
-        self.fp: Dict[int, List[PackedLayer]] = {}
+        #: FP2-FP4 (keys 1-3): (layer 1, layer 2), both run by pvn3d_mlp_fp2 with the interpolation fused into the
+        #: operand producer of layer 1
+        self.fp: Dict[int, Tuple[PackedLayer, PackedLayer]] = {}
         for i, fp in enumerate(model.FP_modules):
             if i == 0:
                 continue
@@ -295,7 +321,10 @@ class FusedPointnet2MSG:
                 pl = PackedLayer(*fold_conv_bn(layer), prev_pad)
                 prev_pad = pl.n_pad
                 layers.append(pl)
-            self.fp[i] = layers
+            if len(layers) != 2 or not fp2_fits(*layers):
+                raise ValueError(f"FP{i + 1}: no fused kernel takes its layers "
+                                 f"({' -> '.join(str(x) for x in [layers[0].k] + [l.n for l in layers])} channels)")
+            self.fp[i] = (layers[0], layers[1])
         #: FP1, factored: W1 = [W_k (known columns) | W_s (skip columns)] as (P layer W_k, S layer W_s + b1, layer 2).
         #: The skip of FP1 is the raw cloud: W_s reads it through the level-0 factor table [f | hi x | lo x].
         fp1 = model.FP_modules[0].mlp
@@ -428,11 +457,8 @@ class FusedPointnet2MSG:
             unknown, known = l_xyz[i], l_xyz[i + 1]
             nn_idx, nn_w = plan.nn[i]
             sptr, lds, c1 = feats[i]
-            layers = self.fp[i]
-            h = mlp_fp_first(l_feat[i + 1], nn_idx, nn_w, sptr, lds, c1, layers[0], round_out=True, reserve=rs)
-            for li2, lyr in enumerate(layers[1:]):
-                last = li2 == len(layers) - 2        # level tables stay full fp32
-                h = mlp_dense(h, lyr, round_out=not last, a_tf32=True, reserve=rs)
+            l1, l2 = self.fp[i]
+            h = mlp_fp2(l_feat[i + 1], nn_idx, nn_w, sptr, lds, c1, l1, l2, reserve=rs)   # level tables stay full fp32
             l_feat[i] = h.view(b, unknown.size(1), -1)
             self._m("mlp")
         # FP1, factored -- it pays only where the known descriptors are much wider than the layer and the skip is
