@@ -436,6 +436,28 @@ int pvn3d_icp_refine_batch_clustered(const void *models, const float *pcld, cons
                                      double *err_out, uint8_t *refined_out, int *cluster_pts_out,
                                      void *workspace, size_t workspace_bytes, pvn3d_stream_t stream);
 
+/* The full-resolution scene of eval_icp's refinement (pvn3d/eval_icp.py:224-291, 388-422).
+ *
+ * pvn3d_depth_to_cloud: Basic_Utils.dpt_2_cld (lib/utils/basic_utils.py:381-399) for every pixel, in
+ * raster order.  depth [B,H,W] f32, K [B,3,3] f32 (per frame), cam_scale [B] f32 ->
+ * cloud [B,H*W,3] f32, valid [B,H*W] u8.  A pixel is valid when dpt > 1e-6; then, one float32
+ * operation per step, pt2 = dpt / cam_scale, pt0 = ((col - cx) * pt2) / fx,
+ * pt1 = ((row - cy) * pt2) / fy.  An invalid pixel gets (0, 0, 0) and valid = 0.
+ * B*H*W < 2^31, else PVN3D_ERR_UNSUPPORTED (nothing launched). */
+int pvn3d_depth_to_cloud(const float *depth, const float *K, const float *cam_scale, int b, int h, int w,
+                         float *cloud, uint8_t *valid, pvn3d_stream_t stream);
+/* pvn3d_label_fill: eval_icp's fill_label_item.  Every valid pixel of cloud [B,hw,3] / valid [B,hw]
+ * takes point_labels[b, j] of the sampled point j of pcld [B,N,3] f32 nearest to it: float64 squared
+ * distance (dx*dx + dy*dy) + dz*dz without FMA, lowest j on exact ties.  labels_out [B,hw] i32;
+ * nn_idx_out [B,hw] i32 (j; NULL to skip).  Invalid pixels get label 0 and index -1.
+ * Each call builds the search grid of every frame's pcld into the workspace
+ * (pvn3d_label_fill_workspace_bytes(b, n), 256-B aligned; 0 = unsupported) on the stream.
+ * B*hw < 2^31, B*N < 2^31 and B <= 65535, else PVN3D_ERR_UNSUPPORTED (nothing launched). */
+size_t pvn3d_label_fill_workspace_bytes(int b, int n);
+int pvn3d_label_fill(const float *cloud, const uint8_t *valid, int hw, const float *pcld, const int *point_labels,
+                     int b, int n, int *labels_out, int *nn_idx_out, void *workspace, size_t workspace_bytes,
+                     pvn3d_stream_t stream);
+
 /* ------------------------------------------------------------------------------------------
  * Callers either side of the path (SURVEY section 8 f4)
  * ---------------------------------------------------------------------------------------- */

@@ -103,6 +103,9 @@ _SIGNATURES = {
     "pvn3d_icp_clustered_workspace_bytes": (c_size_t, [c_int, c_int, c_int, c_int]),
     "pvn3d_icp_refine_batch_clustered": (c_int, [_P, _P, _P, c_int, c_int, c_int, _P, _P, c_int, c_int, c_int, c_double,
                                                  c_double, c_int, _P, _P, _P, _P, _P, _P, c_size_t, _P]),
+    "pvn3d_depth_to_cloud": (c_int, [_P, _P, _P, c_int, c_int, c_int, _P, _P, _P]),
+    "pvn3d_label_fill_workspace_bytes": (c_size_t, [c_int, c_int]),
+    "pvn3d_label_fill": (c_int, [_P, _P, c_int, _P, _P, c_int, c_int, _P, _P, _P, c_size_t, _P]),
 }
 FLAT_MS_MAX_PTS = 4096   # PVN3D_FLAT_MS_MAX_PTS
 EXPORTED_SYMBOLS = tuple(_SIGNATURES)

@@ -404,6 +404,79 @@ __device__ void nn_search(const ModelHdr &H, const int *__restrict__ cs, const u
 }
 
 // ------------------------------------------------------------------------------------------------
+// eval_icp's fill_label_item: every valid pixel of a back-projected depth image takes the label of its
+// nearest sampled point.  Each frame's sampled cloud is a "model" of the set (icp_build_kernel, model
+// b = points [b*n, (b+1)*n)), searched at the identity pose: P a is then a itself and the camera-frame
+// distance is the float64 squared distance of the pixel to the point, so the match equals a float64
+// brute-force scan with the lowest point index on exact ties (sklearn's 1-NN up to its own ties).
+// ------------------------------------------------------------------------------------------------
+constexpr int kFillThreads = 256;
+
+// the models directory and model_off = b*n of the per-frame sets, written on the stream (no host copy)
+__global__ void label_fill_setup_kernel(ModelsDir L, int b, int n, int *__restrict__ off,
+                                        unsigned char *__restrict__ buf) {
+  const int t = blockIdx.x * blockDim.x + threadIdx.x;
+  if (t == 0) *reinterpret_cast<ModelsDir *>(buf) = L;
+  if (t <= b) off[t] = t * n;
+}
+
+__global__ void __launch_bounds__(kFillThreads)
+label_fill_kernel(const unsigned char *__restrict__ models, const float *__restrict__ cloud,
+                  const uint8_t *__restrict__ valid, int hw, int total, const int *__restrict__ point_labels,
+                  int n, int *__restrict__ labels_out, int *__restrict__ nn_out) {
+  __shared__ double s_eye[12];
+  if (threadIdx.x < 12) s_eye[threadIdx.x] = (threadIdx.x % 5 == 0) ? 1.0 : 0.0;  // [I | 0]
+  __syncthreads();
+  const int g = blockIdx.x * kFillThreads + threadIdx.x;
+  if (g >= total) return;
+  if (!valid[g]) {
+    labels_out[g] = 0;
+    if (nn_out) nn_out[g] = -1;
+    return;
+  }
+  const int b = g / hw;
+  const ModelsView mv = models_view(models);
+  const ModelHdr H = mv.hdr[b];
+  const double q[3] = {cloud[static_cast<size_t>(g) * 3 + 0], cloud[static_cast<size_t>(g) * 3 + 1],
+                       cloud[static_cast<size_t>(g) * 3 + 2]};
+  int pos;
+  double d2;
+  unsigned tests = 0;
+  nn_search(H, mv.cell_start + static_cast<size_t>(b) * (kMaxCells + 1), mv.dt + static_cast<size_t>(b) * kMaxCells,
+            mv.pts + H.pt_off, s_eye, 1.0, q, q, pos, d2, tests);
+  const int j = static_cast<int>(mv.pts[H.pt_off + pos].w);
+  labels_out[g] = point_labels[static_cast<size_t>(b) * n + j];
+  if (nn_out) nn_out[g] = j;
+}
+
+// Basic_Utils.dpt_2_cld per pixel, in raster order: valid = dpt > 1e-6; pt2 = dpt / cam_scale,
+// pt0 = (col - cx) * pt2 / fx, pt1 = (row - cy) * pt2 / fy, each step one float32 operation
+__global__ void __launch_bounds__(kFillThreads)
+depth_to_cloud_kernel(const float *__restrict__ depth, const float *__restrict__ K,
+                      const float *__restrict__ cam_scale, int h, int w, int total, float *__restrict__ cloud,
+                      uint8_t *__restrict__ valid) {
+  const int g = blockIdx.x * kFillThreads + threadIdx.x;
+  if (g >= total) return;
+  const int hw = h * w, b = g / hw, p = g - b * hw, row = p / w, col = p - row * w;
+  const float d = depth[g];
+  float *o = cloud + static_cast<size_t>(g) * 3;
+  if (!(d > 1e-6f)) {
+    o[0] = 0.f;
+    o[1] = 0.f;
+    o[2] = 0.f;
+    valid[g] = 0;
+    return;
+  }
+  const float *k = K + static_cast<size_t>(b) * 9;
+  const float fx = k[0], cx = k[2], fy = k[4], cy = k[5];
+  const float pt2 = __fdiv_rn(d, cam_scale[b]);
+  o[0] = __fdiv_rn(__fmul_rn(__fsub_rn(static_cast<float>(col), cx), pt2), fx);
+  o[1] = __fdiv_rn(__fmul_rn(__fsub_rn(static_cast<float>(row), cy), pt2), fy);
+  o[2] = pt2;
+  valid[g] = 1;
+}
+
+// ------------------------------------------------------------------------------------------------
 // the fit: one CTA per (frame, class) of a batch, or one CTA for an explicit scene set
 // ------------------------------------------------------------------------------------------------
 struct FitParams {
@@ -947,4 +1020,64 @@ extern "C" int pvn3d_icp_fit(const void *models, int model, const float *scene, 
   p.tests_out = reinterpret_cast<unsigned long long *>(ws + L.stats);
   icp_fit_kernel<false><<<1, kFitThreads, 0, st>>>(p);
   return check_launch("icp_fit_kernel");
+}
+
+namespace pvn3d {
+namespace {
+
+// the label fill's workspace: the per-frame model set, then model_off [b+1]
+struct FillWsLayout {
+  ModelsDir models;
+  size_t off, total;
+};
+FillWsLayout fill_ws_layout(int b, int n) {
+  FillWsLayout L;
+  L.models = models_layout(b, b * n);
+  L.off = L.models.total;
+  L.total = L.off + align_up(static_cast<size_t>(b + 1) * 4, 256);
+  return L;
+}
+
+// B*H*W pixels (and B*N points) are indexed with 32-bit ints
+bool fits_int32(long long b, long long per) { return b * per < 0x80000000ll; }
+
+}  // namespace
+}  // namespace pvn3d
+
+extern "C" int pvn3d_depth_to_cloud(const float *depth, const float *K, const float *cam_scale, int b, int h,
+                                    int w, float *cloud, uint8_t *valid, pvn3d_stream_t stream) {
+  if (!depth || !K || !cam_scale || !cloud || !valid || b < 1 || h < 1 || w < 1) return PVN3D_ERR_INVALID_ARG;
+  if (!fits_int32(b, static_cast<long long>(h) * w)) return PVN3D_ERR_UNSUPPORTED;
+  const int total = b * h * w;
+  depth_to_cloud_kernel<<<ceil_div(total, kFillThreads), kFillThreads, 0, as_stream(stream)>>>(
+      depth, K, cam_scale, h, w, total, cloud, valid);
+  return check_launch("depth_to_cloud_kernel");
+}
+
+extern "C" size_t pvn3d_label_fill_workspace_bytes(int b, int n) {
+  if (b < 1 || n < 1 || b > 65535 || !fits_int32(b, n)) return 0;
+  return fill_ws_layout(b, n).total;
+}
+
+extern "C" int pvn3d_label_fill(const float *cloud, const uint8_t *valid, int hw, const float *pcld,
+                                const int *point_labels, int b, int n, int *labels_out, int *nn_idx_out,
+                                void *workspace, size_t workspace_bytes, pvn3d_stream_t stream) {
+  if (!cloud || !valid || !pcld || !point_labels || !labels_out || !models_ok(workspace) || hw < 1 || b < 1 ||
+      n < 1)
+    return PVN3D_ERR_INVALID_ARG;
+  if (b > 65535 || !fits_int32(b, hw) || !fits_int32(b, n)) return PVN3D_ERR_UNSUPPORTED;
+  const FillWsLayout L = fill_ws_layout(b, n);
+  if (workspace_bytes < L.total) return PVN3D_ERR_WORKSPACE;
+  unsigned char *buf = static_cast<unsigned char *>(workspace);
+  int *off = reinterpret_cast<int *>(buf + L.off);
+  cudaStream_t st = as_stream(stream);
+  label_fill_setup_kernel<<<ceil_div(b + 1, 256), 256, 0, st>>>(L.models, b, n, off, buf);
+  int rc = check_launch("label_fill_setup_kernel");
+  if (rc != PVN3D_OK) return rc;
+  icp_build_kernel<<<b, kBuildThreads, 0, st>>>(pcld, off, buf);
+  if ((rc = check_launch("icp_build_kernel")) != PVN3D_OK) return rc;
+  const int total = b * hw;
+  label_fill_kernel<<<ceil_div(total, kFillThreads), kFillThreads, 0, st>>>(buf, cloud, valid, hw, total,
+                                                                           point_labels, n, labels_out, nn_idx_out);
+  return check_launch("label_fill_kernel");
 }

@@ -6,6 +6,8 @@ float64 by csrc/icp.cu.
     poses64, iters, err, refined = ref.refine(pcld, mask, poses, present)          # batched, sync-free
     p3ds = get_cld_bigest_clus(p3ds, radius=0.06)    # eval_icp's biggest flat mean-shift cluster
     ref = IcpRefiner(..., cluster_bandwidth=0.06)    # the same filter before every batched fit
+    ref = DepthIcpRefiner(models, n_cls, batch)      # eval_icp's settings on full-resolution depth
+    poses64, iters, err, refined = ref.refine(depth, K, cam_scale, poses, present, pcld=pcld, point_labels=mask)
 
 The batched form takes FramePoseSolver.solve()'s poses and present flags as they come out and runs
 one fit per (frame, class) on the current stream, as pvn3d/eval_icp.py:94-185 does per object.
@@ -201,6 +203,181 @@ class IcpRefiner:
                     self._ws_ptr, self.ws_bytes, cur.cuda_stream)
         check(rc, "pvn3d_icp_refine_batch" + ("" if self.cluster_bw is None else "_clustered"))
         return self.poses[:b], self.iters[:b], self.err[:b], self.refined[:b]
+
+
+_INT32_LIMIT = 1 << 31
+
+
+def _check_dev(t: torch.Tensor, dt, dev, what: str) -> None:
+    if not (t.is_cuda and t.is_contiguous() and t.dtype == dt and (dev is None or t.device == dev)):
+        raise ValueError(f"{what}: expected a contiguous {dt} CUDA tensor" + ("" if dev is None else f" on {dev}"))
+
+
+def depth_to_cloud(depth: torch.Tensor, K: torch.Tensor, cam_scale: torch.Tensor, *, out=None):
+    """Basic_Utils.dpt_2_cld (lib/utils/basic_utils.py:381-399) for every pixel of a batch, on device.
+    depth [B,H,W] f32 (convert a uint16 depth PNG with .float(), as the reference's .astype(np.float32)),
+    K [B,3,3] f32 (per frame), cam_scale [B] f32.  Returns (cloud [B,H*W,3] f32, valid [B,H*W] u8) in
+    raster order: valid = depth > 1e-6; pt2 = depth / cam_scale, pt0 = (col - cx) * pt2 / fx,
+    pt1 = (row - cy) * pt2 / fy in float32; invalid pixels hold (0, 0, 0).  `out` = (cloud, valid)
+    to write into.  Runs on the current stream, no host sync."""
+    if depth.dim() != 3 or K.shape != (depth.size(0), 3, 3) or cam_scale.shape != (depth.size(0),):
+        raise ValueError(f"depth_to_cloud: expected depth [B,H,W], K [B,3,3], cam_scale [B]; got "
+                         f"{tuple(depth.shape)}, {tuple(K.shape)}, {tuple(cam_scale.shape)}")
+    dev = depth.device
+    for t, name in ((depth, "depth"), (K, "K"), (cam_scale, "cam_scale")):
+        _check_dev(t, torch.float32, dev, f"depth_to_cloud: {name}")
+    b, h, w = depth.shape
+    if b * h * w >= _INT32_LIMIT:
+        raise ValueError(f"depth_to_cloud: B*H*W = {b * h * w} pixels needs 64-bit indexing")
+    if out is None:
+        cloud = torch.empty((b, h * w, 3), dtype=torch.float32, device=dev)
+        valid = torch.empty((b, h * w), dtype=torch.uint8, device=dev)
+    else:
+        cloud, valid = out
+        if cloud.shape != (b, h * w, 3) or valid.shape != (b, h * w):
+            raise ValueError("depth_to_cloud: `out` shapes do not match the depth batch")
+        _check_dev(cloud, torch.float32, dev, "depth_to_cloud: out cloud")
+        _check_dev(valid, torch.uint8, dev, "depth_to_cloud: out valid")
+    lib = _lib.load()
+    with torch.cuda.device(dev):
+        rc = lib.pvn3d_depth_to_cloud(ptr(depth), ptr(K), ptr(cam_scale), b, h, w, ptr(cloud), ptr(valid),
+                                      torch.cuda.current_stream(dev).cuda_stream)
+    check(rc, "pvn3d_depth_to_cloud")
+    return cloud, valid
+
+
+def fill_label(cloud: torch.Tensor, valid: torch.Tensor, pcld: torch.Tensor, point_labels: torch.Tensor, *,
+               out=None, nn_idx=None) -> torch.Tensor:
+    """pvn3d/eval_icp.py:388-422 (fill_label_item) on device: every valid pixel of cloud [B,P,3] f32 /
+    valid [B,P] u8 takes point_labels[b, j] [B,N] i32 of its nearest sampled point j of pcld [B,N,3] f32
+    -- float64 distance (dx*dx + dy*dy) + dz*dz, lowest j on exact ties, which is sklearn
+    NearestNeighbors(n_neighbors=1)'s answer wherever the two best distances differ.  Invalid pixels
+    get 0.  Returns labels [B,P] i32 (`out` if given); `nn_idx` [B,P] i32, if given, receives j (-1 for
+    invalid pixels).  Runs on the current stream, no host sync."""
+    if cloud.dim() != 3 or cloud.size(2) != 3 or pcld.dim() != 3 or pcld.size(2) != 3:
+        raise ValueError(f"fill_label: expected cloud [B,P,3] and pcld [B,N,3]; got {tuple(cloud.shape)}, "
+                         f"{tuple(pcld.shape)}")
+    b, p = cloud.shape[:2]
+    n = pcld.size(1)
+    if valid.shape != (b, p) or pcld.size(0) != b or point_labels.shape != (b, n) or n < 1 or p < 1:
+        raise ValueError(f"fill_label: shapes do not agree: cloud {tuple(cloud.shape)}, valid {tuple(valid.shape)}, "
+                         f"pcld {tuple(pcld.shape)}, point_labels {tuple(point_labels.shape)}")
+    dev = cloud.device
+    for t, dt, name in ((cloud, torch.float32, "cloud"), (valid, torch.uint8, "valid"), (pcld, torch.float32, "pcld"),
+                        (point_labels, torch.int32, "point_labels")):
+        _check_dev(t, dt, dev, f"fill_label: {name}")
+    lib = _lib.load()
+    ws_bytes = int(lib.pvn3d_label_fill_workspace_bytes(b, n))
+    if ws_bytes == 0 or b * p >= _INT32_LIMIT:
+        raise ValueError(f"fill_label: B={b}, P={p}, N={n} needs 64-bit indexing")
+    labels = torch.empty((b, p), dtype=torch.int32, device=dev) if out is None else out
+    for t, name in ((labels, "out"), (nn_idx, "nn_idx")):
+        if t is not None:
+            if t.shape != (b, p):
+                raise ValueError(f"fill_label: {name} must be [B,P]")
+            _check_dev(t, torch.int32, dev, f"fill_label: {name}")
+    ws, ws_ptr = _aligned(ws_bytes, dev)
+    with torch.cuda.device(dev):
+        rc = lib.pvn3d_label_fill(ptr(cloud), ptr(valid), p, ptr(pcld), ptr(point_labels), b, n, ptr(labels),
+                                  ptr(nn_idx), ws_ptr, ws_bytes, torch.cuda.current_stream(dev).cuda_stream)
+    check(rc, "pvn3d_label_fill")
+    return labels
+
+
+def dpt_2_cld(dpt, cam_scale, K, device="cuda"):
+    """lib/utils/basic_utils.py:381-399 for one frame, computed on the GPU: dpt [H,W] (or [H,W,C]: channel
+    0), cam_scale and K [3,3] -> (cld [n,3] float32, choose [n] uint32) over the n pixels with dpt > 1e-6,
+    in raster order; (None, None) when there is none.  dpt, K and cam_scale are taken as float32: the
+    reference's arithmetic for float32 K (eval_icp's cam_scale is float32), and for any K under NumPy 1.x."""
+    dev = _cuda_device(device, "dpt_2_cld (pvn3d_b200)")
+    d = dpt.detach().cpu().numpy() if torch.is_tensor(dpt) else np.asarray(dpt)
+    if d.ndim > 2:
+        d = d[:, :, 0]
+    if d.ndim != 2:
+        raise ValueError(f"dpt_2_cld: expected an [H,W] depth image, got shape {d.shape}")
+    k = K.detach().cpu().numpy() if torch.is_tensor(K) else np.asarray(K)
+    k = np.ascontiguousarray(k, np.float32).reshape(1, 3, 3)
+    h, w = d.shape
+    td = torch.from_numpy(np.ascontiguousarray(d, np.float32)).reshape(1, h, w).to(dev)
+    cs = torch.tensor([float(np.float32(cam_scale))], dtype=torch.float32).to(dev)
+    cloud, valid = depth_to_cloud(td, torch.from_numpy(k).to(dev), cs)
+    v = valid[0].cpu().numpy().astype(bool)
+    choose = np.nonzero(v)[0].astype(np.uint32)
+    if len(choose) < 1:
+        return None, None
+    return cloud[0].cpu().numpy()[v], choose
+
+
+class DepthIcpRefiner:
+    """eval_icp's refinement (pvn3d/eval_icp.py:224-291, label_type='predmsk') on full-resolution depth,
+    batched and sync-free: back-project every pixel (depth_to_cloud), give each valid pixel a label
+    (fill_label from the network's sampled cloud, or a given label image), then run IcpRefiner with
+    n_pts = H*W on the pixel cloud -- invalid pixels carry class 0 and are never selected.  So each
+    object's scene set is its pixels in raster order: max_pts of them by the stride
+    floor(j*cnt/max_pts), skipped below min_pts, the biggest flat mean-shift cluster, then my_icp.
+
+    Defaults are eval_icp's: max_pts=2000 (n_sample_points), min_pts=1500, cluster_bandwidth=0.06,
+    max_iter=500, tol=1e-9.  Deliberate differences from the reference, shared with IcpRefiner: the
+    stride replaces np.random.shuffle's subset, and a class the solver did not find passes its pose
+    through (the reference runs ICP from a zero pose)."""
+
+    def __init__(self, models, n_cls: int, batch: int, height: int = 480, width: int = 640, *, max_pts: int = 2000,
+                 min_pts: int = 1500, cluster_bandwidth=0.06, max_iter: int = 500, tol: float = 1e-9,
+                 cluster_max_iter: int = 300, device="cuda"):
+        self.dev = _cuda_device(device, "DepthIcpRefiner")
+        self.h, self.w, self.b = int(height), int(width), int(batch)
+        if self.h < 1 or self.w < 1 or self.b < 1:
+            raise ValueError(f"batch={batch}, height={height}, width={width}: all must be >= 1")
+        if self.b * self.h * self.w >= _INT32_LIMIT:
+            raise ValueError(f"DepthIcpRefiner: {self.b}x{self.h}x{self.w} pixels needs 64-bit indexing")
+        hw = self.h * self.w
+        self.icp = IcpRefiner(models, n_cls, self.b, hw, max_pts=max_pts, min_pts=min_pts, max_iter=max_iter, tol=tol,
+                              cluster_bandwidth=cluster_bandwidth, cluster_max_iter=cluster_max_iter, device=self.dev)
+        self.n_cls = self.icp.n_cls
+        #: the pixel cloud [B,H*W,3] f32, its validity [B,H*W] u8 and per-pixel labels [B,H*W] i32 (0 where
+        #: invalid) of the last refine(): refiner-owned, valid until the next refine() on the same stream
+        self.cloud = torch.empty((self.b, hw, 3), dtype=torch.float32, device=self.dev)
+        self.valid = torch.empty((self.b, hw), dtype=torch.uint8, device=self.dev)
+        self.labels = torch.empty((self.b, hw), dtype=torch.int32, device=self.dev)
+
+    @property
+    def cluster_pts(self):
+        """[B,n_cls] i32: pixels each fit of the last refine() used after the cluster filter (0 when skipped)"""
+        return self.icp.cluster_pts
+
+    def kept_points(self) -> torch.Tensor:
+        """IcpRefiner.kept_points over the pixel cloud: the fits' pixel indices (row-major y*W + x)"""
+        return self.icp.kept_points()
+
+    def refine(self, depth: torch.Tensor, K: torch.Tensor, cam_scale: torch.Tensor, poses: torch.Tensor,
+               present: torch.Tensor, *, pcld: torch.Tensor = None, point_labels: torch.Tensor = None,
+               label_image: torch.Tensor = None):
+        """depth [B,H,W] f32, K [B,3,3] f32, cam_scale [B] f32, poses [B,n_cls,3,4] f32 and present
+        [B,n_cls] u8 (FramePoseSolver.solve()), and the labels as either
+          pcld [B,N,3] f32 + point_labels [B,N] i32: the network's sampled cloud and its labels (the
+            solver's new_mask, or seg_argmax), filled to every pixel (eval_icp's fill_label_item); or
+          label_image [B,H,W] integer: a label per pixel (eval_icp's eval_item, the ground-truth mask).
+        Returns IcpRefiner.refine's (poses f64, iters, err, refined), views of refiner-owned buffers.
+        Everything runs on the current stream; no host sync."""
+        b = depth.size(0) if depth.dim() == 3 else -1
+        if not (1 <= b <= self.b and depth.shape[1:] == (self.h, self.w)):
+            raise ValueError(f"DepthIcpRefiner.refine: depth must be [B<={self.b},{self.h},{self.w}], "
+                             f"got {tuple(depth.shape)}")
+        if (label_image is None) == (pcld is None and point_labels is None):
+            raise ValueError("DepthIcpRefiner.refine: pass either pcld and point_labels, or label_image")
+        if label_image is None and (pcld is None or point_labels is None):
+            raise ValueError("DepthIcpRefiner.refine: pcld and point_labels go together")
+        cloud, valid, labels = self.cloud[:b], self.valid[:b], self.labels[:b]
+        with torch.cuda.device(self.dev):
+            depth_to_cloud(depth, K, cam_scale, out=(cloud, valid))
+            if label_image is None:
+                fill_label(cloud, valid, pcld, point_labels, out=labels)
+            else:
+                if label_image.shape != (b, self.h, self.w) or label_image.device != self.dev:
+                    raise ValueError(f"DepthIcpRefiner.refine: label_image must be [{b},{self.h},{self.w}] on "
+                                     f"{self.dev}")
+                torch.mul(label_image.reshape(b, -1), valid, out=labels)
+            return self.icp.refine(cloud, labels, poses, present)
 
 
 def my_icp(A, B, init_pose=None, max_iterations=20, tolerance=0.001, device="cuda"):

@@ -215,6 +215,16 @@ def perturb_pose(R, t, angle_deg: float, offset: float, rng):
     return dR @ R, t + offset * d / np.linalg.norm(d)
 
 
+def _box_models(n_cls: int, model_pts: int, rng):
+    """per-class box extents [n_cls,3] (sorted descending, 3-12 cm) and surface models (None for class 0)"""
+    extents = np.zeros((n_cls, 3))
+    models = [None] * n_cls
+    for c in range(1, n_cls):
+        extents[c] = np.sort(rng.uniform(0.03, 0.12, size=3))[::-1]
+        models[c] = box_surface(extents[c], model_pts, rng)
+    return extents, models
+
+
 def make_icp_batch(batch: int, n_obj: int, pts_per_obj: int, seed: int = 0, n_cls: int = fixtures.YCB_N_CLASSES,
                    model_pts: int = 3000, noise: float = 0.001, outlier_frac: float = 0.0, n_bg: int = 2000,
                    angle_deg: float = 5.0, offset: float = 0.01, n_stray: int = 0) -> dict:
@@ -229,11 +239,7 @@ def make_icp_batch(batch: int, n_obj: int, pts_per_obj: int, seed: int = 0, n_cl
     pcld [B,N,3] f32, mask [B,N] i32, gt [B,n_cls,3,4] f64, init [B,n_cls,3,4] f32 (gt perturbed by
     angle_deg / offset; identity for absent classes), present [B,n_cls] u8)."""
     rng = np.random.default_rng(seed)
-    extents = np.zeros((n_cls, 3))
-    models = [None] * n_cls
-    for c in range(1, n_cls):
-        extents[c] = np.sort(rng.uniform(0.03, 0.12, size=3))[::-1]
-        models[c] = box_surface(extents[c], model_pts, rng)
+    extents, models = _box_models(n_cls, model_pts, rng)
     n = n_obj * (pts_per_obj + n_stray) + n_bg
     pcld = np.zeros((batch, n, 3), np.float32)
     mask = np.zeros((batch, n), np.int32)
@@ -273,3 +279,94 @@ def make_icp_batch(batch: int, n_obj: int, pts_per_obj: int, seed: int = 0, n_cl
         pcld[b] = np.concatenate(pts, 0)[order]
         mask[b] = np.concatenate(lab, 0)[order]
     return dict(models=models, extents=extents, pcld=pcld, mask=mask, gt=gt, init=init, present=present)
+
+
+def _ray_box_depth(R, t, extents, dirs):
+    """depth (camera z) of the first hit of rays dirs [P,3] (z component 1, from the origin) on the box
+    (pose R, t), inf where they miss"""
+    o = -(R.T @ t)                                   # camera origin in the object frame
+    d = dirs @ R                                     # ray directions in the object frame
+    half = 0.5 * np.asarray(extents, np.float64)
+    with np.errstate(divide="ignore", invalid="ignore"):
+        t1 = (-half - o) / d
+        t2 = (half - o) / d
+    tmin = np.nanmax(np.minimum(t1, t2), axis=1)
+    tmax = np.nanmin(np.maximum(t1, t2), axis=1)
+    return np.where((tmax >= tmin) & (tmin > 0), tmin, np.inf)
+
+
+def make_icp_depth_batch(batch: int, n_obj: int = 5, seed: int = 0, n_cls: int = fixtures.YCB_N_CLASSES,
+                         n_sample: int = fixtures.N_SAMPLE_POINTS, height: int = H, width: int = W,
+                         model_pts: int = 3000, noise: float = 0.001, hole_frac: float = 0.02, n_hole_boxes: int = 3,
+                         flip_frac: float = 0.03, angle_deg: float = 5.0, offset: float = 0.01,
+                         cam_scale: float = 10000.0) -> dict:
+    """Full-resolution inputs for DepthIcpRefiner: the box models of make_icp_batch(seed=seed) and, per
+    frame, n_obj distinct classes under random poses (the same layout as make_icp_batch) ray-cast into a
+    depth image over a background plane at z = 1.2 m (label 0), with N(0, noise) depth noise, stored as
+    a depth PNG would be (round(z * cam_scale), float32), hole_frac of the pixels and n_hole_boxes
+    rectangles zeroed (no depth), and the YCB intrinsics K_YCB1 (float32).  The network's input is
+    stood in for by n_sample valid pixels in raster order, back-projected as Basic_Utils.dpt_2_cld does,
+    with the ground-truth labels except that flip_frac * n_sample of the points near object borders
+    take the label of a neighbouring region.  Returns dict(models, extents, depth [B,H,W] f32,
+    K [B,3,3] f32, cam_scale [B] f32, label [B,H,W] i32 (ground truth, also where depth is missing),
+    gt [B,n_cls,3,4] f64, init [B,n_cls,3,4] f32 (gt perturbed; identity for absent classes),
+    present [B,n_cls] u8, pcld [B,n_sample,3] f32, labels [B,n_sample] i32, choose [B,n_sample] i64)."""
+    rng = np.random.default_rng(seed)
+    extents, models = _box_models(n_cls, model_pts, rng)
+    h, w = int(height), int(width)
+    K = K_YCB1.astype(np.float32)
+    fx, fy, cx, cy = (float(K[0, 0]), float(K[1, 1]), float(K[0, 2]), float(K[1, 2]))
+    v, u = np.mgrid[0:h, 0:w]
+    dirs = np.stack([((u - cx) / fx).ravel(), ((v - cy) / fy).ravel(), np.ones(h * w)], 1)
+    rows = np.repeat(np.arange(h, dtype=np.float32), w)
+    cols = np.tile(np.arange(w, dtype=np.float32), h)
+    out = dict(models=models, extents=extents, depth=np.zeros((batch, h, w), np.float32),
+               K=np.repeat(K[None], batch, 0), cam_scale=np.full(batch, cam_scale, np.float32),
+               label=np.zeros((batch, h, w), np.int32), gt=np.zeros((batch, n_cls, 3, 4)),
+               init=np.zeros((batch, n_cls, 3, 4), np.float32), present=np.zeros((batch, n_cls), np.uint8),
+               pcld=np.zeros((batch, n_sample, 3), np.float32), labels=np.zeros((batch, n_sample), np.int32),
+               choose=np.zeros((batch, n_sample), np.int64))
+    out["init"][:, :, :3, :3] = np.eye(3, dtype=np.float32)
+    out["gt"][:, :, :3, :3] = np.eye(3)
+    grid = [(-0.15, -0.1), (0.0, -0.1), (0.15, -0.1), (-0.15, 0.1), (0.0, 0.1), (0.15, 0.1), (-0.3, 0.0), (0.3, 0.0)]
+    for b in range(batch):
+        z = np.full(h * w, 1.2)
+        lab = np.zeros(h * w, np.int32)
+        for k, c in enumerate(np.sort(rng.choice(np.arange(1, n_cls), size=n_obj, replace=False))):
+            R = _haar_rotation(rng)
+            gx, gy = grid[k % len(grid)]
+            t = np.array([gx, gy, rng.uniform(0.6, 1.0)])
+            hit = _ray_box_depth(R, t, extents[c], dirs)
+            closer = hit < z
+            z = np.where(closer, hit, z)
+            lab = np.where(closer, c, lab)
+            out["gt"][b, c, :, :3], out["gt"][b, c, :, 3] = R, t
+            Ri, ti = perturb_pose(R, t, angle_deg, offset, rng)
+            out["init"][b, c, :, :3], out["init"][b, c, :, 3] = Ri, ti
+            out["present"][b, c] = 1
+        dpt = np.round((z + rng.normal(0.0, noise, size=z.shape)) * cam_scale).astype(np.float32)
+        dpt[rng.random(h * w) < hole_frac] = 0.0
+        dpt = dpt.reshape(h, w)
+        for _ in range(n_hole_boxes):
+            y0, x0 = int(rng.integers(0, h)), int(rng.integers(0, w))
+            dpt[y0:y0 + int(rng.integers(5, 30)), x0:x0 + int(rng.integers(5, 30))] = 0.0
+        lab = lab.reshape(h, w)
+        out["depth"][b], out["label"][b] = dpt, lab
+        # the sampled cloud: dpt_2_cld's float32 arithmetic at n_sample valid pixels, raster order
+        valid = np.nonzero(dpt.ravel() > np.float32(1e-6))[0]
+        choose = np.sort(rng.choice(valid, size=n_sample, replace=False))
+        pt2 = dpt.ravel()[choose] / np.float32(cam_scale)
+        out["pcld"][b] = np.stack([((cols[choose] - K[0, 2]) * pt2) / K[0, 0],
+                                   ((rows[choose] - K[1, 2]) * pt2) / K[1, 1], pt2], 1)
+        out["choose"][b] = choose
+        # segmentation errors at borders: the label of a region 4 px away, where it differs
+        other = np.zeros((h, w), np.int32)
+        for dy, dx in ((0, 4), (0, -4), (4, 0), (-4, 0)):
+            sh = np.roll(lab, (dy, dx), axis=(0, 1))
+            other = np.where((other == 0) & (sh != lab), sh + 1, other)    # +1: tells label 0 from none
+        border = np.nonzero(other.ravel()[choose] > 0)[0]
+        pl = lab.ravel()[choose].copy()
+        flip = rng.choice(border, size=min(len(border), int(round(flip_frac * n_sample))), replace=False)
+        pl[flip] = other.ravel()[choose[flip]] - 1
+        out["labels"][b] = pl
+    return out
