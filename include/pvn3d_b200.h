@@ -249,8 +249,8 @@ int pvn3d_mlp_sa_fact2w_supported(const pvn3d_mlp_layer_t *layer2, const pvn3d_m
  * Both layers apply ReLU; flags: PVN3D_MLP_ROUND_OUT (output) and PVN3D_MLP_RESERVE_SMS(n).  Weight pointers must be
  * 16-byte aligned (else PVN3D_ERR_INVALID_ARG, before any CUDA call).
  * PVN3D_ERR_UNSUPPORTED (nothing launched) unless pvn3d_mlp_fp2_supported(layer1, layer2) is 1: layer1->n_pad 256 or
- * 512, layer2->k_pad == layer1->n_pad, layer2->n_pad a multiple of 128, and the layer-1 tile, four operand stages and
- * three weight stages within a block's shared memory.  The query is host-only and touches no device memory. */
+ * 512, layer2->k_pad == layer1->n_pad, layer2->n_pad a multiple of 128, and the layer-1 tile, three operand stages and
+ * four weight stages within a block's shared memory.  The query is host-only and touches no device memory. */
 int pvn3d_mlp_fp2(const float *known_feat_pm, int c2, const int *nn_idx, const float *nn_w, const float *skip_pm, int lds,
                   int c1, int b, int n_unknown, int m_known, const pvn3d_mlp_layer_t *layer1, const pvn3d_mlp_layer_t *layer2,
                   int flags, float *out, int ldo, int col0, pvn3d_stream_t stream);

@@ -1938,16 +1938,17 @@ __global__ void __launch_bounds__(kFp2Threads, 1) mlp_fp2_kernel(const __grid_co
 
 // pvn3d_mlp_fp2's ring stages for a module (A ring, weight ring); false: the module is not covered -- a first layer of
 // other than 256 or 512 columns, a second layer not a multiple of 128 columns, a layer-2 K other than the layer-1
-// width, or H + four A stages + three weight stages beyond the shared memory of a block
+// width, or H + three A stages + four weight stages beyond the shared memory of a block
 bool fp2_stages(int k1_pad, int n1_pad, int k2_pad, int n2_pad, int *a_stages, int *w_stages) {
   if ((n1_pad != 256 && n1_pad != 512) || n2_pad <= 0 || n2_pad % 128 || k2_pad != n1_pad || k1_pad <= 0 || k1_pad % 32)
     return false;
   const uint32_t fixed = fp2_smem(k2_pad, 0, 0).bytes;
-  const uint32_t least = 4u * kFp2AStageBytes + 3u * kFp2WStageBytes;
+  const uint32_t least = 3u * kFp2AStageBytes + 4u * kFp2WStageBytes;
   if (fixed + least > static_cast<uint32_t>(kMlpSmemMax)) return false;
-  // the A ring first (the gathering producers are the slower side), at least three weight stages
+  // at least four weight stages -- with three, each warpgroup has one chunk of look-ahead and the ring's round trip
+  // stalls it (N1 = 512 beside the 128 KB H tile: 3 A + 4 W stages, not 5 A + 3 W) -- then the A ring, then the rest
   const uint32_t avail = static_cast<uint32_t>(kMlpSmemMax) - fixed;
-  const int sa = std::min<int>(kFp2MaxStages, static_cast<int>((avail - 3u * kFp2WStageBytes) / kFp2AStageBytes));
+  const int sa = std::min<int>(kFp2MaxStages, static_cast<int>((avail - 4u * kFp2WStageBytes) / kFp2AStageBytes));
   const int sw = std::min<int>(kFp2MaxStages, static_cast<int>((avail - static_cast<uint32_t>(sa) * kFp2AStageBytes) / kFp2WStageBytes));
   *a_stages = sa;
   *w_stages = sw;
