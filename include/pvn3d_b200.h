@@ -264,6 +264,20 @@ int pvn3d_mlp_fp2_supported(const pvn3d_mlp_layer_t *layer1, const pvn3d_mlp_lay
 int pvn3d_mlp_fp_fact(const float *p, const float *s, int ld, int c_valid, const int *nn_idx, const float *nn_w,
                       int b, int n_unknown, int m_known, const float *w, const float *bias, int k_pad, int n_pad,
                       int flags, float *out, int ldo, int col0, pvn3d_stream_t stream);
+/* The skip term and the second layer of a factored FP module whose skip is an SA factor table (FP1), in one launch:
+ * S never goes through HBM.  Same result, bit for bit, as
+ *   pvn3d_mlp_dense(table, k, k, b*n_unknown, layer_s, PVN3D_MLP_A_TF32) -> s    (k = layer_s->k_pad, no ReLU)
+ *   pvn3d_mlp_fp_fact(p, s, 128, 128, nn_idx, nn_w, b, n_unknown, m_known, layer2,
+ *                     PVN3D_MLP_RELU | PVN3D_MLP_OUT_CN) -> out [b][128][n_unknown]
+ * for ANY n_unknown (a tile may hold the end of one frame and the start of the next).
+ *   p [b*m_known, 128], table [b*n_unknown, 32] TF32-rounded (pvn3d_sa_factor_table), both 16-byte aligned.
+ * flags: PVN3D_MLP_RESERVE_SMS(n) only.  Pointers not 16-byte aligned or other flags: PVN3D_ERR_INVALID_ARG, before any
+ * CUDA call.  PVN3D_ERR_UNSUPPORTED (nothing launched) unless pvn3d_mlp_fp_fact2_supported(layer_s, layer2) is 1:
+ * layer_s 32 -> 128 (k_pad 32, n_pad 128) and layer2 128 -> 128.  The query is host-only and touches no device memory. */
+int pvn3d_mlp_fp_fact2(const float *p, const float *table, const int *nn_idx, const float *nn_w, int b, int n_unknown,
+                       int m_known, const pvn3d_mlp_layer_t *layer_s, const pvn3d_mlp_layer_t *layer2, int flags, float *out,
+                       pvn3d_stream_t stream);
+int pvn3d_mlp_fp_fact2_supported(const pvn3d_mlp_layer_t *layer_s, const pvn3d_mlp_layer_t *layer2);
 /* weight[p,0:3] = (1/(sqrt(dist2)+1e-8)) / sum  (pointnet2_modules.py:184-186), fp32 IEEE ops */
 int pvn3d_three_nn_weights(const float *dist2, long long rows, float *weight, pvn3d_stream_t stream);
 

@@ -1976,6 +1976,261 @@ int launch_fp2(Fp2Args &g, cudaStream_t st) {
   return check_launch("mlp_fp2_kernel");
 }
 
+// =====================================================================================================
+// The skip term and the second layer of a FACTORED FP module whose skip is the SA1 factor table (FP1), in ONE
+// persistent kernel.
+//
+// As two launches (pvn3d_mlp_dense for S = W1s . table + b1, then pvn3d_mlp_fp_fact with OUT_CN) S goes to HBM and
+// straight back: 201 + 201 MB per 32-frame batch of 12288 points.  Here it never leaves the SM.  Per 64-row tile:
+//   loader    (warp 16)     brings W_s and W2 into shared memory once (TMA), then the tile's 32-column table rows by
+//                           TMA (SWIZZLE_128B: the wgmma layout) into a ring slot;
+//   producers (warps 0-7)   warp w gathers K chunk w / 2 of rows 32 (w & 1).. : sum_t w_t P[idx_t] (fp32, unrounded)
+//                           into the slot's K-major SWIZZLE_128B operand tile, row state in shared memory as
+//                           mlp_fp2_kernel keeps it;
+//   MMA       (warps 8-15)  warpgroup wg takes the slots it % 2 == wg: S = table . W_s^T (wgmma m64n128k8, the four K
+//                           steps of the 32 columns) into registers, then in place over its fragment of the operand
+//                           tile tf32(relu(interp + (S + b1))) (dead rows zero), fence.proxy.async, layer 2 from the
+//                           tile (W2 resident, K 0..127), the slot released, relu(acc + b2) stored channel-major
+//                           [b][128][n_unknown] from the fragment: the 8 rows of a lane quad are 8 consecutive points,
+//                           whole 32-byte sectors of one channel.
+// Every output element keeps the operands, the wgmma shape, K order and epilogue arithmetic of the two launches, so
+// the results are bit-identical.
+constexpr int kFpf2BM = 64;
+constexpr int kFpf2ProWarps = 8;
+constexpr int kFpf2LoaderWarp = kFpf2ProWarps + kMlpMmaWarps;   // warp 16
+constexpr int kFpf2Threads = (kFpf2LoaderWarp + 1) * 32;
+constexpr int kFpf2MaxStages = 4;
+constexpr uint32_t kFpf2AChunk = kFpf2BM * 128u;                 // one K chunk of the operand tile: 64 rows x 32 fp32
+constexpr uint32_t kFpf2ABytes = 4u * kFpf2AChunk;               // the operand tile: 64 rows x K 128
+constexpr uint32_t kFpf2TBytes = kFpf2BM * 128u;                 // the table rows of a tile: 64 x 32 fp32
+
+struct FpFact2Args {
+  MlpArgs a;   // PRO_FP_INTERP row fields (known_feat = P, c2 = 128, nn_idx, nn_w, n_unknown, m_known, rows), out; tmap: table
+  alignas(64) CUtensorMap tmap_s, tmap_w2;
+  const float *bias_s, *bias2;
+};
+
+struct FpFact2SmemCtl {
+  uint64_t t_full[kFpf2MaxStages];   // the loader's arrive.expect_tx + the TMA bytes of the slot's table rows
+  uint64_t a_full[kFpf2MaxStages];   // 256 arrivals: every producer thread, once its part of the operand tile is stored
+  uint64_t empty[kFpf2MaxStages];    // 4 arrivals: the warps of the warpgroup that consumed the slot
+  uint64_t w_full;                   // the loader's arrive.expect_tx + the TMA bytes of W_s and W2
+};
+
+// shared-memory layout behind the 1024-byte aligned base (kernel, launcher and pvn3d_mlp_fp_fact2_supported use the
+// same function): [W2: 4 chunks of 128 x 128 B][W_s: 128 x 128 B][operand tiles: stages x 32 KB][table rows: stages x
+// 8 KB][row states: 32 B per row of each producer warp][barriers]
+struct FpFact2Smem {
+  uint32_t w2, ws, a, t, rows, ctl, bytes;   // offsets from the aligned base; bytes = dynamic size incl. alignment slack
+};
+static inline __host__ __device__ FpFact2Smem fpf2_smem(int stages) {
+  FpFact2Smem s;
+  s.w2 = 0;
+  s.ws = s.w2 + 4u * 128u * 128u;
+  s.a = s.ws + 128u * 128u;
+  s.t = s.a + static_cast<uint32_t>(stages) * kFpf2ABytes;
+  s.rows = s.t + static_cast<uint32_t>(stages) * kFpf2TBytes;
+  s.ctl = s.rows + kFpf2ProWarps * 32u * 32u;
+  s.bytes = 1024u + s.ctl + static_cast<uint32_t>(sizeof(FpFact2SmemCtl));
+  return s;
+}
+// ring slots pvn3d_mlp_fp_fact2 runs with (3: 209 KB); 0 if the layers are not covered (a skip layer other than K 32 ->
+// 128, a second layer other than 128 -> 128)
+int fpf2_stages(int ks_pad, int ns_pad, int k2_pad, int n2_pad) {
+  if (ks_pad != 32 || ns_pad != 128 || k2_pad != 128 || n2_pad != 128) return 0;
+  const uint32_t fixed = fpf2_smem(0).bytes;
+  const int stages = std::min<int>(kFpf2MaxStages, static_cast<int>((kMlpSmemMax - fixed) / (kFpf2ABytes + kFpf2TBytes)));
+  return stages >= 2 ? stages : 0;
+}
+
+// K chunk k0 / 32 of the producer's 8 rows: sum_t w_t P[idx_t] with the contraction of stage_a_chunk<PRO_FP_FACT>,
+// fma(p3,w3, fma(p1,w1, p2*w2)), stored unrounded (the MMA warpgroup adds S, applies the ReLU and rounds); dead rows 0
+__device__ __forceinline__ void fpf2_stage_chunk(const MlpArgs &a, uint32_t rst, int r_first, int sub, int k0, uint32_t sa) {
+  const float *kf = a.known_feat + k0 + 4 * sub;
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {  // two halves: 12 LDG.128 in flight each
+    float4 p1[4], p2[4], p3[4];
+#pragma unroll
+    for (int jj = 0; jj < 4; ++jj) {
+      const int4 gi = lds128i(rst + 128u * (h * 4 + jj));
+      p1[jj] = ldg128(kf + static_cast<size_t>(gi.x) * a.c2);
+      p2[jj] = ldg128(kf + static_cast<size_t>(gi.y) * a.c2);
+      p3[jj] = ldg128(kf + static_cast<size_t>(gi.z) * a.c2);
+    }
+#pragma unroll
+    for (int jj = 0; jj < 4; ++jj) {
+      const int j = h * 4 + jj;
+      const float4 w = lds128(rst + 128u * j + 16u);
+      float4 v;
+      v.x = __fmaf_rn(p3[jj].x, w.z, __fmaf_rn(p1[jj].x, w.x, __fmul_rn(p2[jj].x, w.y)));
+      v.y = __fmaf_rn(p3[jj].y, w.z, __fmaf_rn(p1[jj].y, w.x, __fmul_rn(p2[jj].y, w.y)));
+      v.z = __fmaf_rn(p3[jj].z, w.z, __fmaf_rn(p1[jj].z, w.x, __fmul_rn(p2[jj].z, w.y)));
+      v.w = __fmaf_rn(p3[jj].w, w.z, __fmaf_rn(p1[jj].w, w.x, __fmul_rn(p2[jj].w, w.y)));
+      if (w.w == 0.f) v = make_float4(0.f, 0.f, 0.f, 0.f);
+      sts128(sa + sw128_off(r_first + 4 * j, sub), v.x, v.y, v.z, v.w);
+    }
+  }
+}
+
+__global__ void __launch_bounds__(kFpf2Threads, 1) mlp_fp_fact2_kernel(const __grid_constant__ FpFact2Args g) {
+  const MlpArgs &a = g.a;
+  extern __shared__ unsigned char mlp_smem_raw[];
+  const uint32_t raw = smem_u32(mlp_smem_raw);
+  const uint32_t base = (raw + 1023u) & ~1023u;   // SWIZZLE_128B atoms are 8 rows x 128 B
+  const int S = a.stages;
+  const FpFact2Smem L = fpf2_smem(S);
+  FpFact2SmemCtl &ctl = *reinterpret_cast<FpFact2SmemCtl *>(mlp_smem_raw + (base - raw) + L.ctl);
+  const int t = threadIdx.x;
+  const unsigned warp = t >> 5, lane = t & 31u;
+  const int tiles = static_cast<int>((a.rows + kFpf2BM - 1) / kFpf2BM);   // the launcher checks tiles < 2^31
+
+  if (t == 0) {
+    for (int s = 0; s < S; ++s) {
+      mbar_init(&ctl.t_full[s], 1);
+      mbar_init(&ctl.a_full[s], kFpf2ProWarps * 32);
+      mbar_init(&ctl.empty[s], 4);
+    }
+    mbar_init(&ctl.w_full, 1);
+    mbar_fence_init();
+  }
+  __syncthreads();
+
+  if (warp < kFpf2ProWarps) {
+    // ================= producers: warp w stages K chunk w / 2 of rows 32 (w & 1) .. +31 of every tile ============
+    const int kc = static_cast<int>(warp >> 1);
+    const int sub = static_cast<int>(lane & 7u), r_first = 32 * static_cast<int>(warp & 1u) + static_cast<int>(lane >> 3);
+    const uint32_t rst = base + L.rows + warp * 1024u + (lane >> 3) * 32u;
+    int it = 0;
+    for (int tile = blockIdx.x; tile < tiles; tile += gridDim.x, ++it) {
+      const int s = it % S;
+      const long long p_first = static_cast<long long>(tile) * kFpf2BM + r_first;
+      {
+        RowState rs;
+        rows_setup<PRO_FP_INTERP>(a, p_first, rs);
+        __syncwarp();   // every lane is done with the previous tile's row state
+        fp2_rows_store(rs, rst, static_cast<unsigned>(sub));
+        __syncwarp();
+      }
+      mbar_wait(&ctl.empty[s], static_cast<unsigned>(((it / S) & 1) ^ 1));
+      fpf2_stage_chunk(a, rst, r_first, sub, kc * 32, base + L.a + static_cast<uint32_t>(s) * kFpf2ABytes + kc * kFpf2AChunk);
+      mbar_arrive(&ctl.a_full[s]);
+    }
+  } else if (warp == kFpf2LoaderWarp) {
+    // ================= loader: the resident weights once, then every tile's table rows, in ring order ==========
+    if (lane == 0) {
+      mbar_expect_tx(&ctl.w_full, 5u * 128u * 128u);
+      tma_load_2d(base + L.ws, &g.tmap_s, 0, 0, &ctl.w_full);
+      for (int kc = 0; kc < 4; ++kc) tma_load_2d(base + L.w2 + kc * 128u * 128u, &g.tmap_w2, kc * 32, 0, &ctl.w_full);
+      int it = 0;
+      for (int tile = blockIdx.x; tile < tiles; tile += gridDim.x, ++it) {
+        const int s = it % S;
+        mbar_wait(&ctl.empty[s], static_cast<unsigned>(((it / S) & 1) ^ 1));
+        mbar_expect_tx(&ctl.t_full[s], kFpf2TBytes);   // a ragged last tile: TMA fills the rows past the end with zeros
+        tma_load_2d(base + L.t + static_cast<uint32_t>(s) * kFpf2TBytes, &a.tmap, 0, tile * kFpf2BM, &ctl.t_full[s]);
+      }
+    }
+  } else {
+    // ================= MMA + epilogue: warpgroup wg takes the slots it % 2 == wg, warp w4 rows 16 w4 .. +15 =======
+    const unsigned mw = warp - kFpf2ProWarps, wg = mw >> 2, w4 = mw & 3u;
+    const int frag_row = static_cast<int>(16 * w4 + (lane >> 2));
+    const uint64_t ws_desc = smem_desc_sw128(base + L.ws);
+    const long long n_unk = a.n_unknown;
+    float d[64];
+    mbar_wait(&ctl.w_full, 0u);
+    int it = static_cast<int>(wg);
+    for (int tile = blockIdx.x + static_cast<int>(wg) * gridDim.x; tile < tiles; tile += 2 * gridDim.x, it += 2) {
+      const int s = it % S;
+      const unsigned par = static_cast<unsigned>((it / S) & 1);
+      const uint32_t a_s = base + L.a + static_cast<uint32_t>(s) * kFpf2ABytes;
+      // ---- S = table . W_s^T: the MMA of pvn3d_mlp_dense (K 32: four k8 steps, zero columns included)
+      mbar_wait(&ctl.t_full[s], par);
+      {
+        const uint64_t tdesc = smem_desc_sw128(base + L.t + static_cast<uint32_t>(s) * kFpf2TBytes);
+        wgmma_fence();
+#pragma unroll
+        for (int k4 = 0; k4 < 4; ++k4)
+          wgmma_tf32<128>(d, tdesc + static_cast<uint64_t>(k4 * 2), ws_desc + static_cast<uint64_t>(k4 * 2), k4 > 0 ? 1u : 0u);
+        wgmma_commit();
+        wgmma_wait<0>();
+        acc_fence(d);
+      }
+      // ---- the layer-2 operand in place: tf32(relu(interp + (S + b1))), the producer of pvn3d_mlp_fp_fact
+      const long long r0 = static_cast<long long>(tile) * kFpf2BM + frag_row;
+      const bool on0 = r0 < a.rows, on1 = r0 + 8 < a.rows;
+      mbar_wait(&ctl.a_full[s], par);
+#pragma unroll
+      for (int j = 0; j < 16; ++j) {
+        const int c = 8 * j + 2 * static_cast<int>(lane & 3u);
+        const float b0 = __ldg(g.bias_s + c), b1 = __ldg(g.bias_s + c + 1);
+        const uint32_t off = static_cast<uint32_t>(c >> 5) * kFpf2AChunk + static_cast<uint32_t>(frag_row) * 128u +
+                             ((static_cast<uint32_t>(((c & 31) >> 2) ^ (frag_row & 7))) << 4) + (c & 3) * 4u;
+        float x0, x1, y0, y1;
+        asm volatile("ld.shared.v2.f32 {%0,%1}, [%2];" : "=f"(x0), "=f"(x1) : "r"(a_s + off));
+        asm volatile("ld.shared.v2.f32 {%0,%1}, [%2];" : "=f"(y0), "=f"(y1) : "r"(a_s + off + 8u * 128u));
+        x0 = on0 ? to_tf32(fmaxf(x0 + (d[4 * j] + b0), 0.f)) : 0.f;
+        x1 = on0 ? to_tf32(fmaxf(x1 + (d[4 * j + 1] + b1), 0.f)) : 0.f;
+        y0 = on1 ? to_tf32(fmaxf(y0 + (d[4 * j + 2] + b0), 0.f)) : 0.f;
+        y1 = on1 ? to_tf32(fmaxf(y1 + (d[4 * j + 3] + b1), 0.f)) : 0.f;
+        asm volatile("st.shared.v2.f32 [%0], {%1,%2};" ::"r"(a_s + off), "f"(x0), "f"(x1) : "memory");
+        asm volatile("st.shared.v2.f32 [%0], {%1,%2};" ::"r"(a_s + off + 8u * 128u), "f"(y0), "f"(y1) : "memory");
+      }
+      fence_proxy_async_smem();   // generic-proxy stores of the operand -> visible to the tensor core
+      named_bar_sync(1 + static_cast<int>(wg), 128);
+      // ---- layer 2: K 0..127 in order against the resident W2
+      wgmma_fence();
+#pragma unroll
+      for (int kc = 0; kc < 4; ++kc) {
+        const uint64_t adesc = smem_desc_sw128(a_s + static_cast<uint32_t>(kc) * kFpf2AChunk);
+        const uint64_t bdesc = smem_desc_sw128(base + L.w2 + static_cast<uint32_t>(kc) * 128u * 128u);
+#pragma unroll
+        for (int k4 = 0; k4 < 4; ++k4)
+          wgmma_tf32<128>(d, adesc + static_cast<uint64_t>(k4 * 2), bdesc + static_cast<uint64_t>(k4 * 2), (kc > 0 || k4 > 0) ? 1u : 0u);
+      }
+      wgmma_commit();
+      wgmma_wait<0>();
+      acc_fence(d);
+      if (lane == 0) mbar_arrive(&ctl.empty[s]);   // the slot (operand tile and table rows) may be refilled
+      // ---- out[b][c][i] = relu(acc + b2[c]): a lane quad's rows are 8 consecutive points of one channel
+      const long long fb0 = r0 / n_unk, fb1 = (r0 + 8) / n_unk;
+      float *o0 = a.out + fb0 * 128 * n_unk + (r0 - fb0 * n_unk);
+      float *o1 = a.out + fb1 * 128 * n_unk + (r0 + 8 - fb1 * n_unk);
+#pragma unroll
+      for (int j = 0; j < 16; ++j) {
+        const int c = 8 * j + 2 * static_cast<int>(lane & 3u);
+        const float b0 = __ldg(g.bias2 + c), b1 = __ldg(g.bias2 + c + 1);
+        if (on0) {
+          stg_stream(o0 + c * n_unk, fmaxf(d[4 * j] + b0, 0.f));
+          stg_stream(o0 + (c + 1) * n_unk, fmaxf(d[4 * j + 1] + b1, 0.f));
+        }
+        if (on1) {
+          stg_stream(o1 + c * n_unk, fmaxf(d[4 * j + 2] + b0, 0.f));
+          stg_stream(o1 + (c + 1) * n_unk, fmaxf(d[4 * j + 3] + b1, 0.f));
+        }
+      }
+    }
+  }
+}
+
+int launch_fp_fact2(FpFact2Args &g, const float *table, const float *ws, const float *w2, cudaStream_t st) {
+  MlpArgs &a = g.a;
+  if (a.rows <= 0) return PVN3D_OK;
+  const size_t smem = fpf2_smem(a.stages).bytes;
+  const long long tiles = (a.rows + kFpf2BM - 1) / kFpf2BM;
+  // the kernel counts tiles and ring items in 32 bits; TMA addresses table rows with a 32-bit coordinate
+  if (tiles * kFpf2BM > 0x7fffffffll) return PVN3D_ERR_UNSUPPORTED;
+  if (!weight_tensor_map(&a.tmap, table, 32, static_cast<int>(a.rows), kFpf2BM) ||
+      !weight_tensor_map(&g.tmap_s, ws, 32, 128, 128) || !weight_tensor_map(&g.tmap_w2, w2, 128, 128, 128))
+    return PVN3D_ERR_UNSUPPORTED;
+  const int sms = std::max(1, sm_count() - a.reserve_sms);
+  auto kern = mlp_fp_fact2_kernel;
+  static PerDeviceOnce once;
+  PVN3D_ONCE_PER_DEVICE(once, cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, kMlpSmemMax),
+                        "mlp fp_fact2 smem attr");
+  const unsigned grid = static_cast<unsigned>(std::min<long long>(tiles, sms));
+  kern<<<grid, kFpf2Threads, smem, st>>>(g);
+  return check_launch("mlp_fp_fact2_kernel");
+}
+
 int dispatch(MlpArgs &a, int pro, int pool, cudaStream_t st) {
   if (pool) {
     if (pool != 8 && pool != 16 && pool != 32) return PVN3D_ERR_UNSUPPORTED;
@@ -2280,6 +2535,33 @@ extern "C" int pvn3d_mlp_fp_fact(const float *p, const float *s, int ld, int c_v
     return launch_mlp<PRO_FP_FACT, EPI_STORE_T>(a, as_stream(stream));
   }
   return dispatch(a, PRO_FP_FACT, 0, as_stream(stream));
+}
+
+extern "C" int pvn3d_mlp_fp_fact2(const float *p, const float *table, const int *nn_idx, const float *nn_w, int b,
+                                  int n_unknown, int m_known, const pvn3d_mlp_layer_t *layer_s,
+                                  const pvn3d_mlp_layer_t *layer2, int flags, float *out, pvn3d_stream_t stream) {
+  if (!p || !table || !nn_idx || !nn_w || !layer_s || !layer2 || !layer_s->w || !layer_s->bias || !layer2->w ||
+      !layer2->bias || !out || b < 0 || n_unknown < 0 || m_known <= 0 || (flags & ~0xff00) ||
+      (reinterpret_cast<uintptr_t>(p) & 15u) || (reinterpret_cast<uintptr_t>(table) & 15u) ||
+      (reinterpret_cast<uintptr_t>(layer_s->w) & 15u) || (reinterpret_cast<uintptr_t>(layer2->w) & 15u))
+    return PVN3D_ERR_INVALID_ARG;
+  const int stages = fpf2_stages(layer_s->k_pad, layer_s->n_pad, layer2->k_pad, layer2->n_pad);
+  if (!stages) return PVN3D_ERR_UNSUPPORTED;
+  if (static_cast<long long>(b) * m_known > 0x7fffffffll || n_unknown > 0x3fffffff) return PVN3D_ERR_UNSUPPORTED;
+  FpFact2Args g{};
+  MlpArgs &a = g.a;
+  a.rows = static_cast<long long>(b) * n_unknown;
+  a.known_feat = p; a.c2 = layer_s->n_pad; a.nn_idx = nn_idx; a.nn_w = nn_w;
+  a.n_unknown = n_unknown; a.m_known = m_known;
+  a.out = out; a.stages = stages;
+  a.reserve_sms = (flags >> 8) & 0xff;
+  g.bias_s = layer_s->bias; g.bias2 = layer2->bias;
+  return launch_fp_fact2(g, table, layer_s->w, layer2->w, as_stream(stream));
+}
+
+extern "C" int pvn3d_mlp_fp_fact2_supported(const pvn3d_mlp_layer_t *layer_s, const pvn3d_mlp_layer_t *layer2) {
+  if (!layer_s || !layer2) return 0;
+  return fpf2_stages(layer_s->k_pad, layer_s->n_pad, layer2->k_pad, layer2->n_pad) ? 1 : 0;
 }
 
 extern "C" int pvn3d_mlp_dense_frame_bias(const float *a, int lda, int a_cols, long long rows, int rows_per_frame,

@@ -13,9 +13,9 @@ matrix + bias, and runs `Pointnet2MSG.forward` (reference pvn3d/lib/pvn3d.py:126
   per FP level : three_nn -> inverse-distance weights ->
                  FP2-4: both layers in ONE launch (pvn3d_mlp_fp2): three_interpolate + concat fused into the
                         tensor-core operand producer, the layer-1 activations kept in shared memory
-                 FP1  : factored first layer (P = W1k . known, S = W1s . skip + b1 by pvn3d_mlp_dense) ->
-                        second layer on relu(interpolated P + S) (pvn3d_mlp_fp_fact), stored channel-major
-                        [B,128,N], the layout the reference returns (when N % 32 == 0; else a transpose follows)
+                 FP1  : factored first layer, P = W1k . known once per known point (pvn3d_mlp_dense) ->
+                        S = W1s . skip + b1 and the second layer on relu(interpolated P + S) in ONE launch
+                        (pvn3d_mlp_fp_fact2), stored channel-major [B,128,N], the layout the reference returns
 
 The grouped tensors [B,3+C,M,S] and the interpolated tensors [B,C,n] are never materialised; no
 cuDNN / cuBLAS / ATen kernel runs in this path.
@@ -245,6 +245,31 @@ def mlp_fp_fact(p: torch.Tensor, s_: torch.Tensor, nn_idx: torch.Tensor, nn_w: t
     return out
 
 
+def fp_fact2_fits(layer_s: PackedLayer, layer2: PackedLayer) -> bool:
+    """whether pvn3d_mlp_fp_fact2 takes a factored FP module (the library's own rule: a skip layer 32 -> 128 over an SA
+    factor table, a second layer 128 -> 128 -- FP1)"""
+    ls, l2 = _layer_struct(layer_s), _layer_struct(layer2)
+    return bool(_lib.load().pvn3d_mlp_fp_fact2_supported(ctypes.addressof(ls), ctypes.addressof(l2)))
+
+
+def mlp_fp_fact2(p: torch.Tensor, table: torch.Tensor, nn_idx: torch.Tensor, nn_w: torch.Tensor, m_known: int,
+                 layer_s: PackedLayer, layer2: PackedLayer, reserve=0):
+    """the skip term and the second layer of a factored FP module in one launch (pvn3d_mlp_fp_fact2) -> [b, 128,
+    n_unknown]: the same bits as mlp_fp_fact(p, mlp_dense(table, layer_s, relu=False, a_tf32=True), .., layer2,
+    out_cn=True)"""
+    lib = _lib.load()
+    b, n_unknown = nn_idx.shape[0], nn_idx.shape[1]
+    assert p.size(-1) == layer_s.n_pad and table.size(-1) == layer_s.k_pad and table.size(0) == b * n_unknown
+    out = torch.empty((b, layer2.n_pad, n_unknown), dtype=torch.float32, device=p.device)
+    ls, l2 = _layer_struct(layer_s), _layer_struct(layer2)
+    with torch.cuda.device(p.device):
+        rc = lib.pvn3d_mlp_fp_fact2(ptr(p), ptr(table), ptr(nn_idx), ptr(nn_w), b, n_unknown, m_known,
+                                    ctypes.addressof(ls), ctypes.addressof(l2), _flags(False, reserve=reserve), ptr(out),
+                                    _stream(p.device))
+    check(rc, "pvn3d_mlp_fp_fact2")
+    return out
+
+
 def three_nn_weights(dist2: torch.Tensor) -> torch.Tensor:
     lib = _lib.load()
     w = torch.empty_like(dist2)
@@ -333,7 +358,11 @@ class FusedPointnet2MSG:
         lk = PackedLayer(w[:, :c2].contiguous(), torch.zeros_like(bias))
         ws = torch.cat([w[:, c2:], torch.zeros((w.size(0), 6), dtype=w.dtype, device=w.device)], dim=1)
         ls = PackedLayer(ws.contiguous(), bias)
-        self.fp1 = (lk, ls, PackedLayer(*fold_conv_bn(fp1[1]), lk.n_pad))
+        l2 = PackedLayer(*fold_conv_bn(fp1[1]), lk.n_pad) if len(fp1) == 2 else None
+        if l2 is None or not fp_fact2_fits(ls, l2):
+            raise ValueError(f"FP1: no fused kernel takes its skip term and second layer "
+                             f"({len(fp1)} layers, {ws.size(1)} skip columns -> {ls.n} channels)")
+        self.fp1 = (lk, ls, l2)
         self._marks = None
 
     def _m(self, family: str) -> None:
@@ -421,7 +450,7 @@ class FusedPointnet2MSG:
         MLP kernels leave free for kernels of other streams (the next batch's sampling); reserve_levels: the SA levels
         0 .. reserve_levels-1 do so (5: the FP modules too) -- the sampling of the next batch is over well before the
         MLPs are, and the later layers then take the whole machine."""
-        b, n0, width = pointcloud.shape
+        b, _, width = pointcloud.shape
         c0 = width - 3
         rs_all = int(reserve_sms)
         if not plan.ball:
@@ -462,25 +491,16 @@ class FusedPointnet2MSG:
             l_feat[i] = h.view(b, unknown.size(1), -1)
             self._m("mlp")
         # FP1, factored -- it pays only where the known descriptors are much wider than the layer and the skip is
-        # narrow: 256 + 6 -> 128 at 12288 points, 382 vs 420 us; FP2-4 measured 10-40 % SLOWER (DESIGN.md section 9)
+        # narrow: 256 + 6 -> 128 at 12288 points (DESIGN.md section 4)
         lk, ls, l2 = self.fp1
         nn_idx, nn_w = plan.nn[0]
         kf2d = l_feat[1].reshape(-1, l_feat[1].size(-1))
         assert kf2d.size(-1) == lk.k
         pk = mlp_dense(kf2d, lk, relu=False, reserve=rs)                                   # once per known point
-        sk = mlp_dense(table0, ls, relu=False, reserve=rs, a_tf32=True)
-        # the module's output IS the network's: written channel-major ([B,128,N]) straight from the accumulator
-        cn = l2.n_pad in (128, 256) and l2.n == l2.n_pad and n0 % 32 == 0
-        h = mlp_fp_fact(pk, sk, nn_idx, nn_w, l_xyz[1].size(1), l2, round_out=False, reserve=rs, out_cn=cn)
+        # S = W1s . table0 + b1 stays on chip; the module's output IS the network's, written channel-major ([B,128,N])
+        h = mlp_fp_fact2(pk, table0, nn_idx, nn_w, l_xyz[1].size(1), ls, l2, reserve=rs)
         self._m("mlp")
-        if cn:
-            return h
-        out_pm = h.view(b, n0, -1)
-        if out_pm.size(-1) != l2.n:
-            out_pm = out_pm[..., :l2.n].contiguous()
-        out = _ext.transpose_nc_to_cn(out_pm)
-        self._m("glue")
-        return out
+        return h if l2.n == l2.n_pad else h[:, :l2.n].contiguous()
 
     @torch.no_grad()
     def forward(self, pointcloud: torch.Tensor) -> torch.Tensor:

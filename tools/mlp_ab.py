@@ -28,7 +28,8 @@ if os.environ.get("AB_LAUNCHES", "1") == "1":
     with profile(activities=[ProfilerActivity.CUDA]) as prof:
         eng.features(cloud, plan)
         torch.cuda.synchronize()
-    ks = [e for e in prof.events() if any(k in e.name for k in ("mlp_layer_kernel", "mlp_sa_fact2_kernel", "mlp_sa_fact2w_kernel", "mlp_fp2_kernel"))]
+    ks = [e for e in prof.events() if any(k in e.name for k in ("mlp_layer_kernel", "mlp_sa_fact2_kernel", "mlp_sa_fact2w_kernel", "mlp_fp2_kernel",
+                                                                  "mlp_fp_fact2_kernel"))]
     ks.sort(key=lambda e: e.time_range.start)
     print("  launches us:", [round(e.device_time if hasattr(e, "device_time") else e.cuda_time) for e in ks], "sum",
           round(sum((e.device_time if hasattr(e, "device_time") else e.cuda_time) for e in ks)))
