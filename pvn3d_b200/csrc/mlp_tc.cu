@@ -1478,6 +1478,16 @@ __global__ void __launch_bounds__(kSa2wThreads, 1) mlp_sa_fact2w_kernel(const __
         const int cnt = sa2w_pair_blocks(nb2, pp);
         if (static_cast<int>(wg) < cnt) {
           const int nb = pp + static_cast<int>(wg);
+          // the bias of the lane's 32 columns, loaded before the block's MMAs so that they hide the loads' latency.
+          // The producers' gathers stream through L1, so these come from L2; loaded one pair per stored pair after
+          // the MMAs (as the break below forces), they held the tensor cores idle through 16 L2 round trips per block
+          float b2v[32];
+#pragma unroll
+          for (int jj = 0; jj < 16; ++jj) {
+            const int c = 128 * nb + 8 * jj + 2 * static_cast<int>(lane & 3u);
+            b2v[2 * jj] = c < n2 ? __ldg(a.bias + c) : 0.f;
+            b2v[2 * jj + 1] = c + 1 < n2 ? __ldg(a.bias + c + 1) : 0.f;
+          }
           sa2w_block(d, base + L.a, base + L.ring, S, it_base + static_cast<int>(wg), cnt, kc2, ctl.full, ctl.empty, ctl.a_full,
                      static_cast<unsigned>(j & 1), false, lane);
           // both warpgroups have finished the previous tile's layer 3 (its reads of H)
@@ -1489,7 +1499,7 @@ __global__ void __launch_bounds__(kSa2wThreads, 1) mlp_sa_fact2w_kernel(const __
             const int c = 128 * nb + 8 * jj + 2 * static_cast<int>(lane & 3u);
             if (c >= g.k3_pad) break;
             const bool on0 = c < n2, on1 = c + 1 < n2;
-            const float b0 = on0 ? __ldg(a.bias + c) : 0.f, b1 = on1 ? __ldg(a.bias + c + 1) : 0.f;
+            const float b0 = b2v[2 * jj], b1 = b2v[2 * jj + 1];
             const uint32_t off = static_cast<uint32_t>(c >> 5) * kSa2wChunk + static_cast<uint32_t>(frag_row) * 128u +
                                  ((static_cast<uint32_t>(((c & 31) >> 2) ^ (frag_row & 7))) << 4) + (c & 3) * 4u;
             asm volatile("st.shared.v2.f32 [%0], {%1,%2};" ::"r"(base + L.h + off),
@@ -1512,6 +1522,16 @@ __global__ void __launch_bounds__(kSa2wThreads, 1) mlp_sa_fact2w_kernel(const __
         const int cnt = sa2w_pair_blocks(nb3, pp);
         if (static_cast<int>(wg) < cnt) {
           const int nb = pp + static_cast<int>(wg);
+          // the bias of the four columns this lane may store, loaded before the MMAs as in layer 2; the column of
+          // p[i] after the butterfly: io = i + 16 b4 + 8 b3 + 4 b2 (lane bits 4, 3, 2), column 8 (io >> 1) + 2 (lane & 3) + (io & 1)
+          const unsigned b4 = (lane >> 4) & 1u, b3 = (lane >> 3) & 1u, b2 = (lane >> 2) & 1u;
+          float b3v[4];
+#pragma unroll
+          for (int i = 0; i < 4; ++i) {
+            const int io = i + (b4 ? 16 : 0) + (b3 ? 8 : 0) + (b2 ? 4 : 0);
+            const int col = 128 * nb + 8 * (io >> 1) + 2 * static_cast<int>(lane & 3u) + (io & 1);
+            b3v[i] = col < g.n3_pad ? __ldg(g.bias3 + col) : 0.f;
+          }
           const int last = sa2w_block(d, base + L.h, base + L.ring, S, it_base + static_cast<int>(wg), cnt, kc3, ctl.full, ctl.empty, nullptr, 0u,
                                       true, lane);
           // max over the warp's 16 rows: the lane's two rows, then a transposing butterfly over lane bits 4, 3, 2
@@ -1554,14 +1574,13 @@ __global__ void __launch_bounds__(kSa2wThreads, 1) mlp_sa_fact2w_kernel(const __
           if (lane == 0) mbar_arrive(&ctl.empty[last]);
           // the group's rows exist entirely or not at all (rows % pool == 0)
           if (owner && grow * a.pool < a.rows) {
-            const unsigned b4 = (lane >> 4) & 1u, b3 = (lane >> 3) & 1u, b2 = (lane >> 2) & 1u;
             float *o = a.out + grow * a.ldo + a.col0;
 #pragma unroll
             for (int i = 0; i < 4; ++i) {
               const int io = i + (b4 ? 16 : 0) + (b3 ? 8 : 0) + (b2 ? 4 : 0);
               const int col = 128 * nb + 8 * (io >> 1) + 2 * static_cast<int>(lane & 3u) + (io & 1);
               if (col < g.n3_pad) {
-                float r = fmaxf(p[i] + __ldg(g.bias3 + col), 0.f);
+                float r = fmaxf(p[i] + b3v[i], 0.f);
                 if (a.round_out) r = to_tf32(r);
                 o[col] = r;
               }
