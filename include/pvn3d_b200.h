@@ -278,6 +278,26 @@ int pvn3d_mlp_fp_fact2(const float *p, const float *table, const int *nn_idx, co
                        int m_known, const pvn3d_mlp_layer_t *layer_s, const pvn3d_mlp_layer_t *layer2, int flags, float *out,
                        pvn3d_stream_t stream);
 int pvn3d_mlp_fp_fact2_supported(const pvn3d_mlp_layer_t *layer_s, const pvn3d_mlp_layer_t *layer2);
+/* pvn3d_mlp_fp_fact2 with the output POINT-MAJOR in a caller's row table: row r = f * n_unknown + i gets
+ * tf32(relu(acc + b2)) in columns col0 .. col0 + 127 of rows ldo floats apart; other columns are not touched.  The same
+ * bits as tf32(transpose(pvn3d_mlp_fp_fact2's [b][128][n_unknown])).  This is how PVN3D's network forward writes the
+ * PointNet++ features straight into the DenseFusion activation table.  Arguments, flags and coverage as
+ * pvn3d_mlp_fp_fact2; ldo and col0 multiples of 4, col0 >= 0, col0 + 128 <= ldo and out 16-byte aligned, else
+ * PVN3D_ERR_INVALID_ARG before any CUDA call. */
+int pvn3d_mlp_fp_fact2_rows(const float *p, const float *table, const int *nn_idx, const float *nn_w, int b, int n_unknown,
+                            int m_known, const pvn3d_mlp_layer_t *layer_s, const pvn3d_mlp_layer_t *layer2, int flags,
+                            float *out, int ldo, int col0, pvn3d_stream_t stream);
+/* The CNN embedding at the sampled pixels, point-major: PVN3D.forward's
+ *   torch.gather(emb.view(B, C, H*W), 2, choose.repeat(1, C, 1))            (pvn3d.py:288-292)
+ * written as out[f * n + p][col0 + ch] = tf32(emb[f][ch][choose[f][0][p]]) -- bit for bit the reference's gather,
+ * transposed to rows and rounded to TF32 (cvt.rna) -- without the [B, C, N] int64 index the reference materialises.
+ *   emb [b][c][hw] f32 (4-byte aligned), choose [b][1][n] int64 (8-byte aligned), out rows ldo floats apart (16-byte
+ *   aligned; ldo, col0 multiples of 4, col0 + c <= ldo), c a multiple of 4.
+ * An index outside [0, hw) writes a row of NaN (torch.gather raises instead; the library never aborts).
+ * PVN3D_ERR_INVALID_ARG for null pointers, misalignment or a bad column range, PVN3D_ERR_UNSUPPORTED for b * n >= 2^31
+ * or c > 256 -- both before any CUDA call. */
+int pvn3d_gather_pixel_rows(const float *emb, int b, int c, long long hw, const long long *choose, int n, float *out,
+                            int ldo, int col0, pvn3d_stream_t stream);
 /* weight[p,0:3] = (1/(sqrt(dist2)+1e-8)) / sum  (pointnet2_modules.py:184-186), fp32 IEEE ops */
 int pvn3d_three_nn_weights(const float *dist2, long long rows, float *weight, pvn3d_stream_t stream);
 

@@ -84,6 +84,8 @@ _SIGNATURES = {
                                   _P]),
     "pvn3d_mlp_fp_fact2": (c_int, [_P, _P, _P, _P, c_int, c_int, c_int, _P, _P, c_int, _P, _P]),
     "pvn3d_mlp_fp_fact2_supported": (c_int, [_P, _P]),
+    "pvn3d_mlp_fp_fact2_rows": (c_int, [_P, _P, _P, _P, c_int, c_int, c_int, _P, _P, c_int, _P, c_int, c_int, _P]),
+    "pvn3d_gather_pixel_rows": (c_int, [_P, c_int, c_int, ctypes.c_longlong, _P, c_int, _P, c_int, c_int, _P]),
     "pvn3d_three_nn_weights": (c_int, [_P, ctypes.c_longlong, _P, _P]),
     "pvn3d_seg_argmax": (c_int, [_P, ctypes.c_longlong, c_int, _P, _P]),
     "pvn3d_pose_add_adds_workspace_bytes": (c_size_t, [c_int, c_int]),

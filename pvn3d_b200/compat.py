@@ -12,12 +12,16 @@ What install() does (SURVEY section 8b, App. D):
      `lib.utils.meanshift_pytorch.MeanShiftTorch` and
      `lib.utils.pvn3d_eval_utils.{MeanShiftTorch,cal_frame_poses,cal_frame_poses_lm}` to this
      package's implementations (demo.py:22 imports them by name -> call patch_post_modules()
-     after importing demo, or import pvn3d_eval_utils first).
+     after importing demo, or import pvn3d_eval_utils first);
+  4. with patch_model=True, rebinds `lib.pvn3d.PVN3D.forward` (patch_pvn3d_forward): in eval mode, without
+     autograd and on CUDA inputs the network runs on FusedPVN3D (pvn3d_b200.network); anything else -- training,
+     train_*.py, grad-enabled or CPU calls -- runs the reference's own forward.
 Nothing here copies or edits reference files.
 """
 from __future__ import annotations
 
 import importlib
+import itertools
 import sys
 import types
 
@@ -70,7 +74,7 @@ def install_import_shims() -> None:
     _stub("pcl")
 
 
-def install(reference_root: str | None = None, patch_post: bool = False) -> None:
+def install(reference_root: str | None = None, patch_post: bool = False, patch_model: bool = False) -> None:
     from . import _ext
 
     install_import_shims()
@@ -79,6 +83,52 @@ def install(reference_root: str | None = None, patch_post: bool = False) -> None
         sys.path.insert(0, reference_root)
     if patch_post:
         patch_post_modules(import_missing=True)
+    if patch_model:
+        patch_pvn3d_forward(importlib.import_module("lib.pvn3d").PVN3D)
+
+
+def _weights(model):
+    """every parameter and buffer of the module tree, a DataParallel replica's included (replicate() keeps them as plain
+    attributes, listed in _former_parameters, not in _parameters)"""
+    for m in model.modules():
+        for t in itertools.chain(m._parameters.values(), getattr(m, "_former_parameters", {}).values(), m._buffers.values()):
+            if t is not None:
+                yield t
+
+
+def fused_engine(model, device):
+    """The FusedPVN3D of `model` on `device`, cached in the module.  The cache key is (data_ptr, _version) of every
+    parameter and buffer: load_state_dict, an optimiser step or a BatchNorm running-statistics update rebuilds the
+    engine.  A DataParallel replica on the model's own device shares its tensors (and this cache) and hits it; replicas
+    on other devices hold fresh copies and rebuild on every call -- run one process per GPU instead (pvn3d_b200.dist)."""
+    from .network import FusedPVN3D
+
+    key = tuple((t.data_ptr(), t._version) for t in _weights(model))
+    cache = model.__dict__.setdefault("_pvn3d_b200_engines", {})   # plain attribute: copied by reference into replicas
+    hit = cache.get(device)
+    if hit is None or hit[0] != key:
+        hit = cache[device] = (key, FusedPVN3D(model, device))
+    return hit[1]
+
+
+def patch_pvn3d_forward(cls) -> None:
+    """Rebind cls.forward(pointcloud, rgb, choose) (the reference's PVN3D, or a class with the same forward) so that
+    eval-mode, no-grad calls on CUDA inputs run fused_engine(self, device); every other call runs the original forward.
+    Idempotent."""
+    import torch
+
+    if getattr(cls.forward, "_pvn3d_b200_orig", None) is not None:
+        return
+    orig = cls.forward
+
+    def forward(self, pointcloud, rgb, choose):
+        if self.training or torch.is_grad_enabled() or not (pointcloud.is_cuda and rgb.is_cuda and choose.is_cuda):
+            return orig(self, pointcloud, rgb, choose)
+        return fused_engine(self, pointcloud.device)(pointcloud, rgb, choose)
+
+    forward._pvn3d_b200_orig = orig
+    forward.__doc__ = orig.__doc__
+    cls.forward = forward
 
 
 def patch_post_modules(import_missing: bool = False) -> None:

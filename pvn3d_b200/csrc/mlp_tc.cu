@@ -96,6 +96,10 @@ __device__ __forceinline__ float to_tf32(float x) {
   asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(r) : "f"(x));
   return __uint_as_float(r);
 }
+// 8-byte global store kept in program order (the epilogue loop of mlp_fp_fact2_kernel<FPF2_OUT_ROWS> stays in registers)
+__device__ __forceinline__ void stg64(float *p, float x, float y) {
+  asm volatile("st.global.v2.f32 [%0], {%1,%2};" ::"l"(p), "f"(x), "f"(y) : "memory");
+}
 __device__ __forceinline__ void sts128(uint32_t addr, float a, float b, float c, float d) {
   asm volatile("st.shared.v4.f32 [%0], {%1,%2,%3,%4};" ::"r"(addr), "f"(a), "f"(b), "f"(c), "f"(d)
                : "memory");
@@ -2014,6 +2018,11 @@ int launch_fp2(Fp2Args &g, cudaStream_t st) {
 //                           whole 32-byte sectors of one channel.
 // Every output element keeps the operands, the wgmma shape, K order and epilogue arithmetic of the two launches, so
 // the results are bit-identical.
+// Where the layer-2 output goes (the kernel's template parameter):
+//   FPF2_OUT_CN    [b][128][n_unknown] channel-major, streaming stores: the layout Pointnet2MSG.forward returns;
+//   FPF2_OUT_ROWS  relu(acc + b2) rounded to TF32, point-major into columns col0 .. col0+127 of rows ldo apart: a lane
+//                  quad writes each 32-byte row segment (whole sectors), as mlp_fp2_kernel does.  The heads' table.
+enum { FPF2_OUT_CN = 0, FPF2_OUT_ROWS = 1 };
 constexpr int kFpf2BM = 64;
 constexpr int kFpf2ProWarps = 8;
 constexpr int kFpf2LoaderWarp = kFpf2ProWarps + kMlpMmaWarps;   // warp 16
@@ -2091,6 +2100,7 @@ __device__ __forceinline__ void fpf2_stage_chunk(const MlpArgs &a, uint32_t rst,
   }
 }
 
+template <int OUT>
 __global__ void __launch_bounds__(kFpf2Threads, 1) mlp_fp_fact2_kernel(const __grid_constant__ FpFact2Args g) {
   const MlpArgs &a = g.a;
   extern __shared__ unsigned char mlp_smem_raw[];
@@ -2209,27 +2219,41 @@ __global__ void __launch_bounds__(kFpf2Threads, 1) mlp_fp_fact2_kernel(const __g
       wgmma_wait<0>();
       acc_fence(d);
       if (lane == 0) mbar_arrive(&ctl.empty[s]);   // the slot (operand tile and table rows) may be refilled
-      // ---- out[b][c][i] = relu(acc + b2[c]): a lane quad's rows are 8 consecutive points of one channel
-      const long long fb0 = r0 / n_unk, fb1 = (r0 + 8) / n_unk;
-      float *o0 = a.out + fb0 * 128 * n_unk + (r0 - fb0 * n_unk);
-      float *o1 = a.out + fb1 * 128 * n_unk + (r0 + 8 - fb1 * n_unk);
+      if constexpr (OUT == FPF2_OUT_ROWS) {
+        // ---- out[r][col0 + c] = tf32(relu(acc + b2[c])): a lane quad writes 32 contiguous bytes of a row
+        float *o0 = a.out + (r0 * a.ldo + a.col0);
+        float *o1 = o0 + 8 * static_cast<long long>(a.ldo);
 #pragma unroll
-      for (int j = 0; j < 16; ++j) {
-        const int c = 8 * j + 2 * static_cast<int>(lane & 3u);
-        const float b0 = __ldg(g.bias2 + c), b1 = __ldg(g.bias2 + c + 1);
-        if (on0) {
-          stg_stream(o0 + c * n_unk, fmaxf(d[4 * j] + b0, 0.f));
-          stg_stream(o0 + (c + 1) * n_unk, fmaxf(d[4 * j + 1] + b1, 0.f));
+        for (int j = 0; j < 16; ++j) {
+          const int c = 8 * j + 2 * static_cast<int>(lane & 3u);
+          const float2 bb = __ldg(reinterpret_cast<const float2 *>(g.bias2 + c));   // the launcher checks 8-byte alignment
+          if (on0) stg64(o0 + c, to_tf32(fmaxf(d[4 * j] + bb.x, 0.f)), to_tf32(fmaxf(d[4 * j + 1] + bb.y, 0.f)));
+          if (on1) stg64(o1 + c, to_tf32(fmaxf(d[4 * j + 2] + bb.x, 0.f)), to_tf32(fmaxf(d[4 * j + 3] + bb.y, 0.f)));
         }
-        if (on1) {
-          stg_stream(o1 + c * n_unk, fmaxf(d[4 * j + 2] + b0, 0.f));
-          stg_stream(o1 + (c + 1) * n_unk, fmaxf(d[4 * j + 3] + b1, 0.f));
+      } else {
+        // ---- out[b][c][i] = relu(acc + b2[c]): a lane quad's rows are 8 consecutive points of one channel
+        const long long fb0 = r0 / n_unk, fb1 = (r0 + 8) / n_unk;
+        float *o0 = a.out + fb0 * 128 * n_unk + (r0 - fb0 * n_unk);
+        float *o1 = a.out + fb1 * 128 * n_unk + (r0 + 8 - fb1 * n_unk);
+#pragma unroll
+        for (int j = 0; j < 16; ++j) {
+          const int c = 8 * j + 2 * static_cast<int>(lane & 3u);
+          const float b0 = __ldg(g.bias2 + c), b1 = __ldg(g.bias2 + c + 1);
+          if (on0) {
+            stg_stream(o0 + c * n_unk, fmaxf(d[4 * j] + b0, 0.f));
+            stg_stream(o0 + (c + 1) * n_unk, fmaxf(d[4 * j + 1] + b1, 0.f));
+          }
+          if (on1) {
+            stg_stream(o1 + c * n_unk, fmaxf(d[4 * j + 2] + b0, 0.f));
+            stg_stream(o1 + (c + 1) * n_unk, fmaxf(d[4 * j + 3] + b1, 0.f));
+          }
         }
       }
     }
   }
 }
 
+template <int OUT>
 int launch_fp_fact2(FpFact2Args &g, const float *table, const float *ws, const float *w2, cudaStream_t st) {
   MlpArgs &a = g.a;
   if (a.rows <= 0) return PVN3D_OK;
@@ -2241,7 +2265,7 @@ int launch_fp_fact2(FpFact2Args &g, const float *table, const float *ws, const f
       !weight_tensor_map(&g.tmap_s, ws, 32, 128, 128) || !weight_tensor_map(&g.tmap_w2, w2, 128, 128, 128))
     return PVN3D_ERR_UNSUPPORTED;
   const int sms = std::max(1, sm_count() - a.reserve_sms);
-  auto kern = mlp_fp_fact2_kernel;
+  auto kern = mlp_fp_fact2_kernel<OUT>;
   static PerDeviceOnce once;
   PVN3D_ONCE_PER_DEVICE(once, cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, kMlpSmemMax),
                         "mlp fp_fact2 smem attr");
@@ -2321,6 +2345,41 @@ __global__ void nn_weights_kernel(const float *__restrict__ dist2, long long row
   w[p * 3 + 0] = __fdiv_rn(r1, norm);
   w[p * 3 + 1] = __fdiv_rn(r2, norm);
   w[p * 3 + 2] = __fdiv_rn(r3, norm);
+}
+
+// ---- the CNN embedding at the sampled pixels, point-major (PVN3D.forward's torch.gather, pvn3d.py:288-292) ------------
+// out[r][col0 + ch] = tf32(emb[f][ch][choose[r]]) for the rows r = f * n + p.  A CTA takes kGatherPts consecutive rows:
+// lane i of every warp reads one channel of point i (the datasets' ascending `choose` puts neighbouring pixels in the
+// same sectors), the values are transposed through shared memory and every row leaves in whole 16-byte groups.  An
+// index outside [0, hw) writes a row of NaN: the C ABI never aborts.
+constexpr int kGatherPts = 32;
+constexpr int kGatherThreads = 256;
+constexpr int kGatherMaxC = 256;
+
+__global__ void __launch_bounds__(kGatherThreads) gather_pixel_rows_kernel(const float *__restrict__ emb, int c, long long hw,
+                                                                           const long long *__restrict__ choose, int n,
+                                                                           long long rows, float *__restrict__ out, int ldo,
+                                                                           int col0) {
+  __shared__ __align__(16) float tile[kGatherPts * (kGatherMaxC + 4)];   // [point][channel], rows 16-byte aligned
+  const int ld = c + 4;
+  const int lane = static_cast<int>(threadIdx.x & 31u), warp = static_cast<int>(threadIdx.x >> 5);
+  const long long r0 = static_cast<long long>(blockIdx.x) * kGatherPts;
+  const long long r = r0 + lane;
+  const float *src = nullptr;
+  if (r < rows) {
+    const long long idx = __ldg(choose + r);
+    if (idx >= 0 && idx < hw) src = emb + (r / n) * c * hw + idx;
+  }
+#pragma unroll 4
+  for (int ch = warp; ch < c; ch += kGatherThreads / 32)
+    tile[lane * ld + ch] = src ? to_tf32(__ldg(src + ch * hw)) : __int_as_float(0x7fc00000);
+  __syncthreads();
+  const int q4 = c >> 2;
+  for (int i = static_cast<int>(threadIdx.x); i < kGatherPts * q4; i += kGatherThreads) {
+    const int pt = i / q4, q = i - pt * q4;
+    if (r0 + pt < rows)
+      *reinterpret_cast<float4 *>(out + (r0 + pt) * ldo + col0 + 4 * q) = *reinterpret_cast<const float4 *>(tile + pt * ld + 4 * q);
+  }
 }
 
 }  // namespace
@@ -2556,9 +2615,10 @@ extern "C" int pvn3d_mlp_fp_fact(const float *p, const float *s, int ld, int c_v
   return dispatch(a, PRO_FP_FACT, 0, as_stream(stream));
 }
 
-extern "C" int pvn3d_mlp_fp_fact2(const float *p, const float *table, const int *nn_idx, const float *nn_w, int b,
-                                  int n_unknown, int m_known, const pvn3d_mlp_layer_t *layer_s,
-                                  const pvn3d_mlp_layer_t *layer2, int flags, float *out, pvn3d_stream_t stream) {
+// the argument checks and kernel arguments pvn3d_mlp_fp_fact2 and pvn3d_mlp_fp_fact2_rows share
+static int fp_fact2_args(const float *p, const float *table, const int *nn_idx, const float *nn_w, int b, int n_unknown,
+                         int m_known, const pvn3d_mlp_layer_t *layer_s, const pvn3d_mlp_layer_t *layer2, int flags,
+                         float *out, FpFact2Args &g) {
   if (!p || !table || !nn_idx || !nn_w || !layer_s || !layer2 || !layer_s->w || !layer_s->bias || !layer2->w ||
       !layer2->bias || !out || b < 0 || n_unknown < 0 || m_known <= 0 || (flags & ~0xff00) ||
       (reinterpret_cast<uintptr_t>(p) & 15u) || (reinterpret_cast<uintptr_t>(table) & 15u) ||
@@ -2567,7 +2627,6 @@ extern "C" int pvn3d_mlp_fp_fact2(const float *p, const float *table, const int 
   const int stages = fpf2_stages(layer_s->k_pad, layer_s->n_pad, layer2->k_pad, layer2->n_pad);
   if (!stages) return PVN3D_ERR_UNSUPPORTED;
   if (static_cast<long long>(b) * m_known > 0x7fffffffll || n_unknown > 0x3fffffff) return PVN3D_ERR_UNSUPPORTED;
-  FpFact2Args g{};
   MlpArgs &a = g.a;
   a.rows = static_cast<long long>(b) * n_unknown;
   a.known_feat = p; a.c2 = layer_s->n_pad; a.nn_idx = nn_idx; a.nn_w = nn_w;
@@ -2575,7 +2634,45 @@ extern "C" int pvn3d_mlp_fp_fact2(const float *p, const float *table, const int 
   a.out = out; a.stages = stages;
   a.reserve_sms = (flags >> 8) & 0xff;
   g.bias_s = layer_s->bias; g.bias2 = layer2->bias;
-  return launch_fp_fact2(g, table, layer_s->w, layer2->w, as_stream(stream));
+  return PVN3D_OK;
+}
+
+extern "C" int pvn3d_mlp_fp_fact2(const float *p, const float *table, const int *nn_idx, const float *nn_w, int b,
+                                  int n_unknown, int m_known, const pvn3d_mlp_layer_t *layer_s,
+                                  const pvn3d_mlp_layer_t *layer2, int flags, float *out, pvn3d_stream_t stream) {
+  FpFact2Args g{};
+  const int rc = fp_fact2_args(p, table, nn_idx, nn_w, b, n_unknown, m_known, layer_s, layer2, flags, out, g);
+  if (rc != PVN3D_OK) return rc;
+  return launch_fp_fact2<FPF2_OUT_CN>(g, table, layer_s->w, layer2->w, as_stream(stream));
+}
+
+extern "C" int pvn3d_mlp_fp_fact2_rows(const float *p, const float *table, const int *nn_idx, const float *nn_w, int b,
+                                       int n_unknown, int m_known, const pvn3d_mlp_layer_t *layer_s,
+                                       const pvn3d_mlp_layer_t *layer2, int flags, float *out, int ldo, int col0,
+                                       pvn3d_stream_t stream) {
+  if (ldo % 4 || col0 < 0 || col0 % 4 || static_cast<long long>(col0) + 128 > ldo || (reinterpret_cast<uintptr_t>(out) & 15u) ||
+      (layer2 && (reinterpret_cast<uintptr_t>(layer2->bias) & 7u)))
+    return PVN3D_ERR_INVALID_ARG;
+  FpFact2Args g{};
+  const int rc = fp_fact2_args(p, table, nn_idx, nn_w, b, n_unknown, m_known, layer_s, layer2, flags, out, g);
+  if (rc != PVN3D_OK) return rc;
+  g.a.ldo = ldo;
+  g.a.col0 = col0;
+  return launch_fp_fact2<FPF2_OUT_ROWS>(g, table, layer_s->w, layer2->w, as_stream(stream));
+}
+
+extern "C" int pvn3d_gather_pixel_rows(const float *emb, int b, int c, long long hw, const long long *choose, int n,
+                                       float *out, int ldo, int col0, pvn3d_stream_t stream) {
+  if (!emb || !choose || !out || b < 0 || n < 0 || c <= 0 || c % 4 || hw <= 0 || ldo % 4 || col0 < 0 || col0 % 4 ||
+      static_cast<long long>(col0) + c > ldo || (reinterpret_cast<uintptr_t>(emb) & 3u) ||
+      (reinterpret_cast<uintptr_t>(choose) & 7u) || (reinterpret_cast<uintptr_t>(out) & 15u))
+    return PVN3D_ERR_INVALID_ARG;
+  const long long rows = static_cast<long long>(b) * n;
+  if (rows > 0x7fffffffll || c > kGatherMaxC) return PVN3D_ERR_UNSUPPORTED;
+  if (rows == 0) return PVN3D_OK;
+  const unsigned grid = static_cast<unsigned>((rows + kGatherPts - 1) / kGatherPts);
+  gather_pixel_rows_kernel<<<grid, kGatherThreads, 0, as_stream(stream)>>>(emb, c, hw, choose, n, rows, out, ldo, col0);
+  return check_launch("gather_pixel_rows_kernel");
 }
 
 extern "C" int pvn3d_mlp_fp_fact2_supported(const pvn3d_mlp_layer_t *layer_s, const pvn3d_mlp_layer_t *layer2) {

@@ -83,18 +83,34 @@ class FusedHeads:
         self.lb = PackedLayer(w4, b4, 512)
         self.heads = [_Head(s, self.dev) for s in (seg_layer, kpof_layer, ctrof_layer)]
 
+    #: columns of the activation table: [feat_1 = rgb (128) | cld (128)] [feat_2 (512)] [conv3 output (512)]
+    TABLE_COLS = 1280
+    RGB_COL0, CLD_COL0 = 0, 128
+
+    def new_table(self, rows: int) -> torch.Tensor:
+        """an uninitialised activation table for `rows` = B*N points; run() expects its columns RGB_COL0 .. +127 and
+        CLD_COL0 .. +127 filled with the TF32-rounded point-major embeddings"""
+        return torch.empty((rows, self.TABLE_COLS), dtype=torch.float32, device=self.dev)
+
     @torch.no_grad()
     def forward(self, rgb_emb: torch.Tensor, cld_emb: torch.Tensor):
         """rgb_emb [B,128,N] (the CNN embedding gathered at the sampled pixels, pvn3d.py:291-293), cld_emb [B,128,N]
         (Pointnet2MSG.forward) -> (pred_kp_of [B,K,N,3], pred_rgbd_seg [B,N,n_cls], pred_ctr_of [B,1,N,3])"""
         assert rgb_emb.is_cuda and cld_emb.is_cuda and rgb_emb.shape == cld_emb.shape and rgb_emb.size(1) == 128
-        lib = _lib.load()
         b, _, n = cld_emb.shape
         rows = b * n
-        # activation table: [feat_1 = rgb | cld (256)] [feat_2 (512)] [conv3 output (512)]
-        x = torch.empty((rows, 1280), dtype=torch.float32, device=self.dev)
+        x = self.new_table(rows)
         x[:, :128] = tf32_round(_ext.transpose_cn_to_nc(rgb_emb.contiguous().float())).view(rows, 128)
         x[:, 128:256] = tf32_round(_ext.transpose_cn_to_nc(cld_emb.contiguous().float())).view(rows, 128)
+        return self.run(x, b, n)
+
+    @torch.no_grad()
+    def run(self, x: torch.Tensor, b: int, n: int):
+        """DenseFusion and the heads on an activation table x [B*N, TABLE_COLS] (new_table) whose first 256 columns
+        hold feat_1 -> the outputs of forward().  Columns 256.. are overwritten."""
+        assert x.shape == (b * n, self.TABLE_COLS) and x.is_contiguous() and x.is_cuda
+        lib = _lib.load()
+        rows = b * n
         _dense(x.data_ptr(), 1280, 256, rows, self.la, x, col0=256)                      # feat_2 and relu(conv3(feat_1))
         # mean over the points of relu(conv4(.)): 32-row partial sums straight from the accumulator
         groups = (rows + 31) // 32

@@ -270,6 +270,23 @@ def mlp_fp_fact2(p: torch.Tensor, table: torch.Tensor, nn_idx: torch.Tensor, nn_
     return out
 
 
+def mlp_fp_fact2_rows(p: torch.Tensor, table: torch.Tensor, nn_idx: torch.Tensor, nn_w: torch.Tensor, m_known: int,
+                      layer_s: PackedLayer, layer2: PackedLayer, out: torch.Tensor, col0: int, reserve=0) -> torch.Tensor:
+    """mlp_fp_fact2 with its output point-major in columns col0 .. col0+127 of the row table out [b * n_unknown, ldo]
+    (pvn3d_mlp_fp_fact2_rows): tf32_round of the transposed [b, 128, n_unknown], bit for bit"""
+    lib = _lib.load()
+    b, n_unknown = nn_idx.shape[0], nn_idx.shape[1]
+    assert p.size(-1) == layer_s.n_pad and table.size(-1) == layer_s.k_pad and table.size(0) == b * n_unknown
+    assert out.dim() == 2 and out.size(0) == b * n_unknown and out.stride(1) == 1
+    ls, l2 = _layer_struct(layer_s), _layer_struct(layer2)
+    with torch.cuda.device(p.device):
+        rc = lib.pvn3d_mlp_fp_fact2_rows(ptr(p), ptr(table), ptr(nn_idx), ptr(nn_w), b, n_unknown, m_known,
+                                         ctypes.addressof(ls), ctypes.addressof(l2), _flags(False, reserve=reserve), ptr(out),
+                                         out.stride(0), col0, _stream(p.device))
+    check(rc, "pvn3d_mlp_fp_fact2_rows")
+    return out
+
+
 def three_nn_weights(dist2: torch.Tensor) -> torch.Tensor:
     lib = _lib.load()
     w = torch.empty_like(dist2)
@@ -445,11 +462,14 @@ class FusedPointnet2MSG:
         return self.queries(self.sampling(pointcloud, fps_chunk))
 
     @torch.no_grad()
-    def features(self, pointcloud: torch.Tensor, plan: "GeoPlan", reserve_sms: int = 0, reserve_levels: int = 5) -> torch.Tensor:
+    def features(self, pointcloud: torch.Tensor, plan: "GeoPlan", reserve_sms: int = 0, reserve_levels: int = 5,
+                 out_rows: torch.Tensor | None = None, col0: int = 0) -> torch.Tensor:
         """The shared MLPs of all SA / FP levels on a geometry plan -> [B,128,N].  reserve_sms: SMs the persistent
         MLP kernels leave free for kernels of other streams (the next batch's sampling); reserve_levels: the SA levels
         0 .. reserve_levels-1 do so (5: the FP modules too) -- the sampling of the next batch is over well before the
-        MLPs are, and the later layers then take the whole machine."""
+        MLPs are, and the later layers then take the whole machine.
+        out_rows [B*N, ldo]: FP1 writes the features TF32-rounded and point-major into its columns col0 .. col0+127
+        instead (the DenseFusion table of FusedPVN3D), and out_rows is returned."""
         b, _, width = pointcloud.shape
         c0 = width - 3
         rs_all = int(reserve_sms)
@@ -498,13 +518,19 @@ class FusedPointnet2MSG:
         assert kf2d.size(-1) == lk.k
         pk = mlp_dense(kf2d, lk, relu=False, reserve=rs)                                   # once per known point
         # S = W1s . table0 + b1 stays on chip; the module's output IS the network's, written channel-major ([B,128,N])
+        # or into the caller's row table
+        if out_rows is not None:
+            mlp_fp_fact2_rows(pk, table0, nn_idx, nn_w, l_xyz[1].size(1), ls, l2, out_rows, col0, reserve=rs)
+            self._m("mlp")
+            return out_rows
         h = mlp_fp_fact2(pk, table0, nn_idx, nn_w, l_xyz[1].size(1), ls, l2, reserve=rs)
         self._m("mlp")
         return h if l2.n == l2.n_pad else h[:, :l2.n].contiguous()
 
     @torch.no_grad()
-    def forward(self, pointcloud: torch.Tensor) -> torch.Tensor:
-        """pointcloud [B,N,3+C] f32 contiguous on device -> features [B,128,N] (as the reference returns)"""
-        return self.features(pointcloud, self.geometry(pointcloud))
+    def forward(self, pointcloud: torch.Tensor, out_rows: torch.Tensor | None = None, col0: int = 0) -> torch.Tensor:
+        """pointcloud [B,N,3+C] f32 contiguous on device -> features [B,128,N] (as the reference returns), or written
+        into columns col0 .. col0+127 of out_rows [B*N, ldo] (see features)"""
+        return self.features(pointcloud, self.geometry(pointcloud), out_rows=out_rows, col0=col0)
 
     __call__ = forward
