@@ -1040,9 +1040,10 @@ struct Sa2SmemCtl {
 
 // shared-memory layout behind the 1024-byte aligned base (kernel and launcher use the same function):
 // [W2: k2_pad/32 chunks of n2 x 128 B][W3: k3_pad/32 chunks of n3 x 128 B][H: k3_pad/32 chunks of 128 x 128 B]
-// [A ring: stages x 16 KB][pool exchange: 2 warpgroups x 2 warp pairs x max(n3, 32) floats][barriers]
+// [A ring: stages x 16 KB][pool exchange: 2 warpgroups x 2 warp pairs x max(n3, 32) floats][b2: n2 floats]
+// [b3: n3 floats][barriers]
 struct Sa2Smem {
-  uint32_t w2, w3, h, ring, xchg, ctl, bytes;   // offsets from the aligned base; bytes = dynamic size incl. alignment slack
+  uint32_t w2, w3, h, ring, xchg, b2, b3, ctl, bytes;   // offsets from the aligned base; bytes = dynamic size incl. slack
 };
 static inline __host__ __device__ Sa2Smem sa2_smem(int k2_pad, int n2, int k3_pad, int n3, int stages) {
   Sa2Smem s;
@@ -1051,7 +1052,9 @@ static inline __host__ __device__ Sa2Smem sa2_smem(int k2_pad, int n2, int k3_pa
   s.h = s.w3 + static_cast<uint32_t>(k3_pad / 32) * static_cast<uint32_t>(n3) * 128u;
   s.ring = s.h + static_cast<uint32_t>(k3_pad / 32) * kMlpBM * 128u;
   s.xchg = s.ring + static_cast<uint32_t>(stages) * kSa2StageBytes;
-  s.ctl = s.xchg + 4u * static_cast<uint32_t>(n3 > 32 ? n3 : 32) * 4u;   // 32 lanes x max(1, n3 / 32) maxima per warp pair
+  s.b2 = s.xchg + 4u * static_cast<uint32_t>(n3 > 32 ? n3 : 32) * 4u;   // 32 lanes x max(1, n3 / 32) maxima per warp pair
+  s.b3 = s.b2 + static_cast<uint32_t>(n2) * 4u;
+  s.ctl = s.b3 + static_cast<uint32_t>(n3) * 4u;
   s.bytes = 1024u + s.ctl + static_cast<uint32_t>(sizeof(Sa2SmemCtl));
   return s;
 }
@@ -1061,6 +1064,11 @@ __device__ __forceinline__ void named_bar_sync(int id, int threads) {
 }
 __device__ __forceinline__ void named_bar_arrive(int id, int threads) {
   asm volatile("bar.arrive %0, %1;" ::"r"(id), "r"(threads) : "memory");
+}
+
+// `count` floats of a bias -> n floats of shared memory (the rest zero)
+__device__ __forceinline__ void stage_bias(float *dst, const float *bias, int count, int n) {
+  for (int i = threadIdx.x; i < n; i += blockDim.x) dst[i] = i < count ? __ldg(bias + i) : 0.f;
 }
 
 // `rows` rows x `k_pad` columns of a TF32-rounded weight matrix -> n rows of K-major SWIZZLE_128B chunks (rows >= rows zero)
@@ -1075,11 +1083,12 @@ __device__ __forceinline__ void stage_weights(uint32_t dst, const float *w, int 
 
 // Layer 2 of one tile for warpgroup wg: K chunks of the ring x resident W2 into registers, then
 // H[row, c] = tf32(relu(acc + b2[c])) into the warpgroup's rows of the H tile (columns c < k3_pad; the rest of a
-// wgmma N wider than k3_pad is never read).  Stages are released once their MMAs have retired.
+// wgmma N wider than k3_pad is never read).  Stages are released once their MMAs have retired.  b2_s: the bias
+// in shared memory, zero past n_pad.
 template <int N2>
-__device__ __forceinline__ void sa2_layer2(const Sa2Args &g, uint32_t ring, uint32_t w2_s, uint32_t h_s, int S,
-                                           int it_base, int kc2, Sa2SmemCtl &ctl, unsigned wg, int frag_row,
-                                           unsigned lane) {
+__device__ __forceinline__ void sa2_layer2(const Sa2Args &g, uint32_t ring, uint32_t w2_s, uint32_t h_s,
+                                           const float *b2_s, int S, int it_base, int kc2, Sa2SmemCtl &ctl, unsigned wg,
+                                           int frag_row, unsigned lane) {
   float d[N2 / 2];
 #pragma unroll
   for (int i = 0; i < N2 / 2; ++i) d[i] = 0.f;
@@ -1107,22 +1116,27 @@ __device__ __forceinline__ void sa2_layer2(const Sa2Args &g, uint32_t ring, uint
   wgmma_wait<0>();
   acc_fence(d);
   if (lane == 0) mbar_arrive(&ctl.empty[prev]);
+  // the lane's bias pairs, all loaded before the first store (a load between the stores' memory clobbers could not
+  // be hoisted, and each one would hold up the next store)
+  float2 bv[N2 / 8];
+#pragma unroll
+  for (int j = 0; j < N2 / 8; ++j) bv[j] = *reinterpret_cast<const float2 *>(b2_s + 8 * j + 2 * static_cast<int>(lane & 3u));
   // every warp of the warpgroup has finished the previous tile's layer 3 (its reads of H and of the pool exchange)
   named_bar_sync(1 + static_cast<int>(wg), 128);
-  const int n2 = g.a.n_pad;
+  const int k3_pad = g.k3_pad;
 #pragma unroll
   for (int j = 0; j < N2 / 8; ++j) {
-    if (8 * j >= g.k3_pad) break;
-    const int c = 8 * j + 2 * static_cast<int>(lane & 3u);
-    const float b0 = c < n2 ? __ldg(g.a.bias + c) : 0.f, b1 = c + 1 < n2 ? __ldg(g.a.bias + c + 1) : 0.f;
-    const uint32_t off = static_cast<uint32_t>(c >> 5) * (kMlpBM * 128u) + static_cast<uint32_t>(frag_row) * 128u +
-                         ((static_cast<uint32_t>(((c & 31) >> 2) ^ (frag_row & 7))) << 4) + (c & 3) * 4u;
-    asm volatile("st.shared.v2.f32 [%0], {%1,%2};" ::"r"(h_s + off), "f"(to_tf32(fmaxf(d[4 * j] + b0, 0.f))),
-                 "f"(to_tf32(fmaxf(d[4 * j + 1] + b1, 0.f)))
-                 : "memory");
-    asm volatile("st.shared.v2.f32 [%0], {%1,%2};" ::"r"(h_s + off + 8u * 128u), "f"(to_tf32(fmaxf(d[4 * j + 2] + b0, 0.f))),
-                 "f"(to_tf32(fmaxf(d[4 * j + 3] + b1, 0.f)))
-                 : "memory");
+    if (8 * j < k3_pad) {
+      const int c = 8 * j + 2 * static_cast<int>(lane & 3u);
+      const uint32_t off = static_cast<uint32_t>(c >> 5) * (kMlpBM * 128u) + static_cast<uint32_t>(frag_row) * 128u +
+                           ((static_cast<uint32_t>(((c & 31) >> 2) ^ (frag_row & 7))) << 4) + (c & 3) * 4u;
+      asm volatile("st.shared.v2.f32 [%0], {%1,%2};" ::"r"(h_s + off), "f"(to_tf32(fmaxf(d[4 * j] + bv[j].x, 0.f))),
+                   "f"(to_tf32(fmaxf(d[4 * j + 1] + bv[j].y, 0.f)))
+                   : "memory");
+      asm volatile("st.shared.v2.f32 [%0], {%1,%2};" ::"r"(h_s + off + 8u * 128u), "f"(to_tf32(fmaxf(d[4 * j + 2] + bv[j].x, 0.f))),
+                   "f"(to_tf32(fmaxf(d[4 * j + 3] + bv[j].y, 0.f)))
+                   : "memory");
+    }
   }
   fence_proxy_async_smem();   // generic-proxy stores of H -> visible to the tensor core
   named_bar_sync(1 + static_cast<int>(wg), 128);
@@ -1145,23 +1159,28 @@ __device__ __forceinline__ void rowmax_level(float (&p)[NV], unsigned lane) {
   }
 }
 
-template <int N3>
+// N2 = mma_n(layer-2 n_pad), N3 = mma_n(layer-3 n_pad): both MMA widths are compile-time, so no wgmma sits in a
+// branch on a run-time width (ptxas would then fence and serialise every one of them)
+template <int N2, int N3>
 __global__ void __launch_bounds__(kSa2Threads, 1) mlp_sa_fact2_kernel(const __grid_constant__ Sa2Args g) {
   const MlpArgs &a = g.a;
   extern __shared__ unsigned char mlp_smem_raw[];
   const uint32_t raw = smem_u32(mlp_smem_raw);
   const uint32_t base = (raw + 1023u) & ~1023u;   // SWIZZLE_128B atoms are 8 rows x 128 B
-  const int n2_mma = mma_n(a.n_pad);
   const int kc2 = a.k_pad / 32, kc3 = g.k3_pad / 32;
   const int S = a.stages;   // what the launcher's budget left (it computes the layout with the same function)
-  const Sa2Smem L = sa2_smem(a.k_pad, n2_mma, g.k3_pad, N3, S);
+  const Sa2Smem L = sa2_smem(a.k_pad, N2, g.k3_pad, N3, S);
   Sa2SmemCtl &ctl = *reinterpret_cast<Sa2SmemCtl *>(mlp_smem_raw + (base - raw) + L.ctl);
   const int t = threadIdx.x;
   const unsigned warp = t >> 5, lane = t & 31u;
   const int tiles = static_cast<int>((a.rows + kMlpBM - 1) / kMlpBM);   // the launcher checks tiles * kc2 < 2^31
 
-  stage_weights(base + L.w2, a.w, a.n_pad, a.k_pad, n2_mma);
+  stage_weights(base + L.w2, a.w, a.n_pad, a.k_pad, N2);
   stage_weights(base + L.w3, g.w3, g.n3_pad, g.k3_pad, N3);
+  float *const b2_s = reinterpret_cast<float *>(mlp_smem_raw + (base - raw) + L.b2);
+  float *const b3_s = reinterpret_cast<float *>(mlp_smem_raw + (base - raw) + L.b3);
+  stage_bias(b2_s, a.bias, a.n_pad, N2);
+  stage_bias(b3_s, g.bias3, g.n3_pad, N3);
   // H columns past the layer-2 MMA width are K padding of layer 3: zero once, never written again
   for (uint32_t i = t; i < static_cast<uint32_t>(kc3) * kMlpBM * 8u; i += kSa2Threads) sts128(base + L.h + i * 16u, 0.f, 0.f, 0.f, 0.f);
   if (t == 0) {
@@ -1205,26 +1224,37 @@ __global__ void __launch_bounds__(kSa2Threads, 1) mlp_sa_fact2_kernel(const __gr
     const uint32_t xchg = base + L.xchg + (wg * 2u + (w4 >> 1)) * ((N3 > 32 ? N3 : 32) * 4u);
     constexpr int NV = N3 / 4;                 // values per lane after the max over its two rows
     constexpr int NF = NV >= 8 ? NV / 8 : 1;   // ... and after the max over the 8 lane groups
+    // the pooled columns this lane stores (the same for every tile) and their layer-3 bias, held in registers
+    int pool_col[NF];
+    float b3v[NF];
+    {
+      const unsigned b4 = (lane >> 4) & 1u, b3 = (lane >> 3) & 1u, b2 = (lane >> 2) & 1u;
+#pragma unroll
+      for (int i = 0; i < NF; ++i) {
+        const int io = i + (b4 ? NV / 2 : 0) + (b3 && NV >= 4 ? NV / 4 : 0) + (b2 && NV >= 8 ? NV / 8 : 0);
+        pool_col[i] = 8 * (io >> 1) + 2 * static_cast<int>(lane & 3u) + (io & 1);
+        b3v[i] = b3_s[pool_col[i]];
+      }
+    }
     int it_base = 0;
     for (int tile = blockIdx.x; tile < tiles; tile += gridDim.x, it_base += kc2) {
       const long long p0 = static_cast<long long>(tile) * kMlpBM;
-      if (n2_mma == 16) sa2_layer2<16>(g, base + L.ring, base + L.w2, base + L.h, S, it_base, kc2, ctl, wg, frag_row, lane);
-      else if (n2_mma == 32) sa2_layer2<32>(g, base + L.ring, base + L.w2, base + L.h, S, it_base, kc2, ctl, wg, frag_row, lane);
-      else if (n2_mma == 64) sa2_layer2<64>(g, base + L.ring, base + L.w2, base + L.h, S, it_base, kc2, ctl, wg, frag_row, lane);
-      else sa2_layer2<128>(g, base + L.ring, base + L.w2, base + L.h, S, it_base, kc2, ctl, wg, frag_row, lane);
+      sa2_layer2<N2>(g, base + L.ring, base + L.w2, base + L.h, b2_s, S, it_base, kc2, ctl, wg, frag_row, lane);
       // ---- layer 3: A = this warpgroup's 64 rows of H, B = resident W3, same K order as the per-layer kernel
       float d[N3 / 2];
 #pragma unroll
       for (int i = 0; i < N3 / 2; ++i) d[i] = 0.f;
-      wgmma_fence();
+      // one commit group per K chunk: no wgmma of a group sits behind the loop's branch (the run-time kc3 would
+      // otherwise make ptxas fence the accumulator across it)
       for (int kc = 0; kc < kc3; ++kc) {
         const uint64_t adesc = smem_desc_sw128(h_wg + static_cast<uint32_t>(kc) * (kMlpBM * 128u));
         const uint64_t bdesc = smem_desc_sw128(base + L.w3 + static_cast<uint32_t>(kc * N3) * 128u);
+        wgmma_fence();
 #pragma unroll
         for (int k4 = 0; k4 < 4; ++k4)
           wgmma_tf32<N3>(d, adesc + static_cast<uint64_t>(k4 * 2), bdesc + static_cast<uint64_t>(k4 * 2), (kc > 0 || k4 > 0) ? 1u : 0u);
+        wgmma_commit();
       }
-      wgmma_commit();
       wgmma_wait<0>();
       acc_fence(d);
       // ---- max over the warp's 16 rows: the lane's two rows, then a transposing butterfly over lane bits 4, 3, 2
@@ -1261,14 +1291,12 @@ __global__ void __launch_bounds__(kSa2Threads, 1) mlp_sa_fact2_kernel(const __gr
       }
       // the group's rows exist entirely or not at all (rows % pool == 0); NV < 8 leaves duplicates in lane bit 2
       if (owner && grow * a.pool < a.rows && (NV >= 8 || !(lane & 4u))) {
-        const unsigned b4 = (lane >> 4) & 1u, b3 = (lane >> 3) & 1u, b2 = (lane >> 2) & 1u;
         float *o = a.out + grow * a.ldo + a.col0;
 #pragma unroll
         for (int i = 0; i < NF; ++i) {
-          const int io = i + (b4 ? NV / 2 : 0) + (b3 && NV >= 4 ? NV / 4 : 0) + (b2 && NV >= 8 ? NV / 8 : 0);
-          const int col = 8 * (io >> 1) + 2 * static_cast<int>(lane & 3u) + (io & 1);
+          const int col = pool_col[i];
           if (col < g.n3_pad) {
-            float r = fmaxf(p[i] + __ldg(g.bias3 + col), 0.f);
+            float r = fmaxf(p[i] + b3v[i], 0.f);
             if (a.round_out) r = to_tf32(r);
             o[col] = r;
           }
@@ -1288,22 +1316,32 @@ int sa2_stages(int k2_pad, int n2_pad, int k3_pad, int n3_pad, int ns) {
   return stages >= 2 ? stages : 0;   // the two producer groups alternate stages
 }
 
-template <int N3>
+template <int N2, int N3>
 int launch_sa_fact2(Sa2Args &g, int stages, cudaStream_t st) {
   MlpArgs &a = g.a;
   if (a.rows <= 0) return PVN3D_OK;
   a.stages = stages;
-  const size_t smem = sa2_smem(a.k_pad, mma_n(a.n_pad), g.k3_pad, N3, stages).bytes;
+  const size_t smem = sa2_smem(a.k_pad, N2, g.k3_pad, N3, stages).bytes;
   const int sms = std::max(1, sm_count() - a.reserve_sms);
   const long long tiles = (a.rows + kMlpBM - 1) / kMlpBM;
   if (tiles * (a.k_pad / 32) > 0x7fffffffll) return PVN3D_ERR_UNSUPPORTED;   // the kernel counts K chunks in 32 bits
-  auto kern = mlp_sa_fact2_kernel<N3>;
+  auto kern = mlp_sa_fact2_kernel<N2, N3>;
   static PerDeviceOnce once;
   PVN3D_ONCE_PER_DEVICE(once, cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, kMlpSmemMax),
                         "mlp sa_fact2 smem attr");
   const unsigned grid = static_cast<unsigned>(std::min<long long>(tiles, sms));
   kern<<<grid, kSa2Threads, smem, st>>>(g);
   return check_launch("mlp_sa_fact2_kernel");
+}
+
+template <int N2>
+int launch_sa_fact2_n3(Sa2Args &g, int stages, cudaStream_t st) {
+  switch (mma_n(g.n3_pad)) {
+    case 16: return launch_sa_fact2<N2, 16>(g, stages, st);
+    case 32: return launch_sa_fact2<N2, 32>(g, stages, st);
+    case 64: return launch_sa_fact2<N2, 64>(g, stages, st);
+    default: return launch_sa_fact2<N2, 128>(g, stages, st);
+  }
 }
 
 // =====================================================================================================
@@ -2504,11 +2542,11 @@ extern "C" int pvn3d_mlp_sa_fact2(const float *u, const float *v, int ldu, int c
   a.round_out = (flags & PVN3D_MLP_ROUND_OUT) ? 1 : 0;
   a.reserve_sms = (flags >> 8) & 0xff;
   g.w3 = layer3->w; g.bias3 = layer3->bias; g.k3_pad = layer3->k_pad; g.n3_pad = layer3->n_pad;
-  switch (mma_n(layer3->n_pad)) {
-    case 16: return launch_sa_fact2<16>(g, stages, as_stream(stream));
-    case 32: return launch_sa_fact2<32>(g, stages, as_stream(stream));
-    case 64: return launch_sa_fact2<64>(g, stages, as_stream(stream));
-    default: return launch_sa_fact2<128>(g, stages, as_stream(stream));
+  switch (mma_n(layer2->n_pad)) {
+    case 16: return launch_sa_fact2_n3<16>(g, stages, as_stream(stream));
+    case 32: return launch_sa_fact2_n3<32>(g, stages, as_stream(stream));
+    case 64: return launch_sa_fact2_n3<64>(g, stages, as_stream(stream));
+    default: return launch_sa_fact2_n3<128>(g, stages, as_stream(stream));
   }
 }
 
