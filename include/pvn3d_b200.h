@@ -162,9 +162,6 @@ int pvn3d_three_nn_interpolate(const float *unknown, const float *known, const f
 #define PVN3D_MLP_RELU 1
 #define PVN3D_MLP_ROUND_OUT 2
 #define PVN3D_MLP_A_TF32 4
-#define PVN3D_MLP_OUT_CN 16   /* pvn3d_mlp_fp_fact only: out is [b][n_pad][n_unknown] -- the channel-major [B, C, N] layout
-                                 Pointnet2MSG.forward returns (pvn3d.py:154) -- written straight from the accumulator;
-                                 n_pad 128 or 256, n_unknown % 32 == 0, ldo / col0 ignored (else PVN3D_ERR_UNSUPPORTED) */
 /* leave n SMs (0..255) to kernels running concurrently on other streams: the persistent grid is
  * sm_count - n CTAs instead of one per SM (a persistent CTA that cannot be placed stalls its kernel) */
 #define PVN3D_MLP_RESERVE_SMS(n) (((n) & 0xff) << 8)
@@ -208,17 +205,17 @@ typedef struct {
  *   pvn3d_sa_factor_table: xyz [rows,3], feat_pm [rows, ldf] (c_feat columns) -> out [rows, k_pad] TF32-rounded
  *   pvn3d_sa_centre_term : centres [rows,3], wx [n_pad,3] (TF32-rounded), bias [n_pad] -> out [rows, n_pad]
  *   pvn3d_mlp_sa_fact    : u [B*n, ldu], v [B*m, ldu] (c_valid columns), idx [B,m,ns] -> layer (w, bias) as
- *                          pvn3d_mlp_dense: out rows = B*m*ns (or B*m with pool = ns) */
+ *                          pvn3d_mlp_dense: out rows = B*m*ns */
 int pvn3d_sa_factor_table(const float *xyz, const float *feat_pm, int ldf, int c_feat, long long rows, int k_pad,
                           float *out, pvn3d_stream_t stream);
 int pvn3d_sa_centre_term(const float *centres, const float *wx, const float *bias, long long rows, int n_pad,
                          float *out, pvn3d_stream_t stream);
 int pvn3d_mlp_sa_fact(const float *u, const float *v, int ldu, int c_valid, const int *idx, int b, int n, int m,
-                      int ns, const float *w, const float *bias, int k_pad, int n_pad, int flags, int pool,
-                      float *out, int ldo, int col0, pvn3d_stream_t stream);
+                      int ns, const float *w, const float *bias, int k_pad, int n_pad, int flags, float *out, int ldo,
+                      int col0, pvn3d_stream_t stream);
 /* Layers 2 AND 3 of a factored SA scale plus the max-pool over nsample, in one launch: the layer-2 activations
  * stay in shared memory instead of going through HBM.  Same result, bit for bit, as
- *   pvn3d_mlp_sa_fact(.., layer2, PVN3D_MLP_RELU | PVN3D_MLP_ROUND_OUT, pool = 0)  ->  h
+ *   pvn3d_mlp_sa_fact(.., layer2, PVN3D_MLP_RELU | PVN3D_MLP_ROUND_OUT)  ->  h
  *   pvn3d_mlp_dense(h, .., layer3, PVN3D_MLP_RELU [| PVN3D_MLP_ROUND_OUT], pool = ns) -> out
  * pool must equal ns.  Both layers apply ReLU; flags: PVN3D_MLP_ROUND_OUT (pooled output) and
  * PVN3D_MLP_RESERVE_SMS(n).  layer3->k_pad >= layer2->n_pad.  Any number of layer-2 K chunks.
@@ -267,8 +264,8 @@ int pvn3d_mlp_fp_fact(const float *p, const float *s, int ld, int c_valid, const
 /* The skip term and the second layer of a factored FP module whose skip is an SA factor table (FP1), in one launch:
  * S never goes through HBM.  Same result, bit for bit, as
  *   pvn3d_mlp_dense(table, k, k, b*n_unknown, layer_s, PVN3D_MLP_A_TF32) -> s    (k = layer_s->k_pad, no ReLU)
- *   pvn3d_mlp_fp_fact(p, s, 128, 128, nn_idx, nn_w, b, n_unknown, m_known, layer2,
- *                     PVN3D_MLP_RELU | PVN3D_MLP_OUT_CN) -> out [b][128][n_unknown]
+ *   pvn3d_mlp_fp_fact(p, s, 128, 128, nn_idx, nn_w, b, n_unknown, m_known, layer2, PVN3D_MLP_RELU) -> rows
+ *                     [b*n_unknown][128], transposed per frame -> out [b][128][n_unknown]
  * for ANY n_unknown (a tile may hold the end of one frame and the start of the next).
  *   p [b*m_known, 128], table [b*n_unknown, 32] TF32-rounded (pvn3d_sa_factor_table), both 16-byte aligned.
  * flags: PVN3D_MLP_RESERVE_SMS(n) only.  Pointers not 16-byte aligned or other flags: PVN3D_ERR_INVALID_ARG, before any

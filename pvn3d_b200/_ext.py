@@ -19,8 +19,7 @@ from __future__ import annotations
 
 import torch
 
-from . import _lib
-from ._lib import check, ptr
+from ._lib import call, ptr
 
 
 def _chk_contig(x, name):
@@ -48,13 +47,6 @@ def _need_cuda(x):
         raise RuntimeError("CPU not supported")
 
 
-def _call(fn_name, dev, *args):
-    lib = _lib.load()
-    with torch.cuda.device(dev):
-        rc = getattr(lib, fn_name)(*args, torch.cuda.current_stream(dev).cuda_stream)
-    check(rc, fn_name)
-
-
 def furthest_point_sampling(points: torch.Tensor, nsamples: int) -> torch.Tensor:
     """sampling.cpp:65-86 -- points [B,N,3] f32 -> idx [B,nsamples] i32"""
     _chk_contig(points, "points")
@@ -62,7 +54,7 @@ def furthest_point_sampling(points: torch.Tensor, nsamples: int) -> torch.Tensor
     _need_cuda(points)
     b, n = points.size(0), points.size(1)
     out = torch.empty((b, nsamples), dtype=torch.int32, device=points.device)
-    _call("pvn3d_furthest_point_sampling", points.device, ptr(points), b, n, int(nsamples), ptr(out))
+    call("pvn3d_furthest_point_sampling", points.device, ptr(points), b, n, int(nsamples), ptr(out))
     return out
 
 
@@ -78,7 +70,7 @@ def gather_points(points: torch.Tensor, idx: torch.Tensor) -> torch.Tensor:
     b, c, n = points.shape
     m = idx.size(1)
     out = torch.empty((b, c, m), dtype=torch.float32, device=points.device)
-    _call("pvn3d_gather_points", points.device, ptr(points), ptr(idx), b, c, n, m, ptr(out))
+    call("pvn3d_gather_points", points.device, ptr(points), ptr(idx), b, c, n, m, ptr(out))
     return out
 
 
@@ -90,7 +82,7 @@ def gather_xyz(xyz: torch.Tensor, idx: torch.Tensor) -> torch.Tensor:
     b, n, _ = xyz.shape
     m = idx.size(1)
     out = torch.empty((b, m, 3), dtype=torch.float32, device=xyz.device)
-    _call("pvn3d_gather_xyz", xyz.device, ptr(xyz), ptr(idx), b, n, m, ptr(out))
+    call("pvn3d_gather_xyz", xyz.device, ptr(xyz), ptr(idx), b, n, m, ptr(out))
     return out
 
 
@@ -105,7 +97,7 @@ def gather_points_grad(grad_out: torch.Tensor, idx: torch.Tensor, n: int) -> tor
     _need_cuda(grad_out)
     b, c, m = grad_out.shape
     out = torch.empty((b, c, int(n)), dtype=torch.float32, device=grad_out.device)
-    _call("pvn3d_gather_points_grad", grad_out.device, ptr(grad_out), ptr(idx), b, c, int(n), m, ptr(out))
+    call("pvn3d_gather_points_grad", grad_out.device, ptr(grad_out), ptr(idx), b, c, int(n), m, ptr(out))
     return out
 
 
@@ -121,7 +113,7 @@ def ball_query(new_xyz: torch.Tensor, xyz: torch.Tensor, radius: float, nsample:
     b, n = xyz.size(0), xyz.size(1)
     m = new_xyz.size(1)
     idx = torch.empty((new_xyz.size(0), m, int(nsample)), dtype=torch.int32, device=new_xyz.device)
-    _call("pvn3d_ball_query", new_xyz.device, ptr(new_xyz), ptr(xyz), b, n, m, float(radius), int(nsample), ptr(idx))
+    call("pvn3d_ball_query", new_xyz.device, ptr(new_xyz), ptr(xyz), b, n, m, float(radius), int(nsample), ptr(idx))
     return idx
 
 
@@ -137,7 +129,7 @@ def group_points(points: torch.Tensor, idx: torch.Tensor) -> torch.Tensor:
     b, c, n = points.shape
     m, s = idx.size(1), idx.size(2)
     out = torch.empty((b, c, m, s), dtype=torch.float32, device=points.device)
-    _call("pvn3d_group_points", points.device, ptr(points), ptr(idx), b, c, n, m, s, ptr(out))
+    call("pvn3d_group_points", points.device, ptr(points), ptr(idx), b, c, n, m, s, ptr(out))
     return out
 
 
@@ -153,7 +145,7 @@ def group_points_grad(grad_out: torch.Tensor, idx: torch.Tensor, n: int) -> torc
     b, c = grad_out.size(0), grad_out.size(1)
     m, s = idx.size(1), idx.size(2)
     out = torch.empty((b, c, int(n)), dtype=torch.float32, device=grad_out.device)
-    _call("pvn3d_group_points_grad", grad_out.device, ptr(grad_out), ptr(idx), b, c, int(n), m, s, ptr(out))
+    call("pvn3d_group_points_grad", grad_out.device, ptr(grad_out), ptr(idx), b, c, int(n), m, s, ptr(out))
     return out
 
 
@@ -170,7 +162,7 @@ def three_nn(unknowns: torch.Tensor, knows: torch.Tensor):
     m = knows.size(1)
     idx = torch.empty((b, n, 3), dtype=torch.int32, device=unknowns.device)
     dist2 = torch.empty((b, n, 3), dtype=torch.float32, device=unknowns.device)
-    _call("pvn3d_three_nn", unknowns.device, ptr(unknowns), ptr(knows), b, n, m, ptr(dist2), ptr(idx))
+    call("pvn3d_three_nn", unknowns.device, ptr(unknowns), ptr(knows), b, n, m, ptr(dist2), ptr(idx))
     return [dist2, idx]
 
 
@@ -189,7 +181,7 @@ def three_interpolate(points: torch.Tensor, idx: torch.Tensor, weight: torch.Ten
     b, c, m = points.shape
     n = idx.size(1)
     out = torch.empty((b, c, n), dtype=torch.float32, device=points.device)
-    _call("pvn3d_three_interpolate", points.device, ptr(points), ptr(idx), ptr(weight), b, c, m, n, ptr(out))
+    call("pvn3d_three_interpolate", points.device, ptr(points), ptr(idx), ptr(weight), b, c, m, n, ptr(out))
     return out
 
 
@@ -207,7 +199,7 @@ def three_interpolate_grad(grad_out: torch.Tensor, idx: torch.Tensor, weight: to
     _need_cuda(grad_out)
     b, c, n = grad_out.shape
     out = torch.empty((b, c, int(m)), dtype=torch.float32, device=grad_out.device)
-    _call("pvn3d_three_interpolate_grad", grad_out.device, ptr(grad_out), ptr(idx), ptr(weight), b, c, n, int(m), ptr(out))
+    call("pvn3d_three_interpolate_grad", grad_out.device, ptr(grad_out), ptr(idx), ptr(weight), b, c, n, int(m), ptr(out))
     return out
 
 
@@ -218,7 +210,7 @@ def transpose_cn_to_nc(x: torch.Tensor) -> torch.Tensor:
     _chk_contig(x, "x"); _chk_float(x, "x"); _need_cuda(x)
     b, c, n = x.shape
     out = torch.empty((b, n, c), dtype=torch.float32, device=x.device)
-    _call("pvn3d_transpose_cn_to_nc", x.device, ptr(x), b, c, n, ptr(out))
+    call("pvn3d_transpose_cn_to_nc", x.device, ptr(x), b, c, n, ptr(out))
     return out
 
 
@@ -227,7 +219,7 @@ def transpose_nc_to_cn(x: torch.Tensor) -> torch.Tensor:
     _chk_contig(x, "x"); _chk_float(x, "x"); _need_cuda(x)
     b, n, c = x.shape
     out = torch.empty((b, c, n), dtype=torch.float32, device=x.device)
-    _call("pvn3d_transpose_nc_to_cn", x.device, ptr(x), b, n, c, ptr(out))
+    call("pvn3d_transpose_nc_to_cn", x.device, ptr(x), b, n, c, ptr(out))
     return out
 
 
@@ -248,7 +240,7 @@ def query_and_group(xyz, new_xyz, feat_pm, radius: float, nsample: int, ldf=None
         ldf, c = 0, 0
     out = torch.empty((b, 3 + c, m, int(nsample)), dtype=torch.float32, device=xyz.device)
     idx = torch.empty((b, m, int(nsample)), dtype=torch.int32, device=xyz.device) if want_idx else None
-    _call("pvn3d_query_and_group", xyz.device, ptr(xyz), ptr(new_xyz), ptr(feat_pm), ldf, b, n, m, c,
+    call("pvn3d_query_and_group", xyz.device, ptr(xyz), ptr(new_xyz), ptr(feat_pm), ldf, b, n, m, c,
           float(radius), int(nsample), ptr(idx), ptr(out))
     return out, idx
 
@@ -269,7 +261,7 @@ def query_and_group2(xyz, new_xyz, feat_pm, radii, nsamples, ldf=None, c=None, w
     outs = [torch.empty((b, 3 + c, m, int(ns)), dtype=torch.float32, device=xyz.device) if want_out else None
             for ns in nsamples]
     idxs = [torch.empty((b, m, int(ns)), dtype=torch.int32, device=xyz.device) if want_idx else None for ns in nsamples]
-    _call("pvn3d_query_and_group2", xyz.device, ptr(xyz), ptr(new_xyz), ptr(feat_pm) if want_out else 0, ldf, b, n, m, c,
+    call("pvn3d_query_and_group2", xyz.device, ptr(xyz), ptr(new_xyz), ptr(feat_pm) if want_out else 0, ldf, b, n, m, c,
           float(radii[0]), int(nsamples[0]), ptr(idxs[0]), ptr(outs[0]),
           float(radii[1]), int(nsamples[1]), ptr(idxs[1]), ptr(outs[1]))
     return outs, idxs
@@ -294,6 +286,6 @@ def three_nn_interpolate(unknown, known, known_feat_pm, out_pm=None, col0=0, wan
     ldo = out_pm.size(2)
     dist2 = torch.empty((b, n, 3), dtype=torch.float32, device=unknown.device) if want_nn else None
     idx = torch.empty((b, n, 3), dtype=torch.int32, device=unknown.device) if want_nn else None
-    _call("pvn3d_three_nn_interpolate", unknown.device, ptr(unknown), ptr(known), ptr(known_feat_pm),
+    call("pvn3d_three_nn_interpolate", unknown.device, ptr(unknown), ptr(known), ptr(known_feat_pm),
           b, n, m, c, ptr(out_pm), ldo, int(col0), ptr(dist2), ptr(idx))
     return out_pm, dist2, idx

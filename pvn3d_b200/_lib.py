@@ -70,8 +70,8 @@ _SIGNATURES = {
     "pvn3d_mlp_fp_first": (c_int, [_P, c_int, _P, _P, _P, c_int, c_int, c_int, c_int, c_int, _P, _P, c_int, c_int, c_int, _P, c_int, c_int, _P]),
     "pvn3d_sa_factor_table": (c_int, [_P, _P, c_int, c_int, ctypes.c_longlong, c_int, _P, _P]),
     "pvn3d_sa_centre_term": (c_int, [_P, _P, _P, ctypes.c_longlong, c_int, _P, _P]),
-    "pvn3d_mlp_sa_fact": (c_int, [_P, _P, c_int, c_int, _P, c_int, c_int, c_int, c_int, _P, _P, c_int, c_int, c_int, c_int, _P,
-                                  c_int, c_int, _P]),
+    "pvn3d_mlp_sa_fact": (c_int, [_P, _P, c_int, c_int, _P, c_int, c_int, c_int, c_int, _P, _P, c_int, c_int, c_int, _P, c_int,
+                                  c_int, _P]),
     "pvn3d_mlp_sa_fact2": (c_int, [_P, _P, c_int, c_int, _P, c_int, c_int, c_int, c_int, _P, _P, c_int, c_int, _P, c_int,
                                    c_int, _P]),
     "pvn3d_mlp_sa_fact2_supported": (c_int, [_P, _P, c_int]),
@@ -152,6 +152,17 @@ def check(rc: int, what: str) -> None:
         detail = lib.pvn3d_last_cuda_error()
         msg += f": {detail.decode() if detail else '?'}"
     raise Pvn3dError(f"{what}: {msg}")
+
+
+def call(fn_name: str, dev, *args) -> None:
+    """fn_name(*args, stream) with `dev` the current device and stream its current stream; raises Pvn3dError on a
+    non-zero return code"""
+    import torch
+
+    lib = load()
+    with torch.cuda.device(dev):
+        rc = getattr(lib, fn_name)(*args, torch.cuda.current_stream(dev).cuda_stream)
+    check(rc, fn_name)
 
 
 def ptr(t) -> int:

@@ -27,6 +27,10 @@
 // point-major row or reduce over the nsample rows of each centre with a transposing shuffle butterfly
 // (max-pool) and store one 128-byte line per centre.
 //
+// The engines run this per-layer kernel only for dense layers (the factor tables, the heads); the SA / FP
+// modules run on the fused kernels further down, and the other producers and the pooled form stay as the
+// two-launch references those kernels are tested against, bit for bit.
+//
 // TF32: operands are rounded to nearest (cvt.rna.tf32.f32) when staged, accumulation is fp32 -- the
 // precision class of the reference's default cuDNN convolutions (torch.backends.cudnn.allow_tf32).
 #include <cuda.h>  // CUtensorMap + the cuTensorMapEncodeTiled prototype (entry point fetched through the runtime)
@@ -45,13 +49,12 @@ constexpr int kMlpMaxStages = 6;
 constexpr int kMlpSmemMax = 227 * 1024;  // dynamic shared memory a block may opt into on sm_90
 
 enum : int { PRO_DENSE = 0, PRO_FP_INTERP = 2, PRO_SA_FACT = 3, PRO_FP_FACT = 4 };
-enum : int { EPI_STORE = 0, EPI_MAXPOOL = 1, EPI_SUMPOOL = 2, EPI_MAXPOOL_T = 3, EPI_STORE_T = 4 };
+enum : int { EPI_STORE = 0, EPI_MAXPOOL = 1, EPI_SUMPOOL = 2 };
 
 struct MlpArgs {
   // W as a TMA tensor map ([n_pad][k_pad] fp32, box 32 columns x bn rows, SWIZZLE_128B): one
-  // cp.async.bulk.tensor.2d per K chunk lands the B operand in the wgmma layout (use_tma, else cp.async)
+  // cp.async.bulk.tensor.2d per K chunk lands the B operand in the wgmma layout
   alignas(64) CUtensorMap tmap;
-  int use_tma;
   // GEMM
   const float *w;     // [n_pad][k_pad]
   const float *bias;  // [n_pad]
@@ -81,7 +84,6 @@ struct MlpArgs {
   int pool;       // nsample of the max-pool epilogue (8, 16 or 32)
   int reserve_sms;  // host only: SMs left to concurrent kernels (PVN3D_MLP_RESERVE_SMS in flags)
   int bias_npb;     // > 0: bias is [rows / bias_npb][n_pad] -- one vector per batch element (bias_npb % 128 == 0)
-  int out_cn;       // STORE_T: points per frame; out is [rows / out_cn][n_pad][out_cn] (channel-major frames, out_cn % 32 == 0)
 };
 
 // ---- PTX wrappers --------------------------------------------------------------------------------
@@ -199,8 +201,8 @@ __device__ __forceinline__ uint64_t smem_desc_sw128(uint32_t saddr) {
 }
 
 // ---- shared-memory accumulator tile: 128 rows x acc_ld floats (acc_ld a multiple of 32), the 16-byte
-// chunks of every 128-byte line XOR-swizzled by row & 7 so that a thread per row (epilogue), a thread
-// per column (transposed epilogues) and the wgmma fragment stores all run without bank conflicts
+// chunks of every 128-byte line XOR-swizzled by row & 7 so that a thread per row (epilogue) and the
+// wgmma fragment stores both run without bank conflicts
 __device__ __forceinline__ uint32_t acc_off(int r, int c, int ld) {
   return static_cast<uint32_t>(r * ld * 4 + ((c >> 5) << 7) + ((((c >> 2) & 7) ^ (r & 7)) << 4) + (c & 3) * 4);
 }
@@ -225,12 +227,6 @@ __device__ __forceinline__ void acc_ld_row(uint32_t acc_s, int ld, int r, int c0
     if (q < 4 || cols == 32) x = lds128(acc_s + acc_off(r, c0 + 4 * q, ld));
     v[4 * q + 0] = x.x; v[4 * q + 1] = x.y; v[4 * q + 2] = x.z; v[4 * q + 3] = x.w;
   }
-}
-// column c, rows r0..r0+31
-__device__ __forceinline__ void acc_ld_col(uint32_t acc_s, int ld, int r0, int c, float (&v)[32]) {
-#pragma unroll
-  for (int i = 0; i < 32; ++i)
-    asm volatile("ld.shared.f32 %0, [%1];" : "=f"(v[i]) : "r"(acc_s + acc_off(r0 + i, c, ld)));
 }
 
 // wgmma N for `n_pad` columns: the narrowest of 16 / 32 / 64 / 128 that covers them (wider layers: 128-column tiles;
@@ -653,7 +649,6 @@ __global__ void __launch_bounds__(kMlpThreads, 1) mlp_layer_kernel(const __grid_
       const int nb = static_cast<int>(tile - rt * n_blocks);
       const long long p0 = rt * kMlpBM;
       const int n0 = nb * a.bn;
-      const int bn = min(a.bn, a.n_pad - n0);
       const long long p_first = p0 + r_first;
       RowState rs;
       rows_setup<PRO>(a, p_first, rs);
@@ -673,17 +668,11 @@ __global__ void __launch_bounds__(kMlpThreads, 1) mlp_layer_kernel(const __grid_
         mbar_wait(&ctl.empty[s], static_cast<unsigned>(((it / S) & 1) ^ 1));
         const uint32_t sa = ring + static_cast<uint32_t>(s) * stage_bytes;
         const uint32_t sb = sa + a_bytes;
-        // weights: rows n0..n0+bn of W, columns kc*32..+32 (TF32-rounded, zero-padded): global -> smem
-        if (a.use_tma) {
-          if (pt == 0) {   // one tensor-map copy, completing on the stage's `full` barrier in bytes
-            mbar_expect_tx_only(&ctl.full[s], static_cast<unsigned>(a.bn) * 128u);
-            tma_load_2d(sb, &a.tmap, kc * 32, n0, &ctl.full[s]);
-          }
-        } else {
-          for (int i = pt; i < bn * 8; i += 128) {
-            const int n = i >> 3, c = i & 7;
-            cp_async16(sb + sw128_off(n, c), a.w + static_cast<size_t>(n0 + n) * a.k_pad + kc * 32 + c * 4);
-          }
+        // weights: rows n0..n0+bn of W, columns kc*32..+32 (TF32-rounded, zero-padded): one tensor-map copy,
+        // completing on the stage's `full` barrier in bytes
+        if (pt == 0) {
+          mbar_expect_tx_only(&ctl.full[s], static_cast<unsigned>(a.bn) * 128u);
+          tma_load_2d(sb, &a.tmap, kc * 32, n0, &ctl.full[s]);
         }
         if (a_async) {
           const int k = kc * 32 + 4 * sub;
@@ -697,7 +686,7 @@ __global__ void __launch_bounds__(kMlpThreads, 1) mlp_layer_kernel(const __grid_
         } else {
           cp_async_commit();
           stage_a_chunk<PRO>(a, rs, p_first, r_first, sub, kc * 32, sa, vec_ok);
-          cp_async_wait<0>();        // the weights of this chunk and every asynchronous chunk still pending have landed
+          cp_async_wait<0>();        // every asynchronous chunk still pending has landed
           fence_proxy_async_smem();  // generic-proxy stores / copies -> visible to the tensor-core proxy
           if (npend >= 1) mbar_arrive(&ctl.full[pend0]);
           if (npend == 2) mbar_arrive(&ctl.full[pend1]);
@@ -739,12 +728,7 @@ __global__ void __launch_bounds__(kMlpThreads, 1) mlp_layer_kernel(const __grid_
         const bool col_on = static_cast<int>(chunk) * 4 < cw;
         float4 bq = make_float4(0.f, 0.f, 0.f, 0.f);
         if (EPI == EPI_STORE && col_on) bq = ldg128(bias_t + n0 + c0 + chunk * 4);
-        float bch = 0.f;   // MAXPOOL_T: the lane's channel = n0 + 128 * (c0 / 128) + 32 * warp + lane
-        if (EPI == EPI_MAXPOOL_T || EPI == EPI_STORE_T) bch = __ldg(bias_t + n0 + (c0 & ~127) + warp * 32 + lane);
-        if (EPI == EPI_MAXPOOL_T || EPI == EPI_STORE_T)
-          acc_ld_col(acc_s, a.acc_ld, c0 & 127, (c0 & ~127) + static_cast<int>(warp * 32 + lane), v);   // v[i] = row c0+i
-        else
-          acc_ld_row(acc_s, a.acc_ld, static_cast<int>(warp * 32 + lane), c0, cw, v);
+        acc_ld_row(acc_s, a.acc_ld, static_cast<int>(warp * 32 + lane), c0, cw, v);
         if (EPI == EPI_SUMPOOL) {
           // sum over the 32 rows of the warp of relu(acc + bias): partial sums of a mean over points
           // (DenseFusion's AvgPool1d, pvn3d.py:165,178); rows past the end contribute 0
@@ -761,88 +745,6 @@ __global__ void __launch_bounds__(kMlpThreads, 1) mlp_layer_kernel(const __grid_
           const int col = static_cast<int>(lane);
           if (col < cw && p0 + warp * 32 < a.rows)
             a.out[((p0 + warp * 32) / 32) * a.ldo + a.col0 + n0 + c0 + col] = v[0];
-        } else if (EPI == EPI_STORE_T) {
-          // TRANSPOSED read of the accumulator tile, stored channel-major: lane = channel, registers = 32 consecutive points of one
-          // frame = 128 contiguous bytes of out[frame][channel][:] -- the [B, C, N] layout Pointnet2MSG.forward returns
-          // (pvn3d.py:154) without a transposing pass over the [B*N, C] rows.  Bias / ReLU on the lane's channel, then
-          // through the swizzled staging tile (row = channel) so that one STG.128 writes four full 128-byte lines
-          // (direct stores -- 32 half sectors per instruction -- cost the gathering producers 64 us of LSU time)
-          const long long prow0 = p0 + (c0 & 127);
-#pragma unroll
-          for (int q = 0; q < 8; ++q) {
-            float4 r = make_float4(v[q * 4 + 0] + bch, v[q * 4 + 1] + bch, v[q * 4 + 2] + bch, v[q * 4 + 3] + bch);
-            if (a.relu) {
-              r.x = fmaxf(r.x, 0.f); r.y = fmaxf(r.y, 0.f); r.z = fmaxf(r.z, 0.f); r.w = fmaxf(r.w, 0.f);
-            }
-            if (a.round_out) {
-              r.x = to_tf32(r.x); r.y = to_tf32(r.y); r.z = to_tf32(r.z); r.w = to_tf32(r.w);
-            }
-            sts128(stg + lane * 128u + ((static_cast<uint32_t>(q) ^ (lane & 7u)) << 4), r.x, r.y, r.z, r.w);
-          }
-          __syncwarp();
-          if (prow0 < a.rows) {
-            const long long fb = prow0 / a.out_cn;
-            const long long pt = prow0 - fb * a.out_cn;
-            const int ch0 = n0 + (c0 & ~127) + static_cast<int>(warp * 32 + (lane >> 3));
-            float *o = a.out + (fb * a.n_pad + ch0) * a.out_cn + pt + chunk * 4;
-#pragma unroll
-            for (int i = 0; i < 8; ++i) {
-              const unsigned row = 4u * i + (lane >> 3);
-              const float4 r = lds128(stg + row * 128u + ((chunk ^ (row & 7u)) << 4));
-              *reinterpret_cast<float4 *>(o + static_cast<size_t>(4 * i) * a.out_cn) = r;
-            }
-          }
-          __syncwarp();
-        } else if (EPI == EPI_MAXPOOL_T) {
-          // TRANSPOSED read of the accumulator tile: lane = output channel, register i = row c0 + i of the tile, so
-          // the max over the `pool` consecutive rows of a centre is a max over REGISTERS of one thread -- no
-          // shuffles -- and the 32 lanes of a warp store 32 consecutive channels of one pooled row (128 bytes).
-          // Groups never straddle the end: rows % pool == 0 and 128 % pool == 0.
-          const long long prow0 = p0 + (c0 & 127);          // row of register 0
-          float *o = a.out + a.col0 + n0 + (c0 & ~127) + warp * 32 + lane;
-          if (a.pool == 32) {
-#pragma unroll
-            for (int w = 16; w >= 1; w >>= 1)
-#pragma unroll
-              for (int i = 0; i < w; ++i) v[i] = fmaxf(v[i], v[i + w]);
-            if (prow0 < a.rows) {
-              float r = v[0] + bch;
-              if (a.relu) r = fmaxf(r, 0.f);
-              if (a.round_out) r = to_tf32(r);
-              o[(prow0 >> 5) * a.ldo] = r;
-            }
-          } else if (a.pool == 16) {
-#pragma unroll
-            for (int w = 8; w >= 1; w >>= 1)
-#pragma unroll
-              for (int i = 0; i < w; ++i) {
-                v[i] = fmaxf(v[i], v[i + w]);
-                v[16 + i] = fmaxf(v[16 + i], v[16 + i + w]);
-              }
-#pragma unroll
-            for (int g = 0; g < 2; ++g)
-              if (prow0 + 16 * g < a.rows) {
-                float r = v[16 * g] + bch;
-                if (a.relu) r = fmaxf(r, 0.f);
-                if (a.round_out) r = to_tf32(r);
-                o[((prow0 >> 4) + g) * a.ldo] = r;
-              }
-          } else {  // pool == 8
-#pragma unroll
-            for (int w = 4; w >= 1; w >>= 1)
-#pragma unroll
-              for (int i = 0; i < w; ++i)
-#pragma unroll
-                for (int g = 0; g < 4; ++g) v[8 * g + i] = fmaxf(v[8 * g + i], v[8 * g + i + w]);
-#pragma unroll
-            for (int g = 0; g < 4; ++g)
-              if (prow0 + 8 * g < a.rows) {
-                float r = v[8 * g] + bch;
-                if (a.relu) r = fmaxf(r, 0.f);
-                if (a.round_out) r = to_tf32(r);
-                o[((prow0 >> 3) + g) * a.ldo] = r;
-              }
-          }
         } else if (EPI == EPI_STORE) {
           // raw accumulators through a swizzled 4 KB staging tile (thread = row going in, 8 lanes per row coming
           // out: the global stores are 128-byte row segments, 4 rows per STG.128); bias / ReLU / rounding on the
@@ -966,8 +868,8 @@ EncodeTiledFn encode_tiled_fn() {
   return fn;
 }
 
-// tensor map of one weight matrix; false: the driver cannot encode it (mlp_layer_kernel then loads the weights with
-// per-thread cp.async -- the same bytes, 16-byte aligned as launch_mlp requires -- and pvn3d_mlp_sa_fact2w refuses)
+// tensor map of one weight matrix; false: the driver cannot encode it (every launcher then returns
+// PVN3D_ERR_UNSUPPORTED without launching)
 bool weight_tensor_map(CUtensorMap *map, const float *w, int k_pad, int n_pad, int bn) {
   EncodeTiledFn enc = encode_tiled_fn();
   if (!enc || (reinterpret_cast<uintptr_t>(w) & 15u)) return false;
@@ -980,11 +882,23 @@ bool weight_tensor_map(CUtensorMap *map, const float *w, int k_pad, int n_pad, i
              CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
 }
 
+// One persistent launch: a CTA per SM not reserved for other streams (PVN3D_MLP_RESERVE_SMS), at most one per tile.
+// The shared-memory opt-in is made once per kernel and device -- the latch is a static of the instantiation for Kern.
+template <auto Kern, typename Args>
+int launch_persistent(const Args &g, long long tiles, int threads, size_t smem, int reserve_sms, cudaStream_t st,
+                      const char *name) {
+  static PerDeviceOnce once;
+  PVN3D_ONCE_PER_DEVICE(once, cudaFuncSetAttribute(Kern, cudaFuncAttributeMaxDynamicSharedMemorySize, kMlpSmemMax), name);
+  const int sms = std::max(1, sm_count() - reserve_sms);
+  Kern<<<static_cast<unsigned>(std::min<long long>(tiles, sms)), threads, smem, st>>>(g);
+  return check_launch(name);
+}
+
 template <int PRO, int EPI>
 int launch_mlp(MlpArgs &a, cudaStream_t st) {
   if (a.rows <= 0) return PVN3D_OK;
   if (a.k_pad <= 0 || a.k_pad % 32 || a.n_pad <= 0 || a.n_pad % 16 || (reinterpret_cast<uintptr_t>(a.w) & 15u))
-    return PVN3D_ERR_INVALID_ARG;   // the weights are read 16 bytes at a time, by TMA or cp.async
+    return PVN3D_ERR_INVALID_ARG;   // the weights are read 16 bytes at a time, by TMA
   a.bn = mma_n(a.n_pad);
   a.acc_ld = std::max(32, a.bn);
   const size_t stage_bytes = kMlpBM * 128 + align_up(static_cast<size_t>(a.bn) * 128, 1024);
@@ -995,16 +909,9 @@ int launch_mlp(MlpArgs &a, cudaStream_t st) {
   if (stages < 3) return PVN3D_ERR_UNSUPPORTED;
   a.stages = stages;
   const size_t smem = mlp_smem_front(stages, a.bn, a.acc_ld) + kMlpEpiWarps * 4096 + sizeof(MlpSmemCtl);
-  a.use_tma = weight_tensor_map(&a.tmap, a.w, a.k_pad, a.n_pad, a.bn) ? 1 : 0;
-  const int sms = std::max(1, sm_count() - a.reserve_sms);
+  if (!weight_tensor_map(&a.tmap, a.w, a.k_pad, a.n_pad, a.bn)) return PVN3D_ERR_UNSUPPORTED;
   const long long tiles = ((a.rows + kMlpBM - 1) / kMlpBM) * ceil_div(a.n_pad, a.bn);
-  auto kern = mlp_layer_kernel<PRO, EPI>;
-  static PerDeviceOnce once;
-  PVN3D_ONCE_PER_DEVICE(once, cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, kMlpSmemMax),
-                        "mlp smem attr");
-  const unsigned grid = static_cast<unsigned>(std::min<long long>(tiles, sms));
-  kern<<<grid, kMlpThreads, smem, st>>>(a);
-  return check_launch("mlp_layer_kernel");
+  return launch_persistent<mlp_layer_kernel<PRO, EPI>>(a, tiles, kMlpThreads, smem, a.reserve_sms, st, "mlp_layer_kernel");
 }
 
 // =====================================================================================================
@@ -1322,16 +1229,9 @@ int launch_sa_fact2(Sa2Args &g, int stages, cudaStream_t st) {
   if (a.rows <= 0) return PVN3D_OK;
   a.stages = stages;
   const size_t smem = sa2_smem(a.k_pad, N2, g.k3_pad, N3, stages).bytes;
-  const int sms = std::max(1, sm_count() - a.reserve_sms);
   const long long tiles = (a.rows + kMlpBM - 1) / kMlpBM;
   if (tiles * (a.k_pad / 32) > 0x7fffffffll) return PVN3D_ERR_UNSUPPORTED;   // the kernel counts K chunks in 32 bits
-  auto kern = mlp_sa_fact2_kernel<N2, N3>;
-  static PerDeviceOnce once;
-  PVN3D_ONCE_PER_DEVICE(once, cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, kMlpSmemMax),
-                        "mlp sa_fact2 smem attr");
-  const unsigned grid = static_cast<unsigned>(std::min<long long>(tiles, sms));
-  kern<<<grid, kSa2Threads, smem, st>>>(g);
-  return check_launch("mlp_sa_fact2_kernel");
+  return launch_persistent<mlp_sa_fact2_kernel<N2, N3>>(g, tiles, kSa2Threads, smem, a.reserve_sms, st, "mlp_sa_fact2_kernel");
 }
 
 template <int N2>
@@ -1652,20 +1552,13 @@ int launch_sa_fact2w(Sa2wArgs &g, int stages, cudaStream_t st) {
   if (a.rows <= 0) return PVN3D_OK;
   a.stages = stages;
   const size_t smem = sa2w_smem(a.k_pad, g.k3_pad, stages).bytes;
-  const int sms = std::max(1, sm_count() - a.reserve_sms);
   const long long tiles = (a.rows + kSa2wBM - 1) / kSa2wBM;
   const long long chunks = static_cast<long long>(ceil_div(a.n_pad, 128)) * (a.k_pad / 32) +
                            static_cast<long long>(ceil_div(g.n3_pad, 128)) * (g.k3_pad / 32);
   if (tiles * chunks > 0x7fffffffll) return PVN3D_ERR_UNSUPPORTED;   // the kernel counts weight chunks in 32 bits
   if (!weight_tensor_map(&a.tmap, a.w, a.k_pad, a.n_pad, 128) || !weight_tensor_map(&g.tmap3, g.w3, g.k3_pad, g.n3_pad, 128))
     return PVN3D_ERR_UNSUPPORTED;
-  auto kern = mlp_sa_fact2w_kernel;
-  static PerDeviceOnce once;
-  PVN3D_ONCE_PER_DEVICE(once, cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, kMlpSmemMax),
-                        "mlp sa_fact2w smem attr");
-  const unsigned grid = static_cast<unsigned>(std::min<long long>(tiles, sms));
-  kern<<<grid, kSa2wThreads, smem, st>>>(g);
-  return check_launch("mlp_sa_fact2w_kernel");
+  return launch_persistent<mlp_sa_fact2w_kernel>(g, tiles, kSa2wThreads, smem, a.reserve_sms, st, "mlp_sa_fact2w_kernel");
 }
 
 // =====================================================================================================
@@ -2027,21 +1920,14 @@ int launch_fp2(Fp2Args &g, cudaStream_t st) {
     return PVN3D_ERR_UNSUPPORTED;   // the kernel counts ring items in 32 bits
   if (!weight_tensor_map(&a.tmap, a.w, a.k_pad, a.n_pad, 128) || !weight_tensor_map(&g.tmap2, g.w2, g.k2_pad, g.n2_pad, 128))
     return PVN3D_ERR_UNSUPPORTED;
-  const int sms = std::max(1, sm_count() - a.reserve_sms);
-  auto kern = mlp_fp2_kernel;
-  static PerDeviceOnce once;
-  PVN3D_ONCE_PER_DEVICE(once, cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, kMlpSmemMax),
-                        "mlp fp2 smem attr");
-  const unsigned grid = static_cast<unsigned>(std::min<long long>(tiles, sms));
-  kern<<<grid, kFp2Threads, smem, st>>>(g);
-  return check_launch("mlp_fp2_kernel");
+  return launch_persistent<mlp_fp2_kernel>(g, tiles, kFp2Threads, smem, a.reserve_sms, st, "mlp_fp2_kernel");
 }
 
 // =====================================================================================================
 // The skip term and the second layer of a FACTORED FP module whose skip is the SA1 factor table (FP1), in ONE
 // persistent kernel.
 //
-// As two launches (pvn3d_mlp_dense for S = W1s . table + b1, then pvn3d_mlp_fp_fact with OUT_CN) S goes to HBM and
+// As two launches (pvn3d_mlp_dense for S = W1s . table + b1, then pvn3d_mlp_fp_fact) S goes to HBM and
 // straight back: 201 + 201 MB per 32-frame batch of 12288 points.  Here it never leaves the SM.  Per 64-row tile:
 //   loader    (warp 16)     brings W_s and W2 into shared memory once (TMA), then the tile's 32-column table rows by
 //                           TMA (SWIZZLE_128B: the wgmma layout) into a ring slot;
@@ -2055,9 +1941,10 @@ int launch_fp2(Fp2Args &g, cudaStream_t st) {
 //                           [b][128][n_unknown] from the fragment: the 8 rows of a lane quad are 8 consecutive points,
 //                           whole 32-byte sectors of one channel.
 // Every output element keeps the operands, the wgmma shape, K order and epilogue arithmetic of the two launches, so
-// the results are bit-identical.
+// the results are bit-identical to their point-major rows, transposed.
 // Where the layer-2 output goes (the kernel's template parameter):
-//   FPF2_OUT_CN    [b][128][n_unknown] channel-major, streaming stores: the layout Pointnet2MSG.forward returns;
+//   FPF2_OUT_CN    [b][128][n_unknown] channel-major, streaming stores: the layout Pointnet2MSG.forward returns,
+//                  written from the fragment with no transposing pass;
 //   FPF2_OUT_ROWS  relu(acc + b2) rounded to TF32, point-major into columns col0 .. col0+127 of rows ldo apart: a lane
 //                  quad writes each 32-byte row segment (whole sectors), as mlp_fp2_kernel does.  The heads' table.
 enum { FPF2_OUT_CN = 0, FPF2_OUT_ROWS = 1 };
@@ -2302,31 +2189,7 @@ int launch_fp_fact2(FpFact2Args &g, const float *table, const float *ws, const f
   if (!weight_tensor_map(&a.tmap, table, 32, static_cast<int>(a.rows), kFpf2BM) ||
       !weight_tensor_map(&g.tmap_s, ws, 32, 128, 128) || !weight_tensor_map(&g.tmap_w2, w2, 128, 128, 128))
     return PVN3D_ERR_UNSUPPORTED;
-  const int sms = std::max(1, sm_count() - a.reserve_sms);
-  auto kern = mlp_fp_fact2_kernel<OUT>;
-  static PerDeviceOnce once;
-  PVN3D_ONCE_PER_DEVICE(once, cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, kMlpSmemMax),
-                        "mlp fp_fact2 smem attr");
-  const unsigned grid = static_cast<unsigned>(std::min<long long>(tiles, sms));
-  kern<<<grid, kFpf2Threads, smem, st>>>(g);
-  return check_launch("mlp_fp_fact2_kernel");
-}
-
-int dispatch(MlpArgs &a, int pro, int pool, cudaStream_t st) {
-  if (pool) {
-    if (pool != 8 && pool != 16 && pool != 32) return PVN3D_ERR_UNSUPPORTED;
-    a.pool = pool;
-    // 128-channel pooled layers: transposed read of the accumulator tile, register max instead of shuffles
-    if (pro == PRO_DENSE && a.n_pad == 128) return launch_mlp<PRO_DENSE, EPI_MAXPOOL_T>(a, st);
-    if (pro == PRO_DENSE) return launch_mlp<PRO_DENSE, EPI_MAXPOOL>(a, st);
-    if (pro == PRO_SA_FACT) return launch_mlp<PRO_SA_FACT, EPI_MAXPOOL>(a, st);
-    return PVN3D_ERR_INVALID_ARG;
-  }
-  a.pool = 0;
-  if (pro == PRO_DENSE) return launch_mlp<PRO_DENSE, EPI_STORE>(a, st);
-  if (pro == PRO_SA_FACT) return launch_mlp<PRO_SA_FACT, EPI_STORE>(a, st);
-  if (pro == PRO_FP_FACT) return launch_mlp<PRO_FP_FACT, EPI_STORE>(a, st);
-  return launch_mlp<PRO_FP_INTERP, EPI_STORE>(a, st);
+  return launch_persistent<mlp_fp_fact2_kernel<OUT>>(g, tiles, kFpf2Threads, smem, a.reserve_sms, st, "mlp_fp_fact2_kernel");
 }
 
 // ---- factored first layer of an SA scale -------------------------------------------------------------
@@ -2425,6 +2288,58 @@ __global__ void __launch_bounds__(kGatherThreads) gather_pixel_rows_kernel(const
 
 using namespace pvn3d;
 
+// the shapes a pair of layers must have, `first` feeding `second`: K a positive multiple of 32, N one of 16, and the
+// second layer's K covering the first one's N
+static bool layer_pair_ok(const pvn3d_mlp_layer_t *first, const pvn3d_mlp_layer_t *second) {
+  return first && second && first->k_pad > 0 && first->k_pad % 32 == 0 && first->n_pad > 0 && first->n_pad % 16 == 0 &&
+         second->k_pad >= first->n_pad && second->k_pad % 32 == 0 && second->n_pad > 0 && second->n_pad % 16 == 0;
+}
+// both pointers of a layer set, w 16-byte aligned (it is read 16 bytes at a time)
+static bool layer_ptrs_ok(const pvn3d_mlp_layer_t *l) {
+  return l->w && l->bias && !(reinterpret_cast<uintptr_t>(l->w) & 15u);
+}
+
+// the operand checks and kernel arguments of a layer on relu(U[idx] - V), the second of a factored SA scale
+// (pvn3d_mlp_sa_fact, pvn3d_mlp_sa_fact2, pvn3d_mlp_sa_fact2w): PVN3D_ERR_INVALID_ARG for a bad operand, then
+// PVN3D_ERR_UNSUPPORTED for sizes beyond the kernels' 32-bit row arithmetic
+static int sa_fact_args(const float *u, const float *v, int ldu, int c_valid, const int *idx, int b, int n, int m, int ns,
+                        const pvn3d_mlp_layer_t &layer, int flags, float *out, int ldo, int col0, MlpArgs &a) {
+  if (!u || !v || !idx || !layer.w || !layer.bias || !out || b < 0 || n <= 0 || m < 0 || ns <= 0 || c_valid <= 0 ||
+      c_valid % 4 || ldu < c_valid || ldu % 4 || layer.k_pad < c_valid || ldo % 4 || col0 % 4 ||
+      (reinterpret_cast<uintptr_t>(u) & 15u) || (reinterpret_cast<uintptr_t>(v) & 15u))
+    return PVN3D_ERR_INVALID_ARG;
+  if (static_cast<long long>(m) * ns > 0x3fffffffll || static_cast<long long>(b) * n > 0x7fffffffll ||
+      static_cast<long long>(b) * m > 0x7fffffffll)
+    return PVN3D_ERR_UNSUPPORTED;
+  a.w = layer.w; a.bias = layer.bias; a.k_pad = layer.k_pad; a.n_pad = layer.n_pad;
+  a.rows = static_cast<long long>(b) * m * ns;
+  a.feat = u; a.new_xyz = v; a.ldf = ldu; a.c_feat = c_valid; a.idx = idx;
+  a.n = n; a.m = m; a.ns = ns;
+  a.out = out; a.ldo = ldo; a.col0 = col0;
+  a.relu = flags & PVN3D_MLP_RELU; a.round_out = (flags & PVN3D_MLP_ROUND_OUT) ? 1 : 0;
+  a.reserve_sms = (flags >> 8) & 0xff;
+  return PVN3D_OK;
+}
+
+// the same for a layer on [interpolated known descriptors | skip], the first of an FP module (pvn3d_mlp_fp_first,
+// pvn3d_mlp_fp2)
+static int fp_interp_args(const float *known_feat_pm, int c2, const int *nn_idx, const float *nn_w, const float *skip_pm,
+                          int lds, int c1, int b, int n_unknown, int m_known, const pvn3d_mlp_layer_t &layer, int flags,
+                          float *out, int ldo, int col0, MlpArgs &a) {
+  if (!known_feat_pm || !nn_idx || !nn_w || !layer.w || !layer.bias || !out || b < 0 || n_unknown < 0 || m_known <= 0 ||
+      c2 <= 0 || c1 < 0 || (c1 > 0 && (!skip_pm || lds < c1)) || layer.k_pad < c2 + c1 || ldo % 4 || col0 % 4)
+    return PVN3D_ERR_INVALID_ARG;
+  if (static_cast<long long>(b) * m_known > 0x7fffffffll || n_unknown > 0x3fffffff) return PVN3D_ERR_UNSUPPORTED;
+  a.w = layer.w; a.bias = layer.bias; a.k_pad = layer.k_pad; a.n_pad = layer.n_pad;
+  a.rows = static_cast<long long>(b) * n_unknown;
+  a.known_feat = known_feat_pm; a.c2 = c2; a.nn_idx = nn_idx; a.nn_w = nn_w; a.skip = skip_pm;
+  a.lds = lds; a.c1 = c1; a.n_unknown = n_unknown; a.m_known = m_known;
+  a.out = out; a.ldo = ldo; a.col0 = col0;
+  a.relu = flags & PVN3D_MLP_RELU; a.round_out = (flags & PVN3D_MLP_ROUND_OUT) ? 1 : 0;
+  a.reserve_sms = (flags >> 8) & 0xff;
+  return PVN3D_OK;
+}
+
 extern "C" int pvn3d_mlp_dense(const float *a, int lda, int a_cols, long long rows, const float *w,
                                const float *bias, int k_pad, int n_pad, int flags, int pool,
                                float *out, int ldo, int col0, pvn3d_stream_t stream) {
@@ -2439,7 +2354,10 @@ extern "C" int pvn3d_mlp_dense(const float *a, int lda, int a_cols, long long ro
   m.relu = flags & PVN3D_MLP_RELU; m.round_out = (flags & PVN3D_MLP_ROUND_OUT) ? 1 : 0;
   m.a_tf32 = (flags & PVN3D_MLP_A_TF32) ? 1 : 0;
   m.reserve_sms = (flags >> 8) & 0xff;
-  return dispatch(m, PRO_DENSE, pool, as_stream(stream));
+  if (!pool) return launch_mlp<PRO_DENSE, EPI_STORE>(m, as_stream(stream));
+  if (pool != 8 && pool != 16 && pool != 32) return PVN3D_ERR_UNSUPPORTED;
+  m.pool = pool;
+  return launch_mlp<PRO_DENSE, EPI_MAXPOOL>(m, as_stream(stream));
 }
 
 extern "C" int pvn3d_mlp_fp_first(const float *known_feat_pm, int c2, const int *nn_idx,
@@ -2447,20 +2365,11 @@ extern "C" int pvn3d_mlp_fp_first(const float *known_feat_pm, int c2, const int 
                                   int n_unknown, int m_known, const float *w, const float *bias,
                                   int k_pad, int n_pad, int flags, float *out, int ldo, int col0,
                                   pvn3d_stream_t stream) {
-  if (!known_feat_pm || !nn_idx || !nn_w || !w || !bias || !out || b < 0 || n_unknown < 0 ||
-      m_known <= 0 || c2 <= 0 || c1 < 0 || (c1 > 0 && (!skip_pm || lds < c1)) || k_pad < c2 + c1 ||
-      ldo % 4 || col0 % 4)
-    return PVN3D_ERR_INVALID_ARG;
-  if (static_cast<long long>(b) * m_known > 0x7fffffffll || n_unknown > 0x3fffffff)
-    return PVN3D_ERR_UNSUPPORTED;
   MlpArgs a{};
-  a.w = w; a.bias = bias; a.rows = static_cast<long long>(b) * n_unknown; a.k_pad = k_pad; a.n_pad = n_pad;
-  a.known_feat = known_feat_pm; a.c2 = c2; a.nn_idx = nn_idx; a.nn_w = nn_w; a.skip = skip_pm;
-  a.lds = lds; a.c1 = c1; a.n_unknown = n_unknown; a.m_known = m_known;
-  a.out = out; a.ldo = ldo; a.col0 = col0;
-  a.relu = flags & PVN3D_MLP_RELU; a.round_out = (flags & PVN3D_MLP_ROUND_OUT) ? 1 : 0;
-  a.reserve_sms = (flags >> 8) & 0xff;
-  return dispatch(a, PRO_FP_INTERP, 0, as_stream(stream));
+  const int rc = fp_interp_args(known_feat_pm, c2, nn_idx, nn_w, skip_pm, lds, c1, b, n_unknown, m_known,
+                                pvn3d_mlp_layer_t{w, bias, k_pad, n_pad}, flags, out, ldo, col0, a);
+  if (rc != PVN3D_OK) return rc;
+  return launch_mlp<PRO_FP_INTERP, EPI_STORE>(a, as_stream(stream));
 }
 
 extern "C" int pvn3d_three_nn_weights(const float *dist2, long long rows, float *weight,
@@ -2497,51 +2406,37 @@ extern "C" int pvn3d_sa_centre_term(const float *centres, const float *wx, const
 
 extern "C" int pvn3d_mlp_sa_fact(const float *u, const float *v, int ldu, int c_valid, const int *idx, int b, int n,
                                  int m, int ns, const float *w, const float *bias, int k_pad, int n_pad, int flags,
-                                 int pool, float *out, int ldo, int col0, pvn3d_stream_t stream) {
-  if (!u || !v || !idx || !w || !bias || !out || b < 0 || n <= 0 || m < 0 || ns <= 0 || c_valid <= 0 ||
-      c_valid % 4 || ldu < c_valid || ldu % 4 || k_pad < c_valid || ldo % 4 || col0 % 4 ||
-      (reinterpret_cast<uintptr_t>(u) & 15u) || (reinterpret_cast<uintptr_t>(v) & 15u))
-    return PVN3D_ERR_INVALID_ARG;
-  if (pool && pool != ns) return PVN3D_ERR_INVALID_ARG;
-  if (static_cast<long long>(m) * ns > 0x3fffffffll || static_cast<long long>(b) * n > 0x7fffffffll ||
-      static_cast<long long>(b) * m > 0x7fffffffll)
-    return PVN3D_ERR_UNSUPPORTED;
+                                 float *out, int ldo, int col0, pvn3d_stream_t stream) {
   MlpArgs a{};
-  a.w = w; a.bias = bias; a.rows = static_cast<long long>(b) * m * ns; a.k_pad = k_pad; a.n_pad = n_pad;
-  a.feat = u; a.new_xyz = v; a.ldf = ldu; a.c_feat = c_valid; a.idx = idx;
-  a.n = n; a.m = m; a.ns = ns;
-  a.out = out; a.ldo = ldo; a.col0 = col0;
-  a.relu = flags & PVN3D_MLP_RELU; a.round_out = (flags & PVN3D_MLP_ROUND_OUT) ? 1 : 0;
-  a.reserve_sms = (flags >> 8) & 0xff;
-  return dispatch(a, PRO_SA_FACT, pool, as_stream(stream));
+  const int rc = sa_fact_args(u, v, ldu, c_valid, idx, b, n, m, ns, pvn3d_mlp_layer_t{w, bias, k_pad, n_pad}, flags, out,
+                              ldo, col0, a);
+  if (rc != PVN3D_OK) return rc;
+  return launch_mlp<PRO_SA_FACT, EPI_STORE>(a, as_stream(stream));
+}
+
+// the argument checks and kernel arguments pvn3d_mlp_sa_fact2 (G = Sa2Args) and pvn3d_mlp_sa_fact2w (Sa2wArgs) share
+template <typename G>
+static int sa_fact2_args(const float *u, const float *v, int ldu, int c_valid, const int *idx, int b, int n, int m, int ns,
+                         const pvn3d_mlp_layer_t *layer2, const pvn3d_mlp_layer_t *layer3, int flags, int pool, float *out,
+                         int ldo, int col0, G &g) {
+  if (!layer_pair_ok(layer2, layer3) || !layer_ptrs_ok(layer2) || !layer_ptrs_ok(layer3) || pool != ns)
+    return PVN3D_ERR_INVALID_ARG;
+  const int rc = sa_fact_args(u, v, ldu, c_valid, idx, b, n, m, ns, *layer2, flags, out, ldo, col0, g.a);
+  if (rc != PVN3D_OK) return rc;
+  g.a.relu = 1;
+  g.a.pool = ns;
+  g.w3 = layer3->w; g.bias3 = layer3->bias; g.k3_pad = layer3->k_pad; g.n3_pad = layer3->n_pad;
+  return PVN3D_OK;
 }
 
 extern "C" int pvn3d_mlp_sa_fact2(const float *u, const float *v, int ldu, int c_valid, const int *idx, int b, int n,
                                   int m, int ns, const pvn3d_mlp_layer_t *layer2, const pvn3d_mlp_layer_t *layer3,
                                   int flags, int pool, float *out, int ldo, int col0, pvn3d_stream_t stream) {
-  if (!u || !v || !idx || !layer2 || !layer3 || !layer2->w || !layer2->bias || !layer3->w || !layer3->bias || !out ||
-      b < 0 || n <= 0 || m < 0 || ns <= 0 || c_valid <= 0 || c_valid % 4 || ldu < c_valid || ldu % 4 ||
-      layer2->k_pad < c_valid || layer2->k_pad <= 0 || layer2->k_pad % 32 || layer2->n_pad <= 0 || layer2->n_pad % 16 ||
-      layer3->k_pad < layer2->n_pad || layer3->k_pad % 32 || layer3->n_pad <= 0 || layer3->n_pad % 16 || ldo % 4 ||
-      col0 % 4 || (reinterpret_cast<uintptr_t>(u) & 15u) || (reinterpret_cast<uintptr_t>(v) & 15u) ||
-      (reinterpret_cast<uintptr_t>(layer2->w) & 15u) || (reinterpret_cast<uintptr_t>(layer3->w) & 15u))
-    return PVN3D_ERR_INVALID_ARG;
-  if (pool != ns) return PVN3D_ERR_INVALID_ARG;
+  Sa2Args g{};
+  const int rc = sa_fact2_args(u, v, ldu, c_valid, idx, b, n, m, ns, layer2, layer3, flags, pool, out, ldo, col0, g);
+  if (rc != PVN3D_OK) return rc;
   const int stages = sa2_stages(layer2->k_pad, layer2->n_pad, layer3->k_pad, layer3->n_pad, ns);
   if (!stages) return PVN3D_ERR_UNSUPPORTED;
-  if (static_cast<long long>(m) * ns > 0x3fffffffll || static_cast<long long>(b) * n > 0x7fffffffll ||
-      static_cast<long long>(b) * m > 0x7fffffffll)
-    return PVN3D_ERR_UNSUPPORTED;
-  Sa2Args g{};
-  MlpArgs &a = g.a;
-  a.w = layer2->w; a.bias = layer2->bias; a.k_pad = layer2->k_pad; a.n_pad = layer2->n_pad;
-  a.rows = static_cast<long long>(b) * m * ns;
-  a.feat = u; a.new_xyz = v; a.ldf = ldu; a.c_feat = c_valid; a.idx = idx;
-  a.n = n; a.m = m; a.ns = ns; a.pool = pool;
-  a.out = out; a.ldo = ldo; a.col0 = col0; a.relu = 1;
-  a.round_out = (flags & PVN3D_MLP_ROUND_OUT) ? 1 : 0;
-  a.reserve_sms = (flags >> 8) & 0xff;
-  g.w3 = layer3->w; g.bias3 = layer3->bias; g.k3_pad = layer3->k_pad; g.n3_pad = layer3->n_pad;
   switch (mma_n(layer2->n_pad)) {
     case 16: return launch_sa_fact2_n3<16>(g, stages, as_stream(stream));
     case 32: return launch_sa_fact2_n3<32>(g, stages, as_stream(stream));
@@ -2551,78 +2446,43 @@ extern "C" int pvn3d_mlp_sa_fact2(const float *u, const float *v, int ldu, int c
 }
 
 extern "C" int pvn3d_mlp_sa_fact2_supported(const pvn3d_mlp_layer_t *layer2, const pvn3d_mlp_layer_t *layer3, int ns) {
-  if (!layer2 || !layer3 || layer2->k_pad <= 0 || layer2->k_pad % 32 || layer2->n_pad <= 0 || layer2->n_pad % 16 ||
-      layer3->k_pad < layer2->n_pad || layer3->k_pad % 32 || layer3->n_pad <= 0 || layer3->n_pad % 16)
-    return 0;
+  if (!layer_pair_ok(layer2, layer3)) return 0;
   return sa2_stages(layer2->k_pad, layer2->n_pad, layer3->k_pad, layer3->n_pad, ns) ? 1 : 0;
 }
 
 extern "C" int pvn3d_mlp_sa_fact2w(const float *u, const float *v, int ldu, int c_valid, const int *idx, int b, int n,
                                    int m, int ns, const pvn3d_mlp_layer_t *layer2, const pvn3d_mlp_layer_t *layer3,
                                    int flags, int pool, float *out, int ldo, int col0, pvn3d_stream_t stream) {
-  if (!u || !v || !idx || !layer2 || !layer3 || !layer2->w || !layer2->bias || !layer3->w || !layer3->bias || !out ||
-      b < 0 || n <= 0 || m < 0 || ns <= 0 || c_valid <= 0 || c_valid % 4 || ldu < c_valid || ldu % 4 ||
-      layer2->k_pad < c_valid || layer2->k_pad <= 0 || layer2->k_pad % 32 || layer2->n_pad <= 0 || layer2->n_pad % 16 ||
-      layer3->k_pad < layer2->n_pad || layer3->k_pad % 32 || layer3->n_pad <= 0 || layer3->n_pad % 16 || ldo % 4 ||
-      col0 % 4 || (reinterpret_cast<uintptr_t>(u) & 15u) || (reinterpret_cast<uintptr_t>(v) & 15u) ||
-      (reinterpret_cast<uintptr_t>(layer2->w) & 15u) || (reinterpret_cast<uintptr_t>(layer3->w) & 15u))
-    return PVN3D_ERR_INVALID_ARG;
-  if (pool != ns) return PVN3D_ERR_INVALID_ARG;
+  Sa2wArgs g{};
+  const int rc = sa_fact2_args(u, v, ldu, c_valid, idx, b, n, m, ns, layer2, layer3, flags, pool, out, ldo, col0, g);
+  if (rc != PVN3D_OK) return rc;
   const int stages = sa2w_stages(layer2->k_pad, layer2->n_pad, layer3->k_pad, layer3->n_pad, ns);
   if (!stages) return PVN3D_ERR_UNSUPPORTED;
-  if (static_cast<long long>(m) * ns > 0x3fffffffll || static_cast<long long>(b) * n > 0x7fffffffll ||
-      static_cast<long long>(b) * m > 0x7fffffffll)
-    return PVN3D_ERR_UNSUPPORTED;
-  Sa2wArgs g{};
-  MlpArgs &a = g.a;
-  a.w = layer2->w; a.bias = layer2->bias; a.k_pad = layer2->k_pad; a.n_pad = layer2->n_pad;
-  a.rows = static_cast<long long>(b) * m * ns;
-  a.feat = u; a.new_xyz = v; a.ldf = ldu; a.c_feat = c_valid; a.idx = idx;
-  a.n = n; a.m = m; a.ns = ns; a.pool = pool;
-  a.out = out; a.ldo = ldo; a.col0 = col0; a.relu = 1;
-  a.round_out = (flags & PVN3D_MLP_ROUND_OUT) ? 1 : 0;
-  a.reserve_sms = (flags >> 8) & 0xff;
-  g.w3 = layer3->w; g.bias3 = layer3->bias; g.k3_pad = layer3->k_pad; g.n3_pad = layer3->n_pad;
   return launch_sa_fact2w(g, stages, as_stream(stream));
 }
 
 extern "C" int pvn3d_mlp_sa_fact2w_supported(const pvn3d_mlp_layer_t *layer2, const pvn3d_mlp_layer_t *layer3, int ns) {
-  if (!layer2 || !layer3 || layer2->k_pad <= 0 || layer2->k_pad % 32 || layer2->n_pad <= 0 || layer2->n_pad % 16 ||
-      layer3->k_pad < layer2->n_pad || layer3->k_pad % 32 || layer3->n_pad <= 0 || layer3->n_pad % 16)
-    return 0;
+  if (!layer_pair_ok(layer2, layer3)) return 0;
   return sa2w_stages(layer2->k_pad, layer2->n_pad, layer3->k_pad, layer3->n_pad, ns) ? 1 : 0;
 }
 
 extern "C" int pvn3d_mlp_fp2(const float *known_feat_pm, int c2, const int *nn_idx, const float *nn_w, const float *skip_pm,
                              int lds, int c1, int b, int n_unknown, int m_known, const pvn3d_mlp_layer_t *layer1,
                              const pvn3d_mlp_layer_t *layer2, int flags, float *out, int ldo, int col0, pvn3d_stream_t stream) {
-  if (!known_feat_pm || !nn_idx || !nn_w || !layer1 || !layer2 || !layer1->w || !layer1->bias || !layer2->w || !layer2->bias ||
-      !out || b < 0 || n_unknown < 0 || m_known <= 0 || c2 <= 0 || c1 < 0 || (c1 > 0 && (!skip_pm || lds < c1)) ||
-      layer1->k_pad < c2 + c1 || layer1->k_pad % 32 || layer1->n_pad <= 0 || layer1->n_pad % 16 || layer2->k_pad < layer1->n_pad ||
-      layer2->k_pad % 32 || layer2->n_pad <= 0 || layer2->n_pad % 16 || ldo % 4 || col0 % 4 ||
-      (reinterpret_cast<uintptr_t>(layer1->w) & 15u) || (reinterpret_cast<uintptr_t>(layer2->w) & 15u))
-    return PVN3D_ERR_INVALID_ARG;
-  int a_stages = 0, w_stages = 0;
-  if (!fp2_stages(layer1->k_pad, layer1->n_pad, layer2->k_pad, layer2->n_pad, &a_stages, &w_stages)) return PVN3D_ERR_UNSUPPORTED;
-  if (static_cast<long long>(b) * m_known > 0x7fffffffll || n_unknown > 0x3fffffff) return PVN3D_ERR_UNSUPPORTED;
+  if (!layer_pair_ok(layer1, layer2) || !layer_ptrs_ok(layer1) || !layer_ptrs_ok(layer2)) return PVN3D_ERR_INVALID_ARG;
   Fp2Args g{};
-  MlpArgs &a = g.a;
-  a.w = layer1->w; a.bias = layer1->bias; a.k_pad = layer1->k_pad; a.n_pad = layer1->n_pad;
-  a.rows = static_cast<long long>(b) * n_unknown;
-  a.known_feat = known_feat_pm; a.c2 = c2; a.nn_idx = nn_idx; a.nn_w = nn_w; a.skip = skip_pm;
-  a.lds = lds; a.c1 = c1; a.n_unknown = n_unknown; a.m_known = m_known;
-  a.out = out; a.ldo = ldo; a.col0 = col0; a.relu = 1;
-  a.round_out = (flags & PVN3D_MLP_ROUND_OUT) ? 1 : 0;
-  a.reserve_sms = (flags >> 8) & 0xff;
+  const int rc = fp_interp_args(known_feat_pm, c2, nn_idx, nn_w, skip_pm, lds, c1, b, n_unknown, m_known, *layer1, flags,
+                                out, ldo, col0, g.a);
+  if (rc != PVN3D_OK) return rc;
+  if (!fp2_stages(layer1->k_pad, layer1->n_pad, layer2->k_pad, layer2->n_pad, &g.a_stages, &g.w_stages))
+    return PVN3D_ERR_UNSUPPORTED;
+  g.a.relu = 1;
   g.w2 = layer2->w; g.bias2 = layer2->bias; g.k2_pad = layer2->k_pad; g.n2_pad = layer2->n_pad;
-  g.a_stages = a_stages; g.w_stages = w_stages;
   return launch_fp2(g, as_stream(stream));
 }
 
 extern "C" int pvn3d_mlp_fp2_supported(const pvn3d_mlp_layer_t *layer1, const pvn3d_mlp_layer_t *layer2) {
-  if (!layer1 || !layer2 || layer1->k_pad <= 0 || layer1->k_pad % 32 || layer1->n_pad <= 0 || layer1->n_pad % 16 ||
-      layer2->k_pad < layer1->n_pad || layer2->k_pad % 32 || layer2->n_pad <= 0 || layer2->n_pad % 16)
-    return 0;
+  if (!layer_pair_ok(layer1, layer2)) return 0;
   int a_stages = 0, w_stages = 0;
   return fp2_stages(layer1->k_pad, layer1->n_pad, layer2->k_pad, layer2->n_pad, &a_stages, &w_stages) ? 1 : 0;
 }
@@ -2643,14 +2503,7 @@ extern "C" int pvn3d_mlp_fp_fact(const float *p, const float *s, int ld, int c_v
   a.out = out; a.ldo = ldo; a.col0 = col0;
   a.relu = flags & PVN3D_MLP_RELU; a.round_out = (flags & PVN3D_MLP_ROUND_OUT) ? 1 : 0;
   a.reserve_sms = (flags >> 8) & 0xff;
-  if (flags & PVN3D_MLP_OUT_CN) {
-    // out = [b][n_pad][n_unknown]: one or two 128-channel accumulators per tile, 32-point groups inside a frame
-    if ((n_pad != 128 && n_pad != 256) || n_unknown % 32 || (reinterpret_cast<uintptr_t>(out) & 15u))
-      return PVN3D_ERR_UNSUPPORTED;
-    a.out_cn = n_unknown; a.pool = 0; a.ldo = n_pad; a.col0 = 0;
-    return launch_mlp<PRO_FP_FACT, EPI_STORE_T>(a, as_stream(stream));
-  }
-  return dispatch(a, PRO_FP_FACT, 0, as_stream(stream));
+  return launch_mlp<PRO_FP_FACT, EPI_STORE>(a, as_stream(stream));
 }
 
 // the argument checks and kernel arguments pvn3d_mlp_fp_fact2 and pvn3d_mlp_fp_fact2_rows share
@@ -2732,7 +2585,7 @@ extern "C" int pvn3d_mlp_dense_frame_bias(const float *a, int lda, int a_cols, l
   m.a_tf32 = (flags & PVN3D_MLP_A_TF32) ? 1 : 0;
   m.reserve_sms = (flags >> 8) & 0xff;
   m.bias_npb = rows_per_frame;
-  return dispatch(m, PRO_DENSE, 0, as_stream(stream));
+  return launch_mlp<PRO_DENSE, EPI_STORE>(m, as_stream(stream));
 }
 
 extern "C" int pvn3d_mlp_dense_sum32(const float *a, int lda, int a_cols, long long rows, const float *w,

@@ -24,9 +24,9 @@ from typing import List, Tuple
 
 import torch
 
-from . import _ext, _lib
-from ._lib import check, ptr
-from .mlp import PackedLayer, _flags, _stream, fold_conv_bn, tf32_round
+from . import _ext
+from ._lib import call, ptr
+from .mlp import PackedLayer, _flags, fold_conv_bn, tf32_round
 
 
 def _conv1d_wb(conv: torch.nn.Conv1d) -> Tuple[torch.Tensor, torch.Tensor]:
@@ -37,12 +37,8 @@ def _conv1d_wb(conv: torch.nn.Conv1d) -> Tuple[torch.Tensor, torch.Tensor]:
 
 def _dense(a_ptr: int, lda: int, a_cols: int, rows: int, layer: PackedLayer, out: torch.Tensor, col0: int = 0, relu=True,
            round_out=True, a_tf32=True):
-    lib = _lib.load()
-    dev = out.device
-    with torch.cuda.device(dev):
-        rc = lib.pvn3d_mlp_dense(a_ptr, lda, a_cols, rows, ptr(layer.w), ptr(layer.bias), layer.k_pad, layer.n_pad,
-                                 _flags(relu, round_out, a_tf32), 0, ptr(out), out.size(-1), col0, _stream(dev))
-    check(rc, "pvn3d_mlp_dense")
+    call("pvn3d_mlp_dense", out.device, a_ptr, lda, a_cols, rows, ptr(layer.w), ptr(layer.bias), layer.k_pad, layer.n_pad,
+         _flags(relu, round_out, a_tf32), 0, ptr(out), out.size(-1), col0)
     return out
 
 
@@ -109,17 +105,13 @@ class FusedHeads:
         """DenseFusion and the heads on an activation table x [B*N, TABLE_COLS] (new_table) whose first 256 columns
         hold feat_1 -> the outputs of forward().  Columns 256.. are overwritten."""
         assert x.shape == (b * n, self.TABLE_COLS) and x.is_contiguous() and x.is_cuda
-        lib = _lib.load()
         rows = b * n
         _dense(x.data_ptr(), 1280, 256, rows, self.la, x, col0=256)                      # feat_2 and relu(conv3(feat_1))
         # mean over the points of relu(conv4(.)): 32-row partial sums straight from the accumulator
         groups = (rows + 31) // 32
         part = torch.empty((groups, self.lb.n_pad), dtype=torch.float32, device=self.dev)
-        with torch.cuda.device(self.dev):
-            rc = lib.pvn3d_mlp_dense_sum32(x.data_ptr() + 768 * 4, 1280, 512, rows, ptr(self.lb.w), ptr(self.lb.bias),
-                                           self.lb.k_pad, self.lb.n_pad, _flags(True, a_tf32=True), ptr(part), part.size(-1), 0,
-                                           _stream(self.dev))
-        check(rc, "pvn3d_mlp_dense_sum32")
+        call("pvn3d_mlp_dense_sum32", self.dev, x.data_ptr() + 768 * 4, 1280, 512, rows, ptr(self.lb.w), ptr(self.lb.bias),
+             self.lb.k_pad, self.lb.n_pad, _flags(True, a_tf32=True), ptr(part), part.size(-1), 0)
         if n % 32 == 0:
             ap = part.view(b, n // 32, -1).double().sum(1) / n                           # [B, 1024] AvgPool1d(num_points)
         else:   # 32-row groups straddle frames: per-point activations through the plain layer, then the mean
@@ -133,11 +125,8 @@ class FusedHeads:
             fbp[:, : fb.size(1)] = fb
             h = torch.empty((rows, hd.first.n_pad), dtype=torch.float32, device=self.dev)
             if n % 128 == 0:
-                with torch.cuda.device(self.dev):
-                    rc = lib.pvn3d_mlp_dense_frame_bias(x.data_ptr(), 1280, 768, rows, n, ptr(hd.first.w), ptr(fbp), hd.first.k_pad,
-                                                        hd.first.n_pad, _flags(True, True, True), ptr(h), h.size(-1), 0,
-                                                        _stream(self.dev))
-                check(rc, "pvn3d_mlp_dense_frame_bias")
+                call("pvn3d_mlp_dense_frame_bias", self.dev, x.data_ptr(), 1280, 768, rows, n, ptr(hd.first.w), ptr(fbp),
+                     hd.first.k_pad, hd.first.n_pad, _flags(True, True, True), ptr(h), h.size(-1), 0)
             else:       # a 128-row tile may straddle frames: one launch per frame with that frame's bias
                 for bi in range(b):
                     layer = PackedLayer.__new__(PackedLayer)

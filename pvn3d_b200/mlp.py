@@ -28,7 +28,7 @@ from typing import Callable, Dict, List, Tuple
 import torch
 
 from . import _ext, _lib
-from ._lib import check, ptr
+from ._lib import call, ptr
 from .pointnet2 import SA_SPEC
 
 
@@ -68,7 +68,7 @@ class PackedLayer:
         self.bias[:n] = bias
 
 
-MLP_RELU, MLP_ROUND_OUT, MLP_A_TF32, MLP_OUT_CN = 1, 2, 4, 16      # include/pvn3d_b200.h PVN3D_MLP_*
+MLP_RELU, MLP_ROUND_OUT, MLP_A_TF32 = 1, 2, 4      # include/pvn3d_b200.h PVN3D_MLP_*
 
 
 def _flags(relu, round_out=False, a_tf32=False, reserve=0):
@@ -77,101 +77,25 @@ def _flags(relu, round_out=False, a_tf32=False, reserve=0):
             | ((int(reserve) & 0xFF) << 8))
 
 
-def _stream(dev):
-    return torch.cuda.current_stream(dev).cuda_stream
-
-
 def mlp_dense(a2d: torch.Tensor, layer: PackedLayer, relu=True, pool=0, out=None, col0=0, round_out=False,
               a_tf32=False, reserve=0):
     """a2d [rows, lda] point-major activations (all lda columns valid or zero).  a_tf32: a2d came out of
     a layer run with round_out=True (values already TF32) -> asynchronous copy path."""
-    lib = _lib.load()
     rows, lda = a2d.shape
     if out is None:
         out = torch.empty((rows // pool if pool else rows, layer.n_pad), dtype=torch.float32, device=a2d.device)
-    with torch.cuda.device(a2d.device):
-        rc = lib.pvn3d_mlp_dense(ptr(a2d), lda, lda, rows, ptr(layer.w), ptr(layer.bias), layer.k_pad, layer.n_pad,
-                                 _flags(relu, round_out, a_tf32, reserve), pool, ptr(out), out.size(-1), col0, _stream(a2d.device))
-    check(rc, "pvn3d_mlp_dense")
+    call("pvn3d_mlp_dense", a2d.device, ptr(a2d), lda, lda, rows, ptr(layer.w), ptr(layer.bias), layer.k_pad, layer.n_pad,
+         _flags(relu, round_out, a_tf32, reserve), pool, ptr(out), out.size(-1), col0)
     return out
 
 
 def mlp_fp_first(known_feat_pm, nn_idx, nn_w, skip_ptr, lds, c1, layer: PackedLayer, relu=True, round_out=False, reserve=0):
-    lib = _lib.load()
     b, m_known, c2 = known_feat_pm.shape
     n_unknown = nn_idx.shape[1]
     out = torch.empty((b * n_unknown, layer.n_pad), dtype=torch.float32, device=known_feat_pm.device)
-    with torch.cuda.device(known_feat_pm.device):
-        rc = lib.pvn3d_mlp_fp_first(ptr(known_feat_pm), c2, ptr(nn_idx), ptr(nn_w), skip_ptr, lds, c1, b, n_unknown,
-                                    m_known, ptr(layer.w), ptr(layer.bias), layer.k_pad, layer.n_pad,
-                                    _flags(relu, round_out, reserve=reserve), ptr(out), out.size(-1), 0,
-                                    _stream(known_feat_pm.device))
-    check(rc, "pvn3d_mlp_fp_first")
-    return out
-
-
-def fp2_fits(layer1: PackedLayer, layer2: PackedLayer) -> bool:
-    """whether pvn3d_mlp_fp2 takes a two-layer FP module (the library's own rule: a first layer of 256 or 512 columns, a
-    second layer of a multiple of 128 columns over exactly those, tiles and stages within shared memory -- FP2-FP4)"""
-    l1, l2 = _layer_struct(layer1), _layer_struct(layer2)
-    return bool(_lib.load().pvn3d_mlp_fp2_supported(ctypes.addressof(l1), ctypes.addressof(l2)))
-
-
-def mlp_fp2(known_feat_pm, nn_idx, nn_w, skip_ptr, lds, c1, layer1: PackedLayer, layer2: PackedLayer, out=None, col0=0,
-            round_out=False, reserve=0):
-    """both layers of an FP module in one launch (pvn3d_mlp_fp2): the same bits as
-    mlp_fp_first(.., layer1, round_out=True) -> mlp_dense(.., layer2, a_tf32=True, round_out=round_out)"""
-    lib = _lib.load()
-    b, m_known, c2 = known_feat_pm.shape
-    n_unknown = nn_idx.shape[1]
-    if out is None:
-        out = torch.empty((b * n_unknown, layer2.n_pad), dtype=torch.float32, device=known_feat_pm.device)
-    l1, l2 = _layer_struct(layer1), _layer_struct(layer2)
-    with torch.cuda.device(known_feat_pm.device):
-        rc = lib.pvn3d_mlp_fp2(ptr(known_feat_pm), c2, ptr(nn_idx), ptr(nn_w), skip_ptr, lds, c1, b, n_unknown, m_known,
-                               ctypes.addressof(l1), ctypes.addressof(l2), _flags(True, round_out, reserve=reserve), ptr(out),
-                               out.size(-1), col0, _stream(known_feat_pm.device))
-    check(rc, "pvn3d_mlp_fp2")
-    return out
-
-
-def sa_factor_table(xyz: torch.Tensor, feat_ptr: int, ldf: int, c_feat: int, k_pad: int) -> torch.Tensor:
-    """[B,n,3] coordinates + point-major descriptors -> [B*n, k_pad] rows [tf32(f) | hi(x) | lo(x) | 0] (see
-    pvn3d_sa_factor_table in include/pvn3d_b200.h)"""
-    lib = _lib.load()
-    rows = xyz.size(0) * xyz.size(1)
-    out = torch.empty((rows, k_pad), dtype=torch.float32, device=xyz.device)
-    with torch.cuda.device(xyz.device):
-        rc = lib.pvn3d_sa_factor_table(ptr(xyz), feat_ptr, ldf, c_feat, rows, k_pad, ptr(out), _stream(xyz.device))
-    check(rc, "pvn3d_sa_factor_table")
-    return out
-
-
-def sa_centre_term(new_xyz: torch.Tensor, wx: torch.Tensor, bias: torch.Tensor) -> torch.Tensor:
-    """V[i] = Wx . c_i - bias for every sampled centre: new_xyz [B,m,3], wx [n_pad,3], bias [n_pad] -> [B*m, n_pad]"""
-    lib = _lib.load()
-    rows = new_xyz.size(0) * new_xyz.size(1)
-    n_pad = wx.size(0)
-    out = torch.empty((rows, n_pad), dtype=torch.float32, device=new_xyz.device)
-    with torch.cuda.device(new_xyz.device):
-        rc = lib.pvn3d_sa_centre_term(ptr(new_xyz), ptr(wx), ptr(bias), rows, n_pad, ptr(out), _stream(new_xyz.device))
-    check(rc, "pvn3d_sa_centre_term")
-    return out
-
-
-def mlp_sa_fact(u: torch.Tensor, v: torch.Tensor, idx: torch.Tensor, n: int, layer: PackedLayer, relu=True, pool=0,
-                out=None, col0=0, round_out=False, reserve=0):
-    """second layer of a factored SA scale: rows relu(U[idx] - V) -> layer (pvn3d_mlp_sa_fact)"""
-    lib = _lib.load()
-    b, m, ns = idx.shape
-    rows = b * m * ns
-    if out is None:
-        out = torch.empty((rows // pool if pool else rows, layer.n_pad), dtype=torch.float32, device=u.device)
-    with torch.cuda.device(u.device):
-        rc = lib.pvn3d_mlp_sa_fact(ptr(u), ptr(v), u.size(-1), u.size(-1), ptr(idx), b, n, m, ns, ptr(layer.w), ptr(layer.bias),
-                                   layer.k_pad, layer.n_pad, _flags(relu, round_out, reserve=reserve), pool, ptr(out),
-                                   out.size(-1), col0, _stream(u.device))
-    check(rc, "pvn3d_mlp_sa_fact")
+    call("pvn3d_mlp_fp_first", known_feat_pm.device, ptr(known_feat_pm), c2, ptr(nn_idx), ptr(nn_w), skip_ptr, lds, c1, b,
+         n_unknown, m_known, ptr(layer.w), ptr(layer.bias), layer.k_pad, layer.n_pad, _flags(relu, round_out, reserve=reserve),
+         ptr(out), out.size(-1), 0)
     return out
 
 
@@ -179,94 +103,128 @@ def _layer_struct(layer: PackedLayer) -> _lib.MlpLayer:
     return _lib.MlpLayer(layer.w.data_ptr(), layer.bias.data_ptr(), layer.k_pad, layer.n_pad)
 
 
+def _supported(query: str, *layers: PackedLayer, ns=None) -> bool:
+    """a fused kernel's host-only `_supported` query on the layers' shapes"""
+    structs = [_layer_struct(layer) for layer in layers]
+    args = [ctypes.addressof(st) for st in structs] + ([] if ns is None else [ns])
+    return bool(getattr(_lib.load(), query)(*args))
+
+
+def fp2_fits(layer1: PackedLayer, layer2: PackedLayer) -> bool:
+    """whether pvn3d_mlp_fp2 takes a two-layer FP module (the library's own rule: a first layer of 256 or 512 columns, a
+    second layer of a multiple of 128 columns over exactly those, tiles and stages within shared memory -- FP2-FP4)"""
+    return _supported("pvn3d_mlp_fp2_supported", layer1, layer2)
+
+
+def mlp_fp2(known_feat_pm, nn_idx, nn_w, skip_ptr, lds, c1, layer1: PackedLayer, layer2: PackedLayer, out=None, col0=0,
+            round_out=False, reserve=0):
+    """both layers of an FP module in one launch (pvn3d_mlp_fp2): the same bits as
+    mlp_fp_first(.., layer1, round_out=True) -> mlp_dense(.., layer2, a_tf32=True, round_out=round_out)"""
+    b, m_known, c2 = known_feat_pm.shape
+    n_unknown = nn_idx.shape[1]
+    if out is None:
+        out = torch.empty((b * n_unknown, layer2.n_pad), dtype=torch.float32, device=known_feat_pm.device)
+    l1, l2 = _layer_struct(layer1), _layer_struct(layer2)
+    call("pvn3d_mlp_fp2", known_feat_pm.device, ptr(known_feat_pm), c2, ptr(nn_idx), ptr(nn_w), skip_ptr, lds, c1, b,
+         n_unknown, m_known, ctypes.addressof(l1), ctypes.addressof(l2), _flags(True, round_out, reserve=reserve), ptr(out),
+         out.size(-1), col0)
+    return out
+
+
+def sa_factor_table(xyz: torch.Tensor, feat_ptr: int, ldf: int, c_feat: int, k_pad: int) -> torch.Tensor:
+    """[B,n,3] coordinates + point-major descriptors -> [B*n, k_pad] rows [tf32(f) | hi(x) | lo(x) | 0] (see
+    pvn3d_sa_factor_table in include/pvn3d_b200.h)"""
+    rows = xyz.size(0) * xyz.size(1)
+    out = torch.empty((rows, k_pad), dtype=torch.float32, device=xyz.device)
+    call("pvn3d_sa_factor_table", xyz.device, ptr(xyz), feat_ptr, ldf, c_feat, rows, k_pad, ptr(out))
+    return out
+
+
+def sa_centre_term(new_xyz: torch.Tensor, wx: torch.Tensor, bias: torch.Tensor) -> torch.Tensor:
+    """V[i] = Wx . c_i - bias for every sampled centre: new_xyz [B,m,3], wx [n_pad,3], bias [n_pad] -> [B*m, n_pad]"""
+    rows = new_xyz.size(0) * new_xyz.size(1)
+    n_pad = wx.size(0)
+    out = torch.empty((rows, n_pad), dtype=torch.float32, device=new_xyz.device)
+    call("pvn3d_sa_centre_term", new_xyz.device, ptr(new_xyz), ptr(wx), ptr(bias), rows, n_pad, ptr(out))
+    return out
+
+
+def mlp_sa_fact(u: torch.Tensor, v: torch.Tensor, idx: torch.Tensor, n: int, layer: PackedLayer, relu=True, out=None,
+                col0=0, round_out=False, reserve=0):
+    """second layer of a factored SA scale: rows relu(U[idx] - V) -> layer (pvn3d_mlp_sa_fact)"""
+    b, m, ns = idx.shape
+    if out is None:
+        out = torch.empty((b * m * ns, layer.n_pad), dtype=torch.float32, device=u.device)
+    call("pvn3d_mlp_sa_fact", u.device, ptr(u), ptr(v), u.size(-1), u.size(-1), ptr(idx), b, n, m, ns, ptr(layer.w),
+         ptr(layer.bias), layer.k_pad, layer.n_pad, _flags(relu, round_out, reserve=reserve), ptr(out), out.size(-1), col0)
+    return out
+
+
 def sa_fact2_fits(layer2: PackedLayer, layer3: PackedLayer, ns: int) -> bool:
     """whether pvn3d_mlp_sa_fact2 takes the scale (the library's own rule: nsample 16 or 32, both layers at most 128
     columns, weights + layer-2 tile within shared memory -- SA1 and SA2)"""
-    l2, l3 = _layer_struct(layer2), _layer_struct(layer3)
-    return bool(_lib.load().pvn3d_mlp_sa_fact2_supported(ctypes.addressof(l2), ctypes.addressof(l3), ns))
-
-
-def mlp_sa_fact2(u: torch.Tensor, v: torch.Tensor, idx: torch.Tensor, n: int, layer2: PackedLayer, layer3: PackedLayer,
-                 out=None, col0=0, round_out=False, reserve=0):
-    """layers 2 and 3 of a factored SA scale + max-pool over nsample in one launch (pvn3d_mlp_sa_fact2): the same bits
-    as mlp_sa_fact(.., layer2, round_out=True) -> mlp_dense(.., layer3, pool=ns, a_tf32=True)"""
-    lib = _lib.load()
-    b, m, ns = idx.shape
-    if out is None:
-        out = torch.empty((b * m, layer3.n_pad), dtype=torch.float32, device=u.device)
-    l2, l3 = _layer_struct(layer2), _layer_struct(layer3)
-    with torch.cuda.device(u.device):
-        rc = lib.pvn3d_mlp_sa_fact2(ptr(u), ptr(v), u.size(-1), u.size(-1), ptr(idx), b, n, m, ns, ctypes.addressof(l2),
-                                    ctypes.addressof(l3), _flags(True, round_out, reserve=reserve), ns, ptr(out), out.size(-1),
-                                    col0, _stream(u.device))
-    check(rc, "pvn3d_mlp_sa_fact2")
-    return out
+    return _supported("pvn3d_mlp_sa_fact2_supported", layer2, layer3, ns=ns)
 
 
 def sa_fact2w_fits(layer2: PackedLayer, layer3: PackedLayer, ns: int) -> bool:
     """whether pvn3d_mlp_sa_fact2w takes the scale (the library's own rule: nsample 16 or 32, a last layer wider than
     128 columns, layer-2 K at most 256, A + H tiles + three weight stages within shared memory -- SA3 and SA4)"""
-    l2, l3 = _layer_struct(layer2), _layer_struct(layer3)
-    return bool(_lib.load().pvn3d_mlp_sa_fact2w_supported(ctypes.addressof(l2), ctypes.addressof(l3), ns))
+    return _supported("pvn3d_mlp_sa_fact2w_supported", layer2, layer3, ns=ns)
 
 
-def mlp_sa_fact2w(u: torch.Tensor, v: torch.Tensor, idx: torch.Tensor, n: int, layer2: PackedLayer, layer3: PackedLayer,
-                  out=None, col0=0, round_out=False, reserve=0):
-    """mlp_sa_fact2 for a wide last layer (pvn3d_mlp_sa_fact2w: weights streamed, both layers in 128-column blocks):
-    the same bits as mlp_sa_fact(.., layer2, round_out=True) -> mlp_dense(.., layer3, pool=ns, a_tf32=True)"""
-    lib = _lib.load()
+def _sa_fact2_call(fn_name: str, u: torch.Tensor, v: torch.Tensor, idx: torch.Tensor, n: int, layer2: PackedLayer,
+                   layer3: PackedLayer, out=None, col0=0, round_out=False, reserve=0):
     b, m, ns = idx.shape
     if out is None:
         out = torch.empty((b * m, layer3.n_pad), dtype=torch.float32, device=u.device)
     l2, l3 = _layer_struct(layer2), _layer_struct(layer3)
-    with torch.cuda.device(u.device):
-        rc = lib.pvn3d_mlp_sa_fact2w(ptr(u), ptr(v), u.size(-1), u.size(-1), ptr(idx), b, n, m, ns, ctypes.addressof(l2),
-                                     ctypes.addressof(l3), _flags(True, round_out, reserve=reserve), ns, ptr(out), out.size(-1),
-                                     col0, _stream(u.device))
-    check(rc, "pvn3d_mlp_sa_fact2w")
+    call(fn_name, u.device, ptr(u), ptr(v), u.size(-1), u.size(-1), ptr(idx), b, n, m, ns, ctypes.addressof(l2),
+         ctypes.addressof(l3), _flags(True, round_out, reserve=reserve), ns, ptr(out), out.size(-1), col0)
     return out
 
 
+def mlp_sa_fact2(u, v, idx, n, layer2, layer3, out=None, col0=0, round_out=False, reserve=0):
+    """layers 2 and 3 of a factored SA scale + max-pool over nsample in one launch (pvn3d_mlp_sa_fact2): the same bits
+    as mlp_sa_fact(.., layer2, round_out=True) -> mlp_dense(.., layer3, pool=ns, a_tf32=True)"""
+    return _sa_fact2_call("pvn3d_mlp_sa_fact2", u, v, idx, n, layer2, layer3, out, col0, round_out, reserve)
+
+
+def mlp_sa_fact2w(u, v, idx, n, layer2, layer3, out=None, col0=0, round_out=False, reserve=0):
+    """mlp_sa_fact2 for a wide last layer (pvn3d_mlp_sa_fact2w: weights streamed, both layers in 128-column blocks),
+    with the same arguments and the same bits"""
+    return _sa_fact2_call("pvn3d_mlp_sa_fact2w", u, v, idx, n, layer2, layer3, out, col0, round_out, reserve)
+
+
 def mlp_fp_fact(p: torch.Tensor, s_: torch.Tensor, nn_idx: torch.Tensor, nn_w: torch.Tensor, m_known: int,
-                layer: PackedLayer, relu=True, round_out=False, reserve=0, out_cn=False):
-    """second layer of a factored FP module: rows relu(sum_t w_t P[idx_t] + S) -> layer (pvn3d_mlp_fp_fact).
-    out_cn: return [b, n_pad, n_unknown] (channel-major frames, PVN3D_MLP_OUT_CN) instead of [b * n_unknown, n_pad]"""
-    lib = _lib.load()
+                layer: PackedLayer, relu=True, round_out=False, reserve=0):
+    """second layer of a factored FP module: rows relu(sum_t w_t P[idx_t] + S) -> layer (pvn3d_mlp_fp_fact),
+    [b * n_unknown, n_pad]"""
     b, n_unknown = nn_idx.shape[0], nn_idx.shape[1]
     ld = p.size(-1)
-    shape = (b, layer.n_pad, n_unknown) if out_cn else (b * n_unknown, layer.n_pad)
-    out = torch.empty(shape, dtype=torch.float32, device=p.device)
-    with torch.cuda.device(p.device):
-        rc = lib.pvn3d_mlp_fp_fact(ptr(p), ptr(s_), ld, ld, ptr(nn_idx), ptr(nn_w), b, n_unknown, m_known, ptr(layer.w),
-                                   ptr(layer.bias), layer.k_pad, layer.n_pad,
-                                   _flags(relu, round_out, reserve=reserve) | (MLP_OUT_CN if out_cn else 0),
-                                   ptr(out), layer.n_pad, 0, _stream(p.device))
-    check(rc, "pvn3d_mlp_fp_fact")
+    out = torch.empty((b * n_unknown, layer.n_pad), dtype=torch.float32, device=p.device)
+    call("pvn3d_mlp_fp_fact", p.device, ptr(p), ptr(s_), ld, ld, ptr(nn_idx), ptr(nn_w), b, n_unknown, m_known,
+         ptr(layer.w), ptr(layer.bias), layer.k_pad, layer.n_pad, _flags(relu, round_out, reserve=reserve), ptr(out),
+         layer.n_pad, 0)
     return out
 
 
 def fp_fact2_fits(layer_s: PackedLayer, layer2: PackedLayer) -> bool:
     """whether pvn3d_mlp_fp_fact2 takes a factored FP module (the library's own rule: a skip layer 32 -> 128 over an SA
     factor table, a second layer 128 -> 128 -- FP1)"""
-    ls, l2 = _layer_struct(layer_s), _layer_struct(layer2)
-    return bool(_lib.load().pvn3d_mlp_fp_fact2_supported(ctypes.addressof(ls), ctypes.addressof(l2)))
+    return _supported("pvn3d_mlp_fp_fact2_supported", layer_s, layer2)
 
 
 def mlp_fp_fact2(p: torch.Tensor, table: torch.Tensor, nn_idx: torch.Tensor, nn_w: torch.Tensor, m_known: int,
                  layer_s: PackedLayer, layer2: PackedLayer, reserve=0):
     """the skip term and the second layer of a factored FP module in one launch (pvn3d_mlp_fp_fact2) -> [b, 128,
-    n_unknown]: the same bits as mlp_fp_fact(p, mlp_dense(table, layer_s, relu=False, a_tf32=True), .., layer2,
-    out_cn=True)"""
-    lib = _lib.load()
+    n_unknown]: the same bits as mlp_fp_fact(p, mlp_dense(table, layer_s, relu=False, a_tf32=True), .., layer2),
+    transposed per frame"""
     b, n_unknown = nn_idx.shape[0], nn_idx.shape[1]
     assert p.size(-1) == layer_s.n_pad and table.size(-1) == layer_s.k_pad and table.size(0) == b * n_unknown
     out = torch.empty((b, layer2.n_pad, n_unknown), dtype=torch.float32, device=p.device)
     ls, l2 = _layer_struct(layer_s), _layer_struct(layer2)
-    with torch.cuda.device(p.device):
-        rc = lib.pvn3d_mlp_fp_fact2(ptr(p), ptr(table), ptr(nn_idx), ptr(nn_w), b, n_unknown, m_known,
-                                    ctypes.addressof(ls), ctypes.addressof(l2), _flags(False, reserve=reserve), ptr(out),
-                                    _stream(p.device))
-    check(rc, "pvn3d_mlp_fp_fact2")
+    call("pvn3d_mlp_fp_fact2", p.device, ptr(p), ptr(table), ptr(nn_idx), ptr(nn_w), b, n_unknown, m_known,
+         ctypes.addressof(ls), ctypes.addressof(l2), _flags(False, reserve=reserve), ptr(out))
     return out
 
 
@@ -274,26 +232,18 @@ def mlp_fp_fact2_rows(p: torch.Tensor, table: torch.Tensor, nn_idx: torch.Tensor
                       layer_s: PackedLayer, layer2: PackedLayer, out: torch.Tensor, col0: int, reserve=0) -> torch.Tensor:
     """mlp_fp_fact2 with its output point-major in columns col0 .. col0+127 of the row table out [b * n_unknown, ldo]
     (pvn3d_mlp_fp_fact2_rows): tf32_round of the transposed [b, 128, n_unknown], bit for bit"""
-    lib = _lib.load()
     b, n_unknown = nn_idx.shape[0], nn_idx.shape[1]
     assert p.size(-1) == layer_s.n_pad and table.size(-1) == layer_s.k_pad and table.size(0) == b * n_unknown
     assert out.dim() == 2 and out.size(0) == b * n_unknown and out.stride(1) == 1
     ls, l2 = _layer_struct(layer_s), _layer_struct(layer2)
-    with torch.cuda.device(p.device):
-        rc = lib.pvn3d_mlp_fp_fact2_rows(ptr(p), ptr(table), ptr(nn_idx), ptr(nn_w), b, n_unknown, m_known,
-                                         ctypes.addressof(ls), ctypes.addressof(l2), _flags(False, reserve=reserve), ptr(out),
-                                         out.stride(0), col0, _stream(p.device))
-    check(rc, "pvn3d_mlp_fp_fact2_rows")
+    call("pvn3d_mlp_fp_fact2_rows", p.device, ptr(p), ptr(table), ptr(nn_idx), ptr(nn_w), b, n_unknown, m_known,
+         ctypes.addressof(ls), ctypes.addressof(l2), _flags(False, reserve=reserve), ptr(out), out.stride(0), col0)
     return out
 
 
 def three_nn_weights(dist2: torch.Tensor) -> torch.Tensor:
-    lib = _lib.load()
     w = torch.empty_like(dist2)
-    rows = dist2.numel() // 3
-    with torch.cuda.device(dist2.device):
-        rc = lib.pvn3d_three_nn_weights(ptr(dist2), rows, ptr(w), _stream(dist2.device))
-    check(rc, "pvn3d_three_nn_weights")
+    call("pvn3d_three_nn_weights", dist2.device, ptr(dist2), dist2.numel() // 3, ptr(w))
     return w
 
 
@@ -424,18 +374,14 @@ class FusedPointnet2MSG:
         xyz = pointcloud[..., :3].contiguous()
         self._m("glue")
         plan = GeoPlan(pointcloud, [xyz])
-        lib = _lib.load()
         for li, (npoint, radii, nsamples, _) in enumerate(SA_SPEC):
             x = plan.l_xyz[-1]
             if fps_chunk and fps_chunk < b:
                 fidx = torch.empty((b, npoint), dtype=torch.int32, device=self.dev)
                 n = x.size(1)
-                with torch.cuda.device(self.dev):
-                    for f0 in range(0, b, fps_chunk):
-                        nb = min(fps_chunk, b - f0)
-                        check(lib.pvn3d_furthest_point_sampling(x.data_ptr() + f0 * n * 12, nb, n, npoint,
-                                                                fidx.data_ptr() + f0 * npoint * 4, _stream(self.dev)),
-                              "pvn3d_furthest_point_sampling")
+                for f0 in range(0, b, fps_chunk):
+                    call("pvn3d_furthest_point_sampling", self.dev, x.data_ptr() + f0 * n * 12, min(fps_chunk, b - f0), n,
+                         npoint, fidx.data_ptr() + f0 * npoint * 4)
             else:
                 fidx = _ext.furthest_point_sampling(x, npoint)
             self._m("fps")

@@ -18,10 +18,9 @@ from __future__ import annotations
 
 import torch
 
-from . import _lib
-from ._lib import check, ptr
+from ._lib import call, ptr
 from .heads import FusedHeads
-from .mlp import FusedPointnet2MSG, _stream
+from .mlp import FusedPointnet2MSG
 
 
 def gather_pixel_rows(emb: torch.Tensor, choose: torch.Tensor, out: torch.Tensor, col0: int = 0) -> torch.Tensor:
@@ -38,11 +37,7 @@ def gather_pixel_rows(emb: torch.Tensor, choose: torch.Tensor, out: torch.Tensor
     n = choose.size(2)
     if out.dim() != 2 or out.size(0) != b * n or out.stride(1) != 1:
         raise ValueError(f"gather_pixel_rows: out must be rows [B*N, ldo], got {tuple(out.shape)}")
-    lib = _lib.load()
-    with torch.cuda.device(emb.device):
-        rc = lib.pvn3d_gather_pixel_rows(ptr(emb), b, c, emb.size(2), ptr(choose), n, ptr(out), out.stride(0), col0,
-                                         _stream(emb.device))
-    check(rc, "pvn3d_gather_pixel_rows")
+    call("pvn3d_gather_pixel_rows", emb.device, ptr(emb), b, c, emb.size(2), ptr(choose), n, ptr(out), out.stride(0), col0)
     return out
 
 

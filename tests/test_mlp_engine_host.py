@@ -35,7 +35,6 @@ def test_misaligned_weights_are_refused_without_launching():
     assert lib.pvn3d_mlp_fp_first(ok, 32, ok, ok, None, 0, 0, 1, 128, 16, w, ok, 32, 16, 1, ok, 16, 0, None) == -1
     # p, s, ld, c_valid, nn_idx, nn_w, b, n_unknown, m_known, w, bias, k_pad, n_pad, flags, out, ldo, col0
     assert lib.pvn3d_mlp_fp_fact(ok, ok, 32, 32, ok, ok, 1, 128, 16, w, ok, 32, 16, 1, ok, 16, 0, None) == -1
-    # u, v, ldu, c_valid, idx, b, n, m, ns, w, bias, k_pad, n_pad, flags, pool, out, ldo, col0
-    assert lib.pvn3d_mlp_sa_fact(ok, ok, 32, 32, ok, 1, 64, 8, 16, w, ok, 32, 16, 1, 0, ok, 16, 0, None) == -1
-    assert lib.pvn3d_mlp_sa_fact(ok, ok, 32, 32, ok, 1, 64, 8, 16, w, ok, 32, 16, 1, 16, ok, 16, 0, None) == -1
+    # u, v, ldu, c_valid, idx, b, n, m, ns, w, bias, k_pad, n_pad, flags, out, ldo, col0
+    assert lib.pvn3d_mlp_sa_fact(ok, ok, 32, 32, ok, 1, 64, 8, 16, w, ok, 32, 16, 1, ok, 16, 0, None) == -1
     assert lib.pvn3d_launch_count() == before

@@ -1,6 +1,6 @@
 """pvn3d_mlp_fp_fact2 (the skip term S = W1s . table + b1 and the second layer of a factored FP module in one launch, S
 kept on chip, the output stored channel-major) against the two launches it replaces: pvn3d_mlp_dense without ReLU on the
-SA1 factor table, then pvn3d_mlp_fp_fact.  Same operands, the same MMA shape and K order per output element and the
+SA1 factor table, then pvn3d_mlp_fp_fact, whose point-major rows are transposed per frame.  Same operands, the same MMA shape and K order per output element and the
 same epilogue arithmetic: the results must be identical, bit for bit."""
 import pytest
 import torch
@@ -30,8 +30,6 @@ def _module(dev, b, n, m, seed, c_feat=6):
 def _two_launches(p, table, nn_idx, nn_w, m, ls, l2, reserve=0):
     b, n = nn_idx.shape[0], nn_idx.shape[1]
     s = mlp.mlp_dense(table, ls, relu=False, a_tf32=True, reserve=reserve)
-    if n % 32 == 0:
-        return mlp.mlp_fp_fact(p, s, nn_idx, nn_w, m, l2, reserve=reserve, out_cn=True)
     pm = mlp.mlp_fp_fact(p, s, nn_idx, nn_w, m, l2, reserve=reserve)
     return pm.view(b, n, -1).transpose(1, 2).contiguous()
 
@@ -42,7 +40,7 @@ def _two_launches(p, table, nn_idx, nn_w, m, ls, l2, reserve=0):
     (1, 96, 40),         # one and a half tiles
 ])
 @pytest.mark.parametrize("reserve", [0, 120])
-def test_fp_fact2_equals_two_launches(cuda_dev, b, n, m, reserve):
+def test_fp_fact2_equals_transposed_two_launches(cuda_dev, b, n, m, reserve):
     p, table, nn_idx, nn_w, ls, l2 = _module(cuda_dev, b, n, m, seed=b + n + m)
     assert mlp.fp_fact2_fits(ls, l2)
     assert bool((table[:, 6:12] != 0).any())          # the hi / lo coordinate columns take part

@@ -30,8 +30,8 @@ def ref_dense(a, w, b, relu, pool):
     # many tiles per persistent CTA (ring and accumulator tile wrap), odd chunk counts, 2 column blocks
     (64000, 96, 128, True, 0), (70005, 32, 32, True, 0), (40960, 64, 64, True, 16), (9000, 544, 512, True, 0),
     (38400, 160, 272, True, 32),
-    # wide pooled layers: transposed accumulator read (channel = lane), every pool size, ragged last tile, 1 / 2 / 4 column
-    # blocks, single-chunk K
+    # wide pooled layers (the shuffle max-pool epilogue on 128-column tiles): every pool size, ragged last tile, 1 / 2 / 4 / 8
+    # column blocks, single-chunk K
     (8192, 96, 128, True, 32), (4144, 64, 128, True, 16), (8000, 224, 256, True, 8), (50016, 224, 256, True, 32),
     (2064, 256, 512, False, 16), (4096, 32, 1024, True, 32), (160, 384, 128, True, 16)])
 def test_dense_layer(cuda_dev, rows, k, n, relu, pool):
@@ -162,7 +162,7 @@ def test_fused_engine_is_deterministic(cuda_dev):
 
 @pytest.mark.parametrize("b,n,m,ns,c_feat,n1,n2", [(2, 1024, 300, 16, 96, 64, 96), (1, 512, 100, 32, 6, 32, 32),
                                                     (3, 700, 129, 8, 256, 128, 208), (2, 2048, 512, 32, 512, 256, 384)])
-def test_factored_sa_first_layer_kernels(cuda_dev, b, n, m, ns, c_feat, n1, n2):
+def test_factored_sa_first_and_second_layer_kernels(cuda_dev, b, n, m, ns, c_feat, n1, n2):
     """pvn3d_sa_factor_table + pvn3d_mlp_dense (U) + pvn3d_sa_centre_term (V): U[idx] - V == W1.[f | x - c] + b1 to fp32
     accuracy (the hi/lo coordinate split), and pvn3d_mlp_sa_fact == relu(tf32(relu(U[idx] - V)) . W2 + b2)"""
     rng = np.random.default_rng(b + n + ns)
@@ -195,8 +195,6 @@ def test_factored_sa_first_layer_kernels(cuda_dev, b, n, m, ns, c_feat, n1, n2):
     a2 = mlp.tf32_round(torch.relu(u.view(b, n, -1)[bi, idx.long()] - v.view(b, m, 1, -1)).reshape(-1, first.n_pad)[:, :n1])
     want2 = ref_dense(a2.cpu(), mlp.tf32_round(w2).cpu(), b2.cpu(), True, 0)
     assert (got2.cpu()[:, :n2] - want2).abs().max() <= 2e-5 * max(1.0, float(want2.abs().max()))
-    got2p = mlp.mlp_sa_fact(u, v, idx, n, l2, pool=ns)
-    assert torch.equal(got2p, got2.view(b * m, ns, -1).max(1).values)
 
 
 def test_factored_fp_first_layer_kernel(cuda_dev):
@@ -216,27 +214,3 @@ def test_factored_fp_first_layer_kernel(cuda_dev):
     want = ref_dense(mlp.tf32_round(a.reshape(-1, n1)).cpu(), l2.w.cpu()[:n2, :n1], l2.bias.cpu()[:n2], True, 0)
     # interpolation order differs in the last ulp before TF32 rounding: one TF32 ulp of the operands
     assert (got.cpu()[:, :n2] - want).abs().max() <= 1e-3 * max(1.0, float(want.abs().max()))
-
-
-@pytest.mark.parametrize("b_,n_u,m_k,n2", [(2, 1024, 333, 128), (3, 4128, 512, 256), (1, 96, 40, 128)])
-def test_factored_fp_layer_channel_major_output(cuda_dev, b_, n_u, m_k, n2):
-    """PVN3D_MLP_OUT_CN: the same numbers as the row-major call, laid out [b, n_pad, n_unknown] (what
-    Pointnet2MSG.forward returns, pvn3d.py:154) -- bit for bit, ragged last tile and frames that end inside a tile"""
-    rng = np.random.default_rng(b_ + n_u)
-    n1 = 128
-    nn = torch.from_numpy(rng.integers(0, m_k, (b_, n_u, 3)).astype(np.int32)).to(cuda_dev)
-    w = rng.uniform(0.05, 1, (b_, n_u, 3)).astype(np.float32)
-    w = torch.from_numpy(w / w.sum(-1, keepdims=True)).to(cuda_dev)
-    p = torch.from_numpy(rng.normal(size=(b_ * m_k, n1)).astype(np.float32)).to(cuda_dev)
-    s_ = torch.from_numpy(rng.normal(size=(b_ * n_u, n1)).astype(np.float32)).to(cuda_dev)
-    g = torch.Generator().manual_seed(n2)
-    l2 = mlp.PackedLayer((torch.randn(n2, n1, generator=g) / np.sqrt(n1)).to(cuda_dev), (torch.randn(n2, generator=g) * 0.1).to(cuda_dev), n1)
-    rows = mlp.mlp_fp_fact(p, s_, nn, w, m_k, l2)
-    cn = mlp.mlp_fp_fact(p, s_, nn, w, m_k, l2, out_cn=True)
-    assert cn.shape == (b_, n2, n_u)
-    assert torch.equal(cn, rows.view(b_, n_u, n2).transpose(1, 2))
-    # unsupported shapes are refused, not mis-stored
-    if n_u % 32 == 0:
-        with pytest.raises(RuntimeError):
-            mlp.mlp_fp_fact(p[:, :n1], s_, nn[:, :n_u - 1].contiguous(), w[:, :n_u - 1].contiguous(), m_k, l2, out_cn=True)
-
