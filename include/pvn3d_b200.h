@@ -295,6 +295,48 @@ int pvn3d_mlp_fp_fact2_rows(const float *p, const float *table, const int *nn_id
  * or c > 256 -- both before any CUDA call. */
 int pvn3d_gather_pixel_rows(const float *emb, int b, int c, long long hw, const long long *choose, int n, float *out,
                             int ldo, int col0, pvn3d_stream_t stream);
+
+/* ------------------------------------------------------------------------------------------
+ * BF16 forms of the dense layer and of the two producers of the DenseFusion activation table (PVN3D's heads in mixed
+ * precision).  A pvn3d_bf16_t holds the bit pattern of one bfloat16 (torch.bfloat16).
+ *      out[p, col0 + 0:n_pad] = act( A[p, 0:k_pad] . W^T + bias )
+ *   a    [rows, lda] bf16 rows, 16-byte aligned, lda and a_cols multiples of 8; columns >= a_cols read as zero
+ *   w    [n_pad, k_pad] bf16 (BN folded, then rounded to nearest even), zero padded, 16-byte aligned; k_pad a multiple
+ *        of 64 (one 128-byte row segment), n_pad a multiple of 16; bias [n_pad] f32
+ *   out  rows of ldo elements of the output type, 16-byte aligned; ldo, col0 multiples of 4, col0 + n_pad <= ldo
+ * Arithmetic: bf16 operands, fp32 accumulation, fp32 bias and ReLU; a bf16 output is rounded to nearest even once.
+ * flags: PVN3D_MLP_RELU, PVN3D_MLP_OUT_BF16 (out is bf16, else f32) and PVN3D_MLP_RESERVE_SMS(n); any other flag, a null
+ * pointer, misalignment or a bad shape: PVN3D_ERR_INVALID_ARG before any CUDA call.
+ * ---------------------------------------------------------------------------------------- */
+typedef uint16_t pvn3d_bf16_t;
+#define PVN3D_MLP_OUT_BF16 8
+int pvn3d_mlp_dense_bf16(const pvn3d_bf16_t *a, int lda, int a_cols, long long rows, const pvn3d_bf16_t *w,
+                         const float *bias, int k_pad, int n_pad, int flags, void *out, int ldo, int col0,
+                         pvn3d_stream_t stream);
+/* pvn3d_mlp_dense_bf16 with one bias vector per batch element, as pvn3d_mlp_dense_frame_bias (rows_per_frame % 128 == 0,
+ * rows % rows_per_frame == 0) */
+int pvn3d_mlp_dense_frame_bias_bf16(const pvn3d_bf16_t *a, int lda, int a_cols, long long rows, int rows_per_frame,
+                                    const pvn3d_bf16_t *w, const float *bias, int k_pad, int n_pad, int flags, void *out,
+                                    int ldo, int col0, pvn3d_stream_t stream);
+/* f32 out[g, :] = sum over the 32 rows p in [32 g, 32 g + 32) of relu(a[p] . W^T + bias), as pvn3d_mlp_dense_sum32: the
+ * sums are fp32 in a fixed order (reproducible).  ReLU always; flags: PVN3D_MLP_RELU and PVN3D_MLP_RESERVE_SMS(n). */
+int pvn3d_mlp_dense_sum32_bf16(const pvn3d_bf16_t *a, int lda, int a_cols, long long rows, const pvn3d_bf16_t *w,
+                               const float *bias, int k_pad, int n_pad, int flags, float *out, int ldo, int col0,
+                               pvn3d_stream_t stream);
+/* pvn3d_mlp_fp_fact2_rows with bf16 rows: the same arithmetic, relu(acc + b2) rounded to nearest even bf16 instead of
+ * TF32 -- the bits of pvn3d_mlp_fp_fact2's [b][128][n_unknown], transposed and converted to bf16.  Arguments, flags and
+ * coverage as pvn3d_mlp_fp_fact2; ldo and col0 (in bf16 elements) multiples of 8, col0 >= 0, col0 + 128 <= ldo and out
+ * 16-byte aligned, else PVN3D_ERR_INVALID_ARG before any CUDA call. */
+int pvn3d_mlp_fp_fact2_rows_bf16(const float *p, const float *table, const int *nn_idx, const float *nn_w, int b,
+                                 int n_unknown, int m_known, const pvn3d_mlp_layer_t *layer_s,
+                                 const pvn3d_mlp_layer_t *layer2, int flags, pvn3d_bf16_t *out, int ldo, int col0,
+                                 pvn3d_stream_t stream);
+/* pvn3d_gather_pixel_rows with bf16 rows: out[f * n + p][col0 + ch] = bf16(emb[f][ch][choose[f][0][p]]).  emb is f32
+ * (emb_bf16 = 0, 4-byte aligned; rounded to nearest even, as torch's .to(torch.bfloat16)) or bf16 (emb_bf16 = 1, 2-byte
+ * aligned; copied), so a CNN that ran under bf16 autocast needs no f32 copy.  c, ldo and col0 multiples of 8, out 16-byte
+ * aligned; otherwise checks, NaN rows and PVN3D_ERR_UNSUPPORTED as pvn3d_gather_pixel_rows. */
+int pvn3d_gather_pixel_rows_bf16(const void *emb, int emb_bf16, int b, int c, long long hw, const long long *choose, int n,
+                                 pvn3d_bf16_t *out, int ldo, int col0, pvn3d_stream_t stream);
 /* weight[p,0:3] = (1/(sqrt(dist2)+1e-8)) / sum  (pointnet2_modules.py:184-186), fp32 IEEE ops */
 int pvn3d_three_nn_weights(const float *dist2, long long rows, float *weight, pvn3d_stream_t stream);
 

@@ -14,7 +14,8 @@ What install() does (SURVEY section 8b, App. D):
      package's implementations (demo.py:22 imports them by name -> call patch_post_modules()
      after importing demo, or import pvn3d_eval_utils first);
   4. with patch_model=True, rebinds `lib.pvn3d.PVN3D.forward` (patch_pvn3d_forward): in eval mode, without
-     autograd and on CUDA inputs the network runs on FusedPVN3D (pvn3d_b200.network); anything else -- training,
+     autograd and on CUDA inputs the network runs on FusedPVN3D (pvn3d_b200.network), with bf16 heads inside a
+     torch.autocast("cuda", dtype=torch.bfloat16) region and TF32 ones otherwise; anything else -- training,
      train_*.py, grad-enabled or CPU calls -- runs the reference's own forward.
 Nothing here copies or edits reference files.
 """
@@ -96,8 +97,9 @@ def _weights(model):
                 yield t
 
 
-def fused_engine(model, device):
-    """The FusedPVN3D of `model` on `device`, cached in the module.  The cache key is (data_ptr, _version) of every
+def fused_engine(model, device, precision="tf32"):
+    """The FusedPVN3D of `model` on `device` at `precision`, cached in the module, one engine per (device, precision).
+    The weight key is (data_ptr, _version) of every
     parameter and buffer: load_state_dict, an optimiser step or a BatchNorm running-statistics update rebuilds the
     engine.  A DataParallel replica on the model's own device shares its tensors (and this cache) and hits it; replicas
     on other devices hold fresh copies and rebuild on every call -- run one process per GPU instead (pvn3d_b200.dist)."""
@@ -105,16 +107,26 @@ def fused_engine(model, device):
 
     key = tuple((t.data_ptr(), t._version) for t in _weights(model))
     cache = model.__dict__.setdefault("_pvn3d_b200_engines", {})   # plain attribute: copied by reference into replicas
-    hit = cache.get(device)
+    hit = cache.get((device, precision))
     if hit is None or hit[0] != key:
-        hit = cache[device] = (key, FusedPVN3D(model, device))
+        hit = cache[(device, precision)] = (key, FusedPVN3D(model, device, precision))
     return hit[1]
+
+
+def autocast_precision() -> str:
+    """the FusedPVN3D precision of a call made here: "bf16" inside torch.autocast("cuda", dtype=torch.bfloat16), "tf32"
+    otherwise (fp16 autocast included: the library has no fp16 heads)"""
+    import torch
+
+    if torch.is_autocast_enabled("cuda") and torch.get_autocast_dtype("cuda") == torch.bfloat16:
+        return "bf16"
+    return "tf32"
 
 
 def patch_pvn3d_forward(cls) -> None:
     """Rebind cls.forward(pointcloud, rgb, choose) (the reference's PVN3D, or a class with the same forward) so that
-    eval-mode, no-grad calls on CUDA inputs run fused_engine(self, device); every other call runs the original forward.
-    Idempotent."""
+    eval-mode, no-grad calls on CUDA inputs run fused_engine(self, device, autocast_precision()); every other call runs
+    the original forward.  Idempotent."""
     import torch
 
     if getattr(cls.forward, "_pvn3d_b200_orig", None) is not None:
@@ -124,7 +136,7 @@ def patch_pvn3d_forward(cls) -> None:
     def forward(self, pointcloud, rgb, choose):
         if self.training or torch.is_grad_enabled() or not (pointcloud.is_cuda and rgb.is_cuda and choose.is_cuda):
             return orig(self, pointcloud, rgb, choose)
-        return fused_engine(self, pointcloud.device)(pointcloud, rgb, choose)
+        return fused_engine(self, pointcloud.device, autocast_precision())(pointcloud, rgb, choose)
 
     forward._pvn3d_b200_orig = orig
     forward.__doc__ = orig.__doc__

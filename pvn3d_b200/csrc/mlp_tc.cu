@@ -102,6 +102,10 @@ __device__ __forceinline__ float to_tf32(float x) {
 __device__ __forceinline__ void stg64(float *p, float x, float y) {
   asm volatile("st.global.v2.f32 [%0], {%1,%2};" ::"l"(p), "f"(x), "f"(y) : "memory");
 }
+// 4-byte global store kept in program order (two bf16 of mlp_fp_fact2_kernel<FPF2_OUT_ROWS_BF16>)
+__device__ __forceinline__ void stg32(uint16_t *p, uint32_t x) {
+  asm volatile("st.global.b32 [%0], %1;" ::"l"(p), "r"(x) : "memory");
+}
 __device__ __forceinline__ void sts128(uint32_t addr, float a, float b, float c, float d) {
   asm volatile("st.shared.v4.f32 [%0], {%1,%2,%3,%4};" ::"r"(addr), "f"(a), "f"(b), "f"(c), "f"(d)
                : "memory");
@@ -187,6 +191,48 @@ __device__ __forceinline__ void wgmma_tf32<128>(float (&d)[64], uint64_t adesc, 
       "wgmma.mma_async.sync.aligned.m64n128k8.f32.tf32.tf32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47,%48,%49,%50,%51,%52,%53,%54,%55,%56,%57,%58,%59,%60,%61,%62,%63}, %64, %65, p, 1, 1;\n\t}\n"
       : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
       : "l"(adesc), "l"(bdesc), "r"(accumulate));
+}
+// D[64 x N] (+)= A[64 x 16] . B[N x 16]^T with bf16 operands, both K-major (no transpose) in shared memory, fp32
+// accumulate; the same fragment layout as wgmma_tf32.  K = 16 bf16 is 32 bytes, as K = 8 tf32 is.
+template <int N>
+__device__ __forceinline__ void wgmma_bf16(float (&d)[N / 2], uint64_t adesc, uint64_t bdesc, uint32_t accumulate);
+template <>
+__device__ __forceinline__ void wgmma_bf16<16>(float (&d)[8], uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %10, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n16k16.f32.bf16.bf16 {%0,%1,%2,%3,%4,%5,%6,%7}, %8, %9, p, 1, 1, 0, 0;\n\t}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
+      : "l"(adesc), "l"(bdesc), "r"(accumulate));
+}
+template <>
+__device__ __forceinline__ void wgmma_bf16<32>(float (&d)[16], uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %18, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n32k16.f32.bf16.bf16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, %16, %17, p, 1, 1, 0, 0;\n\t}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+      : "l"(adesc), "l"(bdesc), "r"(accumulate));
+}
+template <>
+__device__ __forceinline__ void wgmma_bf16<64>(float (&d)[32], uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, %32, %33, p, 1, 1, 0, 0;\n\t}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "l"(adesc), "l"(bdesc), "r"(accumulate));
+}
+template <>
+__device__ __forceinline__ void wgmma_bf16<128>(float (&d)[64], uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47,%48,%49,%50,%51,%52,%53,%54,%55,%56,%57,%58,%59,%60,%61,%62,%63}, %64, %65, p, 1, 1, 0, 0;\n\t}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "l"(adesc), "l"(bdesc), "r"(accumulate));
+}
+// two floats -> bf16x2 (round to nearest even), `lo` in the low half: the element at the lower address
+__device__ __forceinline__ uint32_t pack_bf16x2(float lo, float hi) {
+  uint32_t r;
+  asm("cvt.rn.bf16x2.f32 %0, %1, %2;" : "=r"(r) : "f"(hi), "f"(lo));
+  return r;
 }
 
 // K-major SWIZZLE_128B shared-memory matrix descriptor of wgmma: start >> 4, LBO = 1 (unused for
@@ -590,6 +636,47 @@ __device__ __forceinline__ void mma_tile_n(int n, uint32_t ring, uint32_t stage_
 }
 #undef MLP_MMA_TILE
 
+// One tile of the MMA role of mlp_dense_bf16_kernel: mma_tile with the bf16 MMAs (64 bf16 per stage row, four
+// m64nNk16 steps at the same byte offsets as the tf32 k8 steps).  The ring position (stage s and its phase) is carried
+// from tile to tile in two 32-bit registers instead of being recomputed from a 64-bit chunk count.
+template <int N>
+__device__ __forceinline__ void mma_tile_bf16(uint32_t ring, uint32_t stage_bytes, int S, int &s, unsigned &phase,
+                                              int kc_total, uint64_t *full, uint64_t *empty, uint64_t *acc_full,
+                                              uint64_t *acc_empty, unsigned acc_parity, uint32_t acc_s, int acc_ld,
+                                              unsigned wg, int frag_row, unsigned lane) {
+  float d[N / 2];
+#pragma unroll
+  for (int i = 0; i < N / 2; ++i) d[i] = 0.f;
+  int prev = -1;
+  for (int kc = 0; kc < kc_total; ++kc) {
+    mbar_wait(&full[s], phase);
+    fence_proxy_async_smem();
+    const uint32_t sa = ring + static_cast<uint32_t>(s) * stage_bytes;
+    const uint64_t adesc = smem_desc_sw128(sa + wg * 8192u), bdesc = smem_desc_sw128(sa + kMlpBM * 128u);
+    wgmma_fence();
+#pragma unroll
+    for (int k4 = 0; k4 < 4; ++k4)  // K = 16 bf16 = 32 bytes per instruction: +2 in 16-byte units
+      wgmma_bf16<N>(d, adesc + static_cast<uint64_t>(k4 * 2), bdesc + static_cast<uint64_t>(k4 * 2),
+                    (kc > 0 || k4 > 0) ? 1u : 0u);
+    wgmma_commit();
+    if (prev >= 0) {
+      wgmma_wait<1>();
+      if (lane == 0) mbar_arrive(&empty[prev]);
+    }
+    prev = s;
+    if (++s == S) {
+      s = 0;
+      phase ^= 1u;
+    }
+  }
+  wgmma_wait<0>();
+  acc_fence(d);
+  if (prev >= 0 && lane == 0) mbar_arrive(&empty[prev]);
+  mbar_wait(acc_empty, acc_parity ^ 1u);
+  acc_store<N>(acc_s, acc_ld, frag_row, lane, d);
+  mbar_arrive(acc_full);
+}
+
 // Persistent, warp-specialised: CTA c works on tiles c, c+grid, ... (tile = 128 rows x bn columns).
 //   producers  fill a ring of K-chunk stages (A: 128 rows x 128 B, B: bn rows x 128 B), running ahead
 //              of the tensor core across tile boundaries;
@@ -868,18 +955,19 @@ EncodeTiledFn encode_tiled_fn() {
   return fn;
 }
 
-// tensor map of one weight matrix; false: the driver cannot encode it (every launcher then returns
-// PVN3D_ERR_UNSUPPORTED without launching)
-bool weight_tensor_map(CUtensorMap *map, const float *w, int k_pad, int n_pad, int bn) {
+// tensor map of one weight matrix, fp32 or (bf16) bfloat16 elements, boxes of one 128-byte row segment x bn rows;
+// false: the driver cannot encode it (every launcher then returns PVN3D_ERR_UNSUPPORTED without launching)
+bool weight_tensor_map(CUtensorMap *map, const void *w, int k_pad, int n_pad, int bn, bool bf16 = false) {
   EncodeTiledFn enc = encode_tiled_fn();
   if (!enc || (reinterpret_cast<uintptr_t>(w) & 15u)) return false;
+  const cuuint64_t elem = bf16 ? 2u : 4u;
   const cuuint64_t dims[2] = {static_cast<cuuint64_t>(k_pad), static_cast<cuuint64_t>(n_pad)};
-  const cuuint64_t strides[1] = {static_cast<cuuint64_t>(k_pad) * sizeof(float)};
-  const cuuint32_t box[2] = {32u, static_cast<cuuint32_t>(bn)};
+  const cuuint64_t strides[1] = {static_cast<cuuint64_t>(k_pad) * elem};
+  const cuuint32_t box[2] = {static_cast<cuuint32_t>(128 / elem), static_cast<cuuint32_t>(bn)};
   const cuuint32_t estr[2] = {1u, 1u};
-  return enc(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, const_cast<float *>(w), dims, strides, box, estr,
-             CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-             CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
+  return enc(map, bf16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, const_cast<void *>(w), dims,
+             strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
+             CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
 }
 
 // One persistent launch: a CTA per SM not reserved for other streams (PVN3D_MLP_RESERVE_SMS), at most one per tile.
@@ -894,24 +982,250 @@ int launch_persistent(const Args &g, long long tiles, int threads, size_t smem, 
   return check_launch(name);
 }
 
-template <int PRO, int EPI>
-int launch_mlp(MlpArgs &a, cudaStream_t st) {
-  if (a.rows <= 0) return PVN3D_OK;
-  if (a.k_pad <= 0 || a.k_pad % 32 || a.n_pad <= 0 || a.n_pad % 16 || (reinterpret_cast<uintptr_t>(a.w) & 15u))
-    return PVN3D_ERR_INVALID_ARG;   // the weights are read 16 bytes at a time, by TMA
+// tile width, accumulator tile and ring stages of a layer (mlp_layer_kernel, mlp_dense_bf16_kernel) -> dynamic shared
+// memory bytes, 0 when fewer than 3 stages fit (asynchronous producers keep two chunks in flight)
+size_t mlp_layout(MlpArgs &a) {
   a.bn = mma_n(a.n_pad);
   a.acc_ld = std::max(32, a.bn);
   const size_t stage_bytes = kMlpBM * 128 + align_up(static_cast<size_t>(a.bn) * 128, 1024);
   const size_t fixed = mlp_smem_front(0, a.bn, a.acc_ld) + kMlpEpiWarps * 4096 + sizeof(MlpSmemCtl);
   int stages = static_cast<int>((kMlpSmemMax - fixed) / stage_bytes);
   if (stages > kMlpMaxStages) stages = kMlpMaxStages;
-  // asynchronous producers (pre-rounded dense activations) keep two chunks in flight: >= 3 stages
-  if (stages < 3) return PVN3D_ERR_UNSUPPORTED;
+  if (stages < 3) return 0;
   a.stages = stages;
-  const size_t smem = mlp_smem_front(stages, a.bn, a.acc_ld) + kMlpEpiWarps * 4096 + sizeof(MlpSmemCtl);
+  return mlp_smem_front(stages, a.bn, a.acc_ld) + kMlpEpiWarps * 4096 + sizeof(MlpSmemCtl);
+}
+
+template <int PRO, int EPI>
+int launch_mlp(MlpArgs &a, cudaStream_t st) {
+  if (a.rows <= 0) return PVN3D_OK;
+  if (a.k_pad <= 0 || a.k_pad % 32 || a.n_pad <= 0 || a.n_pad % 16 || (reinterpret_cast<uintptr_t>(a.w) & 15u))
+    return PVN3D_ERR_INVALID_ARG;   // the weights are read 16 bytes at a time, by TMA
+  const size_t smem = mlp_layout(a);
+  if (!smem) return PVN3D_ERR_UNSUPPORTED;
   if (!weight_tensor_map(&a.tmap, a.w, a.k_pad, a.n_pad, a.bn)) return PVN3D_ERR_UNSUPPORTED;
   const long long tiles = ((a.rows + kMlpBM - 1) / kMlpBM) * ceil_div(a.n_pad, a.bn);
   return launch_persistent<mlp_layer_kernel<PRO, EPI>>(a, tiles, kMlpThreads, smem, a.reserve_sms, st, "mlp_layer_kernel");
+}
+
+// =====================================================================================================
+// The dense layer with BF16 operands: the DenseFusion and head layers of FusedHeads at precision "bf16".
+//
+// mlp_layer_kernel<PRO_DENSE, EPI> with the same roles, ring, barriers and accumulator tile, and three differences:
+//   * a K chunk is 64 bf16 (one 128-byte SWIZZLE_128B row segment), so k_pad is a multiple of 64.  The weights
+//     ([n_pad][k_pad] bf16) arrive by TMA, the activation rows (bf16 already, a_cols a multiple of 8) by cp.async;
+//   * the MMAs are wgmma m64nNk16 with bf16 operands and fp32 accumulators, N = BN = mma_n(n_pad) a template parameter
+//     for every tile: a ragged last column block runs the full width on the zero rows TMA fills in past n_pad, and its
+//     epilogue stores only its own columns.  One width per instantiation keeps the MMA role within the 96 registers
+//     of a 640-thread CTA: with the four-way run-time choice of mlp_layer_kernel its loop state spills;
+//   * EPI_STORE writes act(acc + bias) as bf16 rows (OUT_BF16: cvt.rn.bf16x2, round to nearest even) or fp32 rows;
+//     EPI_SUMPOOL sums relu(acc + bias) over 32 rows in fp32, in the fixed order of the TF32 form.
+// MlpArgs::a and ::out carry the bf16 addresses; lda, ldo and col0 count elements of the pointer's own type.
+template <int EPI, bool OUT_BF16, int BN>
+__global__ void __launch_bounds__(kMlpThreads, 1) mlp_dense_bf16_kernel(const __grid_constant__ MlpArgs a) {
+  extern __shared__ unsigned char mlp_smem_raw[];
+  const uint32_t raw = smem_u32(mlp_smem_raw);
+  const uint32_t ring = (raw + 1023u) & ~1023u;   // SWIZZLE_128B atoms are 8 rows x 128 B
+  const uint32_t a_bytes = kMlpBM * 128u;
+  const uint32_t stage_bytes = a_bytes + ((static_cast<uint32_t>(a.bn) * 128u + 1023u) & ~1023u);
+  const uint32_t acc_s = ring + static_cast<uint32_t>(a.stages) * stage_bytes;
+  const uint32_t front = mlp_smem_front(a.stages, a.bn, a.acc_ld);
+  MlpSmemCtl &ctl = *reinterpret_cast<MlpSmemCtl *>(mlp_smem_raw + front + kMlpEpiWarps * 4096);
+
+  const int t = threadIdx.x;
+  const unsigned warp = t >> 5, lane = t & 31u;
+  const int kc_total = a.k_pad / 64;
+  const int S = a.stages;
+  const long long row_tiles = (a.rows + kMlpBM - 1) / kMlpBM;
+  const int n_blocks = (a.n_pad + a.bn - 1) / a.bn;
+  const long long total_tiles = row_tiles * n_blocks;
+
+  if (t == 0) {
+    for (int s = 0; s < S; ++s) {
+      mbar_init(&ctl.full[s], 128);
+      mbar_init(&ctl.empty[s], kMlpMmaWarps);
+    }
+    mbar_init(&ctl.acc_full, kMlpMmaWarps * 32);
+    mbar_init(&ctl.acc_empty, kMlpEpiWarps * 32);
+    mbar_fence_init();
+  }
+  __syncthreads();
+
+  if (warp >= kMlpEpiWarps && warp < kMlpEpiWarps + kMlpProWarps) {
+    // ================= producers: the asynchronous path of mlp_layer_kernel, 8 bf16 per 16-byte copy ============
+    const int pt = (t - kMlpEpiWarps * 32) & 127;
+    const unsigned grp = (warp - kMlpEpiWarps) >> 2;       // group 0 / 1 takes even / odd chunks
+    const int pw = pt >> 5, sub = static_cast<int>(lane & 7u), rg = static_cast<int>(lane >> 3);
+    const int r_first = 32 * pw + rg;
+    const uint16_t *abf = reinterpret_cast<const uint16_t *>(a.a);
+    int pend0 = 0, pend1 = 0, npend = 0;
+    long long it_base = 0;
+    for (long long tile = blockIdx.x; tile < total_tiles; tile += gridDim.x, it_base += kc_total) {
+      if (kc_total == 1 && static_cast<unsigned>(it_base & 1) != grp) continue;  // other group's tile
+      const long long rt = tile / n_blocks;
+      const int nb = static_cast<int>(tile - rt * n_blocks);
+      const long long p_first = rt * kMlpBM + r_first;
+      const int n0 = nb * a.bn;
+      const uint16_t *row[8];
+      unsigned live = 0u;
+#pragma unroll
+      for (int j = 0; j < 8; ++j) {
+        const long long p = p_first + 4 * j;
+        if (p < a.rows) live |= 1u << j;
+        row[j] = abf + (p < a.rows ? p : 0) * a.lda;
+      }
+      for (int kc = 0; kc < kc_total; ++kc) {
+        const long long it = it_base + kc;
+        if (static_cast<unsigned>(it & 1) != grp) continue;
+        const int s = static_cast<int>(it % S);
+        if (npend == 2) {
+          cp_async_wait<1>();
+          fence_proxy_async_smem();
+          mbar_arrive(&ctl.full[pend0]);
+          pend0 = pend1;
+          npend = 1;
+        }
+        mbar_wait(&ctl.empty[s], static_cast<unsigned>(((it / S) & 1) ^ 1));
+        const uint32_t sa = ring + static_cast<uint32_t>(s) * stage_bytes;
+        if (pt == 0) {
+          mbar_expect_tx_only(&ctl.full[s], static_cast<unsigned>(a.bn) * 128u);
+          tma_load_2d(sa + a_bytes, &a.tmap, kc * 64, n0, &ctl.full[s]);
+        }
+        const int k = kc * 64 + 8 * sub;
+        const bool k_on = k < a.a_cols;
+#pragma unroll
+        for (int j = 0; j < 8; ++j)
+          cp_async16(sa + sw128_off(r_first + 4 * j, sub), row[j] + (k_on ? k : 0), (((live >> j) & 1u) && k_on) ? 16u : 0u);
+        cp_async_commit();
+        if (npend == 0) pend0 = s; else pend1 = s;
+        ++npend;
+      }
+    }
+    if (npend == 2) {
+      cp_async_wait<1>();
+      fence_proxy_async_smem();
+      mbar_arrive(&ctl.full[pend0]);
+      pend0 = pend1;
+      npend = 1;
+    }
+    if (npend == 1) {
+      cp_async_wait<0>();
+      fence_proxy_async_smem();
+      mbar_arrive(&ctl.full[pend0]);
+    }
+  } else if (warp < kMlpEpiWarps) {
+    // ================= epilogue: warp w drains rows 32w..32w+31 of the accumulator tile (as mlp_layer_kernel) ======
+    long long j = 0;
+    const uint32_t stg = raw + front + warp * 4096u;
+    for (long long tile = blockIdx.x; tile < total_tiles; tile += gridDim.x, ++j) {
+      const long long rt = tile / n_blocks;
+      const int nb = static_cast<int>(tile - rt * n_blocks);
+      const long long p0 = rt * kMlpBM;
+      const int n0 = nb * a.bn;
+      const int bn = min(a.bn, a.n_pad - n0);
+      mbar_wait(&ctl.acc_full, static_cast<unsigned>(j & 1));
+      const long long prow = p0 + warp * 32 + lane;
+      const float *bias_t = a.bias + (a.bias_npb > 0 ? (p0 / a.bias_npb) * a.n_pad : 0);
+      for (int c0 = 0; c0 < bn; c0 += 32) {
+        float v[32];
+        const int cw = min(32, bn - c0);
+        const unsigned chunk = lane & 7u;
+        const bool col_on = static_cast<int>(chunk) * 4 < cw;
+        float4 bq = make_float4(0.f, 0.f, 0.f, 0.f);
+        if (EPI == EPI_STORE && col_on) bq = ldg128(bias_t + n0 + c0 + chunk * 4);
+        acc_ld_row(acc_s, a.acc_ld, static_cast<int>(warp * 32 + lane), c0, cw, v);
+        if constexpr (EPI == EPI_SUMPOOL) {
+#pragma unroll
+          for (int q = 0; q < 8; ++q) {
+            const float4 bq = q * 4 < cw ? ldg128(bias_t + n0 + c0 + q * 4) : make_float4(0.f, 0.f, 0.f, 0.f);
+            const bool on = prow < a.rows && q * 4 < cw;
+            v[q * 4 + 0] = on ? fmaxf(v[q * 4 + 0] + bq.x, 0.f) : 0.f;
+            v[q * 4 + 1] = on ? fmaxf(v[q * 4 + 1] + bq.y, 0.f) : 0.f;
+            v[q * 4 + 2] = on ? fmaxf(v[q * 4 + 2] + bq.z, 0.f) : 0.f;
+            v[q * 4 + 3] = on ? fmaxf(v[q * 4 + 3] + bq.w, 0.f) : 0.f;
+          }
+          warp_colsum_32(v, lane);
+          const int col = static_cast<int>(lane);
+          if (col < cw && p0 + warp * 32 < a.rows)
+            a.out[((p0 + warp * 32) / 32) * a.ldo + a.col0 + n0 + c0 + col] = v[0];
+        } else {
+          // through the swizzled 4 KB staging tile: 8 lanes per row coming out, each with ONE group of four columns
+          if (cw == 32) {
+#pragma unroll
+            for (int q = 0; q < 8; ++q)
+              sts128(stg + lane * 128u + ((static_cast<uint32_t>(q) ^ (lane & 7u)) << 4), v[q * 4 + 0], v[q * 4 + 1],
+                     v[q * 4 + 2], v[q * 4 + 3]);
+          } else {
+#pragma unroll
+            for (int q = 0; q < 4; ++q)
+              sts128(stg + lane * 128u + ((static_cast<uint32_t>(q) ^ (lane & 7u)) << 4), v[q * 4 + 0], v[q * 4 + 1],
+                     v[q * 4 + 2], v[q * 4 + 3]);
+          }
+          __syncwarp();
+          if (col_on) {
+            const bool full = p0 + kMlpBM <= a.rows;
+            float4 r[8];
+#pragma unroll
+            for (int i = 0; i < 8; ++i) {
+              const unsigned row = 4u * i + (lane >> 3);
+              r[i] = lds128(stg + row * 128u + ((chunk ^ (row & 7u)) << 4));
+            }
+#pragma unroll
+            for (int i = 0; i < 8; ++i) {
+              r[i].x += bq.x; r[i].y += bq.y; r[i].z += bq.z; r[i].w += bq.w;
+              if (a.relu) {
+                r[i].x = fmaxf(r[i].x, 0.f); r[i].y = fmaxf(r[i].y, 0.f); r[i].z = fmaxf(r[i].z, 0.f); r[i].w = fmaxf(r[i].w, 0.f);
+              }
+            }
+            const long long o_off = (p0 + warp * 32 + (lane >> 3)) * a.ldo + a.col0 + n0 + c0 + chunk * 4;
+            if constexpr (OUT_BF16) {
+              uint16_t *o = reinterpret_cast<uint16_t *>(a.out) + o_off;   // 8-byte stores: 4 bf16
+#pragma unroll
+              for (int i = 0; i < 8; ++i)
+                if (full || p0 + warp * 32 + 4 * i + (lane >> 3) < a.rows)
+                  *reinterpret_cast<uint2 *>(o + static_cast<size_t>(4 * i) * a.ldo) =
+                      make_uint2(pack_bf16x2(r[i].x, r[i].y), pack_bf16x2(r[i].z, r[i].w));
+            } else {
+              float *o = a.out + o_off;
+#pragma unroll
+              for (int i = 0; i < 8; ++i)
+                if (full || p0 + warp * 32 + 4 * i + (lane >> 3) < a.rows)
+                  *reinterpret_cast<float4 *>(o + static_cast<size_t>(4 * i) * a.ldo) = r[i];
+            }
+          }
+          __syncwarp();
+        }
+      }
+      mbar_arrive(&ctl.acc_empty);
+    }
+  } else {
+    // ================= warps 12-19: MMA, warpgroup wg takes rows 64wg..64wg+63 of every tile ===========
+    const unsigned mw = warp - (kMlpEpiWarps + kMlpProWarps), wg = mw >> 2;
+    const int frag_row = static_cast<int>(64 * wg + 16 * (mw & 3) + (lane >> 2));
+    int s = 0;
+    unsigned phase = 0u, acc_parity = 0u;
+    for (long long tile = blockIdx.x; tile < total_tiles; tile += gridDim.x, acc_parity ^= 1u)
+      mma_tile_bf16<BN>(ring, stage_bytes, S, s, phase, kc_total, ctl.full, ctl.empty, &ctl.acc_full, &ctl.acc_empty,
+                        acc_parity, acc_s, a.acc_ld, wg, frag_row, lane);
+  }
+}
+
+template <int EPI, bool OUT_BF16>
+int launch_mlp_bf16(MlpArgs &a, cudaStream_t st) {
+  if (a.rows <= 0) return PVN3D_OK;
+  const size_t smem = mlp_layout(a);
+  if (!smem || !weight_tensor_map(&a.tmap, a.w, a.k_pad, a.n_pad, a.bn, true)) return PVN3D_ERR_UNSUPPORTED;
+  const long long tiles = ((a.rows + kMlpBM - 1) / kMlpBM) * ceil_div(a.n_pad, a.bn);
+#define MLP_BF16_LAUNCH(BN)                                                                                          \
+  launch_persistent<mlp_dense_bf16_kernel<EPI, OUT_BF16, BN>>(a, tiles, kMlpThreads, smem, a.reserve_sms, st,          \
+                                                              "mlp_dense_bf16_kernel")
+  switch (a.bn) {
+    case 16: return MLP_BF16_LAUNCH(16);
+    case 32: return MLP_BF16_LAUNCH(32);
+    case 64: return MLP_BF16_LAUNCH(64);
+    default: return MLP_BF16_LAUNCH(128);
+  }
+#undef MLP_BF16_LAUNCH
 }
 
 // =====================================================================================================
@@ -1947,7 +2261,9 @@ int launch_fp2(Fp2Args &g, cudaStream_t st) {
 //                  written from the fragment with no transposing pass;
 //   FPF2_OUT_ROWS  relu(acc + b2) rounded to TF32, point-major into columns col0 .. col0+127 of rows ldo apart: a lane
 //                  quad writes each 32-byte row segment (whole sectors), as mlp_fp2_kernel does.  The heads' table.
-enum { FPF2_OUT_CN = 0, FPF2_OUT_ROWS = 1 };
+//   FPF2_OUT_ROWS_BF16  the same rows rounded to bf16 (cvt.rn: nearest even) instead of TF32, ldo and col0 in bf16
+//                  elements: the heads' table at precision "bf16".  A lane quad writes 16 contiguous bytes of a row.
+enum { FPF2_OUT_CN = 0, FPF2_OUT_ROWS = 1, FPF2_OUT_ROWS_BF16 = 2 };
 constexpr int kFpf2BM = 64;
 constexpr int kFpf2ProWarps = 8;
 constexpr int kFpf2LoaderWarp = kFpf2ProWarps + kMlpMmaWarps;   // warp 16
@@ -2155,6 +2471,17 @@ __global__ void __launch_bounds__(kFpf2Threads, 1) mlp_fp_fact2_kernel(const __g
           if (on0) stg64(o0 + c, to_tf32(fmaxf(d[4 * j] + bb.x, 0.f)), to_tf32(fmaxf(d[4 * j + 1] + bb.y, 0.f)));
           if (on1) stg64(o1 + c, to_tf32(fmaxf(d[4 * j + 2] + bb.x, 0.f)), to_tf32(fmaxf(d[4 * j + 3] + bb.y, 0.f)));
         }
+      } else if constexpr (OUT == FPF2_OUT_ROWS_BF16) {
+        // ---- out[r][col0 + c] = bf16(relu(acc + b2[c])): the arithmetic of FPF2_OUT_ROWS, one bf16x2 per lane and row
+        uint16_t *o0 = reinterpret_cast<uint16_t *>(a.out) + (r0 * a.ldo + a.col0);
+        uint16_t *o1 = o0 + 8 * static_cast<long long>(a.ldo);
+#pragma unroll
+        for (int j = 0; j < 16; ++j) {
+          const int c = 8 * j + 2 * static_cast<int>(lane & 3u);
+          const float2 bb = __ldg(reinterpret_cast<const float2 *>(g.bias2 + c));
+          if (on0) stg32(o0 + c, pack_bf16x2(fmaxf(d[4 * j] + bb.x, 0.f), fmaxf(d[4 * j + 1] + bb.y, 0.f)));
+          if (on1) stg32(o1 + c, pack_bf16x2(fmaxf(d[4 * j + 2] + bb.x, 0.f), fmaxf(d[4 * j + 3] + bb.y, 0.f)));
+        }
       } else {
         // ---- out[b][c][i] = relu(acc + b2[c]): a lane quad's rows are 8 consecutive points of one channel
         const long long fb0 = r0 / n_unk, fb1 = (r0 + 8) / n_unk;
@@ -2280,6 +2607,39 @@ __global__ void __launch_bounds__(kGatherThreads) gather_pixel_rows_kernel(const
     const int pt = i / q4, q = i - pt * q4;
     if (r0 + pt < rows)
       *reinterpret_cast<float4 *>(out + (r0 + pt) * ldo + col0 + 4 * q) = *reinterpret_cast<const float4 *>(tile + pt * ld + 4 * q);
+  }
+}
+
+// the same rows in bf16 (the heads' table at precision "bf16"): out[r][col0 + ch] = bf16(emb[f][ch][choose[r]]), from an
+// fp32 embedding (round to nearest even, as torch's .to(bfloat16)) or a bf16 one (copied).  Rows leave in 16-byte groups
+// of 8 channels; an index outside [0, hw) writes a row of NaN.
+__device__ __forceinline__ uint16_t bf16_bits(float x) { return static_cast<uint16_t>(pack_bf16x2(x, 0.f) & 0xffffu); }
+__device__ __forceinline__ uint16_t bf16_bits(uint16_t x) { return x; }
+
+template <typename T>
+__global__ void __launch_bounds__(kGatherThreads) gather_pixel_rows_bf16_kernel(const T *__restrict__ emb, int c, long long hw,
+                                                                                const long long *__restrict__ choose, int n,
+                                                                                long long rows, uint16_t *__restrict__ out,
+                                                                                int ldo, int col0) {
+  __shared__ __align__(16) uint16_t tile[kGatherPts * (kGatherMaxC + 8)];   // [point][channel], rows 16-byte aligned
+  const int ld = c + 8;
+  const int lane = static_cast<int>(threadIdx.x & 31u), warp = static_cast<int>(threadIdx.x >> 5);
+  const long long r0 = static_cast<long long>(blockIdx.x) * kGatherPts;
+  const long long r = r0 + lane;
+  const T *src = nullptr;
+  if (r < rows) {
+    const long long idx = __ldg(choose + r);
+    if (idx >= 0 && idx < hw) src = emb + (r / n) * c * hw + idx;
+  }
+#pragma unroll 4
+  for (int ch = warp; ch < c; ch += kGatherThreads / 32)
+    tile[lane * ld + ch] = src ? bf16_bits(__ldg(src + ch * hw)) : static_cast<uint16_t>(0x7fc0u);
+  __syncthreads();
+  const int q8 = c >> 3;
+  for (int i = static_cast<int>(threadIdx.x); i < kGatherPts * q8; i += kGatherThreads) {
+    const int pt = i / q8, q = i - pt * q8;
+    if (r0 + pt < rows)
+      *reinterpret_cast<uint4 *>(out + (r0 + pt) * ldo + col0 + 8 * q) = *reinterpret_cast<const uint4 *>(tile + pt * ld + 8 * q);
   }
 }
 
@@ -2602,4 +2962,96 @@ extern "C" int pvn3d_mlp_dense_sum32(const float *a, int lda, int a_cols, long l
   m.reserve_sms = (flags >> 8) & 0xff;
   m.pool = 32;
   return launch_mlp<PRO_DENSE, EPI_SUMPOOL>(m, as_stream(stream));
+}
+
+// ---- BF16 forms (FusedHeads at precision "bf16") ------------------------------------------------------------------------
+// the argument checks and kernel arguments the three bf16 dense entry points share: PVN3D_ERR_INVALID_ARG for a bad
+// operand or a flag outside `allowed` (and the reserved-SM byte), before any CUDA call
+static int dense_bf16_args(const pvn3d_bf16_t *a, int lda, int a_cols, long long rows, const pvn3d_bf16_t *w,
+                           const float *bias, int k_pad, int n_pad, int flags, int allowed, const void *out, int ldo, int col0,
+                           MlpArgs &m) {
+  if (!a || !w || !bias || !out || a_cols < 0 || lda < a_cols || lda % 8 || a_cols % 8 || rows < 0 || k_pad <= 0 ||
+      k_pad % 64 || n_pad <= 0 || n_pad % 16 || ldo % 4 || col0 < 0 || col0 % 4 ||
+      static_cast<long long>(col0) + n_pad > ldo || (flags & ~(allowed | 0xff00)) ||
+      (reinterpret_cast<uintptr_t>(a) & 15u) || (reinterpret_cast<uintptr_t>(w) & 15u) ||
+      (reinterpret_cast<uintptr_t>(out) & 15u))
+    return PVN3D_ERR_INVALID_ARG;
+  m.w = reinterpret_cast<const float *>(w); m.bias = bias; m.rows = rows; m.k_pad = k_pad; m.n_pad = n_pad;
+  m.a = reinterpret_cast<const float *>(a); m.lda = lda; m.a_cols = a_cols;
+  m.out = static_cast<float *>(const_cast<void *>(out)); m.ldo = ldo; m.col0 = col0;
+  m.relu = (flags & PVN3D_MLP_RELU) ? 1 : 0;
+  m.reserve_sms = (flags >> 8) & 0xff;
+  return PVN3D_OK;
+}
+
+extern "C" int pvn3d_mlp_dense_bf16(const pvn3d_bf16_t *a, int lda, int a_cols, long long rows, const pvn3d_bf16_t *w,
+                                    const float *bias, int k_pad, int n_pad, int flags, void *out, int ldo, int col0,
+                                    pvn3d_stream_t stream) {
+  MlpArgs m{};
+  const int rc = dense_bf16_args(a, lda, a_cols, rows, w, bias, k_pad, n_pad, flags, PVN3D_MLP_RELU | PVN3D_MLP_OUT_BF16,
+                                 out, ldo, col0, m);
+  if (rc != PVN3D_OK) return rc;
+  if (flags & PVN3D_MLP_OUT_BF16) return launch_mlp_bf16<EPI_STORE, true>(m, as_stream(stream));
+  return launch_mlp_bf16<EPI_STORE, false>(m, as_stream(stream));
+}
+
+extern "C" int pvn3d_mlp_dense_frame_bias_bf16(const pvn3d_bf16_t *a, int lda, int a_cols, long long rows,
+                                               int rows_per_frame, const pvn3d_bf16_t *w, const float *bias, int k_pad,
+                                               int n_pad, int flags, void *out, int ldo, int col0, pvn3d_stream_t stream) {
+  if (rows_per_frame <= 0 || rows_per_frame % kMlpBM || rows % rows_per_frame) return PVN3D_ERR_INVALID_ARG;
+  MlpArgs m{};
+  const int rc = dense_bf16_args(a, lda, a_cols, rows, w, bias, k_pad, n_pad, flags, PVN3D_MLP_RELU | PVN3D_MLP_OUT_BF16,
+                                 out, ldo, col0, m);
+  if (rc != PVN3D_OK) return rc;
+  m.bias_npb = rows_per_frame;
+  if (flags & PVN3D_MLP_OUT_BF16) return launch_mlp_bf16<EPI_STORE, true>(m, as_stream(stream));
+  return launch_mlp_bf16<EPI_STORE, false>(m, as_stream(stream));
+}
+
+extern "C" int pvn3d_mlp_dense_sum32_bf16(const pvn3d_bf16_t *a, int lda, int a_cols, long long rows, const pvn3d_bf16_t *w,
+                                          const float *bias, int k_pad, int n_pad, int flags, float *out, int ldo, int col0,
+                                          pvn3d_stream_t stream) {
+  MlpArgs m{};
+  const int rc = dense_bf16_args(a, lda, a_cols, rows, w, bias, k_pad, n_pad, flags, PVN3D_MLP_RELU, out, ldo, col0, m);
+  if (rc != PVN3D_OK) return rc;
+  m.relu = 1;
+  m.pool = 32;
+  return launch_mlp_bf16<EPI_SUMPOOL, false>(m, as_stream(stream));
+}
+
+extern "C" int pvn3d_mlp_fp_fact2_rows_bf16(const float *p, const float *table, const int *nn_idx, const float *nn_w, int b,
+                                            int n_unknown, int m_known, const pvn3d_mlp_layer_t *layer_s,
+                                            const pvn3d_mlp_layer_t *layer2, int flags, pvn3d_bf16_t *out, int ldo, int col0,
+                                            pvn3d_stream_t stream) {
+  if (ldo % 8 || col0 < 0 || col0 % 8 || static_cast<long long>(col0) + 128 > ldo || (reinterpret_cast<uintptr_t>(out) & 15u) ||
+      (layer2 && (reinterpret_cast<uintptr_t>(layer2->bias) & 7u)))
+    return PVN3D_ERR_INVALID_ARG;
+  FpFact2Args g{};
+  const int rc = fp_fact2_args(p, table, nn_idx, nn_w, b, n_unknown, m_known, layer_s, layer2, flags,
+                               reinterpret_cast<float *>(out), g);
+  if (rc != PVN3D_OK) return rc;
+  g.a.ldo = ldo;
+  g.a.col0 = col0;
+  return launch_fp_fact2<FPF2_OUT_ROWS_BF16>(g, table, layer_s->w, layer2->w, as_stream(stream));
+}
+
+extern "C" int pvn3d_gather_pixel_rows_bf16(const void *emb, int emb_bf16, int b, int c, long long hw,
+                                            const long long *choose, int n, pvn3d_bf16_t *out, int ldo, int col0,
+                                            pvn3d_stream_t stream) {
+  if (!emb || !choose || !out || (emb_bf16 != 0 && emb_bf16 != 1) || b < 0 || n < 0 || c <= 0 || c % 8 || hw <= 0 ||
+      ldo % 8 || col0 < 0 || col0 % 8 || static_cast<long long>(col0) + c > ldo ||
+      (reinterpret_cast<uintptr_t>(emb) & (emb_bf16 ? 1u : 3u)) || (reinterpret_cast<uintptr_t>(choose) & 7u) ||
+      (reinterpret_cast<uintptr_t>(out) & 15u))
+    return PVN3D_ERR_INVALID_ARG;
+  const long long rows = static_cast<long long>(b) * n;
+  if (rows > 0x7fffffffll || c > kGatherMaxC) return PVN3D_ERR_UNSUPPORTED;
+  if (rows == 0) return PVN3D_OK;
+  const unsigned grid = static_cast<unsigned>((rows + kGatherPts - 1) / kGatherPts);
+  if (emb_bf16)
+    gather_pixel_rows_bf16_kernel<uint16_t><<<grid, kGatherThreads, 0, as_stream(stream)>>>(
+        static_cast<const uint16_t *>(emb), c, hw, choose, n, rows, out, ldo, col0);
+  else
+    gather_pixel_rows_bf16_kernel<float><<<grid, kGatherThreads, 0, as_stream(stream)>>>(
+        static_cast<const float *>(emb), c, hw, choose, n, rows, out, ldo, col0);
+  return check_launch("gather_pixel_rows_bf16_kernel");
 }

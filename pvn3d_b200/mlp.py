@@ -52,18 +52,31 @@ def fold_conv_bn(layer: torch.nn.Module) -> Tuple[torch.Tensor, torch.Tensor]:
     return w.float(), bias.float()
 
 
-class PackedLayer:
-    """one folded layer in the layout pvn3d_mlp_* expects"""
+PRECISIONS = ("tf32", "bf16")
 
-    def __init__(self, w: torch.Tensor, bias: torch.Tensor, k_valid_prev_pad: int | None = None):
+
+def check_precision(precision: str) -> str:
+    if precision not in PRECISIONS:
+        raise ValueError(f"precision must be one of {PRECISIONS}, got {precision!r}")
+    return precision
+
+
+class PackedLayer:
+    """one folded layer in the layout pvn3d_mlp_* expects.  precision "tf32": w [n_pad, k_pad] f32 TF32-rounded, k_pad a
+    multiple of 32; "bf16" (pvn3d_mlp_dense_bf16 and its forms): w bfloat16 rounded to nearest even, k_pad a multiple of
+    64 (one 128-byte row segment per K chunk).  bias [n_pad] f32 either way."""
+
+    def __init__(self, w: torch.Tensor, bias: torch.Tensor, k_valid_prev_pad: int | None = None, precision: str = "tf32"):
         n, k = w.shape
         self.n, self.k = n, k
+        self.precision = check_precision(precision)
         self.n_pad = (n + 15) // 16 * 16
         k_in = k if k_valid_prev_pad is None else k_valid_prev_pad     # width of the producing activation
-        self.k_pad = (max(k, k_in) + 31) // 32 * 32
+        k_mult = 64 if precision == "bf16" else 32
+        self.k_pad = (max(k, k_in) + k_mult - 1) // k_mult * k_mult
         wp = torch.zeros((self.n_pad, self.k_pad), dtype=torch.float32, device=w.device)
         wp[:n, :k] = w
-        self.w = tf32_round(wp).contiguous()
+        self.w = (wp.to(torch.bfloat16) if precision == "bf16" else tf32_round(wp)).contiguous()
         self.bias = torch.zeros((self.n_pad,), dtype=torch.float32, device=w.device)
         self.bias[:n] = bias
 
@@ -231,13 +244,17 @@ def mlp_fp_fact2(p: torch.Tensor, table: torch.Tensor, nn_idx: torch.Tensor, nn_
 def mlp_fp_fact2_rows(p: torch.Tensor, table: torch.Tensor, nn_idx: torch.Tensor, nn_w: torch.Tensor, m_known: int,
                       layer_s: PackedLayer, layer2: PackedLayer, out: torch.Tensor, col0: int, reserve=0) -> torch.Tensor:
     """mlp_fp_fact2 with its output point-major in columns col0 .. col0+127 of the row table out [b * n_unknown, ldo]
-    (pvn3d_mlp_fp_fact2_rows): tf32_round of the transposed [b, 128, n_unknown], bit for bit"""
+    (pvn3d_mlp_fp_fact2_rows): tf32_round of the transposed [b, 128, n_unknown], bit for bit.  A bfloat16 `out` takes
+    the same rows rounded to bf16 instead (pvn3d_mlp_fp_fact2_rows_bf16): the transposed [b, 128, n_unknown]
+    .to(torch.bfloat16), bit for bit."""
     b, n_unknown = nn_idx.shape[0], nn_idx.shape[1]
     assert p.size(-1) == layer_s.n_pad and table.size(-1) == layer_s.k_pad and table.size(0) == b * n_unknown
     assert out.dim() == 2 and out.size(0) == b * n_unknown and out.stride(1) == 1
+    assert out.dtype in (torch.float32, torch.bfloat16)
+    fn = "pvn3d_mlp_fp_fact2_rows_bf16" if out.dtype == torch.bfloat16 else "pvn3d_mlp_fp_fact2_rows"
     ls, l2 = _layer_struct(layer_s), _layer_struct(layer2)
-    call("pvn3d_mlp_fp_fact2_rows", p.device, ptr(p), ptr(table), ptr(nn_idx), ptr(nn_w), b, n_unknown, m_known,
-         ctypes.addressof(ls), ctypes.addressof(l2), _flags(False, reserve=reserve), ptr(out), out.stride(0), col0)
+    call(fn, p.device, ptr(p), ptr(table), ptr(nn_idx), ptr(nn_w), b, n_unknown, m_known, ctypes.addressof(ls),
+         ctypes.addressof(l2), _flags(False, reserve=reserve), ptr(out), out.stride(0), col0)
     return out
 
 
@@ -414,8 +431,9 @@ class FusedPointnet2MSG:
         MLP kernels leave free for kernels of other streams (the next batch's sampling); reserve_levels: the SA levels
         0 .. reserve_levels-1 do so (5: the FP modules too) -- the sampling of the next batch is over well before the
         MLPs are, and the later layers then take the whole machine.
-        out_rows [B*N, ldo]: FP1 writes the features TF32-rounded and point-major into its columns col0 .. col0+127
-        instead (the DenseFusion table of FusedPVN3D), and out_rows is returned."""
+        out_rows [B*N, ldo]: FP1 writes the features TF32-rounded (bf16-rounded for a bfloat16 out_rows) and
+        point-major into its columns col0 .. col0+127 instead (the DenseFusion table of FusedPVN3D), and out_rows is
+        returned."""
         b, _, width = pointcloud.shape
         c0 = width - 3
         rs_all = int(reserve_sms)
