@@ -337,6 +337,35 @@ int pvn3d_mlp_fp_fact2_rows_bf16(const float *p, const float *table, const int *
  * aligned; otherwise checks, NaN rows and PVN3D_ERR_UNSUPPORTED as pvn3d_gather_pixel_rows. */
 int pvn3d_gather_pixel_rows_bf16(const void *emb, int emb_bf16, int b, int c, long long hw, const long long *choose, int n,
                                  pvn3d_bf16_t *out, int ldo, int col0, pvn3d_stream_t stream);
+/* The full-resolution tail of PVN3D's CNN (pspnet.py:88-90 of Modified_PSPNet: up_3 = bilinear x2 with align_corners ->
+ * Conv2d(64,64,3,padding 1) -> BatchNorm2d -> PReLU, then final = Conv2d(64,128,1)) evaluated only at the sampled pixels:
+ * the rows pvn3d_gather_pixel_rows would copy out of the dense [b][128][2h][2w] embedding, to TF32 accuracy, without
+ * the dense maps.  Row r = f * n + p, with (y, x) = divmod(choose[f][0][p], 2w):
+ *     out[r][col0 + 0:128] = tf32( W2 . prelu(W1 . taps + b1) + b2 )
+ *     taps[(3 (dy+1) + (dx+1)) * 64 + c] = the align_corners bilinear sample of x[f][:, :, c] at up-sampled pixel
+ *                                          (y+dy, x+dx), dy, dx in {-1, 0, 1}; zero outside [0, 2h) x [0, 2w)
+ *   x       [b][h][w][64] f32, CHANNELS-LAST, 16-byte aligned: the input of up_3 (the output of up_2); h, w >= 2
+ *   choose  [b][1][n] int64 indices into the 2h x 2w image (8-byte aligned)
+ *   layer1  k_pad 576, n_pad 64: the 3x3 conv with the BatchNorm folded in, K tap-major as above, TF32-rounded;
+ *   layer2  k_pad 64, n_pad 128: final.  Both w 16-byte aligned, layer2->bias 8-byte aligned.
+ *   slope   [64] f32: the PReLU slope of each channel (prelu(v) = v >= 0 ? v : slope * v)
+ *   out     rows ldo floats apart, 16-byte aligned; ldo, col0 multiples of 4, col0 >= 0, col0 + 128 <= ldo; other
+ *           columns are not touched
+ * Arithmetic: taps combined in fp32 and rounded to TF32, TF32 wgmma with fp32 accumulation in both layers, the
+ * layer-1 activation rounded to TF32.  An index outside [0, 4 h w) writes a row of NaN.
+ * flags: PVN3D_MLP_RESERVE_SMS(n) only.  PVN3D_ERR_INVALID_ARG for null pointers, misalignment, other flags or a bad
+ * column range; PVN3D_ERR_UNSUPPORTED unless pvn3d_psp_tail_supported(layer1, layer2) is 1 (the shapes above), for
+ * h or w >= 2^15, b * h * w >= 2^31 or b * n >= 2^31, or when the driver cannot encode the weights' tensor maps -- all
+ * before any launch.  The query is host-only and touches no device memory. */
+int pvn3d_psp_tail_rows(const float *x, int b, int h, int w, const long long *choose, int n,
+                        const pvn3d_mlp_layer_t *layer1, const pvn3d_mlp_layer_t *layer2, const float *slope, int flags,
+                        float *out, int ldo, int col0, pvn3d_stream_t stream);
+int pvn3d_psp_tail_supported(const pvn3d_mlp_layer_t *layer1, const pvn3d_mlp_layer_t *layer2);
+/* pvn3d_psp_tail_rows with bf16 rows: the same arithmetic (TF32 MMAs), acc + b2 rounded to nearest even bf16 instead of
+ * TF32; ldo and col0 (in bf16 elements) multiples of 8. */
+int pvn3d_psp_tail_rows_bf16(const float *x, int b, int h, int w, const long long *choose, int n,
+                             const pvn3d_mlp_layer_t *layer1, const pvn3d_mlp_layer_t *layer2, const float *slope, int flags,
+                             pvn3d_bf16_t *out, int ldo, int col0, pvn3d_stream_t stream);
 /* weight[p,0:3] = (1/(sqrt(dist2)+1e-8)) / sum  (pointnet2_modules.py:184-186), fp32 IEEE ops */
 int pvn3d_three_nn_weights(const float *dist2, long long rows, float *weight, pvn3d_stream_t stream);
 

@@ -2519,6 +2519,337 @@ int launch_fp_fact2(FpFact2Args &g, const float *table, const float *ws, const f
   return launch_persistent<mlp_fp_fact2_kernel<OUT>>(g, tiles, kFpf2Threads, smem, a.reserve_sms, st, "mlp_fp_fact2_kernel");
 }
 
+// =====================================================================================================
+// The full-resolution tail of PVN3D's CNN evaluated ONLY at the sampled pixels, in ONE persistent kernel.
+//
+// Modified_PSPNet ends with up_3 = bilinear x2 (align_corners) -> Conv2d(64,64,3,pad 1) -> BatchNorm -> PReLU and
+// final = Conv2d(64,128,1), both at H x W = 2h x 2w, and PVN3D.forward keeps N of the H*W embedding columns (4 % at
+// 12288 of 480 x 640).  Up to the PReLU every step is linear per pixel, so row r = f * n + p of the heads' table is
+//   out[r] = tf32(W2 . prelu(W1 . taps + b1) + b2),   taps[(3 (dy+1) + (dx+1)) * 64 + c] = up(x)[f][c][y+dy][x+dx]
+// with (y, x) = divmod(choose[r], W), up() the align_corners bilinear sample of the half-resolution map (zero outside
+// [0,H) x [0,W): the conv's padding applies to the up-sampled map) and W1 the 3x3 conv with the BN folded, K tap-major.
+// Per 128-row tile:
+//   loader    (warp 16)     brings W2 into shared memory once, then streams W1's 18 K chunks (64 x 32 fp32 = 8 KB, TMA,
+//                           SWIZZLE_128B) into the ring slot of each chunk.  Streamed, not resident: W1 is 144 KB, which
+//                           beside W2 (32 KB) and H would leave two A stages; the stream is 144 KB of L2 reads per 128
+//                           rows, under the 1.1 MB the same rows gather, and leaves room for a six-deep ring;
+//   producers (warps 0-7)   group q = warp / 4 stages the chunks it % 2 == q, warp w rows 32 (w & 3)..: K chunk kc is
+//                           channels 32 (kc & 1).. of tap kc / 2, the bilinear combination of one contiguous 128-byte
+//                           run of each of four source pixels of the channels-last map, rounded to TF32.  The source
+//                           rows / columns and weights of a row's three tap rows and three tap columns are computed
+//                           once per tile and kept in shared memory (16 words per row);
+//   MMA       (warps 8-15)  warpgroup wg holds rows 64 wg.. : layer 1 (wgmma m64n64k8, 72 K steps) into registers,
+//                           tf32(prelu(acc + b1)) into its rows of the K-major SWIZZLE_128B H tile, fence.proxy.async,
+//                           layer 2 (m64n128k8, 8 K steps) against the resident W2, tf32(acc + b2) (OUT_BF16: rounded
+//                           to bf16 instead) stored a lane quad per row segment as mlp_fp_fact2_kernel<FPF2_OUT_ROWS>.
+// The bilinear index and weight are exact integer arithmetic: i0 = t (h-1) div (H-1), lambda = (t (h-1) mod (H-1)) /
+// (H-1) correctly rounded (torch multiplies by an fp32 scale: the same sample to ~1e-7 * h in lambda).
+// A choose index outside [0, H*W) gives a NaN row: its operand row is NaN and both layers carry it.
+constexpr int kPspBM = 128;
+constexpr int kPspProWarps = 8;
+constexpr int kPspLoaderWarp = kPspProWarps + kMlpMmaWarps;   // warp 16
+constexpr int kPspThreads = (kPspLoaderWarp + 1) * 32;
+constexpr int kPspC = 64;                    // channels of the half-resolution map and of up_3
+constexpr int kPspKc1 = 9 * kPspC / 32;      // K chunks of layer 1: two per tap
+constexpr int kPspN2 = 128;                  // the embedding width
+constexpr int kPspMaxStages = 6;
+constexpr uint32_t kPspAStage = kPspBM * 128u;           // one K chunk of the operand tile: 128 rows x 32 fp32
+constexpr uint32_t kPspWStage = kPspC * 128u;            // one K chunk of W1: 64 rows x 32 fp32
+constexpr uint32_t kPspStage = kPspAStage + kPspWStage;
+constexpr uint32_t kPspRowBytes = 64u;                   // row state, words: [0..2] (f h + i0) w of the tap rows dy = -1, 0, 1,
+                                                         // [3..5] the same for i1, [6..8] lambda_y, [9..11] j0 of the tap
+                                                         // columns, [12..14] lambda_x, [15] mask
+constexpr unsigned kPspNanRow = 64u;                     // mask: bits 0-2 tap row inside the image, 3-5 tap column, 6 NaN row
+
+struct PspTailArgs {
+  alignas(64) CUtensorMap tmap_w1, tmap_w2;
+  const float *x;            // [b][h][w][64] channels-last
+  const long long *choose;   // [b][1][n]
+  const float *bias1, *slope, *bias2;
+  void *out;
+  long long rows;            // b * n
+  int n, h, w, ldo, col0, stages, reserve_sms;
+};
+
+struct PspTailSmemCtl {
+  uint64_t full[kPspMaxStages];    // 128 producer threads + the loader's arrive.expect_tx + the TMA bytes of the W1 chunk
+  uint64_t empty[kPspMaxStages];   // 8 arrivals: the MMA warps
+  uint64_t w2_full;
+};
+
+// shared-memory layout behind the 1024-byte aligned base (kernel, launcher and pvn3d_psp_tail_supported use the same
+// function): [W2: 2 chunks of 128 x 128 B][H: 2 chunks of 128 x 128 B][ring: stages x (16 KB A + 8 KB W1)][row states:
+// 64 B per row of each producer warp][barriers]
+struct PspTailSmem {
+  uint32_t w2, h, ring, rows, ctl, bytes;   // offsets from the aligned base; bytes = dynamic size incl. alignment slack
+};
+static inline __host__ __device__ PspTailSmem psp_tail_smem(int stages) {
+  PspTailSmem s;
+  s.w2 = 0;
+  s.h = s.w2 + 2u * kPspN2 * 128u;
+  s.ring = s.h + 2u * kPspAStage;
+  s.rows = s.ring + static_cast<uint32_t>(stages) * kPspStage;
+  s.ctl = s.rows + kPspProWarps * 32u * kPspRowBytes;
+  s.bytes = 1024u + s.ctl + static_cast<uint32_t>(sizeof(PspTailSmemCtl));
+  return s;
+}
+// ring slots pvn3d_psp_tail_rows runs with (6: 225 KB); 0 if the layers are not 576 -> 64 and 64 -> 128
+int psp_tail_stages(int k1_pad, int n1_pad, int k2_pad, int n2_pad) {
+  if (k1_pad != 9 * kPspC || n1_pad != kPspC || k2_pad != kPspC || n2_pad != kPspN2) return 0;
+  const uint32_t fixed = psp_tail_smem(0).bytes;
+  const int stages = std::min<int>(kPspMaxStages, static_cast<int>((kMlpSmemMax - fixed) / kPspStage));
+  return stages >= 3 ? stages : 0;
+}
+
+__device__ __forceinline__ uint32_t lds32(uint32_t addr) {
+  uint32_t v;
+  asm volatile("ld.shared.b32 %0, [%1];" : "=r"(v) : "r"(addr));
+  return v;
+}
+
+// source index and weight of up-sampled coordinate t (0 <= t < 2 n_src) under align_corners: exact floor and remainder
+__device__ __forceinline__ void psp_axis(int t, int n_src, int &i0, float &lambda) {
+  const int den = 2 * n_src - 1, num = t * (n_src - 1);
+  i0 = num / den;
+  lambda = __fdiv_rn(static_cast<float>(num - i0 * den), static_cast<float>(den));
+}
+
+// the row state of point p (rows past the end: every tap dead, the operand row is zero)
+__device__ __forceinline__ void psp_row_setup(const PspTailArgs &g, long long p, uint32_t dst) {
+  int yo0[3] = {0, 0, 0}, yo1[3] = {0, 0, 0}, xo[3] = {0, 0, 0};
+  float ly[3] = {0.f, 0.f, 0.f}, lx[3] = {0.f, 0.f, 0.f};
+  unsigned mask = 0u;
+  if (p < g.rows) {
+    const long long c = __ldg(g.choose + p);
+    const int H = 2 * g.h, W = 2 * g.w;
+    if (c < 0 || c >= static_cast<long long>(H) * W) {
+      mask = kPspNanRow;
+    } else {
+      const int f = static_cast<int>(p / g.n), y = static_cast<int>(c / W), x = static_cast<int>(c - static_cast<long long>(y) * W);
+#pragma unroll
+      for (int d = 0; d < 3; ++d) {
+        const int ty = y + d - 1, tx = x + d - 1;
+        if (ty >= 0 && ty < H) {
+          int i0;
+          psp_axis(ty, g.h, i0, ly[d]);
+          yo0[d] = (f * g.h + i0) * g.w;
+          yo1[d] = (f * g.h + min(i0 + 1, g.h - 1)) * g.w;
+          mask |= 1u << d;
+        }
+        if (tx >= 0 && tx < W) {
+          psp_axis(tx, g.w, xo[d], lx[d]);
+          mask |= 8u << d;
+        }
+      }
+    }
+  }
+  sts128(dst, __int_as_float(yo0[0]), __int_as_float(yo0[1]), __int_as_float(yo0[2]), __int_as_float(yo1[0]));
+  sts128(dst + 16u, __int_as_float(yo1[1]), __int_as_float(yo1[2]), ly[0], ly[1]);
+  sts128(dst + 32u, ly[2], __int_as_float(xo[0]), __int_as_float(xo[1]), __int_as_float(xo[2]));
+  sts128(dst + 48u, lx[0], lx[1], lx[2], __uint_as_float(mask));
+}
+
+// K chunk kc of the producer's 8 rows: tf32 of tap kc / 2, channels 32 (kc & 1) + 4 sub .. +3.  `rst` is the state of the
+// thread's first row; its rows are 4 apart.
+__device__ __forceinline__ void psp_stage_chunk(const PspTailArgs &g, uint32_t rst, int r_first, int sub, int kc, uint32_t sa) {
+  const int tap = kc >> 1, dy = tap / 3, dx = tap - 3 * dy;
+  const unsigned need = (1u << dy) | (8u << dx);
+  const float *xc = g.x + (kc & 1) * 32 + 4 * sub;
+  const float nan = __int_as_float(0x7fc00000);
+#pragma unroll
+  for (int hh = 0; hh < 2; ++hh) {  // two halves: 16 LDG.128 in flight each
+    float4 v00[4], v01[4], v10[4], v11[4];
+#pragma unroll
+    for (int jj = 0; jj < 4; ++jj) {
+      const uint32_t rs = rst + 4u * kPspRowBytes * (hh * 4 + jj);
+      v00[jj] = v01[jj] = v10[jj] = v11[jj] = make_float4(0.f, 0.f, 0.f, 0.f);
+      if ((lds32(rs + 60u) & need) == need) {
+        const int y0 = static_cast<int>(lds32(rs + 4u * dy)), y1 = static_cast<int>(lds32(rs + 12u + 4u * dy));
+        const int x0 = static_cast<int>(lds32(rs + 36u + 4u * dx)), x1 = min(x0 + 1, g.w - 1);
+        v00[jj] = ldg128(xc + static_cast<size_t>(y0 + x0) * kPspC);
+        v01[jj] = ldg128(xc + static_cast<size_t>(y0 + x1) * kPspC);
+        v10[jj] = ldg128(xc + static_cast<size_t>(y1 + x0) * kPspC);
+        v11[jj] = ldg128(xc + static_cast<size_t>(y1 + x1) * kPspC);
+      }
+    }
+#pragma unroll
+    for (int jj = 0; jj < 4; ++jj) {
+      const int j = hh * 4 + jj;
+      const uint32_t rs = rst + 4u * kPspRowBytes * j;
+      const float ly = __uint_as_float(lds32(rs + 24u + 4u * dy)), lx = __uint_as_float(lds32(rs + 48u + 4u * dx));
+      const float my = 1.f - ly, mx = 1.f - lx;
+      float4 v;
+      v.x = __fmaf_rn(ly, __fmaf_rn(lx, v11[jj].x, mx * v10[jj].x), my * __fmaf_rn(lx, v01[jj].x, mx * v00[jj].x));
+      v.y = __fmaf_rn(ly, __fmaf_rn(lx, v11[jj].y, mx * v10[jj].y), my * __fmaf_rn(lx, v01[jj].y, mx * v00[jj].y));
+      v.z = __fmaf_rn(ly, __fmaf_rn(lx, v11[jj].z, mx * v10[jj].z), my * __fmaf_rn(lx, v01[jj].z, mx * v00[jj].z));
+      v.w = __fmaf_rn(ly, __fmaf_rn(lx, v11[jj].w, mx * v10[jj].w), my * __fmaf_rn(lx, v01[jj].w, mx * v00[jj].w));
+      if (lds32(rs + 60u) & kPspNanRow) v = make_float4(nan, nan, nan, nan);
+      sts_tf32(sa + sw128_off(r_first + 4 * j, sub), v);
+    }
+  }
+}
+
+template <bool OUT_BF16>
+__global__ void __launch_bounds__(kPspThreads, 1) psp_tail_kernel(const __grid_constant__ PspTailArgs g) {
+  extern __shared__ unsigned char mlp_smem_raw[];
+  const uint32_t raw = smem_u32(mlp_smem_raw);
+  const uint32_t base = (raw + 1023u) & ~1023u;   // SWIZZLE_128B atoms are 8 rows x 128 B
+  const int S = g.stages;
+  const PspTailSmem L = psp_tail_smem(S);
+  PspTailSmemCtl &ctl = *reinterpret_cast<PspTailSmemCtl *>(mlp_smem_raw + (base - raw) + L.ctl);
+  const int t = threadIdx.x;
+  const unsigned warp = t >> 5, lane = t & 31u;
+  const int tiles = static_cast<int>((g.rows + kPspBM - 1) / kPspBM);   // the launcher checks the 32-bit counts
+
+  if (t == 0) {
+    for (int s = 0; s < S; ++s) {
+      mbar_init(&ctl.full[s], 128 + 1);
+      mbar_init(&ctl.empty[s], kMlpMmaWarps);
+    }
+    mbar_init(&ctl.w2_full, 1);
+    mbar_fence_init();
+  }
+  __syncthreads();
+
+  if (warp < kPspProWarps) {
+    // ================= producers: group q = warp / 4 stages the items it % 2 == q, warp w rows 32 (w & 3).. ======
+    const unsigned grp = warp >> 2;
+    const int sub = static_cast<int>(lane & 7u), r_first = 32 * static_cast<int>(warp & 3u) + static_cast<int>(lane >> 3);
+    const uint32_t rst_w = base + L.rows + warp * 32u * kPspRowBytes;
+    int it = 0;
+    for (int tile = blockIdx.x; tile < tiles; tile += gridDim.x) {
+      __syncwarp();   // every lane is done with the previous tile's row state
+      psp_row_setup(g, static_cast<long long>(tile) * kPspBM + 32 * static_cast<int>(warp & 3u) + static_cast<int>(lane),
+                    rst_w + lane * kPspRowBytes);
+      __syncwarp();
+      for (int kc = 0; kc < kPspKc1; ++kc, ++it) {
+        if (static_cast<unsigned>(it & 1) != grp) continue;
+        const int s = it % S;
+        mbar_wait(&ctl.empty[s], static_cast<unsigned>(((it / S) & 1) ^ 1));
+        psp_stage_chunk(g, rst_w + (lane >> 3) * kPspRowBytes, r_first, sub, kc, base + L.ring + static_cast<uint32_t>(s) * kPspStage);
+        fence_proxy_async_smem();
+        mbar_arrive(&ctl.full[s]);
+      }
+    }
+  } else if (warp == kPspLoaderWarp) {
+    // ================= loader: W2 once, then the W1 chunk of every item, in ring order ==========================
+    if (lane == 0) {
+      mbar_expect_tx(&ctl.w2_full, 2u * kPspN2 * 128u);
+      for (int kc = 0; kc < 2; ++kc) tma_load_2d(base + L.w2 + kc * kPspN2 * 128u, &g.tmap_w2, kc * 32, 0, &ctl.w2_full);
+      int it = 0;
+      for (int tile = blockIdx.x; tile < tiles; tile += gridDim.x)
+        for (int kc = 0; kc < kPspKc1; ++kc, ++it) {
+          const int s = it % S;
+          mbar_wait(&ctl.empty[s], static_cast<unsigned>(((it / S) & 1) ^ 1));
+          mbar_expect_tx(&ctl.full[s], kPspWStage);
+          tma_load_2d(base + L.ring + static_cast<uint32_t>(s) * kPspStage + kPspAStage, &g.tmap_w1, kc * 32, 0, &ctl.full[s]);
+        }
+    }
+  } else {
+    // ================= MMA + epilogues: warpgroup wg, warp w4 of it holds rows 64 wg + 16 w4 .. +15 of the tile ===
+    const unsigned mw = warp - kPspProWarps, wg = mw >> 2, w4 = mw & 3u;
+    const int frag_row = static_cast<int>(64 * wg + 16 * w4 + (lane >> 2));
+    const uint32_t h_s = base + L.h;
+    mbar_wait(&ctl.w2_full, 0u);
+    int it = 0;
+    for (int tile = blockIdx.x; tile < tiles; tile += gridDim.x) {
+      // ---- layer 1: the 18 K chunks of the ring into registers, each slot released once its MMAs have retired
+      float d1[32];
+#pragma unroll
+      for (int i = 0; i < 32; ++i) d1[i] = 0.f;
+      int prev = -1;
+      for (int kc = 0; kc < kPspKc1; ++kc, ++it) {
+        const int s = it % S;
+        mbar_wait(&ctl.full[s], static_cast<unsigned>((it / S) & 1));
+        fence_proxy_async_smem();
+        const uint32_t slot = base + L.ring + static_cast<uint32_t>(s) * kPspStage;
+        const uint64_t adesc = smem_desc_sw128(slot + wg * 64u * 128u), bdesc = smem_desc_sw128(slot + kPspAStage);
+        wgmma_fence();
+#pragma unroll
+        for (int k4 = 0; k4 < 4; ++k4)
+          wgmma_tf32<64>(d1, adesc + static_cast<uint64_t>(k4 * 2), bdesc + static_cast<uint64_t>(k4 * 2), (kc > 0 || k4 > 0) ? 1u : 0u);
+        wgmma_commit();
+        if (prev >= 0) {
+          wgmma_wait<1>();
+          if (lane == 0) mbar_arrive(&ctl.empty[prev]);
+        }
+        prev = s;
+      }
+      wgmma_wait<0>();
+      acc_fence(d1);
+      if (lane == 0) mbar_arrive(&ctl.empty[prev]);
+      // ---- H[row, c] = tf32(prelu(acc + b1[c])) into the warpgroup's rows, once its warps are past the previous
+      //      tile's layer 2 (the reads of those rows)
+      named_bar_sync(1 + static_cast<int>(wg), 128);
+#pragma unroll
+      for (int j = 0; j < 8; ++j) {
+        const int c = 8 * j + 2 * static_cast<int>(lane & 3u);
+        const float b0 = __ldg(g.bias1 + c), b1 = __ldg(g.bias1 + c + 1), s0 = __ldg(g.slope + c), s1 = __ldg(g.slope + c + 1);
+        const uint32_t off = static_cast<uint32_t>(c >> 5) * kPspAStage + static_cast<uint32_t>(frag_row) * 128u +
+                             ((static_cast<uint32_t>(((c & 31) >> 2) ^ (frag_row & 7))) << 4) + (c & 3) * 4u;
+        float x0 = d1[4 * j] + b0, x1 = d1[4 * j + 1] + b1, y0 = d1[4 * j + 2] + b0, y1 = d1[4 * j + 3] + b1;
+        x0 = x0 >= 0.f ? x0 : s0 * x0;
+        x1 = x1 >= 0.f ? x1 : s1 * x1;
+        y0 = y0 >= 0.f ? y0 : s0 * y0;
+        y1 = y1 >= 0.f ? y1 : s1 * y1;
+        asm volatile("st.shared.v2.f32 [%0], {%1,%2};" ::"r"(h_s + off), "f"(to_tf32(x0)), "f"(to_tf32(x1)) : "memory");
+        asm volatile("st.shared.v2.f32 [%0], {%1,%2};" ::"r"(h_s + off + 8u * 128u), "f"(to_tf32(y0)), "f"(to_tf32(y1)) : "memory");
+      }
+      fence_proxy_async_smem();   // generic-proxy stores of H -> visible to the tensor core
+      named_bar_sync(1 + static_cast<int>(wg), 128);
+      // ---- layer 2: K 0..63 in order against the resident W2
+      float d[64];
+      wgmma_fence();
+#pragma unroll
+      for (int kc = 0; kc < 2; ++kc) {
+        const uint64_t adesc = smem_desc_sw128(h_s + static_cast<uint32_t>(kc) * kPspAStage + wg * 64u * 128u);
+        const uint64_t bdesc = smem_desc_sw128(base + L.w2 + static_cast<uint32_t>(kc) * kPspN2 * 128u);
+#pragma unroll
+        for (int k4 = 0; k4 < 4; ++k4)
+          wgmma_tf32<128>(d, adesc + static_cast<uint64_t>(k4 * 2), bdesc + static_cast<uint64_t>(k4 * 2), (kc > 0 || k4 > 0) ? 1u : 0u);
+      }
+      wgmma_commit();
+      wgmma_wait<0>();
+      acc_fence(d);
+      // ---- out[r][col0 + c] = tf32(acc + b2[c]) (final has no activation): a lane quad writes one row segment
+      const long long r0 = static_cast<long long>(tile) * kPspBM + frag_row;
+      const bool on0 = r0 < g.rows, on1 = r0 + 8 < g.rows;
+      if constexpr (OUT_BF16) {
+        uint16_t *o0 = static_cast<uint16_t *>(g.out) + (r0 * g.ldo + g.col0);
+        uint16_t *o1 = o0 + 8 * static_cast<long long>(g.ldo);
+#pragma unroll
+        for (int j = 0; j < 16; ++j) {
+          const int c = 8 * j + 2 * static_cast<int>(lane & 3u);
+          const float2 bb = __ldg(reinterpret_cast<const float2 *>(g.bias2 + c));   // the launcher checks 8-byte alignment
+          if (on0) stg32(o0 + c, pack_bf16x2(d[4 * j] + bb.x, d[4 * j + 1] + bb.y));
+          if (on1) stg32(o1 + c, pack_bf16x2(d[4 * j + 2] + bb.x, d[4 * j + 3] + bb.y));
+        }
+      } else {
+        float *o0 = static_cast<float *>(g.out) + (r0 * g.ldo + g.col0);
+        float *o1 = o0 + 8 * static_cast<long long>(g.ldo);
+#pragma unroll
+        for (int j = 0; j < 16; ++j) {
+          const int c = 8 * j + 2 * static_cast<int>(lane & 3u);
+          const float2 bb = __ldg(reinterpret_cast<const float2 *>(g.bias2 + c));
+          if (on0) stg64(o0 + c, to_tf32(d[4 * j] + bb.x), to_tf32(d[4 * j + 1] + bb.y));
+          if (on1) stg64(o1 + c, to_tf32(d[4 * j + 2] + bb.x), to_tf32(d[4 * j + 3] + bb.y));
+        }
+      }
+    }
+  }
+}
+
+template <bool OUT_BF16>
+int launch_psp_tail(PspTailArgs &g, const float *w1, const float *w2, cudaStream_t st) {
+  if (g.rows <= 0) return PVN3D_OK;
+  const size_t smem = psp_tail_smem(g.stages).bytes;
+  const long long tiles = (g.rows + kPspBM - 1) / kPspBM;
+  if (tiles * kPspKc1 > 0x7fffffffll) return PVN3D_ERR_UNSUPPORTED;   // the kernel counts ring items in 32 bits
+  if (!weight_tensor_map(&g.tmap_w1, w1, 9 * kPspC, kPspC, kPspC) || !weight_tensor_map(&g.tmap_w2, w2, kPspC, kPspN2, kPspN2))
+    return PVN3D_ERR_UNSUPPORTED;
+  return launch_persistent<psp_tail_kernel<OUT_BF16>>(g, tiles, kPspThreads, smem, g.reserve_sms, st, "psp_tail_kernel");
+}
+
 // ---- factored first layer of an SA scale -------------------------------------------------------------
 // table row j = [ tf32(f_j) (C) | hi(x_j) (3) | lo(x_j) (3) | 0.. ]: x = hi + lo with hi = tf32(x), lo = tf32(x - hi),
 // so that a TF32 GEMM against [W_f | W_x | W_x] evaluates W_x . x to ~2^-21 relative (the coordinates are
@@ -3054,4 +3385,53 @@ extern "C" int pvn3d_gather_pixel_rows_bf16(const void *emb, int emb_bf16, int b
     gather_pixel_rows_bf16_kernel<float><<<grid, kGatherThreads, 0, as_stream(stream)>>>(
         static_cast<const float *>(emb), c, hw, choose, n, rows, out, ldo, col0);
   return check_launch("gather_pixel_rows_bf16_kernel");
+}
+
+// ---- the CNN tail at the sampled pixels (psp_tail_kernel) -----------------------------------------------------------
+// the argument checks and kernel arguments pvn3d_psp_tail_rows and pvn3d_psp_tail_rows_bf16 share; `align` = elements of
+// the output type per 16 bytes
+static int psp_tail_args(const float *x, int b, int h, int w, const long long *choose, int n, const pvn3d_mlp_layer_t *layer1,
+                         const pvn3d_mlp_layer_t *layer2, const float *slope, int flags, void *out, int ldo, int col0,
+                         int align, PspTailArgs &g) {
+  if (!x || !choose || !layer1 || !layer2 || !slope || !out || !layer_ptrs_ok(layer1) || !layer_ptrs_ok(layer2) || b < 0 ||
+      n < 0 || h < 2 || w < 2 || (flags & ~0xff00) || ldo % align || col0 < 0 || col0 % align ||
+      static_cast<long long>(col0) + kPspN2 > ldo || (reinterpret_cast<uintptr_t>(x) & 15u) ||
+      (reinterpret_cast<uintptr_t>(choose) & 7u) || (reinterpret_cast<uintptr_t>(out) & 15u) ||
+      (reinterpret_cast<uintptr_t>(layer2->bias) & 7u))
+    return PVN3D_ERR_INVALID_ARG;
+  g.stages = psp_tail_stages(layer1->k_pad, layer1->n_pad, layer2->k_pad, layer2->n_pad);
+  if (!g.stages) return PVN3D_ERR_UNSUPPORTED;
+  // the kernel addresses source pixels and rows with 32-bit integers, and t (h - 1) of a tap coordinate t < 2 h
+  if (h > 0x7fff || w > 0x7fff || static_cast<long long>(b) * h * w > 0x7fffffffll ||
+      static_cast<long long>(b) * n > 0x7fffffffll)
+    return PVN3D_ERR_UNSUPPORTED;
+  g.x = x; g.choose = choose; g.bias1 = layer1->bias; g.slope = slope; g.bias2 = layer2->bias;
+  g.out = out; g.rows = static_cast<long long>(b) * n;
+  g.n = n; g.h = h; g.w = w; g.ldo = ldo; g.col0 = col0;
+  g.reserve_sms = (flags >> 8) & 0xff;
+  return PVN3D_OK;
+}
+
+extern "C" int pvn3d_psp_tail_rows(const float *x, int b, int h, int w, const long long *choose, int n,
+                                   const pvn3d_mlp_layer_t *layer1, const pvn3d_mlp_layer_t *layer2, const float *slope,
+                                   int flags, float *out, int ldo, int col0, pvn3d_stream_t stream) {
+  PspTailArgs g{};
+  const int rc = psp_tail_args(x, b, h, w, choose, n, layer1, layer2, slope, flags, out, ldo, col0, 4, g);
+  if (rc != PVN3D_OK) return rc;
+  return launch_psp_tail<false>(g, layer1->w, layer2->w, as_stream(stream));
+}
+
+extern "C" int pvn3d_psp_tail_rows_bf16(const float *x, int b, int h, int w, const long long *choose, int n,
+                                        const pvn3d_mlp_layer_t *layer1, const pvn3d_mlp_layer_t *layer2,
+                                        const float *slope, int flags, pvn3d_bf16_t *out, int ldo, int col0,
+                                        pvn3d_stream_t stream) {
+  PspTailArgs g{};
+  const int rc = psp_tail_args(x, b, h, w, choose, n, layer1, layer2, slope, flags, out, ldo, col0, 8, g);
+  if (rc != PVN3D_OK) return rc;
+  return launch_psp_tail<true>(g, layer1->w, layer2->w, as_stream(stream));
+}
+
+extern "C" int pvn3d_psp_tail_supported(const pvn3d_mlp_layer_t *layer1, const pvn3d_mlp_layer_t *layer2) {
+  if (!layer1 || !layer2) return 0;
+  return psp_tail_stages(layer1->k_pad, layer1->n_pad, layer2->k_pad, layer2->n_pad) ? 1 : 0;
 }

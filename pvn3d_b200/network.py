@@ -7,22 +7,27 @@ One call, device resident, in the reference's order:
   1. model.cnn(rgb) unchanged (stock PyTorch / cuDNN);
   2. the embedding at the sampled pixels -> columns 0..127 of the DenseFusion activation table (pvn3d_gather_pixel_rows:
      no [B,128,N] int64 index, no transpose, no copy);
+     for a CNN with the reference's Modified_PSPNet layout (cnn_tail.PspTail.from_cnn) steps 1 and 2 are instead the
+     CNN up to up_2 on its own modules and ONE kernel for up_3 + final at the sampled pixels only
+     (pvn3d_psp_tail_rows): the full-resolution maps, final_seg and the dense embedding are never computed;
   3. FusedPointnet2MSG, whose last launch (FP1, pvn3d_mlp_fp_fact2_rows) writes columns 128..255 of the same table;
   4. the rest of FusedHeads on that table.
-The outputs are bit-identical to FusedHeads(gathered rgb_emb, FusedPointnet2MSG(pointcloud)).
+With the gathered embedding the outputs are bit-identical to FusedHeads(gathered rgb_emb, FusedPointnet2MSG(pointcloud)).
 
 FusedPVN3D(model, precision="bf16") runs the heads in bf16 (FusedHeads, DESIGN section 5b): the table is bfloat16, the
 gather rounds (or, for a CNN run under bf16 autocast, copies) the embedding into it without an f32 copy of the
 [B,128,H,W] map, and FP1 stores its rows rounded to bf16.  PointNet++ stays TF32; the outputs are f32 in both modes.
 
-Divergence from the reference: a `choose` index outside [0, H*W) gives that point a row of NaN (and NaN outputs)
-where torch.gather would raise.
+Divergences from the reference: a `choose` index outside [0, H*W) gives that point a row of NaN (and NaN outputs)
+where torch.gather would raise; with the sampled tail the embedding columns come from TF32 wgmma instead of cuDNN's
+TF32 convolutions (the same precision class, different low bits).
 """
 from __future__ import annotations
 
 import torch
 
 from ._lib import call, ptr
+from .cnn_tail import PspTail
 from .heads import FusedHeads
 from .mlp import FusedPointnet2MSG, check_precision
 
@@ -66,6 +71,7 @@ class FusedPVN3D:
             raise RuntimeError("FusedPVN3D: CUDA only -- no CPU fallback")
         self.precision = check_precision(precision)
         self.cnn = model.cnn
+        self.tail = PspTail.from_cnn(model.cnn, self.dev)   # None: the CNN runs whole and its embedding is gathered
         self.num_kps = int(model.num_kps)
         ap1 = getattr(model.rgbd_feat, "ap1", None)
         ks = None if ap1 is None else ap1.kernel_size
@@ -81,13 +87,16 @@ class FusedPVN3D:
         if self.num_points is not None and n != self.num_points:
             # the reference fails here too: DenseFusion's AvgPool1d(num_points) does not pool N points to one
             raise ValueError(f"FusedPVN3D: {n} points, but rgbd_feat.ap1 pools over num_points = {self.num_points}")
-        out_rgb, _ = self.cnn(rgb)
-        if out_rgb.size(0) != b or out_rgb.size(1) != 128:
-            raise ValueError(f"FusedPVN3D: the CNN embedding is {tuple(out_rgb.shape)}, expected [{b}, 128, H, W]")
         x = self.heads.new_table(b * n)
-        keep = (torch.float32, torch.bfloat16) if self.precision == "bf16" else (torch.float32,)
-        emb = out_rgb if out_rgb.dtype in keep else out_rgb.float()      # bf16: no f32 copy of a bf16 map
-        gather_pixel_rows(emb.contiguous(), choose, x, col0=FusedHeads.RGB_COL0)
+        if self.tail is not None:
+            self.tail.rows(self.tail.trunk(rgb), choose, x, col0=FusedHeads.RGB_COL0)
+        else:
+            out_rgb, _ = self.cnn(rgb)
+            if out_rgb.size(0) != b or out_rgb.size(1) != 128:
+                raise ValueError(f"FusedPVN3D: the CNN embedding is {tuple(out_rgb.shape)}, expected [{b}, 128, H, W]")
+            keep = (torch.float32, torch.bfloat16) if self.precision == "bf16" else (torch.float32,)
+            emb = out_rgb if out_rgb.dtype in keep else out_rgb.float()      # bf16: no f32 copy of a bf16 map
+            gather_pixel_rows(emb.contiguous(), choose, x, col0=FusedHeads.RGB_COL0)
         self.pointnet2(pointcloud.float().contiguous(), out_rows=x, col0=FusedHeads.CLD_COL0)
         kp, seg, ctr = self.heads.run(x, b, n)
         assert kp.size(1) == self.num_kps

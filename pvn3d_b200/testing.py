@@ -47,6 +47,58 @@ class StandInCNN(torch.nn.Module):
         return emb, self.seg(emb)
 
 
+class _StandInUp(torch.nn.Module):
+    """an up-sampling block in the layout of the reference's PSPUpsample: `.conv` = bilinear x2 (align_corners) ->
+    Conv2d 3x3 -> BatchNorm2d -> PReLU"""
+
+    def __init__(self, c_in: int, c_out: int, prelu_params: int = 1):
+        super().__init__()
+        self.conv = torch.nn.Sequential(torch.nn.Upsample(scale_factor=2, mode="bilinear", align_corners=True),
+                                        torch.nn.Conv2d(c_in, c_out, 3, padding=1), torch.nn.BatchNorm2d(c_out),
+                                        torch.nn.PReLU(prelu_params))
+
+    def forward(self, x):
+        return self.conv(x)
+
+
+class StandInPSPNet(torch.nn.Module):
+    """A small seeded CNN with the attribute names, the tail modules and the forward order of the reference's
+    Modified_PSPNet (whose construction fetches a pretrained checkpoint): a cheap 1/8-resolution `feats` and `psp`, then
+    up_1, up_2, up_3 (64 -> 64), final (64 -> 128) and final_seg.  rgb [B,3,H,W] (H, W multiples of 8) ->
+    ([B,128,H,W] embedding, [B,H,W,n_classes] log-probabilities).  BN statistics randomised, PReLU slopes non-default."""
+
+    def __init__(self, seed: int = 0, prelu_params: int = 1, n_classes: int = 22):
+        super().__init__()
+        torch.manual_seed(seed)
+        self.stem = torch.nn.Conv2d(3, 32, 8, stride=8)
+        self.psp = torch.nn.Sequential(torch.nn.Conv2d(32, 32, 1), torch.nn.ReLU())
+        self.drop_1 = torch.nn.Dropout2d(p=0.3)
+        self.up_1 = _StandInUp(32, 32)
+        self.up_2 = _StandInUp(32, 64)
+        self.up_3 = _StandInUp(64, 64, prelu_params)
+        self.drop_2 = torch.nn.Dropout2d(p=0.15)
+        self.final = torch.nn.Sequential(torch.nn.Conv2d(64, 128, 1))
+        self.final_seg = torch.nn.Sequential(torch.nn.Conv2d(64, n_classes, 1), torch.nn.LogSoftmax(dim=1))
+        randomize_bn_(self, seed + 1)
+        with torch.no_grad():
+            for m in self.modules():
+                if isinstance(m, torch.nn.PReLU):
+                    m.weight.copy_(torch.rand(m.weight.shape) * 0.4 + 0.05)
+        self.eval()
+
+    def feats(self, x):
+        f = self.stem(x)
+        return f, f.mean((2, 3))
+
+    def forward(self, x):
+        f, _ = self.feats(x)
+        p = self.drop_1(self.psp(f))
+        p = self.drop_2(self.up_1(p))
+        p = self.drop_2(self.up_2(p))
+        p = self.up_3(p)
+        return self.final(p), self.final_seg(p).permute(0, 2, 3, 1).contiguous()
+
+
 class StandInPVN3D(torch.nn.Module):
     """A module with the attributes of the reference PVN3D (cnn, pointnet2, rgbd_feat, SEG_layer, KpOF_layer,
     CtrOf_layer, num_kps) built from this package's reference-layout modules, and a module-graph forward that computes
