@@ -52,12 +52,21 @@ class MeanShiftOracle:
             if torch.max(shift) < self.stop_thresh or it > self.max_iter:   # (:42)
                 break
         self.n_iter = it
-        own = A.reshape(n, 1, c).expand(n, n, c)               # Cr rebuilt from the INPUTS (:46)
-        dis = torch.norm(pts - own, dim=2)                     # (:47)
-        num_in = torch.sum(dis < self.bandwidth, dim=1)        # (:48)
-        _, max_idx = torch.max(num_in, 0)                      # first maximal index on CPU (:49)
-        labels = dis[max_idx] < self.bandwidth                 # (:50)
+        _, max_idx, labels = density_labels(A, self.bandwidth)
         return C[max_idx, :], labels
+
+
+def density_labels(A: torch.Tensor, bandwidth: float):
+    """The exact part of fit (:46-50) on A [N,3] float32 CPU -> (num_in [N] int64, max_idx 0-dim int64,
+    labels [N] bool).  It depends on the input points alone, never on the iterations."""
+    n, c = A.shape
+    pts = A.reshape(1, n, c).expand(n, n, c)                   # Ar (:33)
+    own = A.reshape(n, 1, c).expand(n, n, c)                   # Cr rebuilt from the INPUTS (:46)
+    dis = torch.norm(pts - own, dim=2)                         # (:47)
+    num_in = torch.sum(dis < bandwidth, dim=1)                 # (:48)
+    _, max_idx = torch.max(num_in, 0)                          # first maximal index on CPU (:49)
+    labels = dis[max_idx] < bandwidth                          # (:50)
+    return num_in, max_idx, labels
 
 
 def best_fit_transform(A: np.ndarray, B: np.ndarray) -> np.ndarray:

@@ -23,7 +23,9 @@ __device__ inline void svd3_jacobi(const double h[3][3], double u[3][3], double 
           beta += a[i][q] * a[i][q];
           gamma += a[i][p] * a[i][q];
         }
-        const double lim = 1e-30 + 1e-16 * sqrt(alpha * beta);
+        // purely relative: an absolute floor would leave small columns (|a_p||a_q| below it, e.g. the second and
+        // third of a nearly collinear H at a 1e-4 m scale) unrotated, and U far from orthonormal
+        const double lim = 1e-16 * sqrt(alpha * beta);
         if (fabs(gamma) <= lim) continue;
         offd = fmax(offd, fabs(gamma) / (sqrt(alpha * beta) + 1e-300));
         const double zeta = (beta - alpha) / (2.0 * gamma);
