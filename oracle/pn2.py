@@ -58,6 +58,14 @@ def opt_n_threads(n: int) -> int:
     return int(lib().oracle_opt_n_threads(ctypes.c_int(n)))
 
 
+def sqdist(q, pts):
+    """q [nq,3], pts [n,3] -> [nq,n] f32: the squared distance of the ops below, bit for bit (oracle_sqdist)"""
+    q, qp = _f(q); pts, pp = _f(pts)
+    out = np.zeros((q.shape[0], pts.shape[0]), np.float32)
+    lib().oracle_sqdist(qp, q.shape[0], pp, pts.shape[0], out.ctypes.data_as(ctypes.c_void_p))
+    return out
+
+
 def furthest_point_sampling(xyz, m, threads=None):
     xyz, _ = _f(xyz)
     b, n, _3 = xyz.shape

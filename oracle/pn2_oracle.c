@@ -25,6 +25,16 @@ static inline float ref_sqdist(float dx, float dy, float dz) {
   return fmaf(dz, dz, fmaf(dx, dx, dy * dy));
 }
 
+/* out[i * n + k] = the squared distance every op below evaluates between q[i] and pts[k] (q - pts, the operand
+ * order of ball_query and three_nn; the square is symmetric).  Lets the tests place points within one ulp of a
+ * radius and restate single rows of an op in numpy without re-deriving the contraction. */
+void oracle_sqdist(const float *q, int nq, const float *pts, int n, float *out) {
+  for (int i = 0; i < nq; ++i)
+    for (int k = 0; k < n; ++k)
+      out[(size_t)i * n + k] = ref_sqdist(q[i * 3 + 0] - pts[k * 3 + 0], q[i * 3 + 1] - pts[k * 3 + 1],
+                                          q[i * 3 + 2] - pts[k * 3 + 2]);
+}
+
 /* cuda_utils.h:15-19 */
 int oracle_opt_n_threads(int work_size) {
   const int pow_2 = (int)(log((double)work_size) / log(2.0));

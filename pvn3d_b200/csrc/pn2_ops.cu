@@ -273,9 +273,16 @@ __global__ void __launch_bounds__(512) nn_sort_known_kernel(const float *__restr
   known += static_cast<size_t>(blockIdx.x) * m * 3;
   sorted += static_cast<size_t>(blockIdx.x) * m_pad;
   const float inf = __int_as_float(0x7f800000);
-  for (int i = threadIdx.x; i < m_pad; i += blockDim.x)
-    s_k[i] = i < m ? make_float4(__ldg(known + i * 3), __ldg(known + i * 3 + 1), __ldg(known + i * 3 + 2), __int_as_float(i))
-                   : make_float4(inf, inf, inf, __int_as_float(0x7fffffff));
+  // a NaN x orders against nothing and would leave the copy unsorted for every other point: it is keyed (and stored)
+  // as +inf.  Its distance is then inf or NaN instead of NaN -- never selected either way, as in the reference cascade
+  for (int i = threadIdx.x; i < m_pad; i += blockDim.x) {
+    float4 v = make_float4(inf, inf, inf, __int_as_float(0x7fffffff));
+    if (i < m) {
+      const float x = __ldg(known + i * 3);
+      v = make_float4(x == x ? x : inf, __ldg(known + i * 3 + 1), __ldg(known + i * 3 + 2), __int_as_float(i));
+    }
+    s_k[i] = v;
+  }
   __syncthreads();
   for (int k = 2; k <= m_pad; k <<= 1) {          // bitonic sort by (x, index)
     for (int j = k >> 1; j > 0; j >>= 1) {

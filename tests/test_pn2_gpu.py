@@ -37,7 +37,7 @@ def test_fps_ties_duplicates_and_origin_points(cuda_dev):
     rng = np.random.default_rng(3)
     ref = load_ref_ext()
     for n, m in [(512, 64), (1024, 300), (700, 128), (128, 32), (37, 20), (3000, 257), (12288, 200), (5000, 130),
-                 (6100, 90)]:          # 4097..12288 points: the thread-block-cluster kernel (3 or 6 points per thread)
+                 (6100, 90)]:          # 4097..12288 points: fps_regs_kernel through launch_regs<12> and <24> (points per thread)
         base = rng.uniform(0.2, 1.0, size=(2, max(4, n // 3), 3)).astype(np.float32)
         xyz = np.concatenate([base] * 4, 1)[:, :n].copy()          # wrap-padded duplicates => exact ties
         xyz[:, 5] = [0.01, 0.01, 0.01]                              # |p|^2 <= 1e-3: never selected
