@@ -560,6 +560,50 @@ int pvn3d_label_fill(const float *cloud, const uint8_t *valid, int hw, const flo
                      int b, int n, int *labels_out, int *nn_idx_out, void *workspace, size_t workspace_bytes,
                      pvn3d_stream_t stream);
 
+/* The network input of an RGB-D frame: the datasets' get_item (pvn3d/datasets/ycb/ycb_dataset.py:185-233,
+ * pvn3d/datasets/linemod/linemod_dataset.py:211-271) after depth_to_cloud, batched and sync-free.
+ *
+ * pvn3d_frame_sample: choose_2 and the assembly of the network's input, per frame b of cloud [B,hw,3] f32 /
+ * valid [B,hw] u8 (pvn3d_depth_to_cloud's outputs).  n_v = the number of valid pixels.
+ *   key(p) = mix(mix(seed + (b + 1) * 0x9E3779B97F4A7C15) + p) in uint64 arithmetic (wrapping), mix = the
+ *   splitmix64 finaliser z ^= z >> 30; z *= 0xBF58476D1CE4E5B9; z ^= z >> 27; z *= 0x94D049BB133111EB;
+ *   z ^= z >> 31.  The keys of one frame are distinct.
+ *   n_v > N: the N valid pixels with the smallest keys; 400 <= n_v <= N: every valid pixel, repeated
+ *   cyclically to N (np.pad 'wrap'); both in ascending pixel order within each cycle.  n_v < 400: ok = 0 and
+ *   every output row of the frame is zero.
+ * outputs: choose [B,N] i64 (pixel indices), ok [B] u8, cld_rgb_nrm rows b*N + j with row_stride (>= 6)
+ *   floats: columns 0..2 = cloud[b, choose], 3..5 = rgb[b, c, choose] as f32 (rgb [B,3,hw], u8 when
+ *   rgb_u8 = 1, else f32); pcld [B,N,3] f32 = cloud[b, choose]; labels_out [B,N] i32 =
+ *   label_image[b, choose] (label_image [B,hw] i32; labels_out NULL to skip).
+ * Workspace: pvn3d_frame_sample_workspace_bytes(b, hw, n), 256-B aligned; 0 = unsupported.
+ * B*hw < 2^31 and B*N < 2^31, else PVN3D_ERR_UNSUPPORTED (nothing launched). */
+size_t pvn3d_frame_sample_workspace_bytes(int b, int hw, int n);
+int pvn3d_frame_sample(const float *cloud, const uint8_t *valid, const void *rgb, int rgb_u8, const int *label_image,
+                       int b, int hw, int n, unsigned long long seed, float *cld_rgb_nrm, long long row_stride,
+                       float *pcld, long long *choose, int *labels_out, uint8_t *ok, void *workspace,
+                       size_t workspace_bytes, pvn3d_stream_t stream);
+/* pvn3d_knn_normals: PCL's NormalEstimation with setKSearch(50) (get_normal) at n_query query points of each
+ * frame.  Reference set of frame b: the points ref[b, i] [B,n_ref,3] f32 with ref_valid[b, i] != 0 (ref_valid
+ * NULL: all) and finite coordinates.  Query j of frame b: query[b, j] [B,n_query,3] f32.
+ *   neighbours: the 50 reference points with the smallest float64 (dx*dx + dy*dy) + dz*dz of the float32
+ *   coordinates (no FMA), lowest index first on exact ties; a query that is a reference point is its own
+ *   neighbour at distance 0.
+ *   C = (1/50) sum (p - mean)(p - mean)^T in float64 (two passes); n = the unit eigenvector of C's smallest
+ *   eigenvalue lambda0, negated when n . q > 0 (flipped towards the viewpoint at the origin); curvature =
+ *   lambda0 / trace(C).  trace(C) == 0, fewer than 50 reference points, a non-finite query or
+ *   frame_ok[b] == 0 (frame_ok NULL: every frame) give n = (0, 0, 0) and curvature 0.
+ * outputs: normals_out rows b*n_query + j with row_stride (>= 3) floats (n as f32); curv_out [B,n_query] f32,
+ *   normals64_out [B,n_query,3] f64 and nn_idx_out [B,n_query,50] i32 (reference indices by rank, -1 where
+ *   there is none) when not NULL.
+ * Each call builds a search grid of every frame's reference set into the workspace
+ * (pvn3d_knn_normals_workspace_bytes(b, n_ref, n_query), 256-B aligned; 0 = unsupported) on the stream.
+ * B*(2*n_ref + 65) < 2^31, B*n_query*32 < 2^31 and B <= 65535, else PVN3D_ERR_UNSUPPORTED (nothing launched). */
+size_t pvn3d_knn_normals_workspace_bytes(int b, int n_ref, int n_query);
+int pvn3d_knn_normals(const float *ref, const uint8_t *ref_valid, int n_ref, const float *query, int n_query, int b,
+                      const uint8_t *frame_ok, float *normals_out, long long row_stride, float *curv_out,
+                      double *normals64_out, int *nn_idx_out, void *workspace, size_t workspace_bytes,
+                      pvn3d_stream_t stream);
+
 /* ------------------------------------------------------------------------------------------
  * Callers either side of the path (SURVEY section 8 f4)
  * ---------------------------------------------------------------------------------------- */
