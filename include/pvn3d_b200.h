@@ -604,6 +604,43 @@ int pvn3d_knn_normals(const float *ref, const uint8_t *ref_valid, int n_ref, con
                       double *normals64_out, int *nn_idx_out, void *workspace, size_t workspace_bytes,
                       pvn3d_stream_t stream);
 
+/* pvn3d_depth_fill: Basic_Utils.fill_missing(dpt, cam_scale, scale_2_80m) (lib/utils/basic_utils.py:436-456), i.e.
+ * ip_basic's fill_in_multiscale with max_depth M = 3, extrapolate False and blur 'bilateral'
+ * (lib/utils/ip_basic/ip_basic/depth_map_utils_ycb.py:290-443), per frame b of depth [B,H,W] f32 (raw units, as
+ * the depth PNG holds them; finite) with cam_scale[b] ([B] f32, device) -> out [B,H,W] f32.  T = 0.01f; "under
+ * top" means row >= top[col], where top[col] is the first row with a value > T (0 when the column has none).
+ *   1  d = (depth / cam_scale) * scale_2_80m; s1 = M - d where d > T, else d.  Bins: near T < d <= 1,
+ *      med 1 < d <= 2, far d > 2.  Depth beyond 3 m makes s1 negative, which stays invalid to the end and is
+ *      returned negative (after the rescale of step 11).
+ *   2  s2 = s1, overwritten where > T by the dilation of s1*far (cross 3), then s1*med (cross 5), then s1*near
+ *      (cross 7).  3  s3 = 5x5 dilation, then 5x5 erosion.  4  s4 = 5x5 median of s3 where s3 > T.
+ *   5  top1 from s4.  6  s5 = 9x9 dilation of s4 where !(s4 > T) and under top1.  7  top2 from s5.
+ *   8  six times: s = 5x5 dilation of s where s < T (not <=) and under top2.
+ *   9  V = (s > T) & under top2, then s = 5x5 median of s at V.
+ *  10  s = cv2.bilateralFilter(s, 5, 0.5, 2.0) at V (filtering the whole image).
+ *  11  s = M - s where s > T; out = (s / scale_2_80m) * cam_scale.
+ * Dilations ignore pixels outside the image, erosions likewise; medians replicate the edge.  Every
+ * arithmetic step is one round-to-nearest float32 operation, so steps 1-9 (s4, s5, the pre-bilateral image
+ * and both top rows) are bit-exact against a float32 restatement (equal as values: -0 == +0).
+ * The bilateral is cv2's float32 algorithm: over [min, max] of the whole pre-bilateral image (zero and
+ * negative pixels included) len = (float)(max - min), scale = 4096 / len, lut[i] = (float)exp(-2 (i / scale)^2),
+ * i < 4098; max - min < FLT_EPSILON returns the image unfiltered.  The 13 taps with dy^2 + dx^2 <= 4, reflect-101
+ * border, weight w = (float)exp(-r^2 / 8) * interp(lut, |val - s| * scale), each in float32 as cv2 does, and
+ * sum(val w) / sum(w) accumulated in float32 in a fixed tap order.  Against the same weights summed in float64
+ * the result differs by at most 3 * 2^-20 * max(|min|, |max|): the sums of 13 products carry at most
+ * 13u and 12u relative error (u = 2^-24) of sum |val| w <= max|val| sum w, the quotient one more u, and the
+ * comparison's own rounding of the float64 result one more: 27u, under 48u = 3 * 2^-20, which leaves room for
+ * a one-ulp difference in a lut entry (device exp).
+ * Optional outputs: stages [B,4,H,W] f32 = s4, s5, the pre-bilateral image (after step 9) and the image after
+ * step 10; top_rows [B,2,W] i32 = top1, top2.  Either may be NULL.
+ * Workspace: pvn3d_depth_fill_workspace_bytes(b, h, w) (two [B,H,W] images and per-frame tables), 256-B aligned;
+ * 0 = unsupported.  scale_2_80m must be finite and > 0.  B*H*W < 2^31, B <= 65535 and ceil(H/8) <= 65535, else
+ * PVN3D_ERR_UNSUPPORTED; a workspace that is too small gives PVN3D_ERR_WORKSPACE (nothing launched).  15
+ * launches on the stream, no host sync. */
+size_t pvn3d_depth_fill_workspace_bytes(int b, int h, int w);
+int pvn3d_depth_fill(const float *depth, const float *cam_scale, float scale_2_80m, int b, int h, int w, float *out,
+                     float *stages, int *top_rows, void *workspace, size_t workspace_bytes, pvn3d_stream_t stream);
+
 /* ------------------------------------------------------------------------------------------
  * Callers either side of the path (SURVEY section 8 f4)
  * ---------------------------------------------------------------------------------------- */

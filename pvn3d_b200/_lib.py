@@ -126,6 +126,8 @@ _SIGNATURES = {
     "pvn3d_knn_normals_workspace_bytes": (c_size_t, [c_int, c_int, c_int]),
     "pvn3d_knn_normals": (c_int, [_P, _P, c_int, _P, c_int, c_int, _P, _P, ctypes.c_longlong, _P, _P, _P, _P, c_size_t,
                                   _P]),
+    "pvn3d_depth_fill_workspace_bytes": (c_size_t, [c_int, c_int, c_int]),
+    "pvn3d_depth_fill": (c_int, [_P, _P, c_float, c_int, c_int, c_int, _P, _P, _P, _P, c_size_t, _P]),
 }
 FLAT_MS_MAX_PTS = 4096   # PVN3D_FLAT_MS_MAX_PTS
 EXPORTED_SYMBOLS = tuple(_SIGNATURES)

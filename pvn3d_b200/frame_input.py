@@ -15,7 +15,8 @@ Deliberate differences from get_item, all documented in INTEGRATION.md section 2
     get_item's `normal[np.isnan(normal)] = 0.0` makes of PCL's NaN there;
   * a frame with fewer than 400 valid pixels is not dropped (get_item returns None) but flagged ok = 0
     and zero-filled, so the batch keeps its shape;
-  * depth is taken as given: Basic_Utils.fill_missing (YCB) is the caller's.
+  * depth is taken as given unless fill="multiscale", which runs Basic_Utils.fill_missing (YCB's
+    get_item fills every frame) on the GPU first (depth_fill.DepthFiller).
 """
 from __future__ import annotations
 
@@ -24,11 +25,13 @@ import torch
 
 from . import _lib
 from ._lib import check, ptr
+from .depth_fill import DepthFiller
 from .icp import _INT32_LIMIT, _aligned, _check_dev, _cuda_device, depth_to_cloud
 
 K_SEARCH = 50        #: neighbours per normal (the reference's ne.set_KSearch(50))
 MIN_VALID = 400      #: get_item returns None below this many valid pixels
 NORMAL_MODES = ("full", "sampled")
+FILL_MODES = (None, "multiscale")
 
 
 def _knn_normals(lib, ref, ref_valid, query, frame_ok, normals_out, row_stride, *, curv=None, normals64=None,
@@ -58,18 +61,23 @@ class FrameInputBuilder:
                points' normals are computed: the values are the same);
              "sampled": among the frame's N sampled points, wrap duplicates included, as
                linemod_dataset.py:269-270 does.
+    fill     None: build() takes depth as given; "multiscale": build() first fills it as YCB's get_item does
+             (Basic_Utils.fill_missing(dpt, cam_scale, 1), ycb_dataset.py:206) into `filled` [B,H,W] f32 and
+             back-projects that.
     debug    keep the neighbour indices [B,N,50] i32 (`nn_idx`: pixel indices in "full" mode, sample
              indices in "sampled" mode), the float64 normals [B,N,3] (`normals64`) and the curvature
              [B,N] f32 (`curvature`) of the last build().
     """
 
     def __init__(self, batch: int, n_points: int = 12288, height: int = 480, width: int = 640, *,
-                 normals: str = "full", debug: bool = False, device="cuda"):
+                 normals: str = "full", fill: str = None, debug: bool = False, device="cuda"):
         self.dev = _cuda_device(device, "FrameInputBuilder")
         self.b, self.n, self.h, self.w = int(batch), int(n_points), int(height), int(width)
         if normals not in NORMAL_MODES:
             raise ValueError(f"normals={normals!r}: one of {NORMAL_MODES}")
         self.mode = normals
+        if fill not in FILL_MODES:
+            raise ValueError(f"fill={fill!r}: one of {FILL_MODES}")
         if self.b < 1 or self.h < 1 or self.w < 1:
             raise ValueError(f"batch={batch}, height={height}, width={width}: all must be >= 1")
         if self.n < K_SEARCH:
@@ -94,6 +102,11 @@ class FrameInputBuilder:
         self.pcld = torch.empty((self.b, self.n, 3), **f32)
         self.ok = torch.empty((self.b,), dtype=torch.uint8, device=self.dev)
         self.labels = torch.empty((self.b, self.n), dtype=torch.int32, device=self.dev)
+        self.filler = self.filled = None
+        if fill == "multiscale":
+            self.filler = DepthFiller(self.b, self.h, self.w, device=self.dev)
+            #: the filled depth [B,H,W] f32 of the last build()
+            self.filled = self.filler.out
         self.nn_idx = self.normals64 = self.curvature = None
         if debug:
             self.nn_idx = torch.empty((self.b, self.n, K_SEARCH), dtype=torch.int32, device=self.dev)
@@ -102,7 +115,7 @@ class FrameInputBuilder:
 
     def build(self, depth: torch.Tensor, K: torch.Tensor, cam_scale: torch.Tensor, rgb: torch.Tensor, seed: int, *,
               label_image: torch.Tensor = None):
-        """depth [B,H,W] f32 (already filled where the dataset fills it), K [B,3,3] f32, cam_scale [B] f32, rgb
+        """depth [B,H,W] f32 (filled first when the builder was made with fill="multiscale"), K [B,3,3] f32, cam_scale [B] f32, rgb
         [B,3,H,W] uint8 or float32 (the CHW image the network takes: BGR for LineMOD, RGB for YCB), seed a
         non-negative int (the subset is a function of seed, frame index and pixel index).
 
@@ -131,6 +144,8 @@ class FrameInputBuilder:
         cloud, valid, ok = self.cloud[:b], self.valid[:b], self.ok[:b]
         cld, pcld, choose, labels = self.cld_rgb_nrm[:b], self.pcld[:b], self.choose[:b], self.labels[:b]
         with torch.cuda.device(self.dev):
+            if self.filler is not None:
+                depth = self.filler.fill(depth, cam_scale)
             depth_to_cloud(depth, K, cam_scale, out=(cloud, valid))
             rc = self.lib.pvn3d_frame_sample(
                 ptr(cloud), ptr(valid), ptr(rgb), int(rgb.dtype == torch.uint8), ptr(lab), b, hw, self.n, seed,
