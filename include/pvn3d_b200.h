@@ -67,7 +67,12 @@ int pvn3d_gather_points(const float *points, const int *idx, int b, int c, int n
  * gather_operation(xyz.transpose(1,2), idx).transpose(1,2) (pointnet2_modules.py:47-53), no transposes */
 int pvn3d_gather_xyz(const float *xyz, const int *idx, int b, int n, int m, float *out, pvn3d_stream_t stream);
 /* gather_points_grad(grad_out[B,C,M], idx[B,M], N) -> grad_points[B,C,N]  (sampling_gpu.cu:34-57);
- * grad_points is zero-filled by the callee, then scatter-added. */
+ * grad_points is zero-filled by the callee, then scatter-added.
+ * Precision of the three *_grad entry points: fp32 atomic scatter-adds, so the summation order is unspecified and
+ * results are not bit-reproducible from run to run.  Each element is within gamma_k * sum|t| of the exact sum of its
+ * k contributions t (gamma_k = k u / (1 - k u), u = 2^-24; three_interpolate_grad's t = g * w, its product rounding
+ * included); k = 0 gives +0.0 and k = 1 gives fl32(t).  Integer-valued inputs (and dyadic weights) whose partial sums
+ * stay below 2^24 are exact.  An input with no elements may be null. */
 int pvn3d_gather_points_grad(const float *grad_out, const int *idx, int b, int c, int n, int m,
                              float *grad_points, pvn3d_stream_t stream);
 
@@ -81,7 +86,8 @@ int pvn3d_ball_query(const float *new_xyz, const float *xyz, int b, int n, int m
 /* group_points(points[B,C,N], idx[B,M,S]) -> out[B,C,M,S]       (group_points_gpu.cu:8-39) */
 int pvn3d_group_points(const float *points, const int *idx, int b, int c, int n, int npoints,
                        int nsample, float *out, pvn3d_stream_t stream);
-/* group_points_grad(grad_out[B,C,M,S], idx[B,M,S], N) -> grad_points[B,C,N]  (:43-75) */
+/* group_points_grad(grad_out[B,C,M,S], idx[B,M,S], N) -> grad_points[B,C,N]  (:43-75)
+ * Zero-filled, then scatter-added; precision as gather_points_grad above. */
 int pvn3d_group_points_grad(const float *grad_out, const int *idx, int b, int c, int n,
                             int npoints, int nsample, float *grad_points, pvn3d_stream_t stream);
 
@@ -98,7 +104,8 @@ int pvn3d_three_interpolate(const float *points, const int *idx, const float *we
                             int m, int n, float *out, pvn3d_stream_t stream);
 /* three_interpolate_grad(grad_out[B,C,N], idx, weight, M) -> grad_points[B,C,M].
  * NOTE: implements the mathematically correct scatter of interpolate_gpu.cu:116-143; the
- * reference host wrapper launches the forward kernel by mistake (interpolate.cpp:89-93). */
+ * reference host wrapper launches the forward kernel by mistake (interpolate.cpp:89-93).
+ * Zero-filled, then scatter-added; precision as gather_points_grad above. */
 int pvn3d_three_interpolate_grad(const float *grad_out, const int *idx, const float *weight, int b,
                                  int c, int n, int m, float *grad_points, pvn3d_stream_t stream);
 

@@ -528,9 +528,10 @@ extern "C" int pvn3d_gather_points(const float *points, const int *idx, int b, i
 
 extern "C" int pvn3d_gather_points_grad(const float *grad_out, const int *idx, int b, int c, int n,
                                         int m, float *grad_points, pvn3d_stream_t stream) {
-  if (!grad_out || !idx || !grad_points || b < 0 || c < 0 || n <= 0 || m < 0)
-    return PVN3D_ERR_INVALID_ARG;
+  if (b < 0 || c < 0 || n <= 0 || m < 0) return PVN3D_ERR_INVALID_ARG;
   if (b == 0 || c == 0) return PVN3D_OK;
+  // an input with no elements may be null: torch hands out null data pointers for empty tensors
+  if (!grad_points || (m > 0 && (!grad_out || !idx))) return PVN3D_ERR_INVALID_ARG;
   if (b > 65535) return PVN3D_ERR_UNSUPPORTED;
   PVN3D_CUDA_TRY(cudaMemsetAsync(grad_points, 0, sizeof(float) * b * c * (size_t)n,
                                  as_stream(stream)),
@@ -579,10 +580,10 @@ extern "C" int pvn3d_group_points(const float *points, const int *idx, int b, in
 extern "C" int pvn3d_group_points_grad(const float *grad_out, const int *idx, int b, int c, int n,
                                        int npoints, int nsample, float *grad_points,
                                        pvn3d_stream_t stream) {
-  if (!grad_out || !idx || !grad_points || b < 0 || c < 0 || n <= 0 || npoints < 0 || nsample < 0)
-    return PVN3D_ERR_INVALID_ARG;
+  if (b < 0 || c < 0 || n <= 0 || npoints < 0 || nsample < 0) return PVN3D_ERR_INVALID_ARG;
   if (b == 0 || c == 0) return PVN3D_OK;
   const long long slots_ll = static_cast<long long>(npoints) * nsample;
+  if (!grad_points || (slots_ll > 0 && (!grad_out || !idx))) return PVN3D_ERR_INVALID_ARG;
   if (b > 65535 || slots_ll > 0x7fffffffll) return PVN3D_ERR_UNSUPPORTED;
   PVN3D_CUDA_TRY(cudaMemsetAsync(grad_points, 0, sizeof(float) * b * c * (size_t)n,
                                  as_stream(stream)),
@@ -649,9 +650,9 @@ extern "C" int pvn3d_three_interpolate(const float *points, const int *idx, cons
 extern "C" int pvn3d_three_interpolate_grad(const float *grad_out, const int *idx,
                                             const float *weight, int b, int c, int n, int m,
                                             float *grad_points, pvn3d_stream_t stream) {
-  if (!grad_out || !idx || !weight || !grad_points || b < 0 || c < 0 || m <= 0 || n < 0)
-    return PVN3D_ERR_INVALID_ARG;
+  if (b < 0 || c < 0 || m <= 0 || n < 0) return PVN3D_ERR_INVALID_ARG;
   if (b == 0 || c == 0) return PVN3D_OK;
+  if (!grad_points || (n > 0 && (!grad_out || !idx || !weight))) return PVN3D_ERR_INVALID_ARG;
   if (b > 65535) return PVN3D_ERR_UNSUPPORTED;
   PVN3D_CUDA_TRY(cudaMemsetAsync(grad_points, 0, sizeof(float) * b * c * (size_t)m,
                                  as_stream(stream)),
