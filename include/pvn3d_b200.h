@@ -668,6 +668,34 @@ int pvn3d_pose_add_adds(const float *pred_rt, const float *gt_rt, int n_poses, c
                         int n_points, float *add, float *adds, void *workspace, size_t workspace_bytes,
                         pvn3d_stream_t stream);
 
+/* ADD and ADD-S of every ground-truth object of a batch in one call: TorchEval's eval_metric (YCB) and
+ * eval_metric_lm (LineMOD), pvn3d_eval_utils.py:113-137,204-220, over the pose table of pvn3d_frame_poses_batch /
+ * pvn3d_icp_refine_batch.
+ *   poses [b,n_cls,3,4] f32, present [b,n_cls] u8       predicted pose and presence of each class
+ *   gt_rt [b,slots,3,4] f32, cls_ids [b,slots] i32      ground-truth pose and class of each slot
+ *   meshes [mesh_off[n_cls],3] f32                      object-frame points of every class, class c at rows
+ *                                                        mesh_off[c] .. mesh_off[c+1]-1
+ *   mesh_off [n_cls+1] i32, HOST memory                  read at call time: it sizes the grid and travels to the
+ *                                                        kernels by value (a captured graph keeps those values)
+ *   absent  PVN3D_ADD_ABSENT_ZEROS: a class with present == 0 is scored with the zero pose (YCB,
+ *           pvn3d_eval_utils.py:123-124); PVN3D_ADD_ABSENT_IDENTITY: with [I | 0] (LineMOD's empty mask, :172-173)
+ *   add, adds [b,slots] f32 (either may be NULL).  Slot (f, i) is scored when cls_ids[f, 0..i] holds no 0 (the
+ *           `break` at :118-119) and cls_ids[f, i] lies in [1, n_cls); every other slot is written as NaN.
+ * The arithmetic per slot is pvn3d_pose_add_adds's (same kernels): with n_cls = 2, one mesh at class 1, all ids 1 and
+ * all present, the outputs equal pvn3d_pose_add_adds's bit for bit.  No host sync; the grid depends only on b, slots
+ * and the largest mesh, so the call can be captured in a CUDA graph.
+ * Refused before any launch: mesh_off[0] != 0, a class c >= 1 without points, n_cls < 2 or an unknown `absent`
+ * (PVN3D_ERR_INVALID_ARG); n_cls > PVN3D_ADD_MAX_CLASSES, b*slots > 65535 or mesh_off[n_cls] > (2^31-1)/3
+ * (PVN3D_ERR_UNSUPPORTED).  Workspace: pvn3d_frame_add_adds_workspace_bytes(b, slots, largest mesh of classes >= 1),
+ * 8-byte aligned. */
+#define PVN3D_ADD_ABSENT_ZEROS 0
+#define PVN3D_ADD_ABSENT_IDENTITY 1
+#define PVN3D_ADD_MAX_CLASSES 64
+size_t pvn3d_frame_add_adds_workspace_bytes(int b, int slots, int max_points);
+int pvn3d_frame_add_adds(const float *poses, const uint8_t *present, int n_cls, const float *gt_rt, const int *cls_ids,
+                         int b, int slots, const float *meshes, const int *mesh_off, int absent, float *add,
+                         float *adds, void *workspace, size_t workspace_bytes, pvn3d_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif

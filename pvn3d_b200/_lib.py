@@ -100,6 +100,8 @@ _SIGNATURES = {
     "pvn3d_seg_argmax": (c_int, [_P, ctypes.c_longlong, c_int, _P, _P]),
     "pvn3d_pose_add_adds_workspace_bytes": (c_size_t, [c_int, c_int]),
     "pvn3d_pose_add_adds": (c_int, [_P, _P, c_int, _P, c_int, _P, _P, _P, c_size_t, _P]),
+    "pvn3d_frame_add_adds_workspace_bytes": (c_size_t, [c_int, c_int, c_int]),
+    "pvn3d_frame_add_adds": (c_int, [_P, _P, c_int, _P, _P, c_int, c_int, _P, _P, c_int, _P, _P, _P, c_size_t, _P]),
     "pvn3d_meanshift_workspace_bytes": (c_size_t, [c_int, c_int, c_int]),
     "pvn3d_meanshift_workspace_counts_offset": (c_size_t, [c_int, c_int, c_int]),
     "pvn3d_meanshift_fit_batch": (c_int, [_P, _P, _P, c_int, c_int, c_double, c_int, c_uint, _P, _P, _P, _P, _P, c_size_t, _P]),

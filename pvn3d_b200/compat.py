@@ -16,7 +16,11 @@ What install() does (SURVEY section 8b, App. D):
   4. with patch_model=True, rebinds `lib.pvn3d.PVN3D.forward` (patch_pvn3d_forward): in eval mode, without
      autograd and on CUDA inputs the network runs on FusedPVN3D (pvn3d_b200.network), with bf16 heads inside a
      torch.autocast("cuda", dtype=torch.bfloat16) region and TF32 ones otherwise; anything else -- training,
-     train_*.py, grad-enabled or CPU calls -- runs the reference's own forward.
+     train_*.py, grad-enabled or CPU calls -- runs the reference's own forward;
+  5. with patch_eval=True, rebinds `TorchEval.eval_pose_parallel` (patch_eval_pose_parallel): the poses of the whole
+     batch in one FramePoseSolver.solve, every ground-truth object scored in one pvn3d_frame_add_adds launch, one
+     device -> host read, and the distance lists appended exactly as eval_metric / eval_metric_lm would -- the
+     reference's cal_auc / cal_lm_add then run unchanged.
 Nothing here copies or edits reference files.
 """
 from __future__ import annotations
@@ -75,7 +79,8 @@ def install_import_shims() -> None:
     _stub("pcl")
 
 
-def install(reference_root: str | None = None, patch_post: bool = False, patch_model: bool = False) -> None:
+def install(reference_root: str | None = None, patch_post: bool = False, patch_model: bool = False,
+            patch_eval: bool = False) -> None:
     from . import _ext
 
     install_import_shims()
@@ -86,6 +91,13 @@ def install(reference_root: str | None = None, patch_post: bool = False, patch_m
         patch_post_modules(import_missing=True)
     if patch_model:
         patch_pvn3d_forward(importlib.import_module("lib.pvn3d").PVN3D)
+    if patch_eval:
+        ev = importlib.import_module("lib.utils.pvn3d_eval_utils")
+        patch_eval_pose_parallel(ev.TorchEval)
+        for name in ("train.train_ycb_pvn3d", "train.train_linemod_pvn3d"):
+            mod = sys.modules.get(name)
+            if mod is not None and getattr(mod, "TorchEval", None) is not None:
+                patch_eval_pose_parallel(mod.TorchEval)
 
 
 def _weights(model):
@@ -170,3 +182,80 @@ def patch_post_modules(import_missing: bool = False) -> None:
             continue
         for k, v in attrs.items():
             setattr(mod, k, v)
+
+
+def _batch_evaluator(ref, ds_type: str, obj_id: int, device):
+    """the PoseEvaluator of one dataset (and LineMOD object) on `device`, cached in the reference module.  Meshes come
+    from the reference's own bs_utils.get_pointxyz_cuda, once per class: LineMOD's loader draws a random 2000-point
+    subset and caches it, so this evaluator and the reference's eval_metric_lm score the same points."""
+    from .eval_utils import PoseEvaluator
+
+    cache = ref.__dict__.setdefault("_pvn3d_b200_evaluators", {})
+    key = (ds_type, obj_id if ds_type != "ycb" else None, str(device))
+    ev = cache.get(key)
+    if ev is None:
+        if ds_type == "ycb":
+            meshes = {c: ref.bs_utils.get_pointxyz_cuda(ref.cls_lst[c - 1]) for c in range(1, len(ref.cls_lst) + 1)}
+            ev = PoseEvaluator(meshes, ref.config.ycb_sym_cls_ids, absent="zeros", device=device)
+        else:
+            mesh = ref.bs_utils_lm.get_pointxyz_cuda(obj_id, ds_type="linemod")
+            ev = PoseEvaluator({1: mesh}, [], absent="identity", device=device)
+        cache[key] = ev
+    return ev
+
+
+def patch_eval_pose_parallel(cls) -> None:
+    """Rebind cls.eval_pose_parallel (the reference's TorchEval, pvn3d_eval_utils.py:345-387) to a batched form with
+    the same arguments and the same effect on self.cls_add_dis / self.cls_adds_dis: cal_frame_poses(_lm) for every
+    frame in one FramePoseSolver.solve (ds_type, use_ctr_clus_flter and obj_id as there), eval_metric(_lm) for every
+    ground-truth object in one pvn3d_frame_add_adds launch, one device -> host read.  Idempotent."""
+    if getattr(cls.eval_pose_parallel, "_pvn3d_b200_orig", None) is not None:
+        return
+    orig = cls.eval_pose_parallel
+    ref = sys.modules[cls.__module__]
+
+    def eval_pose_parallel(self, pclds, rgbs, masks, pred_ctr_ofs, gt_ctr_ofs, labels, cnt, cls_ids, RTs, pred_kp_ofs,
+                           min_cnt=20, merge_clus=False, bbox=False, ds="YCB", cls_type=None, use_p2d=False,
+                           vote_type=None, use_ctr_clus_flter=True, use_ctr=True, ds_type="ycb", obj_id=0):
+        import torch
+
+        from . import eval_utils
+
+        if not use_ctr:
+            raise NotImplementedError("use_ctr=False is never exercised by the reference callers")
+        bs, n_kps, n_pts, _ = pred_kp_ofs.size()
+        dev = pred_kp_ofs.device
+        pcld = pclds.reshape(bs, n_pts, 3).float().contiguous()
+        ctr = pred_ctr_ofs.reshape(bs, -1, n_pts, 3)[:, 0].float().contiguous()
+        kp = pred_kp_ofs.float().contiguous()
+        ycb = ds_type == "ycb"
+        masks = masks.reshape(bs, n_pts)
+        if ycb:
+            m32 = masks.to(torch.int32).contiguous()
+            s = eval_utils._solver("ycb", n_pts, n_kps, self.n_cls, bool(use_ctr_clus_flter), dev, batch=bs)
+            gt, ids = RTs, cls_ids.reshape(bs, -1)
+        else:
+            m32 = (masks == 1).to(torch.int32).contiguous()      # cls_msk = mask == 1 (:171)
+            s = eval_utils._solver("lm", n_pts, n_kps, max(self.n_cls, 2), bool(use_ctr_clus_flter), dev,
+                                   obj_id=obj_id, batch=bs)     # the solver cal_frame_poses_lm uses, batched
+            gt, ids = RTs[:, :1], torch.ones((bs, 1), dtype=torch.int32, device=dev)   # RTs[0] only (:211)
+        ev = _batch_evaluator(ref, ds_type if ycb else "linemod", obj_id, dev)
+        with s.lock:
+            poses, present, _, _ = s.solve(pcld, m32, ctr, kp)
+            if not ycb:
+                poses, present = poses[:, :2], present[:, :2]          # class 1 only
+            ev.reset()
+            ev.add_batch(poses, present, gt, ids)
+            add, adds = ev.distances()
+        if ycb:
+            for c in range(len(self.cls_add_dis)):
+                self.cls_add_dis[c] += add[c] if c < len(add) else []
+                self.cls_adds_dis[c] += adds[c] if c < len(adds) else []
+        else:
+            for dst, src in ((self.cls_add_dis, add), (self.cls_adds_dis, adds)):
+                dst[obj_id] += src[1]
+                dst[0] += src[0]
+
+    eval_pose_parallel._pvn3d_b200_orig = orig
+    eval_pose_parallel.__doc__ = orig.__doc__
+    cls.eval_pose_parallel = eval_pose_parallel
