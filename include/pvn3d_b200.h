@@ -96,6 +96,27 @@ int pvn3d_group_points_grad(const float *grad_out, const int *idx, int b, int c,
  * (first index wins ties); unused slots when m < 3 hold +inf / 0. */
 int pvn3d_three_nn(const float *unknown, const float *known, int b, int n, int m, float *dist2,
                    int *idx, pvn3d_stream_t stream);
+/* three_nn and the inverse-distance weights of pvn3d_three_nn_weights for nlev <= 4 levels of one batch in one call:
+ * level l is unknown[l][B,n[l],3] against known[l][B,m[l],3] -> dist2[l], idx[l] (as pvn3d_three_nn) and weight[l]
+ * [B,n[l],3] (as pvn3d_three_nn_weights), bit for bit.  The levels pvn3d_three_nn_grid_supported takes are searched on
+ * per-frame cell grids of their known points: one launch builds every grid, one searches every level and writes the
+ * weights.  Other levels run pvn3d_three_nn and pvn3d_three_nn_weights.  The pointer arrays are host memory; no host
+ * sync, scratch from the stream-ordered pool. */
+int pvn3d_three_nn_grid_supported(int n, int m);
+int pvn3d_three_nn_weights_levels(int nlev, const float *const *unknown, const float *const *known, const int *n,
+                                  const int *m, int b, float *const *dist2, int *const *idx, float *const *weight,
+                                  pvn3d_stream_t stream);
+/* ball query of both radii of nlev <= 4 MSG levels of one batch in one call: level l searches xyz[l][B,n[l],3] around
+ * new_xyz[l][B,m[l],3] -> idx0[l][B,m[l],ns0[l]] (radius0[l]) and idx1[l][B,m[l],ns1[l]] (radius1[l]), the same values
+ * as pvn3d_query_and_group2 (first ns in index order, padded with the first hit, zeros for an empty ball).  The levels
+ * pvn3d_ball_grid_supported takes are binned into per-frame cell grids no finer than the larger radius (one launch
+ * for every grid) and searched a warp per centre (one launch); a centre with more hits than the warp buffers scans the
+ * whole cloud in index order.  Other levels run pvn3d_query_and_group2.  The arrays are host memory; no host sync,
+ * scratch from the stream-ordered pool. */
+int pvn3d_ball_grid_supported(int n, int m, int ns0, int ns1);
+int pvn3d_ball_query2_levels(int nlev, const float *const *xyz, const float *const *new_xyz, const int *n, const int *m,
+                             int b, const float *radius0, const int *ns0, int *const *idx0, const float *radius1,
+                             const int *ns1, int *const *idx1, pvn3d_stream_t stream);
 
 /* three_interpolate(points[B,C,M], idx[B,N,3], weight[B,N,3]) -> out[B,C,N]
  * (interpolate_gpu.cu:72-111); p1*w1 + p2*w2 + p3*w3 contracted as the reference SASS does

@@ -166,6 +166,65 @@ def three_nn(unknowns: torch.Tensor, knows: torch.Tensor):
     return [dist2, idx]
 
 
+def three_nn_weights_levels(unknowns, knowns):
+    """three_nn and the inverse-distance weights of up to four levels of one batch in one call
+    (pvn3d_three_nn_weights_levels): unknowns[l] [B,n_l,3], knowns[l] [B,m_l,3] -> [(dist2, idx, weight)] per level,
+    the same bits as three_nn followed by pvn3d_three_nn_weights."""
+    import ctypes
+    nlev = len(unknowns)
+    if nlev != len(knowns) or nlev > 4:
+        raise ValueError("three_nn_weights_levels: at most four (unknown, known) pairs")
+    for t in (*unknowns, *knowns):
+        _chk_contig(t, "xyz")
+        _chk_float(t, "xyz")
+        _need_cuda(t)
+    if nlev == 0:
+        return []
+    b = unknowns[0].size(0)
+    if any(t.size(0) != b or t.dim() != 3 or t.size(2) != 3 for t in (*unknowns, *knowns)):
+        raise ValueError("three_nn_weights_levels: every cloud must be [B,*,3] with the same B")
+    dev = unknowns[0].device
+    outs = [(torch.empty((b, u.size(1), 3), dtype=torch.float32, device=dev),
+             torch.empty((b, u.size(1), 3), dtype=torch.int32, device=dev),
+             torch.empty((b, u.size(1), 3), dtype=torch.float32, device=dev)) for u in unknowns]
+    arr = lambda xs: (ctypes.c_void_p * nlev)(*[x.data_ptr() for x in xs])       # noqa: E731
+    ints = lambda xs: (ctypes.c_int * nlev)(*xs)                                  # noqa: E731
+    call("pvn3d_three_nn_weights_levels", dev, nlev, arr(unknowns), arr(knowns), ints([u.size(1) for u in unknowns]),
+         ints([k.size(1) for k in knowns]), b, arr([o[0] for o in outs]), arr([o[1] for o in outs]),
+         arr([o[2] for o in outs]))
+    return outs
+
+
+def ball_query2_levels(centres, clouds, radii, nsamples):
+    """ball_query2 of up to four MSG levels of one batch in one call (pvn3d_ball_query2_levels): centres[l] [B,m_l,3]
+    searched in clouds[l] [B,n_l,3] with radii[l] = (r0, r1), nsamples[l] = (ns0, ns1) -> [(idx0, idx1)] per level,
+    the same values as ball_query2."""
+    import ctypes
+    nlev = len(centres)
+    if not (nlev == len(clouds) == len(radii) == len(nsamples)) or nlev > 4:
+        raise ValueError("ball_query2_levels: at most four levels, one radius and nsample pair each")
+    for x in (*centres, *clouds):
+        _chk_contig(x, "xyz")
+        _chk_float(x, "xyz")
+        _need_cuda(x)
+    if nlev == 0:
+        return []
+    b = centres[0].size(0)
+    if any(x.size(0) != b or x.dim() != 3 or x.size(2) != 3 for x in (*centres, *clouds)):
+        raise ValueError("ball_query2_levels: every cloud must be [B,*,3] with the same B")
+    dev = centres[0].device
+    outs = [tuple(torch.empty((b, c.size(1), int(ns)), dtype=torch.int32, device=dev) for ns in nss)
+            for c, nss in zip(centres, nsamples)]
+    arr = lambda xs: (ctypes.c_void_p * nlev)(*[x.data_ptr() for x in xs])       # noqa: E731
+    ints = lambda xs: (ctypes.c_int * nlev)(*[int(x) for x in xs])                # noqa: E731
+    flts = lambda xs: (ctypes.c_float * nlev)(*[float(x) for x in xs])            # noqa: E731
+    call("pvn3d_ball_query2_levels", dev, nlev, arr(clouds), arr(centres), ints([x.size(1) for x in clouds]),
+         ints([c.size(1) for c in centres]), b, flts([r[0] for r in radii]), ints([s[0] for s in nsamples]),
+         arr([o[0] for o in outs]), flts([r[1] for r in radii]), ints([s[1] for s in nsamples]),
+         arr([o[1] for o in outs]))
+    return outs
+
+
 def three_interpolate(points: torch.Tensor, idx: torch.Tensor, weight: torch.Tensor) -> torch.Tensor:
     """interpolate.cpp:42-70 -- points [B,C,M], idx/weight [B,N,3] -> [B,C,N]"""
     _chk_contig(points, "points")

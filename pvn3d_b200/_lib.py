@@ -57,6 +57,10 @@ _SIGNATURES = {
     "pvn3d_group_points": (c_int, [_P, _P, c_int, c_int, c_int, c_int, c_int, _P, _P]),
     "pvn3d_group_points_grad": (c_int, [_P, _P, c_int, c_int, c_int, c_int, c_int, _P, _P]),
     "pvn3d_three_nn": (c_int, [_P, _P, c_int, c_int, c_int, _P, _P, _P]),
+    "pvn3d_three_nn_grid_supported": (c_int, [c_int, c_int]),
+    "pvn3d_three_nn_weights_levels": (c_int, [c_int, _P, _P, _P, _P, c_int, _P, _P, _P, _P]),
+    "pvn3d_ball_grid_supported": (c_int, [c_int, c_int, c_int, c_int]),
+    "pvn3d_ball_query2_levels": (c_int, [c_int, _P, _P, _P, _P, c_int, _P, _P, _P, _P, _P, _P, _P]),
     "pvn3d_three_interpolate": (c_int, [_P, _P, _P, c_int, c_int, c_int, c_int, _P, _P]),
     "pvn3d_three_interpolate_grad": (c_int, [_P, _P, _P, c_int, c_int, c_int, c_int, _P, _P]),
     "pvn3d_transpose_cn_to_nc": (c_int, [_P, c_int, c_int, c_int, _P, _P]),

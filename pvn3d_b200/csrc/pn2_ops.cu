@@ -362,6 +362,410 @@ three_nn_slab_kernel(const float *__restrict__ unknown, const float4 *__restrict
   o[0] = best.d1 < inf ? best.i1 : 0; o[1] = best.d2 < inf ? best.i2 : 0; o[2] = best.d3 < inf ? best.i3 : 0;
 }
 
+// dist = sqrt(dist2) (pointnet2_utils.py:126); 1/(dist+1e-8); normalise (modules.py:184-186) -- the IEEE operations of
+// nn_weights_kernel (mlp_tc.cu), so both give the same bits
+__device__ __forceinline__ void nn_inverse_distance_weights(float d1, float d2, float d3, float &w1, float &w2,
+                                                            float &w3) {
+  const float r1 = __fdiv_rn(1.0f, __fadd_rn(__fsqrt_rn(d1), 1e-8f));
+  const float r2 = __fdiv_rn(1.0f, __fadd_rn(__fsqrt_rn(d2), 1e-8f));
+  const float r3 = __fdiv_rn(1.0f, __fadd_rn(__fsqrt_rn(d3), 1e-8f));
+  const float norm = __fadd_rn(__fadd_rn(r1, r2), r3);
+  w1 = __fdiv_rn(r1, norm);
+  w2 = __fdiv_rn(r2, norm);
+  w3 = __fdiv_rn(r3, norm);
+}
+
+// ------------------------------------------------------------------------------------------------
+// three_nn + weights on per-frame cell grids (pvn3d_three_nn_weights_levels).
+// The known set of every (level, frame) is counting-sorted into a uniform grid over its finite bounding box; a query
+// visits the cells in rings of growing Chebyshev distance around its own cell and stops once every unvisited cell lies
+// farther than its third-best distance.  The result is the reference cascade's by the same argument as the x-sorted
+// walk: the three smallest (d2, k) pairs in lexicographic order, d2 by ref_sqdist, in any visiting order.
+//   * Non-finite known points are left out of the grid: their d2 is NaN or inf, which never passes the cascade's
+//     strict '<' against the 1e40 seed.
+//   * The stop test is conservative.  A point binned into cell c lies within [lo + c h, lo + (c+1) h] up to the
+//     rounding of (x - lo) * inv (below 1e-5 h at 64 cells per axis); `tol` covers that and the rounding of the face
+//     coordinate lo + k h, and the factor (1 - 1e-5) the rounding of d2 itself.  Equality with d3 keeps searching.
+//   * Cells are sized for ~kNnGridPts points per cell on a surface (depth clouds are surfaces; a volume cloud gets
+//     smaller cells, which costs rings, not results), at most kNnGridAxis per axis and kNnGridCells in all: a far
+//     outlier makes the cells coarse, never wrong.
+// ------------------------------------------------------------------------------------------------
+constexpr int kNnGridMaxLevels = 4;
+constexpr int kNnGridMaxM = 8192;     // known points per frame the grid path takes
+constexpr int kNnGridCells = 8192;    // cells per grid at most (the counting sort's table: 32 KB of shared memory)
+constexpr int kNnGridAxis = 64;       // cells per axis at most
+constexpr float kNnGridPts = 2.f;     // points per cell aimed at
+constexpr int kNnGridBuildThreads = 512;
+
+struct NnGridHdr {
+  float lo[3];
+  float h, inv, tol;
+  int g[3];
+  int pad;
+};
+struct NnGridLevel {
+  const float *unknown, *known;
+  float *dist2, *weight;
+  int *idx;
+  int n, m;
+  int blk0;            // first blockIdx.x of this level in the search launch
+  float hmin;          // smallest cell side (a ball query's larger radius; 0 for 3-NN)
+  float4 *sorted;      // [B][m]: (x, y, z, index bits), grouped by cell
+  int *cell_start;     // [B][kNnGridCells + 1]
+  NnGridHdr *hdr;      // [B]
+};
+struct NnGridArgs {
+  NnGridLevel lv[kNnGridMaxLevels];
+  int nlev;
+};
+
+__device__ __forceinline__ bool finite3(float x, float y, float z) {
+  return fabsf(x) <= 3.402823466e38f && fabsf(y) <= 3.402823466e38f && fabsf(z) <= 3.402823466e38f;
+}
+__device__ __forceinline__ int nn_cell_axis(const NnGridHdr &g, int d, float v) {
+  const float c = floorf(__fmul_rn(__fsub_rn(v, g.lo[d]), g.inv));
+  return static_cast<int>(fminf(fmaxf(c, 0.f), static_cast<float>(g.g[d] - 1)));   // NaN -> 0 (never queried so)
+}
+__device__ __forceinline__ int nn_cell_of(const NnGridHdr &g, float x, float y, float z) {
+  return (nn_cell_axis(g, 2, z) * g.g[1] + nn_cell_axis(g, 1, y)) * g.g[0] + nn_cell_axis(g, 0, x);
+}
+
+// grid (B, levels): one CTA builds the grid of one frame of one level
+__global__ void __launch_bounds__(kNnGridBuildThreads) nn_grid_build_kernel(NnGridArgs a) {
+  __shared__ int s_cnt[kNnGridCells + 1];
+  __shared__ float s_red[6][kNnGridBuildThreads / 32];
+  __shared__ int s_wsum[kNnGridBuildThreads / 32];
+  __shared__ NnGridHdr s_g;
+  const NnGridLevel &L = a.lv[blockIdx.y];
+  const int b = blockIdx.x, t = threadIdx.x, m = L.m;
+  const unsigned lane = lane_id(), warp = t >> 5;
+  const float *known = L.known + static_cast<size_t>(b) * m * 3;
+  float lo[3] = {3.0e38f, 3.0e38f, 3.0e38f}, hi[3] = {-3.0e38f, -3.0e38f, -3.0e38f};
+  for (int i = t; i < m; i += kNnGridBuildThreads) {
+    const float x = __ldg(known + i * 3), y = __ldg(known + i * 3 + 1), z = __ldg(known + i * 3 + 2);
+    if (finite3(x, y, z)) {
+      lo[0] = fminf(lo[0], x); lo[1] = fminf(lo[1], y); lo[2] = fminf(lo[2], z);
+      hi[0] = fmaxf(hi[0], x); hi[1] = fmaxf(hi[1], y); hi[2] = fmaxf(hi[2], z);
+    }
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) {
+#pragma unroll
+    for (int d = 0; d < 3; ++d) {
+      lo[d] = fminf(lo[d], __shfl_xor_sync(0xffffffffu, lo[d], o));
+      hi[d] = fmaxf(hi[d], __shfl_xor_sync(0xffffffffu, hi[d], o));
+    }
+  }
+  if (lane == 0)
+    for (int d = 0; d < 3; ++d) { s_red[d][warp] = lo[d]; s_red[3 + d][warp] = hi[d]; }
+  for (int c = t; c <= kNnGridCells; c += kNnGridBuildThreads) s_cnt[c] = 0;
+  __syncthreads();
+  if (t == 0) {
+    NnGridHdr g;
+    float e[3];
+    bool any = true;
+    for (int d = 0; d < 3; ++d) {
+      float l = s_red[d][0], h = s_red[3 + d][0];
+      for (int w = 1; w < kNnGridBuildThreads / 32; ++w) { l = fminf(l, s_red[d][w]); h = fmaxf(h, s_red[3 + d][w]); }
+      any = any && l <= h;
+      g.lo[d] = l;
+      e[d] = h - l;   // may round up; the binning clamps
+    }
+    if (!any) {       // no finite point: one empty cell
+      for (int d = 0; d < 3; ++d) { g.lo[d] = 0.f; e[d] = 0.f; }
+    }
+    // the two largest extents span the surface
+    const float e1 = fmaxf(e[0], fmaxf(e[1], e[2]));
+    const float e3 = fminf(e[0], fminf(e[1], e[2]));
+    const float e2 = e[0] + e[1] + e[2] - e1 - e3;
+    const float per = kNnGridPts / static_cast<float>(m);
+    float h = sqrtf(e1 * e2 * per);
+    if (!(h > 0.f)) h = e1 * per;
+    h = fmaxf(h, L.hmin);
+    h = fmaxf(h, e1 / static_cast<float>(kNnGridAxis - 1));   // no axis needs more than kNnGridAxis cells
+    if (!(h > 0.f)) h = 1.f;   // all finite points coincide
+    if (!(e1 < 3.0e38f) || !(h < 3.0e38f)) {   // the extent itself overflows: one cell, every point binned into it
+      g.g[0] = g.g[1] = g.g[2] = 1;
+      h = 1.f;
+      g.inv = 0.f;
+    } else {
+      for (;;) {
+        int cells = 1;
+        for (int d = 0; d < 3; ++d) {
+          g.g[d] = static_cast<int>(fminf(floorf(e[d] / h), static_cast<float>(kNnGridAxis - 1))) + 1;
+          cells *= g.g[d];
+        }
+        if (cells <= kNnGridCells) break;
+        h *= 1.25f;
+      }
+      g.inv = 1.f / h;
+    }
+    g.h = h;
+    float mag = 0.f;
+    for (int d = 0; d < 3; ++d) mag = fmaxf(mag, fmaxf(fabsf(g.lo[d]), fabsf(g.lo[d] + g.g[d] * h)));
+    g.tol = 1e-4f * h + 4e-6f * mag;
+    g.pad = 0;
+    s_g = g;
+    L.hdr[b] = g;
+  }
+  __syncthreads();
+  const NnGridHdr g = s_g;
+  const int ncell = g.g[0] * g.g[1] * g.g[2];
+  for (int i = t; i < m; i += kNnGridBuildThreads) {
+    const float x = __ldg(known + i * 3), y = __ldg(known + i * 3 + 1), z = __ldg(known + i * 3 + 2);
+    if (finite3(x, y, z)) atomicAdd(&s_cnt[nn_cell_of(g, x, y, z)], 1);
+  }
+  __syncthreads();
+  // exclusive scan of the ncell + 1 counts: thread t owns the run [t*per_t, (t+1)*per_t)
+  constexpr int per_t = (kNnGridCells + kNnGridBuildThreads) / kNnGridBuildThreads;   // 17: covers kNnGridCells + 1
+  int run = 0;
+  const int c0 = t * per_t;
+  for (int c = c0; c < c0 + per_t && c <= ncell; ++c) run += s_cnt[c];
+  int incl = run;
+#pragma unroll
+  for (int o = 1; o < 32; o <<= 1) {
+    const int v = __shfl_up_sync(0xffffffffu, incl, o);
+    if (static_cast<int>(lane) >= o) incl += v;
+  }
+  if (lane == 31) s_wsum[warp] = incl;
+  __syncthreads();
+  int acc = incl - run;
+  for (int w = 0; w < static_cast<int>(warp); ++w) acc += s_wsum[w];
+  int *starts = L.cell_start + static_cast<size_t>(b) * (kNnGridCells + 1);
+  for (int c = c0; c < c0 + per_t && c <= ncell; ++c) {
+    const int v = s_cnt[c];
+    s_cnt[c] = acc;
+    starts[c] = acc;
+    acc += v;
+  }
+  __syncthreads();
+  float4 *sorted = L.sorted + static_cast<size_t>(b) * m;
+  for (int i = t; i < m; i += kNnGridBuildThreads) {
+    const float x = __ldg(known + i * 3), y = __ldg(known + i * 3 + 1), z = __ldg(known + i * 3 + 2);
+    if (finite3(x, y, z)) sorted[atomicAdd(&s_cnt[nn_cell_of(g, x, y, z)], 1)] = make_float4(x, y, z, __int_as_float(i));
+  }
+}
+
+// grid (sum over levels of ceil(n / kNnThreads), B): one thread per query point
+__global__ void __launch_bounds__(kNnThreads) three_nn_grid_kernel(NnGridArgs a) {
+  int l = 0;
+  while (l + 1 < a.nlev && static_cast<int>(blockIdx.x) >= a.lv[l + 1].blk0) ++l;
+  const NnGridLevel &L = a.lv[l];
+  const int b = blockIdx.y;
+  const int j = (blockIdx.x - L.blk0) * kNnThreads + threadIdx.x;
+  if (j >= L.n) return;
+  const float *u = L.unknown + (static_cast<size_t>(b) * L.n + j) * 3;
+  const float ux = u[0], uy = u[1], uz = u[2];
+  const NnGridHdr g = L.hdr[b];
+  const float4 *__restrict__ pts = L.sorted + static_cast<size_t>(b) * L.m;
+  const int *__restrict__ start = L.cell_start + static_cast<size_t>(b) * (kNnGridCells + 1);
+  const float inf = __int_as_float(0x7f800000);
+  Best3 best;
+  best3_init(best);
+  best.i1 = best.i2 = best.i3 = 0x7fffffff;   // so that any real pair precedes an empty slot; restored to 0 at the end
+  if (finite3(ux, uy, uz)) {   // a non-finite query has d2 NaN or inf to every point: nothing passes
+    const int cx = nn_cell_axis(g, 0, ux), cy = nn_cell_axis(g, 1, uy), cz = nn_cell_axis(g, 2, uz);
+    const float q[3] = {ux, uy, uz};
+    const int cq[3] = {cx, cy, cz};
+    for (int r = 0;; ++r) {
+      const int y0 = max(cy - r, 0), y1 = min(cy + r, g.g[1] - 1);
+      const int z0 = max(cz - r, 0), z1 = min(cz + r, g.g[2] - 1);
+      const int x0 = max(cx - r, 0), x1 = min(cx + r, g.g[0] - 1);
+      for (int z = z0; z <= z1; ++z) {
+        for (int y = y0; y <= y1; ++y) {
+          const int row = (z * g.g[1] + y) * g.g[0];
+          auto visit = [&](int c_first, int c_last) {   // the points of cells c_first..c_last of this row: one run
+            const int p1 = start[row + c_last + 1];
+            for (int p = start[row + c_first]; p < p1; ++p) {
+              const float4 k = pts[p];
+              best3_push_lex(best, ref_sqdist(ux - k.x, uy - k.y, uz - k.z), __float_as_int(k.w));
+            }
+          };
+          if (abs(z - cz) == r || abs(y - cy) == r) {   // the whole x-run of the row is on ring r
+            visit(x0, x1);
+          } else {                                       // an inner row: its two end cells
+            if (cx - r >= 0) visit(cx - r, cx - r);
+            if (cx + r < g.g[0]) visit(cx + r, cx + r);
+          }
+        }
+      }
+      // every cell within Chebyshev distance r is done; the rest lies beyond the nearest face of that box that has
+      // cells behind it
+      float gap = inf;
+#pragma unroll
+      for (int d = 0; d < 3; ++d) {
+        if (cq[d] - r > 0) gap = fminf(gap, q[d] - (g.lo[d] + static_cast<float>(cq[d] - r) * g.h));
+        if (cq[d] + r < g.g[d] - 1) gap = fminf(gap, (g.lo[d] + static_cast<float>(cq[d] + r + 1) * g.h) - q[d]);
+      }
+      if (gap == inf) break;   // the box covers the grid
+      gap -= g.tol;
+      if (gap > 0.f && gap * gap * (1.f - 1e-5f) > best.d3) break;
+    }
+  }
+  const size_t o = (static_cast<size_t>(b) * L.n + j) * 3;
+  L.dist2[o] = best.d1; L.dist2[o + 1] = best.d2; L.dist2[o + 2] = best.d3;
+  L.idx[o] = best.d1 < inf ? best.i1 : 0;
+  L.idx[o + 1] = best.d2 < inf ? best.i2 : 0;
+  L.idx[o + 2] = best.d3 < inf ? best.i3 : 0;
+  float w1, w2, w3;
+  nn_inverse_distance_weights(best.d1, best.d2, best.d3, w1, w2, w3);
+  L.weight[o] = w1; L.weight[o + 1] = w2; L.weight[o + 2] = w3;
+}
+
+// ------------------------------------------------------------------------------------------------
+// ball query of both radii of an MSG level on per-frame cell grids (pvn3d_ball_query2_levels).
+// The searched cloud of every (level, frame) is binned by nn_grid_build_kernel with cells at least as wide as the larger
+// radius.  A warp per centre visits the cells that can hold a hit, tests every point with ref_sqdist and the strict
+// '<' of both radii, and collects all hits in a per-warp buffer.  Each point sits in exactly one cell, so ranking the
+// buffered hits by index gives the reference's "first ns in index order" for any visiting order.
+//   * Reach: a hit has fl(dx*dx) <= d2 < r2 (monotone rounding), so |c - p| < r (1 + 2^-22) on every axis; the range
+//     c -/+ R with R = 1.001 r + 1e-6 |c| contains it after rounding, and the binning is monotone in the coordinate,
+//     so every hit's cell lies in [cell(c - R), cell(c + R)] -- clamped and misrounded binning included.
+//   * Non-finite points are not binned: their d2 is NaN or inf and never passes '<'.  A non-finite centre has no hit.
+//   * A centre with more than kBgCap hits runs the index-order scan of the whole cloud instead (ball_scan_kernel
+//     without its boxes), so the buffer never decides a result.
+// ------------------------------------------------------------------------------------------------
+constexpr int kBgWarps = 8;
+constexpr int kBgCap = 512;          // buffered hits per centre
+constexpr int kBgMaxNs = 256;        // nsample of either radius the grid path takes
+
+struct BallGridLevel {
+  const float *xyz, *centres;        // searched cloud [B][n][3], centres [B][m][3]
+  int n, m;
+  float r0, r1;
+  int ns0, ns1;
+  int *idx0, *idx1;                  // [B][m][ns0], [B][m][ns1]
+  int blk0;                          // first blockIdx.x of this level
+};
+struct BallGridArgs {
+  BallGridLevel lv[kNnGridMaxLevels];
+  float4 *sorted[kNnGridMaxLevels];
+  int *cell_start[kNnGridMaxLevels];
+  NnGridHdr *hdr[kNnGridMaxLevels];
+  int nlev;
+};
+
+__global__ void __launch_bounds__(kBgWarps * 32) ball_grid_kernel(BallGridArgs a) {
+  __shared__ int s_hit[kBgWarps][kBgCap];
+  int l = 0;
+  while (l + 1 < a.nlev && static_cast<int>(blockIdx.x) >= a.lv[l + 1].blk0) ++l;
+  const BallGridLevel &L = a.lv[l];
+  const int b = blockIdx.y;
+  const unsigned lane = lane_id(), warp = threadIdx.x >> 5;
+  const int j = (blockIdx.x - L.blk0) * kBgWarps + static_cast<int>(warp);
+  if (j >= L.m) return;   // warp-uniform; no CTA barrier below
+  const float *cp = L.centres + (static_cast<size_t>(b) * L.m + j) * 3;
+  const float cx = cp[0], cy = cp[1], cz = cp[2];
+  const float r2a = __fmul_rn(L.r0, L.r0), r2b = __fmul_rn(L.r1, L.r1);   // ball_query_gpu.cu:22
+  int *hits = s_hit[warp];
+  int cnt = 0;
+  if (finite3(cx, cy, cz)) {
+    const NnGridHdr g = a.hdr[l][b];
+    const float4 *__restrict__ pts = a.sorted[l] + static_cast<size_t>(b) * L.n;
+    const int *__restrict__ start = a.cell_start[l] + static_cast<size_t>(b) * (kNnGridCells + 1);
+    const float r = fmaxf(L.r0, L.r1);
+    const float c[3] = {cx, cy, cz};
+    int lo[3], hi[3];
+#pragma unroll
+    for (int d = 0; d < 3; ++d) {
+      const float reach = r * 1.001f + 1e-6f * fabsf(c[d]) + 1e-30f;
+      lo[d] = nn_cell_axis(g, d, c[d] - reach);
+      hi[d] = nn_cell_axis(g, d, c[d] + reach);
+    }
+    for (int z = lo[2]; z <= hi[2]; ++z)
+      for (int y = lo[1]; y <= hi[1]; ++y) {
+        const int row = (z * g.g[1] + y) * g.g[0];
+        const int p1 = start[row + hi[0] + 1];
+        for (int p0 = start[row + lo[0]]; p0 < p1; p0 += 32) {
+          const int p = p0 + static_cast<int>(lane);
+          bool ha = false, hb = false;
+          int k = 0;
+          if (p < p1) {
+            const float4 q = pts[p];
+            const float d2 = ref_sqdist(cx - q.x, cy - q.y, cz - q.z);
+            ha = d2 < r2a;
+            hb = d2 < r2b;
+            k = __float_as_int(q.w);
+          }
+          const unsigned any = __ballot_sync(0xffffffffu, ha || hb);
+          if ((ha || hb)) {
+            const int slot = cnt + __popc(any & lanemask_lt());
+            if (slot < kBgCap) hits[slot] = k | (ha ? 0x40000000 : 0) | (hb ? static_cast<int>(0x80000000u) : 0);
+          }
+          cnt += __popc(any);
+        }
+      }
+  }
+  const size_t cent = static_cast<size_t>(b) * L.m + j;
+  int *out_a = L.idx0 + cent * L.ns0, *out_b = L.idx1 + cent * L.ns1;
+  if (cnt > kBgCap) {
+    // the index-order scan: hits appended in ascending k, the first ns of each radius kept
+    const float *cloud = L.xyz + static_cast<size_t>(b) * L.n * 3;
+    int ca = 0, cb = 0, fa = 0, fb = 0;
+    for (int off = 0; off < L.n && (ca < L.ns0 || cb < L.ns1); off += 32) {
+      const int k = off + static_cast<int>(lane);
+      bool ha = false, hb = false;
+      if (k < L.n) {
+        const float *q = cloud + static_cast<size_t>(k) * 3;
+        const float d2 = ref_sqdist(cx - __ldg(q), cy - __ldg(q + 1), cz - __ldg(q + 2));
+        ha = d2 < r2a;
+        hb = d2 < r2b;
+      }
+      const unsigned ma = __ballot_sync(0xffffffffu, ha), mb = __ballot_sync(0xffffffffu, hb);
+      if (ma) {
+        if (ca == 0) fa = off + __ffs(ma) - 1;
+        const int slot = ca + __popc(ma & lanemask_lt());
+        if (ha && slot < L.ns0) out_a[slot] = k;
+        ca += __popc(ma);
+      }
+      if (mb) {
+        if (cb == 0) fb = off + __ffs(mb) - 1;
+        const int slot = cb + __popc(mb & lanemask_lt());
+        if (hb && slot < L.ns1) out_b[slot] = k;
+        cb += __popc(mb);
+      }
+    }
+    for (int s = static_cast<int>(lane) + min(ca, L.ns0); s < L.ns0; s += 32) out_a[s] = fa;
+    for (int s = static_cast<int>(lane) + min(cb, L.ns1); s < L.ns1; s += 32) out_b[s] = fb;
+    return;
+  }
+  __syncwarp();
+  // rank every buffered hit among the hits of its radius: rank < ns -> slot rank; rank 0 is the first hit
+  int ca = 0, cb = 0, fa = 0x7fffffff, fb = 0x7fffffff;
+  for (int i = static_cast<int>(lane); i < cnt; i += 32) {
+    const int h = hits[i], k = h & 0x3fffffff;
+    const bool ia = (h & 0x40000000) != 0, ib = h < 0;
+    int ra = 0, rb = 0;
+    for (int e = 0; e < cnt; ++e) {
+      const int o = hits[e], ko = o & 0x3fffffff;
+      ra += (ko < k && (o & 0x40000000)) ? 1 : 0;
+      rb += (ko < k && o < 0) ? 1 : 0;
+    }
+    if (ia) {
+      ++ca;
+      fa = min(fa, k);
+      if (ra < L.ns0) out_a[ra] = k;
+    }
+    if (ib) {
+      ++cb;
+      fb = min(fb, k);
+      if (rb < L.ns1) out_b[rb] = k;
+    }
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) {
+    ca += __shfl_xor_sync(0xffffffffu, ca, o);
+    cb += __shfl_xor_sync(0xffffffffu, cb, o);
+    fa = min(fa, __shfl_xor_sync(0xffffffffu, fa, o));
+    fb = min(fb, __shfl_xor_sync(0xffffffffu, fb, o));
+  }
+  // pad: slots >= cnt hold the first hit; an empty ball is zeros (torch::zeros, ball_query.cpp:19-21)
+  if (ca == 0) fa = 0;
+  if (cb == 0) fb = 0;
+  for (int s = static_cast<int>(lane) + min(ca, L.ns0); s < L.ns0; s += 32) out_a[s] = fa;
+  for (int s = static_cast<int>(lane) + min(cb, L.ns1); s < L.ns1; s += 32) out_b[s] = fb;
+}
+
 // ------------------------------------------------------------------------------------------------
 // three_interpolate: out[b,c,j] = sum_t points[b,c,idx[b,j,t]] * w[b,j,t]   (interpolate_gpu.cu:72-101)
 // contraction as in the reference SASS (oracle/_ref build, interpolate_gpu.o):
@@ -446,14 +850,8 @@ three_nn_interp_kernel(const float *__restrict__ unknown, const float *__restric
   Best3 best;
   three_nn_scan(known + static_cast<size_t>(b) * m * 3, m, s_known, u[0], u[1], u[2], best);
   {
-    // dist = sqrt(dist2) (pointnet2_utils.py:126); 1/(dist+1e-8); normalise (modules.py:184-186)
-    const float r1 = __fdiv_rn(1.0f, __fadd_rn(__fsqrt_rn(best.d1), 1e-8f));
-    const float r2 = __fdiv_rn(1.0f, __fadd_rn(__fsqrt_rn(best.d2), 1e-8f));
-    const float r3 = __fdiv_rn(1.0f, __fadd_rn(__fsqrt_rn(best.d3), 1e-8f));
-    const float norm = __fadd_rn(__fadd_rn(r1, r2), r3);
-    s_w[threadIdx.x][0] = __fdiv_rn(r1, norm);
-    s_w[threadIdx.x][1] = __fdiv_rn(r2, norm);
-    s_w[threadIdx.x][2] = __fdiv_rn(r3, norm);
+    nn_inverse_distance_weights(best.d1, best.d2, best.d3, s_w[threadIdx.x][0], s_w[threadIdx.x][1],
+                                s_w[threadIdx.x][2]);
     s_i[threadIdx.x][0] = best.i1;
     s_i[threadIdx.x][1] = best.i2;
     s_i[threadIdx.x][2] = best.i3;
@@ -632,6 +1030,132 @@ extern "C" int pvn3d_three_nn(const float *unknown, const float *known, int b, i
   }
   three_nn_kernel<<<grid, kNnThreads, 0, as_stream(stream)>>>(unknown, known, n, m, dist2, idx);
   return check_launch("three_nn_kernel");
+}
+
+extern "C" int pvn3d_three_nn_grid_supported(int n, int m) { return n >= 1 && m >= 1 && m <= kNnGridMaxM; }
+
+extern "C" int pvn3d_three_nn_weights_levels(int nlev, const float *const *unknown, const float *const *known,
+                                             const int *n, const int *m, int b, float *const *dist2, int *const *idx,
+                                             float *const *weight, pvn3d_stream_t stream) {
+  if (nlev < 0 || nlev > kNnGridMaxLevels || b < 0 || (nlev > 0 && (!unknown || !known || !n || !m || !dist2 || !idx ||
+                                                                     !weight)))
+    return PVN3D_ERR_INVALID_ARG;
+  for (int l = 0; l < nlev; ++l)
+    if (!unknown[l] || !known[l] || !dist2[l] || !idx[l] || !weight[l] || n[l] < 0 || m[l] < 0)
+      return PVN3D_ERR_INVALID_ARG;
+  if (b == 0) return PVN3D_OK;
+  if (b > 65535) return PVN3D_ERR_UNSUPPORTED;
+  cudaStream_t st = as_stream(stream);
+  // levels outside the grid's shape rule: today's 3-NN, then the weights
+  NnGridArgs a{};
+  size_t bytes = 0;
+  long long blocks = 0;
+  for (int l = 0; l < nlev; ++l) {
+    if (!pvn3d_three_nn_grid_supported(n[l], m[l])) {
+      int rc = pvn3d_three_nn(unknown[l], known[l], b, n[l], m[l], dist2[l], idx[l], stream);
+      if (rc == PVN3D_OK) rc = pvn3d_three_nn_weights(dist2[l], static_cast<long long>(b) * n[l], weight[l], stream);
+      if (rc != PVN3D_OK) return rc;
+      continue;
+    }
+    NnGridLevel &L = a.lv[a.nlev++];
+    L.unknown = unknown[l]; L.known = known[l]; L.dist2 = dist2[l]; L.idx = idx[l]; L.weight = weight[l];
+    L.n = n[l]; L.m = m[l];
+    L.blk0 = static_cast<int>(blocks);
+    blocks += ceil_div(n[l], kNnThreads);
+    bytes += align_up(sizeof(float4) * b * m[l], 256) + align_up(sizeof(int) * b * (kNnGridCells + 1), 256) +
+             align_up(sizeof(NnGridHdr) * b, 256);
+  }
+  if (a.nlev == 0) return PVN3D_OK;
+  if (blocks > 0x7fffffffll) return PVN3D_ERR_UNSUPPORTED;
+  int rc = keep_async_pool_warm();
+  if (rc != PVN3D_OK) return rc;
+  unsigned char *scratch = nullptr;
+  PVN3D_CUDA_TRY(cudaMallocAsync(&scratch, bytes, st), "three_nn grid scratch");
+  unsigned char *p = scratch;
+  for (int l = 0; l < a.nlev; ++l) {
+    NnGridLevel &L = a.lv[l];
+    L.sorted = reinterpret_cast<float4 *>(p);
+    p += align_up(sizeof(float4) * b * L.m, 256);
+    L.cell_start = reinterpret_cast<int *>(p);
+    p += align_up(sizeof(int) * b * (kNnGridCells + 1), 256);
+    L.hdr = reinterpret_cast<NnGridHdr *>(p);
+    p += align_up(sizeof(NnGridHdr) * b, 256);
+  }
+  nn_grid_build_kernel<<<dim3(b, a.nlev), kNnGridBuildThreads, 0, st>>>(a);
+  rc = check_launch("nn_grid_build_kernel");
+  if (rc == PVN3D_OK) {
+    three_nn_grid_kernel<<<dim3(static_cast<unsigned>(blocks), b), kNnThreads, 0, st>>>(a);
+    rc = check_launch("three_nn_grid_kernel");
+  }
+  cudaFreeAsync(scratch, st);
+  return rc;
+}
+
+extern "C" int pvn3d_ball_grid_supported(int n, int m, int ns0, int ns1) {
+  return n >= 1 && n < (1 << 30) && m >= 1 && ns0 >= 1 && ns1 >= 1 && ns0 <= kBgMaxNs && ns1 <= kBgMaxNs;
+}
+
+extern "C" int pvn3d_ball_query2_levels(int nlev, const float *const *xyz, const float *const *new_xyz, const int *n,
+                                        const int *m, int b, const float *radius0, const int *ns0, int *const *idx0,
+                                        const float *radius1, const int *ns1, int *const *idx1,
+                                        pvn3d_stream_t stream) {
+  if (nlev < 0 || nlev > kNnGridMaxLevels || b < 0 ||
+      (nlev > 0 && (!xyz || !new_xyz || !n || !m || !radius0 || !ns0 || !idx0 || !radius1 || !ns1 || !idx1)))
+    return PVN3D_ERR_INVALID_ARG;
+  for (int l = 0; l < nlev; ++l)
+    if (!xyz[l] || !new_xyz[l] || !idx0[l] || !idx1[l] || n[l] <= 0 || m[l] < 0 || ns0[l] <= 0 || ns1[l] <= 0)
+      return PVN3D_ERR_INVALID_ARG;
+  if (b == 0) return PVN3D_OK;
+  if (b > 65535) return PVN3D_ERR_UNSUPPORTED;
+  cudaStream_t st = as_stream(stream);
+  NnGridArgs grids{};
+  BallGridArgs a{};
+  size_t bytes = 0;
+  long long blocks = 0;
+  for (int l = 0; l < nlev; ++l) {
+    if (m[l] == 0) continue;
+    if (!pvn3d_ball_grid_supported(n[l], m[l], ns0[l], ns1[l])) {   // levels outside the rule: today's scan
+      const int rc = pvn3d_query_and_group2(xyz[l], new_xyz[l], nullptr, 0, b, n[l], m[l], 0, radius0[l], ns0[l],
+                                            idx0[l], nullptr, radius1[l], ns1[l], idx1[l], nullptr, stream);
+      if (rc != PVN3D_OK) return rc;
+      continue;
+    }
+    NnGridLevel &G = grids.lv[grids.nlev++];
+    G.known = xyz[l];
+    G.m = n[l];
+    G.hmin = fmaxf(radius0[l], radius1[l]);
+    BallGridLevel &L = a.lv[a.nlev++];
+    L.xyz = xyz[l]; L.centres = new_xyz[l]; L.n = n[l]; L.m = m[l];
+    L.r0 = radius0[l]; L.r1 = radius1[l]; L.ns0 = ns0[l]; L.ns1 = ns1[l]; L.idx0 = idx0[l]; L.idx1 = idx1[l];
+    L.blk0 = static_cast<int>(blocks);
+    blocks += ceil_div(m[l], kBgWarps);
+    bytes += align_up(sizeof(float4) * b * (size_t)n[l], 256) + align_up(sizeof(int) * b * (kNnGridCells + 1), 256) +
+             align_up(sizeof(NnGridHdr) * b, 256);
+  }
+  if (a.nlev == 0) return PVN3D_OK;
+  if (blocks > 0x7fffffffll) return PVN3D_ERR_UNSUPPORTED;
+  int rc = keep_async_pool_warm();
+  if (rc != PVN3D_OK) return rc;
+  unsigned char *scratch = nullptr;
+  PVN3D_CUDA_TRY(cudaMallocAsync(&scratch, bytes, st), "ball grid scratch");
+  unsigned char *p = scratch;
+  for (int l = 0; l < grids.nlev; ++l) {
+    NnGridLevel &G = grids.lv[l];
+    a.sorted[l] = G.sorted = reinterpret_cast<float4 *>(p);
+    p += align_up(sizeof(float4) * b * (size_t)G.m, 256);
+    a.cell_start[l] = G.cell_start = reinterpret_cast<int *>(p);
+    p += align_up(sizeof(int) * b * (kNnGridCells + 1), 256);
+    a.hdr[l] = G.hdr = reinterpret_cast<NnGridHdr *>(p);
+    p += align_up(sizeof(NnGridHdr) * b, 256);
+  }
+  nn_grid_build_kernel<<<dim3(b, grids.nlev), kNnGridBuildThreads, 0, st>>>(grids);
+  rc = check_launch("nn_grid_build_kernel");
+  if (rc == PVN3D_OK) {
+    ball_grid_kernel<<<dim3(static_cast<unsigned>(blocks), b), kBgWarps * 32, 0, st>>>(a);
+    rc = check_launch("ball_grid_kernel");
+  }
+  cudaFreeAsync(scratch, st);
+  return rc;
 }
 
 extern "C" int pvn3d_three_interpolate(const float *points, const int *idx, const float *weight,

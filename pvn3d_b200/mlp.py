@@ -10,7 +10,7 @@ matrix + bias, and runs `Pointnet2MSG.forward` (reference pvn3d/lib/pvn3d.py:126
                  and 3 on relu(U[idx] - V) with ReLU + max-pool over nsample in ONE launch
                  (pvn3d_mlp_sa_fact2 for SA1 / SA2, pvn3d_mlp_sa_fact2w for SA3 / SA4), written straight
                  into the level's point-major feature table
-  per FP level : three_nn -> inverse-distance weights ->
+  per FP level : three_nn + inverse-distance weights (all four levels in two launches, on cell grids) ->
                  FP2-4: both layers in ONE launch (pvn3d_mlp_fp2): three_interpolate + concat fused into the
                         tensor-core operand producer, the layer-1 activations kept in shared memory
                  FP1  : factored first layer, P = W1k . known once per known point (pvn3d_mlp_dense) ->
@@ -410,13 +410,14 @@ class FusedPointnet2MSG:
     def queries(self, plan: "GeoPlan") -> "GeoPlan":
         """The wide coordinate-only kernels: ball queries of both radii of every SA level and the 3-NN indices +
         inverse-distance weights of every FP level (pointnet2_modules.py:57-60,183-186).  They fill the machine,
-        so they run on the stream of the MLPs (0.9 ms per 32-frame batch)."""
-        for li, (npoint, radii, nsamples, _) in enumerate(SA_SPEC):
-            plan.ball.append(_ext.ball_query2(plan.l_xyz[li + 1], plan.l_xyz[li], radii, nsamples))   # both radii, one pass
+        so they run on the stream of the MLPs."""
+        # both radii of all four SA levels: two launches
+        plan.ball = _ext.ball_query2_levels(plan.l_xyz[1:], plan.l_xyz[:4], [r for _, r, _, _ in SA_SPEC],
+                                            [ns for _, _, ns, _ in SA_SPEC])
         self._m("ball")
-        for i in range(3, -1, -1):
-            d2, nn_idx = _ext.three_nn(plan.l_xyz[i], plan.l_xyz[i + 1])
-            plan.nn[i] = (nn_idx, three_nn_weights(d2))
+        nn = _ext.three_nn_weights_levels(plan.l_xyz[:4], plan.l_xyz[1:])   # all four FP levels: two launches
+        for i, (_, nn_idx, w) in enumerate(nn):
+            plan.nn[i] = (nn_idx, w)
         self._m("three_nn")
         return plan
 
