@@ -6,6 +6,7 @@ import numpy as np
 import pytest
 
 import normals_ref as nr
+from frame_input_cases import tie_cloud
 from oracle import depth_icp_oracle as dio
 from pvn3d_b200 import _lib, synth
 
@@ -61,19 +62,9 @@ def test_sampling_rule(nv):
 
 
 # ---- the neighbour sets ------------------------------------------------------------------------------------------
-def _tie_cloud(seed, n=600):
-    """dyadic lattice points (exact ties at equal distances), duplicates, and a few random points"""
-    rng = np.random.default_rng(seed)
-    lat = rng.integers(-6, 7, size=(n // 2, 3)).astype(np.float32) / np.float32(8)
-    dup = lat[rng.integers(0, len(lat), size=n // 4)]
-    rnd = rng.normal(size=(n - len(lat) - len(dup), 3)).astype(np.float32)
-    pts = np.concatenate([lat, dup, rnd])
-    return pts[rng.permutation(len(pts))]
-
-
 @pytest.mark.parametrize("seed", range(3))
 def test_knn_matches_brute_force_with_ties_and_duplicates(seed):
-    pts = _tie_cloud(seed)
+    pts = tie_cloud(seed)
     got = nr.knn(pts, pts)
     want = nr.knn_brute(pts, pts)
     assert np.array_equal(got, want)
@@ -86,7 +77,7 @@ def test_knn_matches_brute_force_with_ties_and_duplicates(seed):
 
 
 def test_knn_respects_validity_and_non_finite_points():
-    pts = _tie_cloud(5)
+    pts = tie_cloud(5)
     valid = np.random.default_rng(1).random(len(pts)) < 0.7
     pts[3] = np.nan
     q = pts[:40].copy()
