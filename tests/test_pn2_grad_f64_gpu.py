@@ -24,6 +24,7 @@ import pytest
 import torch
 
 import grad_ref as gr
+from pn2_forward_ref import DISCRETE as _DISCRETE, recorder as _recorder, twin as _twin
 from helpers import SA_LEVELS, load_reference_python
 from pvn3d_b200 import _ext, _lib, pointnet2, synth, testing
 
@@ -404,52 +405,6 @@ def test_mutants_rejected_on_gpu_cases(cuda_dev, plan, mutant):
 
 
 # ---- the network's parameter gradients ------------------------------------------------------------------------------
-_DISCRETE = ("furthest_point_sample", "ball_query", "three_nn")
-
-
-def _t_gather(features, idx):
-    b, c = features.shape[:2]
-    return features.gather(2, idx.long()[:, None].expand(b, c, idx.size(1)))
-
-
-def _t_group(features, idx):
-    b, c = features.shape[:2]
-    return features.gather(2, idx.long().reshape(b, 1, -1).expand(b, c, -1)).reshape(b, c, *idx.shape[1:])
-
-
-def _t_interp(features, idx, weight):
-    return (_t_group(features, idx) * weight[:, None]).sum(-1)
-
-
-def _recorder(log):
-    orig = {k: getattr(pointnet2, k) for k in _DISCRETE}
-
-    def wrap(name):
-        def fn(*a):
-            out = orig[name](*a)
-            log[name].append(out)
-            return out
-        return fn
-    return {k: wrap(k) for k in _DISCRETE}
-
-
-def _twin(log, f64):
-    its = {k: iter(v) for k, v in log.items()}
-
-    def nn(unknown, known):
-        dist, idx = next(its["three_nn"])
-        if f64:                                          # the same neighbours, their float64 distances
-            b, n = idx.shape[:2]
-            k = known.detach().gather(1, idx.long().reshape(b, -1, 1).expand(b, n * 3, 3)).reshape(b, n, 3, 3)
-            dist = (unknown.detach()[:, :, None] - k).square().sum(-1).sqrt()
-        return dist, idx
-
-    return {"furthest_point_sample": lambda xyz, npoint: next(its["furthest_point_sample"]),
-            "ball_query": lambda radius, nsample, xyz, new_xyz: next(its["ball_query"]),
-            "three_nn": nn, "gather_operation": _t_gather, "grouping_operation": _t_group,
-            "three_interpolate": _t_interp}
-
-
 def _arm(model, pc, r, ops, monkeypatch):
     with monkeypatch.context() as mp:
         for k, fn in ops.items():
