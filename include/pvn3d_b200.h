@@ -717,6 +717,75 @@ int pvn3d_frame_add_adds(const float *poses, const uint8_t *present, int n_cls, 
                          int b, int slots, const float *meshes, const int *mesh_off, int absent, float *add,
                          float *adds, void *workspace, size_t workspace_bytes, pvn3d_stream_t stream);
 
+/* ------------------------------------------------------------------------------------------
+ * Training: get_item's regression targets and model_fn's losses (csrc/train.cu)
+ * ---------------------------------------------------------------------------------------- */
+
+/* The offset targets of get_item (ycb_dataset.py:241-278, linemod_dataset.py:275-310) for a batch of sampled clouds.
+ *   pcld [b,n,3] f32, labels [b,n] i32        the sampled points and their labels
+ *   cls_ids [b,s] i32                          class of each meta slot in meta order, 0 = empty slot
+ *   rts [b,s,3,4] f64                          the meta pose of each slot
+ *   kp_table [n_cls,k,3] f32, ctr_table [n_cls,3] f32   object-frame keypoints / centre of each class id
+ * ->kp_targ [b,n,k,3], ctr_targ [b,n,3], kp3ds [b,s,k,3], ctr3ds [b,s,3] f32 (every element written).
+ * kp = kp_f32 . r^T + t and ctr likewise in float64 (numpy promotes to the pose's dtype); an offset is
+ * float32(float64(p) - kp).  A point takes the offsets of the LAST slot whose id equals its label (the reference loop
+ * overwrites); a point whose label is in no slot gets zeros.  A slot id outside [1, n_cls) is an empty slot (zero
+ * kp3ds / ctr3ds, the tables are never read); a label outside [0, n_cls) matches no slot.  LineMOD is s = 2 with
+ * cls_ids = [1, 0].  Refused: b > 65535, n_cls > 4096 or s*(k+1)*24 + 4*n_cls + 1024 > 48 KB (PVN3D_ERR_UNSUPPORTED).
+ * One launch, no host sync. */
+int pvn3d_train_targets(const float *pcld, const int *labels, const int *cls_ids, const double *rts, int b, int n,
+                        int s, const float *kp_table, const float *ctr_table, int n_cls, int k, float *kp_targ,
+                        float *ctr_targ, float *kp3ds, float *ctr3ds, pvn3d_stream_t stream);
+
+/* model_fn's losses (train_ycb_pvn3d.py:172-184, lib/loss.py): any subset of
+ *   focal  FocalLoss(gamma) of seg against seg_target: logpt = log_softmax(z)[t], pt = exp(logpt) DETACHED,
+ *          row loss -(1-pt)^gamma logpt, mean over the rows (seg_mean = 1) or sum (0).  A target outside
+ *          [0, n_cls) makes its row's loss and gradient NaN.  seg is [rows, n_cls] (seg_inner = 1) or
+ *          [rows / inner, n_cls, inner] (the N,C,H,W input FocalLoss reshapes, inner = H*W).
+ *   kp     OFLoss of kp_pred [b,n_kp,n,3] against kp_targ [b,n,n_kp,3] with w = labels[b,n] > 0:
+ *          kp_loss[b,k] = sum_{n,c} w |pred - targ| / (sum_n w + 1e-3), float32 as lib/loss.py
+ *   ctr    the same for ctr_pred [b,n_ctr,n,3] / ctr_targ [b,n,n_ctr,3]
+ * loss = w_seg focal + w_kp sum(kp_loss) + w_ctr sum(ctr_loss); parts = (focal, sum(kp_loss), sum(ctr_loss));
+ * acc = #(first argmax of the row == target) / M.  ok [b] u8 (or NULL; needs seg with rows = b*n) leaves the rows
+ * of frames with ok = 0 out of the focal mean and the accuracy: M = n * #ok, and with no ok frame focal = acc = 0.
+ * A NULL pointer turns a term off.  Sums are per-block partials combined in a fixed order: no atomics, the same bits
+ * on every call.  Limits: n_cls <= 128, n_kp, n_ctr <= 48 (PVN3D_ERR_UNSUPPORTED). */
+typedef struct pvn3d_loss_args {
+  const float *seg;            /* logits, or NULL: no focal term                                    */
+  const long long *seg_target; /* [rows] i64                                                         */
+  long long seg_rows;
+  int n_cls;
+  int seg_inner;
+  float gamma;                 /* >= 0                                                               */
+  int seg_mean;
+  const float *kp_pred, *kp_targ;   /* or NULL */
+  int n_kp;
+  const float *ctr_pred, *ctr_targ; /* or NULL */
+  int n_ctr;
+  const long long *labels;     /* [b,n] i64: the OF weights                                          */
+  int b, n;
+  const uint8_t *ok;           /* [b] or NULL                                                        */
+  float w_seg, w_kp, w_ctr;
+} pvn3d_loss_args_t;
+
+/* workspace of a forward / backward pair (the backward reads what the forward kept there); 0 = invalid arguments.
+ * The workspace must be 256-byte aligned. */
+size_t pvn3d_train_loss_workspace_bytes(const pvn3d_loss_args_t *args);
+/* loss [1], parts [3], kp_loss [b,n_kp], ctr_loss [b,n_ctr], acc [1]: any may be NULL.  Two launches. */
+int pvn3d_train_loss_forward(const pvn3d_loss_args_t *args, float *loss, float *parts, float *kp_loss,
+                             float *ctr_loss, float *acc, void *workspace, size_t workspace_bytes,
+                             pvn3d_stream_t stream);
+/* Gradients of the terms the args enable, after pvn3d_train_loss_forward on the same args and workspace.  The
+ * incoming gradient of the focal term is w_seg g_loss + g_parts[0], of kp_loss[b,k] w_kp g_loss + g_parts[1] +
+ * g_kp[b,k], of ctr_loss[b,k] w_ctr g_loss + g_parts[2] (NULL pointers count as 0; not all NULL).  Writes d_seg (seg's
+ * layout), d_kp [b,n_kp,n,3], d_ctr [b,n_ctr,n,3] in full:
+ *   d_seg[i,j] = (g / M) (-(1-pt_i)^gamma) (delta_jt - p_ij)    (M = 1 for a sum; 0 on ok = 0 rows)
+ *   d_kp[b,k,n,c] = (g[b,k] / den[b]) w[b,n] sgn(diff)          (sgn 0 = 0, as torch.abs's backward)
+ * One launch, no host sync. */
+int pvn3d_train_loss_backward(const pvn3d_loss_args_t *args, const float *g_loss, const float *g_parts,
+                              const float *g_kp, float *d_seg, float *d_kp, float *d_ctr, const void *workspace,
+                              size_t workspace_bytes, pvn3d_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif

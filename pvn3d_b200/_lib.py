@@ -41,6 +41,15 @@ class MlpLayer(ctypes.Structure):
     _fields_ = [("w", c_void_p), ("bias", c_void_p), ("k_pad", c_int), ("n_pad", c_int)]
 
 
+class LossArgs(ctypes.Structure):
+    """pvn3d_loss_args_t (include/pvn3d_b200.h)"""
+    _fields_ = [("seg", c_void_p), ("seg_target", c_void_p), ("seg_rows", ctypes.c_longlong), ("n_cls", c_int),
+                ("seg_inner", c_int), ("gamma", c_float), ("seg_mean", c_int), ("kp_pred", c_void_p),
+                ("kp_targ", c_void_p), ("n_kp", c_int), ("ctr_pred", c_void_p), ("ctr_targ", c_void_p),
+                ("n_ctr", c_int), ("labels", c_void_p), ("b", c_int), ("n", c_int), ("ok", c_void_p),
+                ("w_seg", c_float), ("w_kp", c_float), ("w_ctr", c_float)]
+
+
 # name -> (restype, argtypes); mirrors include/pvn3d_b200.h one to one
 _P = c_void_p
 _SIGNATURES = {
@@ -134,6 +143,10 @@ _SIGNATURES = {
                                   _P]),
     "pvn3d_depth_fill_workspace_bytes": (c_size_t, [c_int, c_int, c_int]),
     "pvn3d_depth_fill": (c_int, [_P, _P, c_float, c_int, c_int, c_int, _P, _P, _P, _P, c_size_t, _P]),
+    "pvn3d_train_targets": (c_int, [_P, _P, _P, _P, c_int, c_int, c_int, _P, _P, c_int, c_int, _P, _P, _P, _P, _P]),
+    "pvn3d_train_loss_workspace_bytes": (c_size_t, [ctypes.POINTER(LossArgs)]),
+    "pvn3d_train_loss_forward": (c_int, [ctypes.POINTER(LossArgs), _P, _P, _P, _P, _P, _P, c_size_t, _P]),
+    "pvn3d_train_loss_backward": (c_int, [ctypes.POINTER(LossArgs), _P, _P, _P, _P, _P, _P, _P, c_size_t, _P]),
 }
 FLAT_MS_MAX_PTS = 4096   # PVN3D_FLAT_MS_MAX_PTS
 EXPORTED_SYMBOLS = tuple(_SIGNATURES)

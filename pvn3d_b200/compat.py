@@ -20,7 +20,11 @@ What install() does (SURVEY section 8b, App. D):
   5. with patch_eval=True, rebinds `TorchEval.eval_pose_parallel` (patch_eval_pose_parallel): the poses of the whole
      batch in one FramePoseSolver.solve, every ground-truth object scored in one pvn3d_frame_add_adds launch, one
      device -> host read, and the distance lists appended exactly as eval_metric / eval_metric_lm would -- the
-     reference's cal_auc / cal_lm_add then run unchanged.
+     reference's cal_auc / cal_lm_add then run unchanged;
+  6. with patch_loss=True, rebinds `lib.loss.FocalLoss` / `lib.loss.OFLoss`, and the same names in
+     `train.train_ycb_pvn3d` / `train.train_linemod_pvn3d` when those are already imported, to the drop-ins of
+     pvn3d_b200.train_utils (import the training script first, then install).  get_item is not patched: it runs in
+     forked DataLoader workers, where CUDA cannot start -- call train_utils.train_batch on the collated batch instead.
 Nothing here copies or edits reference files.
 """
 from __future__ import annotations
@@ -80,7 +84,7 @@ def install_import_shims() -> None:
 
 
 def install(reference_root: str | None = None, patch_post: bool = False, patch_model: bool = False,
-            patch_eval: bool = False) -> None:
+            patch_eval: bool = False, patch_loss: bool = False) -> None:
     from . import _ext
 
     install_import_shims()
@@ -98,6 +102,21 @@ def install(reference_root: str | None = None, patch_post: bool = False, patch_m
             mod = sys.modules.get(name)
             if mod is not None and getattr(mod, "TorchEval", None) is not None:
                 patch_eval_pose_parallel(mod.TorchEval)
+    if patch_loss:
+        patch_loss_modules()
+
+
+def patch_loss_modules() -> None:
+    """Rebind FocalLoss and OFLoss in lib.loss and in the already imported training scripts to
+    pvn3d_b200.train_utils's drop-ins (same constructors and forward signatures, CUDA only)."""
+    from . import train_utils
+
+    mods = [importlib.import_module("lib.loss")]
+    mods += [sys.modules[m] for m in ("train.train_ycb_pvn3d", "train.train_linemod_pvn3d") if m in sys.modules]
+    for mod in mods:
+        for name in ("FocalLoss", "OFLoss"):
+            if name in vars(mod):
+                setattr(mod, name, getattr(train_utils, name))
 
 
 def _weights(model):
