@@ -41,7 +41,7 @@ extern "C" {
 
 typedef void *pvn3d_stream_t; /* cudaStream_t */
 
-int pvn3d_version(void);                 /* ABI version, currently 1                         */
+int pvn3d_version(void);                 /* ABI version, currently 2                         */
 const char *pvn3d_strerror(int code);    /* static string                                    */
 const char *pvn3d_last_cuda_error(void); /* thread-local text of the last PVN3D_ERR_CUDA     */
 int pvn3d_device_sm_count(int *sm_count, int *cc_major, int *cc_minor);
@@ -174,14 +174,14 @@ int pvn3d_three_nn_interpolate(const float *unknown, const float *known, const f
  * Shared-MLP layers of set abstraction / feature propagation on the Hopper tensor cores (wgmma)
  * (reference: SharedMLP = Conv2d 1x1 (no bias) + BatchNorm2d + ReLU, pytorch_utils.py:25-50, and the
  * max-pool over nsample of pointnet2_modules.py:64-67).  One call = one layer:
- *      out[p, col0 + 0:n_pad] = act( A[p, 0:k_pad] . W^T + bias ),   optionally max over `pool` rows
+ *      out[p, col0 + 0:n_pad] = act( A[p, 0:k_pad] . W^T + bias )
  *   w    [n_pad, k_pad] f32, BN folded into rows, values rounded to TF32, zero padded
  *        (k_pad multiple of 32, n_pad multiple of 16), 16-byte aligned (else PVN3D_ERR_INVALID_ARG: it is
  *        read 16 bytes at a time); bias [n_pad] (folded BN shift, 0 in the pad)
- *   out  point-major rows of length ldo (ldo, col0 multiples of 4); pool in {0, 8, 16, 32}
+ *   out  point-major rows of length ldo (ldo, col0 multiples of 4)
  * Arithmetic: TF32 operands (round-to-nearest), fp32 accumulation.
  * flags: PVN3D_MLP_RELU       apply ReLU (flags = 1 / 0 is the plain relu switch)
- *        PVN3D_MLP_ROUND_OUT  store the activations (pooled or not) already rounded to TF32
+ *        PVN3D_MLP_ROUND_OUT  store the activations already rounded to TF32
  *        PVN3D_MLP_A_TF32     (mlp_dense) `a` was produced with ROUND_OUT and is
  *                             16-byte aligned with a leading dimension % 4 == 0: its rows are copied global ->
  *                             shared asynchronously, without the rounding pass (unrounded values would be
@@ -196,8 +196,8 @@ int pvn3d_three_nn_interpolate(const float *unknown, const float *known, const f
 
 /* A = point-major activations a[rows, lda]; columns >= a_cols read as zero. */
 int pvn3d_mlp_dense(const float *a, int lda, int a_cols, long long rows, const float *w,
-                    const float *bias, int k_pad, int n_pad, int flags, int pool, float *out, int ldo,
-                    int col0, pvn3d_stream_t stream);
+                    const float *bias, int k_pad, int n_pad, int flags, float *out, int ldo, int col0,
+                    pvn3d_stream_t stream);
 /* pvn3d_mlp_dense with ONE BIAS VECTOR PER BATCH ELEMENT: bias is [rows / rows_per_frame][n_pad] and row p uses
  * vector p / rows_per_frame (rows_per_frame % 128 == 0).  Lets a layer whose input contains a per-frame constant
  * (DenseFusion's broadcast global feature, pvn3d.py:178-182) drop those K columns: W_c . g_b is folded into the bias. */
@@ -209,12 +209,6 @@ int pvn3d_mlp_dense_frame_bias(const float *a, int lda, int a_cols, long long ro
  * Summation order is fixed (reproducible). */
 int pvn3d_mlp_dense_sum32(const float *a, int lda, int a_cols, long long rows, const float *w, const float *bias,
                           int k_pad, int n_pad, int flags, float *out, int ldo, int col0, pvn3d_stream_t stream);
-/* First layer of an FP module with three_interpolate + concat fused: row (b,j) =
- * [ sum_t nn_w[b,j,t] * known_feat_pm[b, nn_idx[b,j,t], 0:c2] | skip_pm[b, j, 0:c1] | 0.. ] */
-int pvn3d_mlp_fp_first(const float *known_feat_pm, int c2, const int *nn_idx, const float *nn_w,
-                       const float *skip_pm, int lds, int c1, int b, int n_unknown, int m_known,
-                       const float *w, const float *bias, int k_pad, int n_pad, int flags, float *out,
-                       int ldo, int col0, pvn3d_stream_t stream);
 /* one folded layer: w [n_pad][k_pad] TF32-rounded, bias [n_pad] */
 typedef struct {
   const float *w;
@@ -226,26 +220,24 @@ typedef struct {
  *   U_j = W1f.f_j + W1x.x_j   once per POINT    (pvn3d_sa_factor_table + pvn3d_mlp_dense without ReLU), and
  *   V_i = W1x.c_i - b1        once per CENTRE   (pvn3d_sa_centre_term),
  * instead of one GEMM row per (centre, neighbour) pair: 5-16x fewer rows.  The second layer then takes
- * relu(U[idx] - V) as its operand (pvn3d_mlp_sa_fact).  The table carries x as hi + lo TF32 parts (columns
+ * relu(U[idx] - V) as its operand (pvn3d_mlp_sa_fact2(w)).  The table carries x as hi + lo TF32 parts (columns
  * [c_feat, c_feat+3) and [c_feat+3, c_feat+6)), to be multiplied by [W1f | W1x | W1x]: the coordinate term is
  * evaluated to ~2^-21, MORE accurately than rounding the difference x_j - c_i to TF32 as cuDNN's TF32 path
  * does.
  *   pvn3d_sa_factor_table: xyz [rows,3], feat_pm [rows, ldf] (c_feat columns) -> out [rows, k_pad] TF32-rounded
- *   pvn3d_sa_centre_term : centres [rows,3], wx [n_pad,3] (TF32-rounded), bias [n_pad] -> out [rows, n_pad]
- *   pvn3d_mlp_sa_fact    : u [B*n, ldu], v [B*m, ldu] (c_valid columns), idx [B,m,ns] -> layer (w, bias) as
- *                          pvn3d_mlp_dense: out rows = B*m*ns */
+ *   pvn3d_sa_centre_term : centres [rows,3], wx [n_pad,3] (TF32-rounded), bias [n_pad] -> out [rows, n_pad] */
 int pvn3d_sa_factor_table(const float *xyz, const float *feat_pm, int ldf, int c_feat, long long rows, int k_pad,
                           float *out, pvn3d_stream_t stream);
 int pvn3d_sa_centre_term(const float *centres, const float *wx, const float *bias, long long rows, int n_pad,
                          float *out, pvn3d_stream_t stream);
-int pvn3d_mlp_sa_fact(const float *u, const float *v, int ldu, int c_valid, const int *idx, int b, int n, int m,
-                      int ns, const float *w, const float *bias, int k_pad, int n_pad, int flags, float *out, int ldo,
-                      int col0, pvn3d_stream_t stream);
 /* Layers 2 AND 3 of a factored SA scale plus the max-pool over nsample, in one launch: the layer-2 activations
- * stay in shared memory instead of going through HBM.  Same result, bit for bit, as
- *   pvn3d_mlp_sa_fact(.., layer2, PVN3D_MLP_RELU | PVN3D_MLP_ROUND_OUT)  ->  h
- *   pvn3d_mlp_dense(h, .., layer3, PVN3D_MLP_RELU [| PVN3D_MLP_ROUND_OUT], pool = ns) -> out
- * pool must equal ns.  Both layers apply ReLU; flags: PVN3D_MLP_ROUND_OUT (pooled output) and
+ * stay in shared memory instead of going through HBM.
+ *   u [B*n, ldu], v [B*m, ldu] (c_valid columns), idx [B,m,ns]
+ *   A row (b*m + i)*ns + s = relu(u[b*n + idx[b,i,s]] - v[b*m + i])
+ *   pvn3d_mlp_dense(A, .., layer2, PVN3D_MLP_RELU | PVN3D_MLP_ROUND_OUT) -> h
+ *   pvn3d_mlp_dense(h, .., layer3, PVN3D_MLP_RELU [| PVN3D_MLP_ROUND_OUT] | PVN3D_MLP_A_TF32) -> y
+ *   out[b*m + i, col0 + c] = max over s of y[(b*m + i)*ns + s, c]
+ * bit for bit.  pool must equal ns.  Both layers apply ReLU; flags: PVN3D_MLP_ROUND_OUT (pooled output) and
  * PVN3D_MLP_RESERVE_SMS(n).  layer3->k_pad >= layer2->n_pad.  Any number of layer-2 K chunks.
  * PVN3D_ERR_UNSUPPORTED (nothing launched) unless pvn3d_mlp_sa_fact2_supported(layer2, layer3, ns) is 1: ns 16 or 32,
  * both n_pad <= 128, and both weight matrices, the layer-2 tile and two operand stages fit in a block's shared memory.
@@ -256,7 +248,7 @@ int pvn3d_mlp_sa_fact2(const float *u, const float *v, int ldu, int c_valid, con
 int pvn3d_mlp_sa_fact2_supported(const pvn3d_mlp_layer_t *layer2, const pvn3d_mlp_layer_t *layer3, int ns);
 /* The same for a WIDE last layer (layer3->n_pad > 128: SA3, SA4), where the weights cannot stay resident: 64-row
  * tiles, both layers in 128-column blocks, W2 and W3 streamed from L2 by TMA once per tile, the layer-2 activations
- * in shared memory.  Same arguments, same bit-identical result as the two launches above.
+ * in shared memory.  Same arguments, and bit for bit the same operation as pvn3d_mlp_sa_fact2.
  * PVN3D_ERR_UNSUPPORTED (nothing launched) unless pvn3d_mlp_sa_fact2w_supported(layer2, layer3, ns) is 1: ns 16 or
  * 32, layer3->n_pad > 128, layer2->k_pad <= 256, layer3->k_pad within the 128-column blocks of layer 2, the A and H
  * tiles and three weight stages within a block's shared memory.
@@ -265,12 +257,14 @@ int pvn3d_mlp_sa_fact2w(const float *u, const float *v, int ldu, int c_valid, co
                         int ns, const pvn3d_mlp_layer_t *layer2, const pvn3d_mlp_layer_t *layer3, int flags, int pool,
                         float *out, int ldo, int col0, pvn3d_stream_t stream);
 int pvn3d_mlp_sa_fact2w_supported(const pvn3d_mlp_layer_t *layer2, const pvn3d_mlp_layer_t *layer3, int ns);
-/* Both layers of an FP module with a two-layer MLP (FP2-FP4), in one launch: the interpolated first-layer operand is
- * produced once per pair of 128-column blocks instead of once per block, and the layer-1 activations stay in shared
- * memory instead of going through HBM.  Same result, bit for bit, as
- *   pvn3d_mlp_fp_first(.., layer1, PVN3D_MLP_RELU | PVN3D_MLP_ROUND_OUT) -> h [b*n_unknown, layer1->n_pad]
+/* Both layers of an FP module with a two-layer MLP (FP2-FP4), in one launch: three_interpolate and the concat are
+ * fused into the first layer's operand, which is produced once per pair of 128-column blocks, and the layer-1
+ * activations stay in shared memory instead of going through HBM.  Bit for bit:
+ *   A row (b,j) = [ sum_t nn_w[b,j,t] * known_feat_pm[b, nn_idx[b,j,t], 0:c2] | skip_pm[b*n_unknown + j, 0:c1] | 0.. ]
+ *                 (skip rows lds floats apart; the sum as pvn3d_three_interpolate evaluates it)
+ *   pvn3d_mlp_dense(A, .., layer1, PVN3D_MLP_RELU | PVN3D_MLP_ROUND_OUT) -> h [b*n_unknown, layer1->n_pad]
  *   pvn3d_mlp_dense(h, .., layer2, PVN3D_MLP_RELU [| PVN3D_MLP_ROUND_OUT] | PVN3D_MLP_A_TF32) -> out
- * Arguments as pvn3d_mlp_fp_first; out rows = b * n_unknown, columns col0 .. col0 + layer2->n_pad of rows ldo apart.
+ * out rows = b * n_unknown, columns col0 .. col0 + layer2->n_pad of rows ldo apart.
  * Both layers apply ReLU; flags: PVN3D_MLP_ROUND_OUT (output) and PVN3D_MLP_RESERVE_SMS(n).  Weight pointers must be
  * 16-byte aligned (else PVN3D_ERR_INVALID_ARG, before any CUDA call).
  * PVN3D_ERR_UNSUPPORTED (nothing launched) unless pvn3d_mlp_fp2_supported(layer1, layer2) is 1: layer1->n_pad 256 or
@@ -284,16 +278,14 @@ int pvn3d_mlp_fp2_supported(const pvn3d_mlp_layer_t *layer1, const pvn3d_mlp_lay
  *   P = W1k . known      once per KNOWN point   (pvn3d_mlp_dense without ReLU on the known table),
  *   S = W1s . skip + b1  over the skip columns  (pvn3d_mlp_dense without ReLU on the skip table),
  * and the second layer takes relu(sum_t nn_w[b,j,t] * P[b, nn_idx[b,j,t], :] + S[b,j,:]) as its operand:
- * the gathered rows shrink from the known descriptors (256-1024 floats) to the layer width (128-512).
- *   p [B*m_known, ld], s [B*n_unknown, ld], ld == c_valid (multiple of 4) */
-int pvn3d_mlp_fp_fact(const float *p, const float *s, int ld, int c_valid, const int *nn_idx, const float *nn_w,
-                      int b, int n_unknown, int m_known, const float *w, const float *bias, int k_pad, int n_pad,
-                      int flags, float *out, int ldo, int col0, pvn3d_stream_t stream);
+ * the gathered rows shrink from the known descriptors (256-1024 floats) to the layer width (128-512). */
 /* The skip term and the second layer of a factored FP module whose skip is an SA factor table (FP1), in one launch:
- * S never goes through HBM.  Same result, bit for bit, as
+ * S never goes through HBM.  Bit for bit:
  *   pvn3d_mlp_dense(table, k, k, b*n_unknown, layer_s, PVN3D_MLP_A_TF32) -> s    (k = layer_s->k_pad, no ReLU)
- *   pvn3d_mlp_fp_fact(p, s, 128, 128, nn_idx, nn_w, b, n_unknown, m_known, layer2, PVN3D_MLP_RELU) -> rows
- *                     [b*n_unknown][128], transposed per frame -> out [b][128][n_unknown]
+ *   A row (b,j) = relu(sum_t nn_w[b,j,t] * p[b*m_known + nn_idx[b,j,t], :] + s[b*n_unknown + j, :])
+ *                 (the sum as pvn3d_three_interpolate evaluates it, then one fp32 add)
+ *   pvn3d_mlp_dense(A, 128, 128, b*n_unknown, layer2, PVN3D_MLP_RELU) -> rows [b*n_unknown][128], transposed per
+ *                 frame -> out [b][128][n_unknown]
  * for ANY n_unknown (a tile may hold the end of one frame and the start of the next).
  *   p [b*m_known, 128], table [b*n_unknown, 32] TF32-rounded (pvn3d_sa_factor_table), both 16-byte aligned.
  * flags: PVN3D_MLP_RESERVE_SMS(n) only.  Pointers not 16-byte aligned or other flags: PVN3D_ERR_INVALID_ARG, before any

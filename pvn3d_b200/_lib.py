@@ -77,14 +77,11 @@ _SIGNATURES = {
     "pvn3d_query_and_group": (c_int, [_P, _P, _P, c_int, c_int, c_int, c_int, c_int, c_float, c_int, _P, _P, _P]),
     "pvn3d_query_and_group2": (c_int, [_P, _P, _P, c_int, c_int, c_int, c_int, c_int, c_float, c_int, _P, _P, c_float, c_int, _P, _P, _P]),
     "pvn3d_three_nn_interpolate": (c_int, [_P, _P, _P, c_int, c_int, c_int, c_int, _P, c_int, c_int, _P, _P, _P]),
-    "pvn3d_mlp_dense": (c_int, [_P, c_int, c_int, ctypes.c_longlong, _P, _P, c_int, c_int, c_int, c_int, _P, c_int, c_int, _P]),
+    "pvn3d_mlp_dense": (c_int, [_P, c_int, c_int, ctypes.c_longlong, _P, _P, c_int, c_int, c_int, _P, c_int, c_int, _P]),
     "pvn3d_mlp_dense_frame_bias": (c_int, [_P, c_int, c_int, ctypes.c_longlong, c_int, _P, _P, c_int, c_int, c_int, _P, c_int, c_int, _P]),
     "pvn3d_mlp_dense_sum32": (c_int, [_P, c_int, c_int, ctypes.c_longlong, _P, _P, c_int, c_int, c_int, _P, c_int, c_int, _P]),
-    "pvn3d_mlp_fp_first": (c_int, [_P, c_int, _P, _P, _P, c_int, c_int, c_int, c_int, c_int, _P, _P, c_int, c_int, c_int, _P, c_int, c_int, _P]),
     "pvn3d_sa_factor_table": (c_int, [_P, _P, c_int, c_int, ctypes.c_longlong, c_int, _P, _P]),
     "pvn3d_sa_centre_term": (c_int, [_P, _P, _P, ctypes.c_longlong, c_int, _P, _P]),
-    "pvn3d_mlp_sa_fact": (c_int, [_P, _P, c_int, c_int, _P, c_int, c_int, c_int, c_int, _P, _P, c_int, c_int, c_int, _P, c_int,
-                                  c_int, _P]),
     "pvn3d_mlp_sa_fact2": (c_int, [_P, _P, c_int, c_int, _P, c_int, c_int, c_int, c_int, _P, _P, c_int, c_int, _P, c_int,
                                    c_int, _P]),
     "pvn3d_mlp_sa_fact2_supported": (c_int, [_P, _P, c_int]),
@@ -93,8 +90,6 @@ _SIGNATURES = {
     "pvn3d_mlp_sa_fact2w_supported": (c_int, [_P, _P, c_int]),
     "pvn3d_mlp_fp2": (c_int, [_P, c_int, _P, _P, _P, c_int, c_int, c_int, c_int, c_int, _P, _P, c_int, _P, c_int, c_int, _P]),
     "pvn3d_mlp_fp2_supported": (c_int, [_P, _P]),
-    "pvn3d_mlp_fp_fact": (c_int, [_P, _P, c_int, c_int, _P, _P, c_int, c_int, c_int, _P, _P, c_int, c_int, c_int, _P, c_int, c_int,
-                                  _P]),
     "pvn3d_mlp_fp_fact2": (c_int, [_P, _P, _P, _P, c_int, c_int, c_int, _P, _P, c_int, _P, _P]),
     "pvn3d_mlp_fp_fact2_supported": (c_int, [_P, _P]),
     "pvn3d_mlp_fp_fact2_rows": (c_int, [_P, _P, _P, _P, c_int, c_int, c_int, _P, _P, c_int, _P, c_int, c_int, _P]),

@@ -1,6 +1,6 @@
 // mlp_tc.cu -- the shared-MLP contractions of set abstraction / feature propagation on the Hopper
 // tensor cores (wgmma.mma_async tf32, fp32 accumulators in registers), with the PointNet++ data movement
-// fused into the operand producer and the activation / max-pool fused into the epilogue.
+// fused into the operand producers and the activation / max-pool fused into the epilogues.
 //
 // Replaces, per SharedMLP layer of the reference (pytorch_utils.py:25-50: Conv2d 1x1 (no bias) ->
 // BatchNorm2d -> ReLU, plus F.max_pool2d over nsample at pointnet2_modules.py:64-67): one cuDNN conv,
@@ -9,27 +9,21 @@
 //
 //   out[p, :] = act( A[p, :] . W^T + bias )            W: BN folded, K-major, TF32-rounded
 //
-// A-operand producers (warps 4-11, eight lanes per row of the 128-row tile):
-//   DENSE      rows of a point-major activation matrix [P, lda]
-//   SA_FACT    row (b,i,s): relu(U[b, idx[b,i,s], :] - V[b, i, :]) -- the second layer of a factored SA scale
-//              (QueryAndGroup.forward, pointnet2_utils.py:311-321, and the first layer never materialised)
-//   FP_INTERP  row (b,j): [ sum_t w_t * known_feat_pm[b, idx_t, 0:C2] | skip[b, j, 0:C1] | 0 ... ]
-//              (three_interpolate + torch.cat of PointnetFPModule.forward, pointnet2_modules.py:188-199)
-//   FP_FACT    row (b,j): relu(sum_t w_t * P[b, idx_t, :] + S[b, j, :]) -- the second layer of a factored FP module
-// Operands are staged in shared memory in the canonical K-major SWIZZLE_128B layout (32 fp32 = 128 B
-// per row per stage; weights arrive by TMA, pre-rounded activations by cp.async).  Two MMA warpgroups
-// (warps 12-19) each issue wgmma m64nNk8 (N = 16, 32, 64 or 128 columns per tile) for one 64-row half
-// of the tile, keep the accumulator in registers, release stages once wgmma.wait_group has retired the
-// MMAs that read them, and hand each finished tile to the epilogue through a swizzled shared-memory
-// accumulator tile; the kernel is persistent (one CTA per SM, tiles strided), so staging of tile j+1
-// and the epilogue of tile j-1 overlap the MMAs of tile j.  The epilogue warps (0-3) read the
-// accumulator tile one row per thread, add the folded-BN bias, apply ReLU and either store the
-// point-major row or reduce over the nsample rows of each centre with a transposing shuffle butterfly
-// (max-pool) and store one 128-byte line per centre.
+// mlp_layer_kernel runs one dense layer on the rows of a point-major matrix [P, lda] (SA factor tables, FP1's P, the
+// heads, DenseFusion).  Its producers (warps 4-11, eight lanes per row of the 128-row tile) stage the operands in the
+// canonical K-major SWIZZLE_128B layout (32 fp32 = 128 B per row per stage; weights arrive by TMA, pre-rounded
+// activations by cp.async).  Two MMA warpgroups (warps 12-19) each issue wgmma m64nNk8 (N = 16, 32, 64 or 128 columns
+// per tile) for one 64-row half of the tile, keep the accumulator in registers, release stages once wgmma.wait_group
+// has retired the MMAs that read them, and hand each finished tile to the epilogue through a swizzled shared-memory
+// accumulator tile; the kernel is persistent (one CTA per SM, tiles strided), so staging of tile j+1 and the epilogue
+// of tile j-1 overlap the MMAs of tile j.  The epilogue warps (0-3) read the accumulator tile one row per thread, add
+// the folded-BN bias, apply ReLU and store the row, or sum relu(row) over 32 rows (DenseFusion's average pool).
 //
-// The engines run this per-layer kernel only for dense layers (the factor tables, the heads); the SA / FP
-// modules run on the fused kernels further down, and the other producers and the pooled form stay as the
-// two-launch references those kernels are tested against, bit for bit.
+// The SA and FP modules run on the fused kernels further down, which build the rows of their first contracted layer
+// on chip: relu(U[b, idx[b,i,s]] - V[b, i]) for SA (the factored QueryAndGroup rows, pointnet2_utils.py:311-321, then
+// a max over nsample), [three_interpolate(known) | skip | 0] for FP2-FP4 (pointnet2_modules.py:188-199) and
+// relu(three_interpolate(P) + S) for FP1.  Each rounds its rows to TF32 as the dense producer does and keeps the dense
+// layer's MMA order and epilogue arithmetic, so it equals mlp_layer_kernel run on those rows, bit for bit.
 //
 // TF32: operands are rounded to nearest (cvt.rna.tf32.f32) when staged, accumulation is fp32 -- the
 // precision class of the reference's default cuDNN convolutions (torch.backends.cudnn.allow_tf32).
@@ -48,8 +42,8 @@ constexpr int kMlpThreads = (kMlpEpiWarps + kMlpProWarps + kMlpMmaWarps) * 32;
 constexpr int kMlpMaxStages = 6;
 constexpr int kMlpSmemMax = 227 * 1024;  // dynamic shared memory a block may opt into on sm_90
 
-enum : int { PRO_DENSE = 0, PRO_FP_INTERP = 2, PRO_SA_FACT = 3, PRO_FP_FACT = 4 };
-enum : int { EPI_STORE = 0, EPI_MAXPOOL = 1, EPI_SUMPOOL = 2 };
+enum : int { PRO_DENSE = 0, PRO_FP_INTERP = 2, PRO_SA_FACT = 3 };   // row layouts of rows_setup / stage_a_chunk
+enum : int { EPI_STORE = 0, EPI_SUMPOOL = 2 };
 
 struct MlpArgs {
   // W as a TMA tensor map ([n_pad][k_pad] fp32, box 32 columns x bn rows, SWIZZLE_128B): one
@@ -81,7 +75,7 @@ struct MlpArgs {
   float *out;
   int ldo, col0, relu;
   int round_out;  // store TF32-rounded values (the next layer then takes them with a_tf32)
-  int pool;       // nsample of the max-pool epilogue (8, 16 or 32)
+  int pool;       // rows per pooled output: nsample of the fused SA kernels (16 or 32), 32 for EPI_SUMPOOL
   int reserve_sms;  // host only: SMs left to concurrent kernels (PVN3D_MLP_RESERVE_SMS in flags)
   int bias_npb;     // > 0: bias is [rows / bias_npb][n_pad] -- one vector per batch element (bias_npb % 128 == 0)
 };
@@ -348,48 +342,12 @@ __device__ __forceinline__ void sts_tf32(uint32_t addr, const float4 &v) {
   sts128(addr, to_tf32(v.x), to_tf32(v.y), to_tf32(v.z), to_tf32(v.w));
 }
 
-// stage columns [k0 + 4*sub, +4) of this thread's 8 rows into the swizzled A tile at `sa`
+// stage columns [k0 + 4*sub, +4) of this thread's 8 rows into the swizzled A tile at `sa` (PRO_DENSE or PRO_SA_FACT)
 template <int PRO>
-__device__ __forceinline__ void stage_a_chunk(const MlpArgs &a, const RowState &s, long long p_first,
-                                              int r_first, int sub, int k0, uint32_t sa, bool vec_ok) {
+__device__ __forceinline__ void stage_a_chunk(const MlpArgs &a, const RowState &s, int r_first, int sub, int k0,
+                                              uint32_t sa, bool vec_ok) {
   const int k = k0 + 4 * sub;
   const float4 zero = make_float4(0.f, 0.f, 0.f, 0.f);
-  if (PRO == PRO_FP_FACT) {
-    // second layer of a FACTORED FP module: row (b,j) = relu( sum_t w_t * P[b, idx_t, :] + S[b, j, :] ) with
-    // P = W1k . known (once per KNOWN point) and S = W1s . skip + b1 (the skip columns only): the first layer is
-    // linear before its ReLU, so three_interpolate commutes with it (pointnet2_modules.py:183-204)
-    if (k >= a.c2) {
-#pragma unroll
-      for (int j = 0; j < 8; ++j) sts128(sa + sw128_off(r_first + 4 * j, sub), 0.f, 0.f, 0.f, 0.f);
-      return;
-    }
-#pragma unroll
-    for (int h = 0; h < 4; ++h) {   // four quarters: 8 LDG.128 in flight each
-      float4 p1[2], p2[2], p3[2], sk[2];
-#pragma unroll
-      for (int jj = 0; jj < 2; ++jj) {
-        const int j = h * 2 + jj;
-        const float *pf = a.known_feat + k;
-        p1[jj] = ldg128(pf + static_cast<size_t>(s.g1[j]) * a.c2);
-        p2[jj] = ldg128(pf + static_cast<size_t>(s.g2[j]) * a.c2);
-        p3[jj] = ldg128(pf + static_cast<size_t>(s.g3[j]) * a.c2);
-        const long long pr = ((s.live >> j) & 1u) ? p_first + 4 * j : 0;
-        sk[jj] = ldg128(a.skip + pr * a.c2 + k);
-      }
-#pragma unroll
-      for (int jj = 0; jj < 2; ++jj) {
-        const int j = h * 2 + jj;
-        float4 v;
-        v.x = fmaxf(__fmaf_rn(p3[jj].x, s.w3[j], __fmaf_rn(p1[jj].x, s.w1[j], __fmul_rn(p2[jj].x, s.w2[j]))) + sk[jj].x, 0.f);
-        v.y = fmaxf(__fmaf_rn(p3[jj].y, s.w3[j], __fmaf_rn(p1[jj].y, s.w1[j], __fmul_rn(p2[jj].y, s.w2[j]))) + sk[jj].y, 0.f);
-        v.z = fmaxf(__fmaf_rn(p3[jj].z, s.w3[j], __fmaf_rn(p1[jj].z, s.w1[j], __fmul_rn(p2[jj].z, s.w2[j]))) + sk[jj].z, 0.f);
-        v.w = fmaxf(__fmaf_rn(p3[jj].w, s.w3[j], __fmaf_rn(p1[jj].w, s.w1[j], __fmul_rn(p2[jj].w, s.w2[j]))) + sk[jj].w, 0.f);
-        if (!((s.live >> j) & 1u)) v = zero;
-        sts_tf32(sa + sw128_off(r_first + 4 * j, sub), v);
-      }
-    }
-    return;
-  }
   if (PRO == PRO_SA_FACT) {
     // second layer of a FACTORED SA scale: row (b,i,s) = relu(U[b, idx[b,i,s], :] - V[b, i, :]), where
     // U = W1 . [f_j | x_j] for every POINT and V = W1x . c_i - bias1 for every CENTRE (the first layer is linear
@@ -418,93 +376,30 @@ __device__ __forceinline__ void stage_a_chunk(const MlpArgs &a, const RowState &
     }
     return;
   }
-  if (PRO == PRO_DENSE) {
-    if (vec_ok && k + 4 <= a.a_cols) {
-      float4 v[8];
+  if (vec_ok && k + 4 <= a.a_cols) {
+    float4 v[8];
 #pragma unroll
-      for (int j = 0; j < 8; ++j) v[j] = (s.live >> j) & 1u ? ldg128(s.row[j] + k) : zero;
+    for (int j = 0; j < 8; ++j) v[j] = (s.live >> j) & 1u ? ldg128(s.row[j] + k) : zero;
 #pragma unroll
-      for (int j = 0; j < 8; ++j) sts_tf32(sa + sw128_off(r_first + 4 * j, sub), v[j]);
-      return;
-    }
-    if (k >= a.a_cols) {
-#pragma unroll
-      for (int j = 0; j < 8; ++j) sts128(sa + sw128_off(r_first + 4 * j, sub), 0.f, 0.f, 0.f, 0.f);
-      return;
-    }
-  } else {
-    if (vec_ok && k + 4 <= a.c2) {
-#pragma unroll
-      for (int h = 0; h < 2; ++h) {  // two halves: 12 LDG.128 in flight each
-        float4 p1[4], p2[4], p3[4];
-#pragma unroll
-        for (int jj = 0; jj < 4; ++jj) {
-          const int j = h * 4 + jj;
-          const float *kf = a.known_feat + k;
-          p1[jj] = ldg128(kf + static_cast<size_t>(s.g1[j]) * a.c2);
-          p2[jj] = ldg128(kf + static_cast<size_t>(s.g2[j]) * a.c2);
-          p3[jj] = ldg128(kf + static_cast<size_t>(s.g3[j]) * a.c2);
-        }
-#pragma unroll
-        for (int jj = 0; jj < 4; ++jj) {
-          const int j = h * 4 + jj;
-          // same contraction as three_interpolate (pn2_ops.cu): fma(p3,w3, fma(p1,w1, p2*w2))
-          float4 v;
-          v.x = __fmaf_rn(p3[jj].x, s.w3[j], __fmaf_rn(p1[jj].x, s.w1[j], __fmul_rn(p2[jj].x, s.w2[j])));
-          v.y = __fmaf_rn(p3[jj].y, s.w3[j], __fmaf_rn(p1[jj].y, s.w1[j], __fmul_rn(p2[jj].y, s.w2[j])));
-          v.z = __fmaf_rn(p3[jj].z, s.w3[j], __fmaf_rn(p1[jj].z, s.w1[j], __fmul_rn(p2[jj].z, s.w2[j])));
-          v.w = __fmaf_rn(p3[jj].w, s.w3[j], __fmaf_rn(p1[jj].w, s.w1[j], __fmul_rn(p2[jj].w, s.w2[j])));
-          if (!((s.live >> j) & 1u)) v = zero;
-          sts_tf32(sa + sw128_off(r_first + 4 * j, sub), v);
-        }
-      }
-      return;
-    }
-    const bool skip_vec = (a.c2 % 4 == 0) && (a.lds % 4 == 0) &&
-                          ((reinterpret_cast<uintptr_t>(a.skip) & 15u) == 0);
-    if (skip_vec && k >= a.c2 && k - a.c2 + 4 <= a.c1) {
-      float4 v[8];
-#pragma unroll
-      for (int j = 0; j < 8; ++j)
-        v[j] = (s.live >> j) & 1u ? ldg128(a.skip + (p_first + 4 * j) * a.lds + (k - a.c2)) : zero;
-#pragma unroll
-      for (int j = 0; j < 8; ++j) sts_tf32(sa + sw128_off(r_first + 4 * j, sub), v[j]);
-      return;
-    }
-    if (k >= a.c2 + a.c1) {
-#pragma unroll
-      for (int j = 0; j < 8; ++j) sts128(sa + sw128_off(r_first + 4 * j, sub), 0.f, 0.f, 0.f, 0.f);
-      return;
-    }
+    for (int j = 0; j < 8; ++j) sts_tf32(sa + sw128_off(r_first + 4 * j, sub), v[j]);
+    return;
   }
-  // generic path (chunks that straddle a segment boundary / unaligned rows).  Which source an element
-  // comes from depends only on its column, not on the row, so the loads of the 8 passes are issued
-  // together as predicated loads -- no per-element branches, one round trip instead of 32.
+  if (k >= a.a_cols) {
+#pragma unroll
+    for (int j = 0; j < 8; ++j) sts128(sa + sw128_off(r_first + 4 * j, sub), 0.f, 0.f, 0.f, 0.f);
+    return;
+  }
+  // generic path (a chunk that straddles a_cols / unaligned rows): the loads of the 8 passes are issued together as
+  // predicated loads (which exist depends on the column only) -- no per-element branches, one round trip instead of 32
   float vv[8][4];
 #pragma unroll
   for (int j = 0; j < 8; ++j) {
     const bool live = (s.live >> j) & 1u;
-    const long long p = p_first + 4 * j;
 #pragma unroll
     for (int e = 0; e < 4; ++e) {
       const int kk = k + e;
-      float v = 0.f;
-      if (PRO == PRO_DENSE) {
-        const bool on = live && kk < a.a_cols;
-        v = on ? __ldg(s.row[j] + (on ? kk : 0)) : 0.f;
-      } else {
-        const bool isk = live && kk < a.c2;
-        const int d = kk - a.c2;
-        const bool iss = live && d >= 0 && d < a.c1;
-        const float *kf = a.known_feat + (isk ? kk : 0);
-        const float p1 = isk ? __ldg(kf + static_cast<size_t>(s.g1[j]) * a.c2) : 0.f;
-        const float p2 = isk ? __ldg(kf + static_cast<size_t>(s.g2[j]) * a.c2) : 0.f;
-        const float p3 = isk ? __ldg(kf + static_cast<size_t>(s.g3[j]) * a.c2) : 0.f;
-        const float sk = iss ? __ldg(a.skip + p * a.lds + (iss ? d : 0)) : 0.f;
-        // same contraction as three_interpolate (pn2_ops.cu): fma(p3,w3, fma(p1,w1, p2*w2))
-        v = isk ? __fmaf_rn(p3, s.w3[j], __fmaf_rn(p1, s.w1[j], __fmul_rn(p2, s.w2[j]))) : sk;
-      }
-      vv[j][e] = v;
+      const bool on = live && kk < a.a_cols;
+      vv[j][e] = on ? __ldg(s.row[j] + (on ? kk : 0)) : 0.f;
     }
   }
 #pragma unroll
@@ -513,19 +408,6 @@ __device__ __forceinline__ void stage_a_chunk(const MlpArgs &a, const RowState &
 }
 
 // ---- epilogue helpers ------------------------------------------------------------------------------
-// After the call, lane l holds in v[0] the max over the 32 lanes of the ORIGINAL v[l] (column l).
-__device__ __forceinline__ void warp_colmax_32(float (&v)[32], unsigned lane) {
-#pragma unroll
-  for (int o = 16; o >= 1; o >>= 1) {
-    const bool hi = (lane & o) != 0;
-#pragma unroll
-    for (int i = 0; i < o; ++i) {
-      const float keep = hi ? v[i + o] : v[i];
-      const float send = hi ? v[i] : v[i + o];
-      v[i] = fmaxf(keep, __shfl_xor_sync(0xffffffffu, send, o));
-    }
-  }
-}
 // After the call, lane l holds in v[0] the SUM over the 32 lanes of the ORIGINAL v[l] (fixed order: reproducible).
 __device__ __forceinline__ void warp_colsum_32(float (&v)[32], unsigned lane) {
 #pragma unroll
@@ -539,35 +421,6 @@ __device__ __forceinline__ void warp_colsum_32(float (&v)[32], unsigned lane) {
     }
   }
 }
-// groups of 16 lanes: lane l (l' = l & 15) ends with columns 2l', 2l'+1 in v[0], v[1]
-__device__ __forceinline__ void warp_colmax_16(float (&v)[32], unsigned lane) {
-#pragma unroll
-  for (int o = 8; o >= 1; o >>= 1) {
-    const bool hi = (lane & o) != 0;
-    const int half = o * 2;  // columns held after this step
-#pragma unroll
-    for (int i = 0; i < half; ++i) {
-      const float keep = hi ? v[i + half] : v[i];
-      const float send = hi ? v[i] : v[i + half];
-      v[i] = fmaxf(keep, __shfl_xor_sync(0xffffffffu, send, o));
-    }
-  }
-}
-// groups of 8 lanes: lane l (l' = l & 7) ends with columns 4l'..4l'+3 in v[0..3]
-__device__ __forceinline__ void warp_colmax_8(float (&v)[32], unsigned lane) {
-#pragma unroll
-  for (int o = 4; o >= 1; o >>= 1) {
-    const bool hi = (lane & o) != 0;
-    const int half = o * 4;
-#pragma unroll
-    for (int i = 0; i < half; ++i) {
-      const float keep = hi ? v[i + half] : v[i];
-      const float send = hi ? v[i] : v[i + half];
-      v[i] = fmaxf(keep, __shfl_xor_sync(0xffffffffu, send, o));
-    }
-  }
-}
-
 struct MlpSmemCtl {
   uint64_t full[kMlpMaxStages];   // 128 arrivals: every producer thread of the filling group
   uint64_t empty[kMlpMaxStages];  // 8 arrivals: one per MMA warp, once its MMAs that read the stage have retired
@@ -682,8 +535,8 @@ __device__ __forceinline__ void mma_tile_bf16(uint32_t ring, uint32_t stage_byte
 //              of the tensor core across tile boundaries;
 //   MMA        two warpgroups accumulate tile j in registers (64 rows each) while the epilogue drains tile j-1
 //              from the shared-memory accumulator tile;
-//   epilogue   bias / ReLU / pooling / stores of the tile in the accumulator tile.
-template <int PRO, int EPI>
+//   epilogue   bias / ReLU / sum-pool / stores of the tile in the accumulator tile.
+template <int EPI>
 __global__ void __launch_bounds__(kMlpThreads, 1) mlp_layer_kernel(const __grid_constant__ MlpArgs a) {
   // dynamic shared memory only: [operand ring: stages x stage_bytes, 1024-byte aligned][accumulator tile
   // 128 x acc_ld floats][epilogue staging 4 x 4 KB][barriers]
@@ -721,13 +574,10 @@ __global__ void __launch_bounds__(kMlpThreads, 1) mlp_layer_kernel(const __grid_
     const unsigned grp = (warp - kMlpEpiWarps) >> 2;       // group 0 / 1 takes even / odd chunks
     const int pw = pt >> 5, sub = static_cast<int>(lane & 7u), rg = static_cast<int>(lane >> 3);
     const int r_first = 32 * pw + rg;
-    bool vec_ok = true;
-    if (PRO == PRO_DENSE) vec_ok = (a.lda % 4 == 0) && ((reinterpret_cast<uintptr_t>(a.a) & 15u) == 0);
-    if (PRO == PRO_FP_INTERP)
-      vec_ok = (a.c2 % 4 == 0) && ((reinterpret_cast<uintptr_t>(a.known_feat) & 15u) == 0);
-    // pre-rounded rows are copied global -> shared asynchronously: DENSE activations of a ROUND_OUT layer
+    const bool vec_ok = (a.lda % 4 == 0) && ((reinterpret_cast<uintptr_t>(a.a) & 15u) == 0);
+    // pre-rounded rows are copied global -> shared asynchronously: activations of a ROUND_OUT layer
     // (PVN3D_MLP_A_TF32); everything else is staged through registers
-    const bool a_async = PRO == PRO_DENSE && a.a_tf32 && vec_ok;
+    const bool a_async = a.a_tf32 && vec_ok;
     int pend0 = 0, pend1 = 0, npend = 0;  // stages whose copies are committed but not yet published
     long long it_base = 0;  // number of K chunks staged before this tile (same in every role)
     for (long long tile = blockIdx.x; tile < total_tiles; tile += gridDim.x, it_base += kc_total) {
@@ -738,7 +588,7 @@ __global__ void __launch_bounds__(kMlpThreads, 1) mlp_layer_kernel(const __grid_
       const int n0 = nb * a.bn;
       const long long p_first = p0 + r_first;
       RowState rs;
-      rows_setup<PRO>(a, p_first, rs);
+      rows_setup<PRO_DENSE>(a, p_first, rs);
       for (int kc = 0; kc < kc_total; ++kc) {
         const long long it = it_base + kc;
         if (static_cast<unsigned>(it & 1) != grp) continue;
@@ -772,7 +622,7 @@ __global__ void __launch_bounds__(kMlpThreads, 1) mlp_layer_kernel(const __grid_
           ++npend;
         } else {
           cp_async_commit();
-          stage_a_chunk<PRO>(a, rs, p_first, r_first, sub, kc * 32, sa, vec_ok);
+          stage_a_chunk<PRO_DENSE>(a, rs, r_first, sub, kc * 32, sa, vec_ok);
           cp_async_wait<0>();        // every asynchronous chunk still pending has landed
           fence_proxy_async_smem();  // generic-proxy stores / copies -> visible to the tensor-core proxy
           if (npend >= 1) mbar_arrive(&ctl.full[pend0]);
@@ -832,7 +682,7 @@ __global__ void __launch_bounds__(kMlpThreads, 1) mlp_layer_kernel(const __grid_
           const int col = static_cast<int>(lane);
           if (col < cw && p0 + warp * 32 < a.rows)
             a.out[((p0 + warp * 32) / 32) * a.ldo + a.col0 + n0 + c0 + col] = v[0];
-        } else if (EPI == EPI_STORE) {
+        } else {
           // raw accumulators through a swizzled 4 KB staging tile (thread = row going in, 8 lanes per row coming
           // out: the global stores are 128-byte row segments, 4 rows per STG.128); bias / ReLU / rounding on the
           // way out, where a lane keeps ONE group of four columns -- its bias is a single float4 (loaded before
@@ -874,51 +724,6 @@ __global__ void __launch_bounds__(kMlpThreads, 1) mlp_layer_kernel(const __grid_
                 *reinterpret_cast<float4 *>(o + static_cast<size_t>(4 * i) * a.ldo) = r[i];
           }
           __syncwarp();
-        } else {
-          // max over the `pool` rows of each centre; rows past the end contribute -inf
-          if (prow >= a.rows) {
-#pragma unroll
-            for (int i = 0; i < 32; ++i) v[i] = -__int_as_float(0x7f800000);
-          }
-          const long long grow0 = (p0 + warp * 32) / a.pool;  // first pooled row of this warp
-          if (a.pool == 32) {
-            warp_colmax_32(v, lane);
-            const int col = static_cast<int>(lane);
-            if (col < cw && p0 + warp * 32 < a.rows) {
-              float r = v[0] + __ldg(bias_t + n0 + c0 + col);
-              if (a.relu) r = fmaxf(r, 0.f);
-              if (a.round_out) r = to_tf32(r);
-              a.out[grow0 * a.ldo + a.col0 + n0 + c0 + col] = r;
-            }
-          } else if (a.pool == 16) {
-            warp_colmax_16(v, lane);
-            const int g = lane >> 4, col = static_cast<int>(lane & 15u) * 2;
-            if (col < cw && p0 + warp * 32 + g * 16 < a.rows) {
-              float2 r;
-              r.x = v[0] + __ldg(bias_t + n0 + c0 + col);
-              r.y = v[1] + __ldg(bias_t + n0 + c0 + col + 1);
-              if (a.relu) { r.x = fmaxf(r.x, 0.f); r.y = fmaxf(r.y, 0.f); }
-              if (a.round_out) { r.x = to_tf32(r.x); r.y = to_tf32(r.y); }
-              *reinterpret_cast<float2 *>(a.out + (grow0 + g) * a.ldo + a.col0 + n0 + c0 + col) = r;
-            }
-          } else {  // pool == 8
-            warp_colmax_8(v, lane);
-            const int g = lane >> 3, col = static_cast<int>(lane & 7u) * 4;
-            if (col < cw && p0 + warp * 32 + g * 8 < a.rows) {
-              float4 r;
-              r.x = v[0] + __ldg(bias_t + n0 + c0 + col);
-              r.y = v[1] + __ldg(bias_t + n0 + c0 + col + 1);
-              r.z = v[2] + __ldg(bias_t + n0 + c0 + col + 2);
-              r.w = v[3] + __ldg(bias_t + n0 + c0 + col + 3);
-              if (a.relu) {
-                r.x = fmaxf(r.x, 0.f); r.y = fmaxf(r.y, 0.f); r.z = fmaxf(r.z, 0.f); r.w = fmaxf(r.w, 0.f);
-              }
-              if (a.round_out) {
-                r.x = to_tf32(r.x); r.y = to_tf32(r.y); r.z = to_tf32(r.z); r.w = to_tf32(r.w);
-              }
-              *reinterpret_cast<float4 *>(a.out + (grow0 + g) * a.ldo + a.col0 + n0 + c0 + col) = r;
-            }
-          }
         }
       }
       mbar_arrive(&ctl.acc_empty);  // the accumulator tile may be overwritten
@@ -996,7 +801,7 @@ size_t mlp_layout(MlpArgs &a) {
   return mlp_smem_front(stages, a.bn, a.acc_ld) + kMlpEpiWarps * 4096 + sizeof(MlpSmemCtl);
 }
 
-template <int PRO, int EPI>
+template <int EPI>
 int launch_mlp(MlpArgs &a, cudaStream_t st) {
   if (a.rows <= 0) return PVN3D_OK;
   if (a.k_pad <= 0 || a.k_pad % 32 || a.n_pad <= 0 || a.n_pad % 16 || (reinterpret_cast<uintptr_t>(a.w) & 15u))
@@ -1005,13 +810,13 @@ int launch_mlp(MlpArgs &a, cudaStream_t st) {
   if (!smem) return PVN3D_ERR_UNSUPPORTED;
   if (!weight_tensor_map(&a.tmap, a.w, a.k_pad, a.n_pad, a.bn)) return PVN3D_ERR_UNSUPPORTED;
   const long long tiles = ((a.rows + kMlpBM - 1) / kMlpBM) * ceil_div(a.n_pad, a.bn);
-  return launch_persistent<mlp_layer_kernel<PRO, EPI>>(a, tiles, kMlpThreads, smem, a.reserve_sms, st, "mlp_layer_kernel");
+  return launch_persistent<mlp_layer_kernel<EPI>>(a, tiles, kMlpThreads, smem, a.reserve_sms, st, "mlp_layer_kernel");
 }
 
 // =====================================================================================================
 // The dense layer with BF16 operands: the DenseFusion and head layers of FusedHeads at precision "bf16".
 //
-// mlp_layer_kernel<PRO_DENSE, EPI> with the same roles, ring, barriers and accumulator tile, and three differences:
+// mlp_layer_kernel<EPI> with the same roles, ring, barriers and accumulator tile, and three differences:
 //   * a K chunk is 64 bf16 (one 128-byte SWIZZLE_128B row segment), so k_pad is a multiple of 64.  The weights
 //     ([n_pad][k_pad] bf16) arrive by TMA, the activation rows (bf16 already, a_cols a multiple of 8) by cp.async;
 //   * the MMAs are wgmma m64nNk16 with bf16 operands and fp32 accumulators, N = BN = mma_n(n_pad) a template parameter
@@ -1231,19 +1036,18 @@ int launch_mlp_bf16(MlpArgs &a, cudaStream_t st) {
 // =====================================================================================================
 // Layers 2 and 3 of a FACTORED SA scale and the max-pool over nsample in ONE persistent kernel.
 //
-// As two launches (pvn3d_mlp_sa_fact with ROUND_OUT, then pvn3d_mlp_dense with pool = ns) the TF32-rounded
-// layer-2 activations H go to HBM and straight back: 67-400 MB per scale and 32-frame batch, far more than
-// L2 holds.  Here they never leave the SM.  Per 128-row tile (whole centres: 128 % ns == 0):
-//   producers (warps 0-7)  stage A1 = tf32(relu(U[idx] - V)) into a ring of K-chunk stages, exactly as the
-//                          PRO_SA_FACT producer of mlp_layer_kernel, running ahead across tiles;
+// As separate launches the TF32-rounded layer-2 activations H would go to HBM and straight back: 67-400 MB per scale
+// and 32-frame batch, far more than L2 holds.  Here they never leave the SM.  Per 128-row tile (whole centres):
+//   producers (warps 0-7)  stage A1 = tf32(relu(U[idx] - V)) into a ring of K-chunk stages (stage_a_chunk<PRO_SA_FACT>),
+//                          running ahead across tiles;
 //   MMA       (warps 8-15) warpgroup wg accumulates rows 64wg..64wg+63 of layer 2 in registers (W2 resident in
 //                          shared memory), writes tf32(relu(acc + b2)) into ITS 64 rows of a K-major SWIZZLE_128B
 //                          H tile, runs layer 3 from that tile (W3 resident), and pools the layer-3 fragment in
 //                          registers: max over the 16 rows of a warp by a transposing shuffle butterfly (a
 //                          32-row centre combines two warps through shared memory), then + b3, ReLU, rounding
 //                          and the store into the column slice col0.. of the level table.
-// Same operands, the same wgmma N and K order per output element and the same epilogue arithmetic as the two
-// launches, so the results are bit-identical (max commutes with the bias add: rounding is monotone).
+// Same operands, wgmma N, K order and epilogue arithmetic as mlp_layer_kernel on A1, then on H: bit-identical to those
+// two layers followed by a max over nsample (the max commutes with the bias add, ReLU and rounding: all monotone).
 constexpr int kSa2Threads = (kMlpProWarps + kMlpMmaWarps) * 32;
 constexpr int kSa2MaxStages = 8;
 constexpr uint32_t kSa2StageBytes = kMlpBM * 128u;   // one A chunk: 128 rows x 32 tf32
@@ -1431,7 +1235,7 @@ __global__ void __launch_bounds__(kSa2Threads, 1) mlp_sa_fact2_kernel(const __gr
         if (static_cast<unsigned>(it & 1) != grp) continue;
         const int s = static_cast<int>(it % S);
         mbar_wait(&ctl.empty[s], static_cast<unsigned>(((it / S) & 1) ^ 1));
-        stage_a_chunk<PRO_SA_FACT>(a, rs, p_first, r_first, sub, kc * 32, base + L.ring + static_cast<uint32_t>(s) * kSa2StageBytes,
+        stage_a_chunk<PRO_SA_FACT>(a, rs, r_first, sub, kc * 32, base + L.ring + static_cast<uint32_t>(s) * kSa2StageBytes,
                                    true);
         fence_proxy_async_smem();
         mbar_arrive(&ctl.full[s]);
@@ -1564,8 +1368,7 @@ int launch_sa_fact2_n3(Sa2Args &g, int stages, cudaStream_t st) {
 // for 256 / 512 output columns neither fits (W3 of SA3 alone is 229 KB).  Here the weights STREAM and both layers
 // run in 128-column blocks, so a thread never holds more than one 64 x 128 fragment.  Per 64-row tile (whole
 // centres: 64 % ns == 0):
-//   producers (warps 0-3)   stage A = tf32(relu(U[idx] - V)) ONCE into a resident A tile (all layer-2 K chunks),
-//                           with the PRO_SA_FACT producer of the per-layer kernel;
+//   producers (warps 0-3)   stage A = tf32(relu(U[idx] - V)) ONCE into a resident A tile (stage_a_chunk<PRO_SA_FACT>);
 //   loader    (warp 12)     streams 32-column K chunks of W2 and W3 (128 output columns each) by TMA through a ring,
 //                           in the order the warpgroups consume them;
 //   MMA       (warps 4-11)  both warpgroups work on the same 64 rows; warpgroup wg takes the column blocks
@@ -1575,7 +1378,7 @@ int launch_sa_fact2_n3(Sa2Args &g, int stages, cudaStream_t st) {
 //                           32-row centre combines two warps through shared memory), + b3, ReLU, rounding, store.
 // The chunks of the two blocks a warpgroup pair works on are interleaved in the ring, so both warpgroups draw
 // from it at once.  Every output column keeps the per-layer kernel's operands, wgmma N (128) and K order, so the
-// results are bit-identical to pvn3d_mlp_sa_fact + pvn3d_mlp_dense(pool = ns).
+// results are bit-identical to mlp_layer_kernel on the rows A, then on H, followed by a max over nsample.
 constexpr int kSa2wBM = 64;
 constexpr int kSa2wProWarps = 4;
 constexpr int kSa2wLoaderWarp = kSa2wProWarps + kMlpMmaWarps;   // warp 12
@@ -1689,7 +1492,7 @@ __global__ void __launch_bounds__(kSa2wThreads, 1) mlp_sa_fact2w_kernel(const __
       rows_setup<PRO_SA_FACT>(a, p_first, rs);
       mbar_wait(&ctl.a_empty, static_cast<unsigned>((j & 1) ^ 1));   // the previous tile's layer 2 is done
       for (int kc = kc_first; kc < kc2; kc += 2) {
-        stage_a_chunk<PRO_SA_FACT>(a, rs, p_first, r_first, sub, kc * 32, base + L.a + static_cast<uint32_t>(kc) * kSa2wChunk,
+        stage_a_chunk<PRO_SA_FACT>(a, rs, r_first, sub, kc * 32, base + L.a + static_cast<uint32_t>(kc) * kSa2wChunk,
                                    true);
         fence_proxy_async_smem();
         mbar_arrive(&ctl.a_full[kc]);
@@ -1879,12 +1682,10 @@ int launch_sa_fact2w(Sa2wArgs &g, int stages, cudaStream_t st) {
 // Both layers of an FP module whose first layer reads the interpolated known descriptors and the skip columns (FP2-FP4),
 // in ONE persistent kernel.
 //
-// As two launches (pvn3d_mlp_fp_first with ROUND_OUT, then pvn3d_mlp_dense) every interpolated operand element is
-// produced once per 128-column block of layer 1 (4 times for 512 columns), and the TF32-rounded layer-1 activations H
-// go to HBM and come back once per layer-2 column block (33-67 MB per module and 32-frame batch).  Per 64-row tile:
-//   producers (warps 0-3)   stage A = [tf32(sum_t w_t known[idx_t]) | tf32(skip) | 0] in 64 x 32 K chunks through a ring,
-//                           as the PRO_FP_INTERP producer of the per-layer kernel does (its per-row neighbour indices
-//                           and weights kept in shared memory, not 48 registers); each chunk is read by BOTH
+// As separate layer launches the TF32-rounded layer-1 activations H would go to HBM and come back once per layer-2
+// column block (33-67 MB per module and 32-frame batch).  Per 64-row tile:
+//   producers (warps 0-3)   stage A = [tf32(sum_t w_t known[idx_t]) | tf32(skip) | 0] in 64 x 32 K chunks through a ring
+//                           (fp2_stage_chunk: row state in shared memory, not 48 registers); each chunk is read by BOTH
 //                           warpgroups, so A is produced once per pair of layer-1 column blocks (once for 256 columns,
 //                           twice for 512), running ahead across passes and tiles;
 //   loader    (warp 12)     streams 32-column K chunks of W1 and W2 (128 output columns each) by TMA through a second
@@ -1893,8 +1694,8 @@ int launch_sa_fact2w(Sa2wArgs &g, int stages, cudaStream_t st) {
 //                           of each layer.  Layer 1: wgmma N = 128 over the A chunks, then tf32(relu(acc + b1)) into
 //                           the block's columns of a K-major SWIZZLE_128B H tile; layer 2: the same from the H tile,
 //                           relu(acc + b2) [rounded with ROUND_OUT] stored point-major, 32-byte row segments per quad.
-// A thread never holds more than one 64 x 128 fragment.  Every output element keeps the per-layer kernels' operands,
-// wgmma N (128), K order and epilogue arithmetic, so the results are bit-identical to the two launches.
+// A thread never holds more than one 64 x 128 fragment.  Every output element keeps the per-layer kernel's operands,
+// wgmma N (128), K order and epilogue arithmetic: bit-identical to mlp_layer_kernel on A (ROUND_OUT), then on H.
 constexpr int kFp2BM = 64;
 constexpr int kFp2ProWarps = 4;   // two pairs, a pair stages one 64-row A chunk (more warps: under 128 registers, spills)
 constexpr int kFp2Pairs = kFp2ProWarps / 2;
@@ -1953,8 +1754,8 @@ __device__ __forceinline__ int4 lds128i(uint32_t addr) {
   return v;
 }
 
-// stage_a_chunk<PRO_FP_INTERP> with the row state read from shared memory (fp2_rows_store): the same loads, the same
-// contraction fma(p3,w3, fma(p1,w1, p2*w2)), the same TF32 rounding and zeros -- the same bits in the A chunk
+// K chunk k0 / 32 of the producer's 8 rows of A = [interpolated known | skip | 0], row state from shared memory
+// (fp2_rows_store): three_interpolate's fma(p3,w3, fma(p1,w1, p2*w2)) (pn2_ops.cu), TF32 rounding, dead rows zero
 __device__ __forceinline__ void fp2_stage_chunk(const MlpArgs &a, uint32_t rst, long long p_first, int r_first, int sub,
                                                 int k0, uint32_t sa, bool vec_ok) {
   const int k = k0 + 4 * sub;
@@ -2157,7 +1958,7 @@ __global__ void __launch_bounds__(kFp2Threads, 1) mlp_fp2_kernel(const __grid_co
         itw += 2 * kc1;
         // both warpgroups have finished the previous tile's layer 2 (its reads of H)
         if (pp == 0) named_bar_sync(1, 2 * 128);
-        // H[row, c] = tf32(relu(acc + b1[c])): the epilogue of pvn3d_mlp_fp_first with RELU | ROUND_OUT
+        // H[row, c] = tf32(relu(acc + b1[c])): the epilogue of mlp_layer_kernel with RELU | ROUND_OUT
 #pragma unroll
         for (int jj = 0; jj < 16; ++jj) {
           const int c = 128 * nb + 8 * jj + 2 * static_cast<int>(lane & 3u);
@@ -2241,7 +2042,7 @@ int launch_fp2(Fp2Args &g, cudaStream_t st) {
 // The skip term and the second layer of a FACTORED FP module whose skip is the SA1 factor table (FP1), in ONE
 // persistent kernel.
 //
-// As two launches (pvn3d_mlp_dense for S = W1s . table + b1, then pvn3d_mlp_fp_fact) S goes to HBM and
+// As separate launches (S = W1s . table + b1, then layer 2 on relu(interpolated P + S)) S would go to HBM and
 // straight back: 201 + 201 MB per 32-frame batch of 12288 points.  Here it never leaves the SM.  Per 64-row tile:
 //   loader    (warp 16)     brings W_s and W2 into shared memory once (TMA), then the tile's 32-column table rows by
 //                           TMA (SWIZZLE_128B: the wgmma layout) into a ring slot;
@@ -2254,8 +2055,8 @@ int launch_fp2(Fp2Args &g, cudaStream_t st) {
 //                           tile (W2 resident, K 0..127), the slot released, relu(acc + b2) stored channel-major
 //                           [b][128][n_unknown] from the fragment: the 8 rows of a lane quad are 8 consecutive points,
 //                           whole 32-byte sectors of one channel.
-// Every output element keeps the operands, the wgmma shape, K order and epilogue arithmetic of the two launches, so
-// the results are bit-identical to their point-major rows, transposed.
+// Every output element keeps the operands, wgmma shape, K order and epilogue arithmetic of mlp_layer_kernel for S and
+// for layer 2 on the rows relu(interp + S): bit-identical to those point-major rows, transposed.
 // Where the layer-2 output goes (the kernel's template parameter):
 //   FPF2_OUT_CN    [b][128][n_unknown] channel-major, streaming stores: the layout Pointnet2MSG.forward returns,
 //                  written from the fragment with no transposing pass;
@@ -2312,7 +2113,7 @@ int fpf2_stages(int ks_pad, int ns_pad, int k2_pad, int n2_pad) {
   return stages >= 2 ? stages : 0;
 }
 
-// K chunk k0 / 32 of the producer's 8 rows: sum_t w_t P[idx_t] with the contraction of stage_a_chunk<PRO_FP_FACT>,
+// K chunk k0 / 32 of the producer's 8 rows: sum_t w_t P[idx_t] with the contraction of three_interpolate (pn2_ops.cu),
 // fma(p3,w3, fma(p1,w1, p2*w2)), stored unrounded (the MMA warpgroup adds S, applies the ReLU and rounds); dead rows 0
 __device__ __forceinline__ void fpf2_stage_chunk(const MlpArgs &a, uint32_t rst, int r_first, int sub, int k0, uint32_t sa) {
   const float *kf = a.known_feat + k0 + 4 * sub;
@@ -2424,7 +2225,7 @@ __global__ void __launch_bounds__(kFpf2Threads, 1) mlp_fp_fact2_kernel(const __g
         wgmma_wait<0>();
         acc_fence(d);
       }
-      // ---- the layer-2 operand in place: tf32(relu(interp + (S + b1))), the producer of pvn3d_mlp_fp_fact
+      // ---- the layer-2 operand in place: tf32(relu(interp + (S + b1))), one plain add, as the dense producer rounds
       const long long r0 = static_cast<long long>(tile) * kFpf2BM + frag_row;
       const bool on0 = r0 < a.rows, on1 = r0 + 8 < a.rows;
       mbar_wait(&ctl.a_full[s], par);
@@ -2991,7 +2792,7 @@ static bool layer_ptrs_ok(const pvn3d_mlp_layer_t *l) {
 }
 
 // the operand checks and kernel arguments of a layer on relu(U[idx] - V), the second of a factored SA scale
-// (pvn3d_mlp_sa_fact, pvn3d_mlp_sa_fact2, pvn3d_mlp_sa_fact2w): PVN3D_ERR_INVALID_ARG for a bad operand, then
+// (pvn3d_mlp_sa_fact2, pvn3d_mlp_sa_fact2w): PVN3D_ERR_INVALID_ARG for a bad operand, then
 // PVN3D_ERR_UNSUPPORTED for sizes beyond the kernels' 32-bit row arithmetic
 static int sa_fact_args(const float *u, const float *v, int ldu, int c_valid, const int *idx, int b, int n, int m, int ns,
                         const pvn3d_mlp_layer_t &layer, int flags, float *out, int ldo, int col0, MlpArgs &a) {
@@ -3012,8 +2813,7 @@ static int sa_fact_args(const float *u, const float *v, int ldu, int c_valid, co
   return PVN3D_OK;
 }
 
-// the same for a layer on [interpolated known descriptors | skip], the first of an FP module (pvn3d_mlp_fp_first,
-// pvn3d_mlp_fp2)
+// the same for a layer on [interpolated known descriptors | skip], the first of an FP module (pvn3d_mlp_fp2)
 static int fp_interp_args(const float *known_feat_pm, int c2, const int *nn_idx, const float *nn_w, const float *skip_pm,
                           int lds, int c1, int b, int n_unknown, int m_known, const pvn3d_mlp_layer_t &layer, int flags,
                           float *out, int ldo, int col0, MlpArgs &a) {
@@ -3031,36 +2831,26 @@ static int fp_interp_args(const float *known_feat_pm, int c2, const int *nn_idx,
   return PVN3D_OK;
 }
 
-extern "C" int pvn3d_mlp_dense(const float *a, int lda, int a_cols, long long rows, const float *w,
-                               const float *bias, int k_pad, int n_pad, int flags, int pool,
-                               float *out, int ldo, int col0, pvn3d_stream_t stream) {
-  if (!a || !w || !bias || !out || lda < a_cols || a_cols < 0 || a_cols % 4 || rows < 0 || ldo % 4 ||
-      col0 % 4)
+// the argument checks and kernel arguments the three TF32 dense entry points share: PVN3D_ERR_INVALID_ARG for a bad
+// operand, before any CUDA call
+static int dense_args(const float *a, int lda, int a_cols, long long rows, const float *w, const float *bias, int k_pad,
+                      int n_pad, int flags, float *out, int ldo, int col0, MlpArgs &m) {
+  if (!a || !w || !bias || !out || lda < a_cols || a_cols < 0 || a_cols % 4 || rows < 0 || ldo % 4 || col0 % 4)
     return PVN3D_ERR_INVALID_ARG;
-  if (pool && rows % pool) return PVN3D_ERR_INVALID_ARG;
-  MlpArgs m{};
   m.w = w; m.bias = bias; m.rows = rows; m.k_pad = k_pad; m.n_pad = n_pad;
   m.a = a; m.lda = lda; m.a_cols = a_cols;
   m.out = out; m.ldo = ldo; m.col0 = col0;
   m.relu = flags & PVN3D_MLP_RELU; m.round_out = (flags & PVN3D_MLP_ROUND_OUT) ? 1 : 0;
   m.a_tf32 = (flags & PVN3D_MLP_A_TF32) ? 1 : 0;
   m.reserve_sms = (flags >> 8) & 0xff;
-  if (!pool) return launch_mlp<PRO_DENSE, EPI_STORE>(m, as_stream(stream));
-  if (pool != 8 && pool != 16 && pool != 32) return PVN3D_ERR_UNSUPPORTED;
-  m.pool = pool;
-  return launch_mlp<PRO_DENSE, EPI_MAXPOOL>(m, as_stream(stream));
+  return PVN3D_OK;
 }
 
-extern "C" int pvn3d_mlp_fp_first(const float *known_feat_pm, int c2, const int *nn_idx,
-                                  const float *nn_w, const float *skip_pm, int lds, int c1, int b,
-                                  int n_unknown, int m_known, const float *w, const float *bias,
-                                  int k_pad, int n_pad, int flags, float *out, int ldo, int col0,
-                                  pvn3d_stream_t stream) {
-  MlpArgs a{};
-  const int rc = fp_interp_args(known_feat_pm, c2, nn_idx, nn_w, skip_pm, lds, c1, b, n_unknown, m_known,
-                                pvn3d_mlp_layer_t{w, bias, k_pad, n_pad}, flags, out, ldo, col0, a);
-  if (rc != PVN3D_OK) return rc;
-  return launch_mlp<PRO_FP_INTERP, EPI_STORE>(a, as_stream(stream));
+extern "C" int pvn3d_mlp_dense(const float *a, int lda, int a_cols, long long rows, const float *w, const float *bias,
+                               int k_pad, int n_pad, int flags, float *out, int ldo, int col0, pvn3d_stream_t stream) {
+  MlpArgs m{};
+  const int rc = dense_args(a, lda, a_cols, rows, w, bias, k_pad, n_pad, flags, out, ldo, col0, m);
+  return rc != PVN3D_OK ? rc : launch_mlp<EPI_STORE>(m, as_stream(stream));
 }
 
 extern "C" int pvn3d_three_nn_weights(const float *dist2, long long rows, float *weight,
@@ -3093,16 +2883,6 @@ extern "C" int pvn3d_sa_centre_term(const float *centres, const float *wx, const
   sa_centre_term_kernel<<<static_cast<unsigned>((rows + 7) / 8), block, 0, as_stream(stream)>>>(centres, wx, bias, rows,
                                                                                                n_pad, out);
   return check_launch("sa_centre_term_kernel");
-}
-
-extern "C" int pvn3d_mlp_sa_fact(const float *u, const float *v, int ldu, int c_valid, const int *idx, int b, int n,
-                                 int m, int ns, const float *w, const float *bias, int k_pad, int n_pad, int flags,
-                                 float *out, int ldo, int col0, pvn3d_stream_t stream) {
-  MlpArgs a{};
-  const int rc = sa_fact_args(u, v, ldu, c_valid, idx, b, n, m, ns, pvn3d_mlp_layer_t{w, bias, k_pad, n_pad}, flags, out,
-                              ldo, col0, a);
-  if (rc != PVN3D_OK) return rc;
-  return launch_mlp<PRO_SA_FACT, EPI_STORE>(a, as_stream(stream));
 }
 
 // the argument checks and kernel arguments pvn3d_mlp_sa_fact2 (G = Sa2Args) and pvn3d_mlp_sa_fact2w (Sa2wArgs) share
@@ -3178,25 +2958,6 @@ extern "C" int pvn3d_mlp_fp2_supported(const pvn3d_mlp_layer_t *layer1, const pv
   return fp2_stages(layer1->k_pad, layer1->n_pad, layer2->k_pad, layer2->n_pad, &a_stages, &w_stages) ? 1 : 0;
 }
 
-extern "C" int pvn3d_mlp_fp_fact(const float *p, const float *s, int ld, int c_valid, const int *nn_idx,
-                                 const float *nn_w, int b, int n_unknown, int m_known, const float *w,
-                                 const float *bias, int k_pad, int n_pad, int flags, float *out, int ldo, int col0,
-                                 pvn3d_stream_t stream) {
-  if (!p || !s || !nn_idx || !nn_w || !w || !bias || !out || b < 0 || n_unknown < 0 || m_known <= 0 || c_valid <= 0 ||
-      c_valid % 4 || ld != c_valid || k_pad < c_valid || ldo % 4 || col0 % 4 || (reinterpret_cast<uintptr_t>(p) & 15u) ||
-      (reinterpret_cast<uintptr_t>(s) & 15u))
-    return PVN3D_ERR_INVALID_ARG;
-  if (static_cast<long long>(b) * m_known > 0x7fffffffll || n_unknown > 0x3fffffff) return PVN3D_ERR_UNSUPPORTED;
-  MlpArgs a{};
-  a.w = w; a.bias = bias; a.rows = static_cast<long long>(b) * n_unknown; a.k_pad = k_pad; a.n_pad = n_pad;
-  a.known_feat = p; a.c2 = ld; a.nn_idx = nn_idx; a.nn_w = nn_w; a.skip = s; a.lds = ld; a.c1 = 0;
-  a.n_unknown = n_unknown; a.m_known = m_known;
-  a.out = out; a.ldo = ldo; a.col0 = col0;
-  a.relu = flags & PVN3D_MLP_RELU; a.round_out = (flags & PVN3D_MLP_ROUND_OUT) ? 1 : 0;
-  a.reserve_sms = (flags >> 8) & 0xff;
-  return launch_mlp<PRO_FP_FACT, EPI_STORE>(a, as_stream(stream));
-}
-
 // the argument checks and kernel arguments pvn3d_mlp_fp_fact2 and pvn3d_mlp_fp_fact2_rows share
 static int fp_fact2_args(const float *p, const float *table, const int *nn_idx, const float *nn_w, int b, int n_unknown,
                          int m_known, const pvn3d_mlp_layer_t *layer_s, const pvn3d_mlp_layer_t *layer2, int flags,
@@ -3265,34 +3026,23 @@ extern "C" int pvn3d_mlp_fp_fact2_supported(const pvn3d_mlp_layer_t *layer_s, co
 extern "C" int pvn3d_mlp_dense_frame_bias(const float *a, int lda, int a_cols, long long rows, int rows_per_frame,
                                           const float *w, const float *bias, int k_pad, int n_pad, int flags,
                                           float *out, int ldo, int col0, pvn3d_stream_t stream) {
-  if (!a || !w || !bias || !out || lda < a_cols || a_cols < 0 || a_cols % 4 || rows < 0 || ldo % 4 || col0 % 4 ||
-      rows_per_frame <= 0 || rows_per_frame % kMlpBM || rows % rows_per_frame)
-    return PVN3D_ERR_INVALID_ARG;
+  if (rows_per_frame <= 0 || rows_per_frame % kMlpBM || rows % rows_per_frame) return PVN3D_ERR_INVALID_ARG;
   MlpArgs m{};
-  m.w = w; m.bias = bias; m.rows = rows; m.k_pad = k_pad; m.n_pad = n_pad;
-  m.a = a; m.lda = lda; m.a_cols = a_cols;
-  m.out = out; m.ldo = ldo; m.col0 = col0;
-  m.relu = flags & PVN3D_MLP_RELU; m.round_out = (flags & PVN3D_MLP_ROUND_OUT) ? 1 : 0;
-  m.a_tf32 = (flags & PVN3D_MLP_A_TF32) ? 1 : 0;
-  m.reserve_sms = (flags >> 8) & 0xff;
+  const int rc = dense_args(a, lda, a_cols, rows, w, bias, k_pad, n_pad, flags, out, ldo, col0, m);
+  if (rc != PVN3D_OK) return rc;
   m.bias_npb = rows_per_frame;
-  return launch_mlp<PRO_DENSE, EPI_STORE>(m, as_stream(stream));
+  return launch_mlp<EPI_STORE>(m, as_stream(stream));
 }
 
 extern "C" int pvn3d_mlp_dense_sum32(const float *a, int lda, int a_cols, long long rows, const float *w,
                                      const float *bias, int k_pad, int n_pad, int flags, float *out, int ldo,
                                      int col0, pvn3d_stream_t stream) {
-  if (!a || !w || !bias || !out || lda < a_cols || a_cols < 0 || a_cols % 4 || rows < 0 || ldo % 4 || col0 % 4)
-    return PVN3D_ERR_INVALID_ARG;
   MlpArgs m{};
-  m.w = w; m.bias = bias; m.rows = rows; m.k_pad = k_pad; m.n_pad = n_pad;
-  m.a = a; m.lda = lda; m.a_cols = a_cols;
-  m.out = out; m.ldo = ldo; m.col0 = col0;
-  m.relu = 1;
-  m.a_tf32 = (flags & PVN3D_MLP_A_TF32) ? 1 : 0;
-  m.reserve_sms = (flags >> 8) & 0xff;
+  const int rc = dense_args(a, lda, a_cols, rows, w, bias, k_pad, n_pad, flags, out, ldo, col0, m);
+  if (rc != PVN3D_OK) return rc;
+  m.relu = 1; m.round_out = 0;   // sums of relu(row), stored unrounded
   m.pool = 32;
-  return launch_mlp<PRO_DENSE, EPI_SUMPOOL>(m, as_stream(stream));
+  return launch_mlp<EPI_SUMPOOL>(m, as_stream(stream));
 }
 
 // ---- BF16 forms (FusedHeads at precision "bf16") ------------------------------------------------------------------------

@@ -55,7 +55,7 @@ int ref_opt_n_threads(int work_size) {
 
 extern "C" {
 
-int pvn3d_version(void) { return 1; }
+int pvn3d_version(void) { return 2; }
 
 unsigned long long pvn3d_launch_count(void) {
   return __atomic_load_n(&pvn3d::g_launches, __ATOMIC_RELAXED);

@@ -51,7 +51,7 @@ def _dense(a_ptr: int, lda: int, a_cols: int, rows: int, layer: PackedLayer, out
              layer.n_pad, _out_flags(relu, out), ptr(out), out.size(-1), col0)
         return out
     call("pvn3d_mlp_dense", out.device, a_ptr, lda, a_cols, rows, ptr(layer.w), ptr(layer.bias), layer.k_pad, layer.n_pad,
-         _flags(relu, round_out, a_tf32), 0, ptr(out), out.size(-1), col0)
+         _flags(relu, round_out, a_tf32), ptr(out), out.size(-1), col0)
     return out
 
 

@@ -90,25 +90,15 @@ def _flags(relu, round_out=False, a_tf32=False, reserve=0):
             | ((int(reserve) & 0xFF) << 8))
 
 
-def mlp_dense(a2d: torch.Tensor, layer: PackedLayer, relu=True, pool=0, out=None, col0=0, round_out=False,
-              a_tf32=False, reserve=0):
+def mlp_dense(a2d: torch.Tensor, layer: PackedLayer, relu=True, out=None, col0=0, round_out=False, a_tf32=False,
+              reserve=0):
     """a2d [rows, lda] point-major activations (all lda columns valid or zero).  a_tf32: a2d came out of
     a layer run with round_out=True (values already TF32) -> asynchronous copy path."""
     rows, lda = a2d.shape
     if out is None:
-        out = torch.empty((rows // pool if pool else rows, layer.n_pad), dtype=torch.float32, device=a2d.device)
+        out = torch.empty((rows, layer.n_pad), dtype=torch.float32, device=a2d.device)
     call("pvn3d_mlp_dense", a2d.device, ptr(a2d), lda, lda, rows, ptr(layer.w), ptr(layer.bias), layer.k_pad, layer.n_pad,
-         _flags(relu, round_out, a_tf32, reserve), pool, ptr(out), out.size(-1), col0)
-    return out
-
-
-def mlp_fp_first(known_feat_pm, nn_idx, nn_w, skip_ptr, lds, c1, layer: PackedLayer, relu=True, round_out=False, reserve=0):
-    b, m_known, c2 = known_feat_pm.shape
-    n_unknown = nn_idx.shape[1]
-    out = torch.empty((b * n_unknown, layer.n_pad), dtype=torch.float32, device=known_feat_pm.device)
-    call("pvn3d_mlp_fp_first", known_feat_pm.device, ptr(known_feat_pm), c2, ptr(nn_idx), ptr(nn_w), skip_ptr, lds, c1, b,
-         n_unknown, m_known, ptr(layer.w), ptr(layer.bias), layer.k_pad, layer.n_pad, _flags(relu, round_out, reserve=reserve),
-         ptr(out), out.size(-1), 0)
+         _flags(relu, round_out, a_tf32, reserve), ptr(out), out.size(-1), col0)
     return out
 
 
@@ -131,8 +121,8 @@ def fp2_fits(layer1: PackedLayer, layer2: PackedLayer) -> bool:
 
 def mlp_fp2(known_feat_pm, nn_idx, nn_w, skip_ptr, lds, c1, layer1: PackedLayer, layer2: PackedLayer, out=None, col0=0,
             round_out=False, reserve=0):
-    """both layers of an FP module in one launch (pvn3d_mlp_fp2): the same bits as
-    mlp_fp_first(.., layer1, round_out=True) -> mlp_dense(.., layer2, a_tf32=True, round_out=round_out)"""
+    """both layers of an FP module in one launch (pvn3d_mlp_fp2): the same bits as mlp_dense(rows, layer1, round_out=True)
+    -> mlp_dense(.., layer2, a_tf32=True, round_out=round_out) on the rows [three_interpolate(known) | skip[:, :c1] | 0]"""
     b, m_known, c2 = known_feat_pm.shape
     n_unknown = nn_idx.shape[1]
     if out is None:
@@ -162,17 +152,6 @@ def sa_centre_term(new_xyz: torch.Tensor, wx: torch.Tensor, bias: torch.Tensor) 
     return out
 
 
-def mlp_sa_fact(u: torch.Tensor, v: torch.Tensor, idx: torch.Tensor, n: int, layer: PackedLayer, relu=True, out=None,
-                col0=0, round_out=False, reserve=0):
-    """second layer of a factored SA scale: rows relu(U[idx] - V) -> layer (pvn3d_mlp_sa_fact)"""
-    b, m, ns = idx.shape
-    if out is None:
-        out = torch.empty((b * m * ns, layer.n_pad), dtype=torch.float32, device=u.device)
-    call("pvn3d_mlp_sa_fact", u.device, ptr(u), ptr(v), u.size(-1), u.size(-1), ptr(idx), b, n, m, ns, ptr(layer.w),
-         ptr(layer.bias), layer.k_pad, layer.n_pad, _flags(relu, round_out, reserve=reserve), ptr(out), out.size(-1), col0)
-    return out
-
-
 def sa_fact2_fits(layer2: PackedLayer, layer3: PackedLayer, ns: int) -> bool:
     """whether pvn3d_mlp_sa_fact2 takes the scale (the library's own rule: nsample 16 or 32, both layers at most 128
     columns, weights + layer-2 tile within shared memory -- SA1 and SA2)"""
@@ -198,7 +177,8 @@ def _sa_fact2_call(fn_name: str, u: torch.Tensor, v: torch.Tensor, idx: torch.Te
 
 def mlp_sa_fact2(u, v, idx, n, layer2, layer3, out=None, col0=0, round_out=False, reserve=0):
     """layers 2 and 3 of a factored SA scale + max-pool over nsample in one launch (pvn3d_mlp_sa_fact2): the same bits
-    as mlp_sa_fact(.., layer2, round_out=True) -> mlp_dense(.., layer3, pool=ns, a_tf32=True)"""
+    as mlp_dense(relu(U[idx] - V), layer2, round_out=True) -> mlp_dense(.., layer3, a_tf32=True), then the max over the
+    nsample rows of each centre"""
     return _sa_fact2_call("pvn3d_mlp_sa_fact2", u, v, idx, n, layer2, layer3, out, col0, round_out, reserve)
 
 
@@ -206,19 +186,6 @@ def mlp_sa_fact2w(u, v, idx, n, layer2, layer3, out=None, col0=0, round_out=Fals
     """mlp_sa_fact2 for a wide last layer (pvn3d_mlp_sa_fact2w: weights streamed, both layers in 128-column blocks),
     with the same arguments and the same bits"""
     return _sa_fact2_call("pvn3d_mlp_sa_fact2w", u, v, idx, n, layer2, layer3, out, col0, round_out, reserve)
-
-
-def mlp_fp_fact(p: torch.Tensor, s_: torch.Tensor, nn_idx: torch.Tensor, nn_w: torch.Tensor, m_known: int,
-                layer: PackedLayer, relu=True, round_out=False, reserve=0):
-    """second layer of a factored FP module: rows relu(sum_t w_t P[idx_t] + S) -> layer (pvn3d_mlp_fp_fact),
-    [b * n_unknown, n_pad]"""
-    b, n_unknown = nn_idx.shape[0], nn_idx.shape[1]
-    ld = p.size(-1)
-    out = torch.empty((b * n_unknown, layer.n_pad), dtype=torch.float32, device=p.device)
-    call("pvn3d_mlp_fp_fact", p.device, ptr(p), ptr(s_), ld, ld, ptr(nn_idx), ptr(nn_w), b, n_unknown, m_known,
-         ptr(layer.w), ptr(layer.bias), layer.k_pad, layer.n_pad, _flags(relu, round_out, reserve=reserve), ptr(out),
-         layer.n_pad, 0)
-    return out
 
 
 def fp_fact2_fits(layer_s: PackedLayer, layer2: PackedLayer) -> bool:
@@ -230,8 +197,8 @@ def fp_fact2_fits(layer_s: PackedLayer, layer2: PackedLayer) -> bool:
 def mlp_fp_fact2(p: torch.Tensor, table: torch.Tensor, nn_idx: torch.Tensor, nn_w: torch.Tensor, m_known: int,
                  layer_s: PackedLayer, layer2: PackedLayer, reserve=0):
     """the skip term and the second layer of a factored FP module in one launch (pvn3d_mlp_fp_fact2) -> [b, 128,
-    n_unknown]: the same bits as mlp_fp_fact(p, mlp_dense(table, layer_s, relu=False, a_tf32=True), .., layer2),
-    transposed per frame"""
+    n_unknown]: the same bits as mlp_dense(relu(three_interpolate(p) + s), layer2) with
+    s = mlp_dense(table, layer_s, relu=False, a_tf32=True), transposed per frame"""
     b, n_unknown = nn_idx.shape[0], nn_idx.shape[1]
     assert p.size(-1) == layer_s.n_pad and table.size(-1) == layer_s.k_pad and table.size(0) == b * n_unknown
     out = torch.empty((b, layer2.n_pad, n_unknown), dtype=torch.float32, device=p.device)

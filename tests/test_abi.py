@@ -29,7 +29,7 @@ def test_binding_table_matches_header():
 
 def test_version_and_strerror():
     lib = _lib.load()
-    assert lib.pvn3d_version() == 1
+    assert lib.pvn3d_version() == 2
     assert lib.pvn3d_strerror(0) == b"ok"
     assert lib.pvn3d_strerror(-2) == b"unsupported size"
 

@@ -1,10 +1,12 @@
 """pvn3d_mlp_fp2 (both layers of a two-layer FP module in one launch: interpolation fused into the operand producer,
-the layer-1 activations kept in shared memory, the weights streamed) against the two launches it replaces:
-pvn3d_mlp_fp_first with ROUND_OUT, then pvn3d_mlp_dense.  Same operands, the same MMA N and K order per output element
-and the same epilogue arithmetic: the results must be identical, bit for bit."""
+the layer-1 activations kept in shared memory, the weights streamed) against the dense layer on the materialised rows
+[three_interpolate(known) | skip | 0]: layer 1 with ROUND_OUT, then layer 2 (mlp_compose.fp2).  Same operands, the
+same MMA N and K order per output element and the same epilogue arithmetic: the results must be identical, bit for
+bit."""
 import pytest
 import torch
 
+import mlp_compose as compose
 from pvn3d_b200 import mlp
 
 pytestmark = pytest.mark.gpu
@@ -24,11 +26,6 @@ def _module(dev, b, n, m, c2, c1, n1, n2, seed, lds=None):
     return known.to(dev), skip.to(dev), nn_idx.to(dev), w.to(dev), lds, l1, l2
 
 
-def _two_launches(known, skip, nn_idx, nn_w, lds, c1, l1, l2, round_out=False, reserve=0):
-    h = mlp.mlp_fp_first(known, nn_idx, nn_w, skip.data_ptr(), lds, c1, l1, round_out=True, reserve=reserve)
-    return mlp.mlp_dense(h, l2, a_tf32=True, round_out=round_out, reserve=reserve)
-
-
 @pytest.mark.parametrize("b,n,m,c2,c1,n1,n2", [
     (32, 512, 128, 1024, 512, 512, 512),     # FP4 at 32 frames: two passes over K, the rings wrap many times
     (32, 1024, 512, 512, 256, 512, 512),     # FP3
@@ -39,30 +36,30 @@ def _two_launches(known, skip, nn_idx, nn_w, lds, c1, l1, l2, round_out=False, r
                                              # three layer-2 blocks: the second warpgroup sits the last one out
 ])
 @pytest.mark.parametrize("reserve", [0, 120])
-def test_fp2_equals_two_launches(cuda_dev, b, n, m, c2, c1, n1, n2, reserve):
+def test_fp2_equals_dense_layers_on_interpolated_rows(cuda_dev, b, n, m, c2, c1, n1, n2, reserve):
     known, skip, nn_idx, nn_w, lds, l1, l2 = _module(cuda_dev, b, n, m, c2, c1, n1, n2, seed=b + n + c2)
     assert mlp.fp2_fits(l1, l2)
-    want = _two_launches(known, skip, nn_idx, nn_w, lds, c1, l1, l2, reserve=reserve)
+    want = compose.fp2(known, skip, nn_idx, nn_w, lds, c1, l1, l2, reserve=reserve)
     got = mlp.mlp_fp2(known, nn_idx, nn_w, skip.data_ptr(), lds, c1, l1, l2, reserve=reserve)
     assert got.shape == want.shape == (b * n, l2.n_pad)
     assert torch.equal(got, want), float((got - want).abs().max())
 
 
-def test_fp2_unaligned_skip_rows_and_rounded_output(cuda_dev):
+def test_fp2_unaligned_skip_rows_equal_dense_layers(cuda_dev):
     """skip rows 4-byte aligned only (lds odd): every skip chunk takes the generic path; ROUND_OUT on the output"""
     known, skip, nn_idx, nn_w, lds, l1, l2 = _module(cuda_dev, 2, 640, 200, 512, 96, 256, 256, seed=5, lds=97)
-    want = _two_launches(known, skip, nn_idx, nn_w, lds, 96, l1, l2, round_out=True)
+    want = compose.fp2(known, skip, nn_idx, nn_w, lds, 96, l1, l2, round_out=True)
     got = mlp.mlp_fp2(known, nn_idx, nn_w, skip.data_ptr(), lds, 96, l1, l2, round_out=True)
     assert torch.equal(got, want)
 
 
-def test_fp2_writes_a_column_slice(cuda_dev):
+def test_fp2_column_slice_equals_dense_layers(cuda_dev):
     b, n, m, c2, c1 = 2, 1000, 300, 512, 256
     known, skip, nn_idx, nn_w, lds, l1, l2 = _module(cuda_dev, b, n, m, c2, c1, 512, 512, seed=17)
     ld, col0 = l2.n_pad + 136, 64
     want = torch.full((b * n, ld), -7.0, device=cuda_dev)
     got = want.clone()
-    want[:, col0:col0 + l2.n_pad] = _two_launches(known, skip, nn_idx, nn_w, lds, c1, l1, l2)
+    want[:, col0:col0 + l2.n_pad] = compose.fp2(known, skip, nn_idx, nn_w, lds, c1, l1, l2)
     mlp.mlp_fp2(known, nn_idx, nn_w, skip.data_ptr(), lds, c1, l1, l2, out=got, col0=col0)
     assert torch.equal(got, want)
 

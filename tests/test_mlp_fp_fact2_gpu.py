@@ -1,10 +1,12 @@
 """pvn3d_mlp_fp_fact2 (the skip term S = W1s . table + b1 and the second layer of a factored FP module in one launch, S
-kept on chip, the output stored channel-major) against the two launches it replaces: pvn3d_mlp_dense without ReLU on the
-SA1 factor table, then pvn3d_mlp_fp_fact, whose point-major rows are transposed per frame.  Same operands, the same MMA shape and K order per output element and the
-same epilogue arithmetic: the results must be identical, bit for bit."""
+kept on chip, the output stored channel-major) against the dense layer without ReLU on the SA1 factor table for S, then
+the dense layer on the materialised rows relu(three_interpolate(P) + S), transposed per frame (mlp_compose.fp_fact2).
+Same operands, the same MMA shape and K order per output element and the same epilogue arithmetic: the results must be
+identical, bit for bit."""
 import pytest
 import torch
 
+import mlp_compose as compose
 from pvn3d_b200 import mlp
 
 pytestmark = pytest.mark.gpu
@@ -27,31 +29,25 @@ def _module(dev, b, n, m, seed, c_feat=6):
     return p, table, nn_idx, nn_w, ls, l2
 
 
-def _two_launches(p, table, nn_idx, nn_w, m, ls, l2, reserve=0):
-    b, n = nn_idx.shape[0], nn_idx.shape[1]
-    s = mlp.mlp_dense(table, ls, relu=False, a_tf32=True, reserve=reserve)
-    pm = mlp.mlp_fp_fact(p, s, nn_idx, nn_w, m, l2, reserve=reserve)
-    return pm.view(b, n, -1).transpose(1, 2).contiguous()
-
-
 @pytest.mark.parametrize("b,n,m", [
     (32, 12288, 2048),   # the bench shape
     (3, 1000, 333),      # frames end inside tiles
     (1, 96, 40),         # one and a half tiles
 ])
 @pytest.mark.parametrize("reserve", [0, 120])
-def test_fp_fact2_equals_transposed_two_launches(cuda_dev, b, n, m, reserve):
+def test_fp_fact2_equals_transposed_dense_layers(cuda_dev, b, n, m, reserve):
     p, table, nn_idx, nn_w, ls, l2 = _module(cuda_dev, b, n, m, seed=b + n + m)
     assert mlp.fp_fact2_fits(ls, l2)
     assert bool((table[:, 6:12] != 0).any())          # the hi / lo coordinate columns take part
-    want = _two_launches(p, table, nn_idx, nn_w, m, ls, l2, reserve=reserve)
+    want = compose.fp_fact2(p, table, nn_idx, nn_w, m, ls, l2, reserve=reserve)
     got = mlp.mlp_fp_fact2(p, table, nn_idx, nn_w, m, ls, l2, reserve=reserve)
     assert got.shape == want.shape == (b, 128, n)
     assert torch.equal(got, want), float((got - want).abs().max())
 
 
-def test_fp_fact2_engine_output_unchanged(cuda_dev):
-    """FusedPointnet2MSG.features: FP1 through the fused launch gives what P -> S -> mlp_fp_fact gives"""
+def test_fp_fact2_engine_output_equals_dense_layers(cuda_dev):
+    """FusedPointnet2MSG.features: FP1 through the fused launch gives what P -> S -> the dense layer on
+    relu(three_interpolate(P) + S) gives"""
     from pvn3d_b200 import synth, testing
 
     host = synth.stack(synth.make_batch("linemod", 2, n_points=3000, config_id=2, lm_obj_id=1))
@@ -73,5 +69,5 @@ def test_fp_fact2_engine_output_unchanged(cuda_dev):
     finally:
         mlp.mlp_fp_fact2 = orig
     assert torch.equal(got, again)
-    want = _two_launches(calls["p"], calls["table"], calls["nn_idx"], calls["nn_w"], calls["m"], ls, l2)
+    want = compose.fp_fact2(calls["p"], calls["table"], calls["nn_idx"], calls["nn_w"], calls["m"], ls, l2)
     assert torch.equal(got, want)

@@ -1,10 +1,12 @@
 """pvn3d_mlp_sa_fact2 (layers 2 and 3 of a factored SA scale + max-pool, the layer-2 activations kept in shared
-memory) against the two launches it replaces: pvn3d_mlp_sa_fact with ROUND_OUT, then pvn3d_mlp_dense with
-pool = nsample.  Same operands, same MMA order per output element: the results must be identical, bit for bit."""
+memory) against the dense layer on the materialised rows relu(U[idx] - V): layer 2 with ROUND_OUT, layer 3, then the
+max over nsample (mlp_compose.sa_fact2).  Same operands, same MMA order per output element: the results must be
+identical, bit for bit."""
 import numpy as np
 import pytest
 import torch
 
+import mlp_compose as compose
 from pvn3d_b200 import mlp
 
 pytestmark = pytest.mark.gpu
@@ -48,24 +50,22 @@ def _factored_scale(dev, b, n, m, ns, c_feat, widths, seed):
     (2, 1024, 300, 32, 6, (256, 32, 64)),
 ])
 @pytest.mark.parametrize("round_out", [False, True])
-def test_sa_fact2_equals_two_launches(cuda_dev, b, n, m, ns, c_feat, widths, round_out):
+def test_sa_fact2_equals_dense_layers_and_max_pool(cuda_dev, b, n, m, ns, c_feat, widths, round_out):
     u, v, idx, l2, l3 = _factored_scale(cuda_dev, b, n, m, ns, c_feat, widths, seed=b + m + ns)
-    h = mlp.mlp_sa_fact(u, v, idx, n, l2, round_out=True)
-    want = mlp.mlp_dense(h, l3, pool=ns, a_tf32=True, round_out=round_out)
+    want = compose.sa_fact2(u, v, idx, n, l2, l3, round_out=round_out)
     got = mlp.mlp_sa_fact2(u, v, idx, n, l2, l3, round_out=round_out)
     assert got.shape == want.shape == (b * m, l3.n_pad)
     assert torch.equal(got, want), float((got - want).abs().max())
 
 
 @pytest.mark.parametrize("ns,c_feat,widths", [(16, 96, (64, 64, 128)), (32, 6, (32, 32, 64))])
-def test_sa_fact2_writes_a_column_slice_of_the_level_table(cuda_dev, ns, c_feat, widths):
+def test_sa_fact2_column_slice_equals_dense_layers(cuda_dev, ns, c_feat, widths):
     b, n, m = 2, 1000, 300
     u, v, idx, l2, l3 = _factored_scale(cuda_dev, b, n, m, ns, c_feat, widths, seed=7 + ns)
     ld, col0 = l3.n_pad + 72, 40
     want = torch.full((b * m, ld), -7.0, device=cuda_dev)
     got = want.clone()
-    h = mlp.mlp_sa_fact(u, v, idx, n, l2, round_out=True)
-    mlp.mlp_dense(h, l3, pool=ns, out=want, col0=col0, a_tf32=True, round_out=True)
+    compose.sa_fact2(u, v, idx, n, l2, l3, round_out=True, out=want, col0=col0)
     mlp.mlp_sa_fact2(u, v, idx, n, l2, l3, out=got, col0=col0, round_out=True)
     assert torch.equal(got, want)
     assert bool((got[:, :col0] == -7.0).all()) and bool((got[:, col0 + l3.n_pad:] == -7.0).all())
