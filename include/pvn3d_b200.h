@@ -778,6 +778,33 @@ int pvn3d_train_loss_backward(const pvn3d_loss_args_t *args, const float *g_loss
                               const float *g_kp, float *d_seg, float *d_kp, float *d_ctr, const void *workspace,
                               size_t workspace_bytes, pvn3d_stream_t stream);
 
+/* ---- pose overlay (csrc/vis.cu): demo.py's mesh drawing, demo.py:122-145 ------------------------------------------ */
+
+/* Stamp plane of the two drawing calls: b*h*w int32, 256-byte aligned; 0 = invalid arguments.  Host only. */
+size_t pvn3d_vis_workspace_bytes(int b, int h, int w);
+
+/* Draw the mesh of every predicted slot into its frame, in place:
+ *   img [b,h,w,3] u8 C-contiguous; mesh_pts [P_total,3] f32 and mesh_off [n_cls+1] i32 on the device
+ *   (eval_utils.pack_meshes), max_pts = the largest mesh's point count; poses [b,n_cls,3,4] f32 (poses_f64 = 0) or f64
+ *   (1); present [b,n_cls] u8; order [b,s] i32 class ids in draw order; k [b,3,3] f64; colors [n_cls,3] u8.
+ * Slot j of frame f draws class c = order[f,j] unless c is outside [1, n_cls) or present[f,c] is 0.  Each mesh point
+ * p (promoted to f64) goes to q = (p . R^T + t) * cam_scale, (u, v, d) = q . K^T (three products summed left to right,
+ * no FMA), d = 1 where d < 1e-8 (NaN stays NaN), x = rint(u / d), y = rint(v / d) converted as numpy does on x86-64
+ * (NaN or outside int32: INT_MIN), clipped to [0, w] and [0, h], and paints the disc dx^2 + dy^2 <= r^2 cut to the
+ * image (cv2.circle(..., -1)).  Where discs of several slots meet, the last slot wins.  Refused: null pointers,
+ * n_cls < 2, s < 1, r < 0 (PVN3D_ERR_INVALID_ARG); b > 65535, s > 65535, r > 32767, h or w >= 65534
+ * (PVN3D_ERR_UNSUPPORTED); a short workspace (PVN3D_ERR_WORKSPACE).  A memset and two launches, no host sync. */
+int pvn3d_vis_draw_poses(uint8_t *img, int b, int h, int w, const float *mesh_pts, const int *mesh_off, int n_cls,
+                         int max_pts, const void *poses, int poses_f64, const uint8_t *present, const int *order, int s,
+                         const double *k, double cam_scale, const uint8_t *colors, int r, void *workspace,
+                         size_t workspace_bytes, pvn3d_stream_t stream);
+
+/* Basic_Utils.draw_p2ds (basic_utils.py:315-323) on one image [h,w,3] u8: p2ds [n,2] i32 on the device are clipped in
+ * place to [0, w] x [0, h] and each paints its disc of radius r in color = c0 | c1 << 8 | c2 << 16 (the three uint8
+ * channels in image order).  n = 0 does nothing.  Refusals as pvn3d_vis_draw_poses.  A memset and two launches. */
+int pvn3d_vis_draw_p2ds(uint8_t *img, int h, int w, int *p2ds, int n, int r, unsigned color, void *workspace,
+                        size_t workspace_bytes, pvn3d_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -142,6 +142,10 @@ _SIGNATURES = {
     "pvn3d_train_loss_workspace_bytes": (c_size_t, [ctypes.POINTER(LossArgs)]),
     "pvn3d_train_loss_forward": (c_int, [ctypes.POINTER(LossArgs), _P, _P, _P, _P, _P, _P, c_size_t, _P]),
     "pvn3d_train_loss_backward": (c_int, [ctypes.POINTER(LossArgs), _P, _P, _P, _P, _P, _P, _P, c_size_t, _P]),
+    "pvn3d_vis_workspace_bytes": (c_size_t, [c_int, c_int, c_int]),
+    "pvn3d_vis_draw_poses": (c_int, [_P, c_int, c_int, c_int, _P, _P, c_int, c_int, _P, c_int, _P, _P, c_int, _P,
+                                     c_double, _P, c_int, _P, c_size_t, _P]),
+    "pvn3d_vis_draw_p2ds": (c_int, [_P, c_int, c_int, _P, c_int, c_int, c_uint, _P, c_size_t, _P]),
 }
 FLAT_MS_MAX_PTS = 4096   # PVN3D_FLAT_MS_MAX_PTS
 EXPORTED_SYMBOLS = tuple(_SIGNATURES)

@@ -24,7 +24,10 @@ What install() does (SURVEY section 8b, App. D):
   6. with patch_loss=True, rebinds `lib.loss.FocalLoss` / `lib.loss.OFLoss`, and the same names in
      `train.train_ycb_pvn3d` / `train.train_linemod_pvn3d` when those are already imported, to the drop-ins of
      pvn3d_b200.train_utils (import the training script first, then install).  get_item is not patched: it runs in
-     forked DataLoader workers, where CUDA cannot start -- call train_utils.train_batch on the collated batch instead.
+     forked DataLoader workers, where CUDA cannot start -- call train_utils.train_batch on the collated batch instead;
+  7. with patch_vis=True, rebinds `lib.utils.basic_utils.Basic_Utils.draw_p2ds` on the class (patch_draw_p2ds), so the
+     instance demo.py already holds draws on the GPU through pvn3d_b200.vis_utils.draw_p2ds; calls it cannot take run
+     the reference's own method.
 Nothing here copies or edits reference files.
 """
 from __future__ import annotations
@@ -84,7 +87,7 @@ def install_import_shims() -> None:
 
 
 def install(reference_root: str | None = None, patch_post: bool = False, patch_model: bool = False,
-            patch_eval: bool = False, patch_loss: bool = False) -> None:
+            patch_eval: bool = False, patch_loss: bool = False, patch_vis: bool = False) -> None:
     from . import _ext
 
     install_import_shims()
@@ -104,6 +107,34 @@ def install(reference_root: str | None = None, patch_post: bool = False, patch_m
                 patch_eval_pose_parallel(mod.TorchEval)
     if patch_loss:
         patch_loss_modules()
+    if patch_vis:
+        patch_vis_modules()
+
+
+def patch_vis_modules() -> None:
+    """Rebind lib.utils.basic_utils.Basic_Utils.draw_p2ds (patch_draw_p2ds)."""
+    patch_draw_p2ds(importlib.import_module("lib.utils.basic_utils").Basic_Utils)
+
+
+def patch_draw_p2ds(cls) -> None:
+    """Rebind cls.draw_p2ds(img, p2ds, r=1, color=(255, 0, 0)) (the reference's Basic_Utils, or a class with the same
+    method) so that the calls vis_utils.gpu_drawable accepts -- a C-contiguous uint8 [H,W,3] image, int32 / int64
+    [n,2] points, an integer r >= 0, a colour of 1 to 4 numbers, a CUDA device -- run vis_utils.draw_p2ds; every other
+    call runs the original method.  Patched on the class, so existing instances pick it up.  Idempotent."""
+    if getattr(cls.draw_p2ds, "_pvn3d_b200_orig", None) is not None:
+        return
+    orig = cls.draw_p2ds
+
+    def draw_p2ds(self, img, p2ds, r=1, color=(255, 0, 0)):
+        from . import vis_utils
+
+        if not vis_utils.gpu_drawable(img, p2ds, r, color):
+            return orig(self, img, p2ds, r, color)
+        return vis_utils.draw_p2ds(img, p2ds, r, color)
+
+    draw_p2ds._pvn3d_b200_orig = orig
+    draw_p2ds.__doc__ = orig.__doc__
+    cls.draw_p2ds = draw_p2ds
 
 
 def patch_loss_modules() -> None:
