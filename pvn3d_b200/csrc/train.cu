@@ -454,7 +454,7 @@ __global__ void __launch_bounds__(kLossTile)
     for (int e = threadIdx.x; e < np * 3; e += blockDim.x) {
       const int p = e / 3, c = e - p * 3;
       const float d = pred[base + e] - s_t[(p * kk + k) * 3 + c];
-      const float sg = d > 0.f ? 1.f : (d < 0.f ? -1.f : (d == 0.f ? 0.f : d));   // torch.sgn: 0 at 0, NaN at NaN
+      const float sg = d > 0.f ? 1.f : (d < 0.f ? -1.f : 0.f);   // torch.abs's backward: sign(0) = sign(NaN) = 0
       grad[base + e] = (q * s_w[p]) * sg;
     }
   }
@@ -528,9 +528,11 @@ int loss_plan(const pvn3d_loss_args_t *a, LossPlan *pl, size_t *smem) {
   return PVN3D_OK;
 }
 
-int loss_smem_setup(size_t smem) {
+// Opt in on every device's first call, whatever this call's footprint: the partials kernel also holds static shared
+// memory (s_red, s_cnt), and the launch limit without the opt-in is 48 KB for static and dynamic together, so a
+// dynamic size just under 48 KB (the focal tile at C = 94, 95) would otherwise be refused.
+int loss_smem_setup() {
   static PerDeviceOnce once;
-  if (smem <= 48 * 1024) return PVN3D_OK;
   PVN3D_ONCE_PER_DEVICE(once,
                         cudaFuncSetAttribute(train_loss_partials_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                              kLossMaxSmem),
@@ -586,7 +588,7 @@ extern "C" int pvn3d_train_loss_forward(const pvn3d_loss_args_t *args, float *lo
   int rc = loss_plan(args, &pl, &smem);
   if (rc != PVN3D_OK) return rc;
   if ((rc = loss_workspace_check(pl, workspace, workspace_bytes)) != PVN3D_OK) return rc;
-  if ((rc = loss_smem_setup(smem)) != PVN3D_OK) return rc;
+  if ((rc = loss_smem_setup()) != PVN3D_OK) return rc;
   unsigned char *ws = static_cast<unsigned char *>(workspace);
   const unsigned grid = static_cast<unsigned>(pl.seg_blocks + pl.kp_blocks + pl.ctr_blocks);
   train_loss_partials_kernel<<<grid, kLossTile, smem, as_stream(stream)>>>(pl, ws);
@@ -605,7 +607,7 @@ extern "C" int pvn3d_train_loss_backward(const pvn3d_loss_args_t *args, const fl
   if ((rc = loss_workspace_check(pl, workspace, workspace_bytes)) != PVN3D_OK) return rc;
   if ((pl.seg_blocks && !d_seg) || (pl.kp_blocks && !d_kp) || (pl.ctr_blocks && !d_ctr) || (!g_loss && !g_parts && !g_kp))
     return PVN3D_ERR_INVALID_ARG;
-  if ((rc = loss_smem_setup(smem)) != PVN3D_OK) return rc;
+  if ((rc = loss_smem_setup()) != PVN3D_OK) return rc;
   const unsigned grid = static_cast<unsigned>(pl.seg_blocks + pl.kp_blocks + pl.ctr_blocks);
   train_loss_backward_kernel<<<grid, kLossTile, smem, as_stream(stream)>>>(
       pl, GradIn{g_loss, g_parts, g_kp}, static_cast<const unsigned char *>(workspace), d_seg, d_kp, d_ctr);

@@ -51,6 +51,18 @@ def _int(t, dt, what):
     return t.to(dt).contiguous()
 
 
+def _ids32(t, what):
+    """integer class ids as int32 for the kernel; an id int32 cannot hold (an int64 label of 2**32 + 1, say) becomes
+    -1, which matches no class and no slot -- as get_item's int64 comparison finds no match for it -- instead of
+    wrapping onto a real class.  On the device, no host sync."""
+    _cuda(t, what)
+    if t.is_floating_point() or t.is_complex():
+        raise ValueError(f"{what}: expected an integer tensor, got {t.dtype}")
+    if t.dtype != torch.bool and (torch.iinfo(t.dtype).min < -2 ** 31 or torch.iinfo(t.dtype).max > 2 ** 31 - 1):
+        t = torch.where((t >= -2 ** 31) & (t <= 2 ** 31 - 1), t, -1)
+    return t.to(torch.int32).contiguous()
+
+
 class TrainTargets:
     """get_item's regression targets on the GPU for a batch of sampled clouds.
 
@@ -103,8 +115,8 @@ class TrainTargets:
             _cuda(t, f"TrainTargets.compute: {what}")
             if t.device != self.dev:
                 raise ValueError(f"TrainTargets.compute: {what} is on {t.device}, the tables on {self.dev}")
-        lab = _int(labels, torch.int32, "TrainTargets.compute: labels")
-        ids = _int(cls_ids, torch.int32, "TrainTargets.compute: cls_ids")
+        lab = _ids32(labels, "TrainTargets.compute: labels")
+        ids = _ids32(cls_ids, "TrainTargets.compute: cls_ids")
         if not RTs.is_floating_point():
             raise ValueError(f"TrainTargets.compute: RTs must be floating point, got {RTs.dtype}")
         rts = RTs.to(torch.float64).contiguous()

@@ -1,5 +1,6 @@
-"""Float64 restatements of get_item's target block and of lib/loss.py's FocalLoss / OFLoss (numpy and CPU torch, no GPU),
-plus the wrong variants ("mutants") the goldens of tests/golden/train_cases.npz must tell apart:
+"""Float64 restatements of get_item's target block and of lib/loss.py's FocalLoss / OFLoss (numpy and torch; the
+loss functions run on whatever device their inputs are on, so the large edge cases can run their float64 reference on
+the GPU), plus the wrong variants ("mutants") the goldens of tests/golden/train_cases.npz must tell apart:
 
     targets_ref   ycb_dataset.py:241-278: kps = kp_f32 . r^T + t and ctr likewise in float64; offset =
                   float32(float64(cld) - kp); the LAST meta slot of a class wins; labels in no slot stay zero
@@ -8,8 +9,13 @@ plus the wrong variants ("mutants") the goldens of tests/golden/train_cases.npz 
     of_ref        OFLoss: [bs, n_kpts] = sum_{n,c} w |pred - targ| / (sum_n w + 1e-3), w = labels > 1e-8.  The
                   denominator counts each labelled point ONCE: the weight tensor lib/loss.py sums is [bs,n_kpts,n_pts,1]
 
+    pvn3d_loss_t  PVN3DLoss: weights . (focal, sum OF kp, sum OF ctr) with an ok frame mask, and the gradient of
+                  g_loss * loss + g_parts . parts
+
 MUTANTS: "first_slot_wins" (targets), "pt_not_detached" (focal), "den_3x" (OF: a denominator of 3x the count, as if w
-were summed over the three coordinates too).
+were summed over the three coordinates too).  The edge cases (tests/train_edge_cases.py) add "gamma_rounded",
+"tail_dropped" and "ok_ignored" (focal), "nhwc" (nchw_rows), "den_no_eps" and "tail_dropped" (OF), and
+"g_parts_ignored" (PVN3DLoss).
 """
 from __future__ import annotations
 
@@ -68,55 +74,118 @@ def targets_ref(pcld, labels, cls_ids, rts, kp_table, ctr_table, mutant=None):
     return tuple(a.astype(np.float32) for a in (kp_t, ctr_t, kp3, ctr3))
 
 
-def focal_ref(z, target, gamma, mean=True, row_mask=None, mutant=None):
-    """float64 FocalLoss of z [M,C] against target [M] -> (loss, d loss / d z [M,C]).  A target outside [0, C) gives a
-    NaN row.  row_mask [M] bool: rows left out (PVN3DLoss's ok = 0 frames); with no row left the loss is 0."""
-    z = torch.as_tensor(np.asarray(z, np.float64)).clone().requires_grad_(True)
-    t = torch.as_tensor(np.asarray(target, np.int64))
-    c = z.shape[1]
+def _f64(x, device=None):
+    t = torch.as_tensor(np.asarray(x) if not torch.is_tensor(x) else x)
+    return t.to(device=device if device is not None else t.device, dtype=torch.float64)
+
+
+def nchw_rows(z, mutant=None):
+    """FocalLoss's rows of an [N,C,*] input: [N * prod(*), C] with row (n, i) = z[n, :, i], as lib/loss.py's
+    view / transpose / view makes them; a 2-D input is its own rows.  Mutant "nhwc": the same memory read as if
+    each row's C values were contiguous."""
+    z = torch.as_tensor(z)
+    if z.dim() == 2:
+        return z
+    n, c = z.shape[:2]
+    if mutant == "nhwc":
+        return z.reshape(-1, c)
+    return z.reshape(n, c, -1).transpose(1, 2).reshape(-1, c)
+
+
+def focal_t(z, target, gamma, mean=True, row_mask=None, g=1.0, mutant=None, tile=128):
+    """float64 FocalLoss on torch tensors, on z's device: z [M,C], target [M] -> (loss [], d (g loss) / d z [M,C]).
+    A target outside [0, C) gives a NaN row.  row_mask [M] bool: rows left out of the sum and the divisor
+    (PVN3DLoss's ok = 0 frames); with no row left the loss is 0.
+    Mutants: "pt_not_detached", "gamma_rounded" (gamma to the nearest integer), "tail_dropped" (the rows after the
+    last full tile of `tile` rows add nothing, the divisor stays M), "ok_ignored" (row_mask is not applied)."""
+    z = _f64(z).clone().requires_grad_(True)
+    t = torch.as_tensor(np.asarray(target) if not torch.is_tensor(target) else target).to(z.device, torch.int64)
+    m, c = z.shape
+    if mutant == "gamma_rounded":
+        gamma = float(round(gamma))
     valid = (t >= 0) & (t < c)
     logp = torch.log_softmax(z, 1)
     logpt = logp.gather(1, torch.where(valid, t, 0)[:, None])[:, 0]
     logpt = torch.where(valid, logpt, torch.full_like(logpt, float("nan")))
     pt = logpt.exp() if mutant == "pt_not_detached" else logpt.detach().exp()
     rows = -1 * (1 - pt) ** gamma * logpt
-    if row_mask is not None:
-        rows = rows[torch.as_tensor(np.asarray(row_mask, bool))]
+    if mutant == "tail_dropped":
+        rows = torch.where(torch.arange(m, device=z.device) < m // tile * tile, rows, torch.zeros_like(rows))
+    if row_mask is not None and mutant != "ok_ignored":
+        rows = rows[torch.as_tensor(np.asarray(row_mask, bool) if not torch.is_tensor(row_mask) else row_mask,
+                                    device=z.device)]
     if rows.numel() == 0:
         loss = (z * 0).sum()
     else:
         loss = rows.mean() if mean else rows.sum()
-    loss.backward()
-    return float(loss), z.grad.numpy()
+    (loss * g).backward()
+    return loss.detach(), z.grad
+
+
+def focal_ref(z, target, gamma, mean=True, row_mask=None, mutant=None):
+    """focal_t with numpy in and out: (loss float, d loss / d z [M,C])"""
+    loss, grad = focal_t(z, target, gamma, mean=mean, row_mask=row_mask, mutant=mutant)
+    return float(loss), grad.cpu().numpy()
+
+
+def of_t(pred, targ, labels, g=None, mutant=None, tile=128):
+    """float64 OFLoss on torch tensors, on pred's device: pred [bs,K,n,3], targ (viewed as [bs,n,K,3]), labels
+    [bs,n] (integer, or float with w = labels > 1e-8) -> (loss [bs,K], d sum(g * loss) / d pred [bs,K,n,3]); g [bs,K]
+    defaults to ones.  Mutants: "den_3x" (three times the count), "den_no_eps" (the count alone), "tail_dropped"
+    (each frame's points after its last full tile of `tile` points are left out)."""
+    pred = _f64(pred).clone().requires_grad_(True)
+    dev = pred.device
+    bs, k, n, _ = pred.shape
+    targ = _f64(targ, dev).reshape(bs, n, k, 3).permute(0, 2, 1, 3)
+    lab = torch.as_tensor(np.asarray(labels) if not torch.is_tensor(labels) else labels).to(dev).reshape(bs, 1, n, 1)
+    w = (lab > 1e-8).float()
+    if mutant == "tail_dropped":
+        w = w * (torch.arange(n, device=dev) < n // tile * tile).reshape(1, 1, n, 1)
+    s = (w * (pred - targ).abs()).sum((2, 3))
+    cnt = w.sum((2, 3)) * (3 if mutant == "den_3x" else 1)
+    # w is float32 in lib/loss.py: its denominator is float32(count + 1e-3)
+    loss = s / (cnt if mutant == "den_no_eps" else cnt + 1e-3)
+    gg = torch.ones(bs, k, dtype=torch.float64, device=dev) if g is None else _f64(g, dev).expand(bs, k)
+    (loss * gg).sum().backward()
+    return loss.detach(), pred.grad
 
 
 def of_ref(pred, targ, labels, g=None, mutant=None):
-    """float64 OFLoss: pred [bs,K,n,3], targ (viewed as [bs,n,K,3]), labels [bs,n] -> (loss [bs,K], d sum(g * loss) /
-    d pred [bs,K,n,3]); g [bs,K] defaults to ones"""
-    pred = torch.as_tensor(np.asarray(pred, np.float64)).clone().requires_grad_(True)
-    bs, k, n, _ = pred.shape
-    targ = torch.as_tensor(np.asarray(targ, np.float64)).reshape(bs, n, k, 3).permute(0, 2, 1, 3)
-    w = torch.as_tensor(np.asarray(labels).reshape(bs, 1, n, 1) > 1e-8).float()
-    s = (w * (pred - targ).abs()).sum((2, 3))
-    cnt = w.sum((2, 3)) * (3 if mutant == "den_3x" else 1)
-    loss = s / (cnt + 1e-3)        # w is float32 in lib/loss.py: its denominator is float32(count + 1e-3)
-    gg = torch.ones(bs, k, dtype=torch.float64) if g is None else torch.as_tensor(np.asarray(g, np.float64))
-    (loss * gg).sum().backward()
-    return loss.detach().numpy(), pred.grad.numpy()
+    """of_t with numpy in and out"""
+    loss, grad = of_t(pred, targ, labels, g=g, mutant=mutant)
+    return loss.cpu().numpy(), grad.cpu().numpy()
+
+
+def pvn3d_loss_t(kp, seg, ctr, kp_targ, ctr_targ, labels, ok=None, weights=(2.0, 1.0, 1.0), gamma=2.0, g_loss=1.0,
+                 g_parts=(0.0, 0.0, 0.0), mutant=None):
+    """PVN3DLoss in float64 on torch tensors, on kp's device: dict(loss, parts [3], acc, d_kp, d_seg, d_ctr) with the
+    gradients of g_loss * loss + g_parts . parts, where loss = weights . parts and parts = (focal over the rows of ok
+    frames, sum of the kp OFLoss, sum of the ctr OFLoss).  Mutants: "ok_ignored", "g_parts_ignored"."""
+    dev = torch.as_tensor(kp).device
+    b, k, n, _ = kp.shape
+    lab = torch.as_tensor(np.asarray(labels) if not torch.is_tensor(labels) else labels).to(dev).reshape(b, n)
+    mask = None
+    if ok is not None:
+        okt = torch.as_tensor(np.asarray(ok) if not torch.is_tensor(ok) else ok).to(dev).reshape(b) != 0
+        mask = okt.repeat_interleave(n)
+    gp = (0.0, 0.0, 0.0) if mutant == "g_parts_ignored" else tuple(float(v) for v in g_parts)
+    gs = [g_loss * w + v for w, v in zip(weights, gp)]      # d (g_loss loss + g_parts . parts) / d parts
+    z = _f64(seg, dev).reshape(b * n, -1)
+    focal, d_seg = focal_t(z, lab.reshape(-1), gamma, row_mask=mask, g=gs[0],
+                           mutant="ok_ignored" if mutant == "ok_ignored" else None)
+    kl, d_kp = of_t(kp, kp_targ, lab, g=gs[1])
+    cl, d_ctr = of_t(ctr, ctr_targ, lab, g=gs[2])
+    parts = torch.stack([focal, kl.sum(), cl.sum()])
+    loss = weights[0] * parts[0] + weights[1] * parts[1] + weights[2] * parts[2]
+    hit = (torch.argmax(z, 1) == lab.reshape(-1)).double()
+    if mask is not None and mutant != "ok_ignored":
+        hit = hit[mask]
+    acc = hit.mean() if hit.numel() else torch.zeros((), dtype=torch.float64, device=dev)
+    return dict(loss=loss, parts=parts, acc=acc, d_kp=d_kp, d_seg=d_seg.reshape(np.shape(seg)), d_ctr=d_ctr)
 
 
 def pvn3d_loss_ref(kp, seg, ctr, kp_targ, ctr_targ, labels, ok=None, weights=(2.0, 1.0, 1.0), gamma=2.0):
-    """PVN3DLoss in float64: (loss, parts [3], acc, d_kp, d_seg, d_ctr) for d loss"""
-    b, k, n, _ = kp.shape
-    lab = np.asarray(labels).reshape(b, n)
-    mask = None if ok is None else np.repeat(np.asarray(ok).reshape(b) != 0, n)
-    z = np.asarray(seg, np.float64).reshape(b * n, -1)
-    focal, d_seg = focal_ref(z, lab.reshape(-1), gamma, row_mask=mask)
-    kl, d_kp = of_ref(kp, kp_targ, lab, g=np.full((b, k), weights[1]))
-    cl, d_ctr = of_ref(ctr, ctr_targ, lab, g=np.full((b, ctr.shape[1]), weights[2]))
-    parts = np.array([focal, kl.sum(), cl.sum()])
-    loss = weights[0] * parts[0] + weights[1] * parts[1] + weights[2] * parts[2]
-    hit = np.argmax(z, 1) == lab.reshape(-1)
-    m = len(hit) if mask is None else int(mask.sum())
-    acc = (hit if mask is None else hit[mask]).sum() / m if m else 0.0
-    return loss, parts, acc, d_kp, weights[0] * d_seg.reshape(np.shape(seg)), d_ctr
+    """pvn3d_loss_t with numpy in and out: (loss, parts [3], acc, d_kp, d_seg, d_ctr) for d loss"""
+    r = pvn3d_loss_t(kp, seg, ctr, kp_targ, ctr_targ, labels, ok, weights, gamma)
+    return (float(r["loss"]), r["parts"].numpy(), float(r["acc"]), r["d_kp"].numpy(), r["d_seg"].numpy(),
+            r["d_ctr"].numpy())
