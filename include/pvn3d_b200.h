@@ -805,6 +805,49 @@ int pvn3d_vis_draw_poses(uint8_t *img, int b, int h, int w, const float *mesh_pt
 int pvn3d_vis_draw_p2ds(uint8_t *img, int h, int w, int *p2ds, int n, int r, unsigned color, void *workspace,
                         size_t workspace_bytes, pvn3d_stream_t stream);
 
+/* ---- fixed-order backward (csrc/determinism.cu): torch.use_deterministic_algorithms ------------------------------- */
+
+/* Workspace of the three *_grad_ordered calls below for b frames of `slots` index entries into n points (gather: m,
+ * group: npoints * nsample, three_interpolate: 3 n): the inverse index (two key and two slot-number buffers of the
+ * radix sort, its per-tile digit counts and their scan, the run starts), 256-byte aligned pieces; 0 = nothing to size
+ * (an empty or refused shape).  Host only: arithmetic on the arguments, no CUDA call. */
+size_t pvn3d_ordered_grad_workspace_bytes(int b, int n, long long slots);
+
+/* The gradients of pvn3d_gather_points_grad, pvn3d_group_points_grad and pvn3d_three_interpolate_grad with a fixed
+ * summation order: each output element is the float32 sum of its contributions, starting from +0.0 and adding one
+ * term at a time in ascending slot order (gather: slot j of idx[b,j]; group: m*S + s of idx[b,m,s]; interpolate:
+ * 3*j + k of idx[b,j,k], whose term is fl(grad_out[b,c,j] * weight[b,j,k])).  The same bits on every call, stream and
+ * schedule.  Indices outside [0, n) contribute nothing.  Argument checks, empty shapes (a zero fill) and the batch
+ * limit as the atomic entry points; a workspace shorter than pvn3d_ordered_grad_workspace_bytes is refused
+ * (PVN3D_ERR_WORKSPACE).  No host sync; 3 + 3 p launches, p = the 8-bit digits of b * n (keys, p radix passes of
+ * count / scan / scatter, run starts, sums). */
+int pvn3d_gather_points_grad_ordered(const float *grad_out, const int *idx, int b, int c, int n, int m,
+                                     float *grad_points, void *workspace, size_t workspace_bytes,
+                                     pvn3d_stream_t stream);
+int pvn3d_group_points_grad_ordered(const float *grad_out, const int *idx, int b, int c, int n, int npoints,
+                                    int nsample, float *grad_points, void *workspace, size_t workspace_bytes,
+                                    pvn3d_stream_t stream);
+int pvn3d_three_interpolate_grad_ordered(const float *grad_out, const int *idx, const float *weight, int b, int c,
+                                         int n, int m, float *grad_points, void *workspace, size_t workspace_bytes,
+                                         pvn3d_stream_t stream);
+
+/* Backward of torch's adaptive_avg_pool2d on NCHW float32: grad_out [nc,oh,ow] -> grad_in [nc,ih,iw], every element
+ * written once.  Bin o of an axis covers [floor(o in / out), ceil((o + 1) in / out)); input element (y, x) sums, in
+ * ascending (oy, ox) over the bins holding it, (g / kW) / kH with kH, kW the bin's height and width (the order of
+ * torch's own backward, pinned against it).  One launch.
+ * Sides of 2^15 or more, or planes above 2^30 elements, are refused (PVN3D_ERR_UNSUPPORTED). */
+int pvn3d_adaptive_avg_pool2d_backward(const float *grad_out, long long nc, int ih, int iw, int oh, int ow,
+                                       float *grad_in, pvn3d_stream_t stream);
+
+/* Backward of torch's upsample_bilinear2d on NCHW float32: grad_out [nc,oh,ow] -> grad_in [nc,ih,iw], every element
+ * written once.  Taps and lambdas as torch computes them (scale (in-1)/(out-1) with align_corners, else 1/scale_h when
+ * scale_h > 0, else in/out; source fma(scale, o + 0.5, -0.5) clamped at 0 without align_corners).  Input element
+ * (y, x) sums, in ascending output index and, within an output, in torch's tap order, fl(fl(lh lw) g) of the taps that
+ * land on it.  One launch; sizes refused as pvn3d_adaptive_avg_pool2d_backward. */
+int pvn3d_upsample_bilinear2d_backward(const float *grad_out, long long nc, int ih, int iw, int oh, int ow,
+                                       int align_corners, double scale_h, double scale_w, float *grad_in,
+                                       pvn3d_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -14,12 +14,25 @@ Contract kept from the reference (SURVEY section 8b):
     made current for the call (the reference has no device guard -- added here).
 Divergence, on purpose: three_interpolate_grad computes the correct gradient (the reference host
 wrapper launches the forward kernel, interpolate.cpp:89-93 -- a training-only bug).
+
+Under torch.use_deterministic_algorithms(True) (warn_only included) the three *_grad functions call the fixed-order
+entry points (pvn3d_*_grad_ordered, csrc/determinism.cu) instead of the atomic ones: the same values up to the order
+of the float additions, and the same bits on every call.
 """
 from __future__ import annotations
 
 import torch
 
-from ._lib import call, ptr
+from ._lib import call, load, ptr
+
+
+def _ordered(fn_name: str, dev, b: int, n: int, slots: int, *args) -> None:
+    """fn_name(*args, workspace, bytes, stream): a fixed-order grad entry point with its inverse-index workspace"""
+    from .icp import _aligned
+
+    nbytes = int(load().pvn3d_ordered_grad_workspace_bytes(b, n, slots)) if b > 0 and n > 0 and slots > 0 else 0
+    ws, ws_ptr = _aligned(nbytes, dev) if nbytes else (None, 0)
+    call(fn_name, dev, *args, ws_ptr, nbytes)
 
 
 def _chk_contig(x, name):
@@ -97,7 +110,11 @@ def gather_points_grad(grad_out: torch.Tensor, idx: torch.Tensor, n: int) -> tor
     _need_cuda(grad_out)
     b, c, m = grad_out.shape
     out = torch.empty((b, c, int(n)), dtype=torch.float32, device=grad_out.device)
-    call("pvn3d_gather_points_grad", grad_out.device, ptr(grad_out), ptr(idx), b, c, int(n), m, ptr(out))
+    if torch.are_deterministic_algorithms_enabled():
+        _ordered("pvn3d_gather_points_grad_ordered", grad_out.device, b, int(n), m,
+                 ptr(grad_out), ptr(idx), b, c, int(n), m, ptr(out))
+    else:
+        call("pvn3d_gather_points_grad", grad_out.device, ptr(grad_out), ptr(idx), b, c, int(n), m, ptr(out))
     return out
 
 
@@ -145,7 +162,11 @@ def group_points_grad(grad_out: torch.Tensor, idx: torch.Tensor, n: int) -> torc
     b, c = grad_out.size(0), grad_out.size(1)
     m, s = idx.size(1), idx.size(2)
     out = torch.empty((b, c, int(n)), dtype=torch.float32, device=grad_out.device)
-    call("pvn3d_group_points_grad", grad_out.device, ptr(grad_out), ptr(idx), b, c, int(n), m, s, ptr(out))
+    if torch.are_deterministic_algorithms_enabled():
+        _ordered("pvn3d_group_points_grad_ordered", grad_out.device, b, int(n), m * s,
+                 ptr(grad_out), ptr(idx), b, c, int(n), m, s, ptr(out))
+    else:
+        call("pvn3d_group_points_grad", grad_out.device, ptr(grad_out), ptr(idx), b, c, int(n), m, s, ptr(out))
     return out
 
 
@@ -258,7 +279,12 @@ def three_interpolate_grad(grad_out: torch.Tensor, idx: torch.Tensor, weight: to
     _need_cuda(grad_out)
     b, c, n = grad_out.shape
     out = torch.empty((b, c, int(m)), dtype=torch.float32, device=grad_out.device)
-    call("pvn3d_three_interpolate_grad", grad_out.device, ptr(grad_out), ptr(idx), ptr(weight), b, c, n, int(m), ptr(out))
+    if torch.are_deterministic_algorithms_enabled():
+        _ordered("pvn3d_three_interpolate_grad_ordered", grad_out.device, b, int(m), 3 * n,
+                 ptr(grad_out), ptr(idx), ptr(weight), b, c, n, int(m), ptr(out))
+    else:
+        call("pvn3d_three_interpolate_grad", grad_out.device, ptr(grad_out), ptr(idx), ptr(weight), b, c, n, int(m),
+             ptr(out))
     return out
 
 

@@ -146,6 +146,13 @@ _SIGNATURES = {
     "pvn3d_vis_draw_poses": (c_int, [_P, c_int, c_int, c_int, _P, _P, c_int, c_int, _P, c_int, _P, _P, c_int, _P,
                                      c_double, _P, c_int, _P, c_size_t, _P]),
     "pvn3d_vis_draw_p2ds": (c_int, [_P, c_int, c_int, _P, c_int, c_int, c_uint, _P, c_size_t, _P]),
+    "pvn3d_ordered_grad_workspace_bytes": (c_size_t, [c_int, c_int, ctypes.c_longlong]),
+    "pvn3d_gather_points_grad_ordered": (c_int, [_P, _P, c_int, c_int, c_int, c_int, _P, _P, c_size_t, _P]),
+    "pvn3d_group_points_grad_ordered": (c_int, [_P, _P, c_int, c_int, c_int, c_int, c_int, _P, _P, c_size_t, _P]),
+    "pvn3d_three_interpolate_grad_ordered": (c_int, [_P, _P, _P, c_int, c_int, c_int, c_int, _P, _P, c_size_t, _P]),
+    "pvn3d_adaptive_avg_pool2d_backward": (c_int, [_P, ctypes.c_longlong, c_int, c_int, c_int, c_int, _P, _P]),
+    "pvn3d_upsample_bilinear2d_backward": (c_int, [_P, ctypes.c_longlong, c_int, c_int, c_int, c_int, c_int, c_double,
+                                                   c_double, _P, _P]),
 }
 FLAT_MS_MAX_PTS = 4096   # PVN3D_FLAT_MS_MAX_PTS
 EXPORTED_SYMBOLS = tuple(_SIGNATURES)

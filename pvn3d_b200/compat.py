@@ -27,7 +27,12 @@ What install() does (SURVEY section 8b, App. D):
      forked DataLoader workers, where CUDA cannot start -- call train_utils.train_batch on the collated batch instead;
   7. with patch_vis=True, rebinds `lib.utils.basic_utils.Basic_Utils.draw_p2ds` on the class (patch_draw_p2ds), so the
      instance demo.py already holds draws on the GPU through pvn3d_b200.vis_utils.draw_p2ds; calls it cannot take run
-     the reference's own method.
+     the reference's own method;
+  8. with patch_deterministic=True, routes lib.pspnet's pooling and bilinear upsampling through
+     pvn3d_b200.deterministic (patch_pspnet): the module's `F` becomes torch.nn.functional with a deterministic-backward
+     `upsample` / `interpolate`, and PSPModule / PSPUpsample give their nn.AdaptiveAvgPool2d / nn.Upsample submodules
+     the deterministic backward on every call, so models built before and after the call are covered.  Forward bits do
+     not change, and the backward is torch's own unless torch.use_deterministic_algorithms is on.
 Nothing here copies or edits reference files.
 """
 from __future__ import annotations
@@ -87,7 +92,8 @@ def install_import_shims() -> None:
 
 
 def install(reference_root: str | None = None, patch_post: bool = False, patch_model: bool = False,
-            patch_eval: bool = False, patch_loss: bool = False, patch_vis: bool = False) -> None:
+            patch_eval: bool = False, patch_loss: bool = False, patch_vis: bool = False,
+            patch_deterministic: bool = False) -> None:
     from . import _ext
 
     install_import_shims()
@@ -109,6 +115,31 @@ def install(reference_root: str | None = None, patch_post: bool = False, patch_m
         patch_loss_modules()
     if patch_vis:
         patch_vis_modules()
+    if patch_deterministic:
+        patch_pspnet(importlib.import_module("lib.pspnet"))
+
+
+def patch_pspnet(mod) -> None:
+    """Route the pooling and bilinear upsampling of `mod` (the reference's lib.pspnet, or a module with the same
+    PSPModule / PSPUpsample) through pvn3d_b200.deterministic: mod.F becomes deterministic.functional(), and
+    PSPModule.forward / PSPUpsample.forward first adopt() their submodules, then run the original forward.
+    Idempotent."""
+    from . import deterministic
+
+    if getattr(mod, "_pvn3d_b200_deterministic", False):
+        return
+    mod.F = deterministic.functional()
+    for cls in (mod.PSPModule, mod.PSPUpsample):
+        orig = cls.forward
+
+        def forward(self, *args, _orig=orig, **kwargs):
+            deterministic.adopt(self)
+            return _orig(self, *args, **kwargs)
+
+        forward._pvn3d_b200_orig = orig
+        forward.__doc__ = orig.__doc__
+        cls.forward = forward
+    mod._pvn3d_b200_deterministic = True
 
 
 def patch_vis_modules() -> None:
