@@ -131,6 +131,33 @@ int pvn3d_three_interpolate_grad(const float *grad_out, const int *idx, const fl
                                  int c, int n, int m, float *grad_points, pvn3d_stream_t stream);
 
 /* ------------------------------------------------------------------------------------------
+ * 16-bit forms of group_points, three_interpolate and their grads, for training under torch.autocast (bf16 or fp16
+ * features; coordinates, idx and weight stay f32 / int32).  `dtype` is PVN3D_F16 (IEEE binary16, torch.float16) or
+ * PVN3D_BF16 (bfloat16, torch.bfloat16); any other code returns PVN3D_ERR_INVALID_ARG before any CUDA call.  The
+ * 16-bit pointers hold elements of that type.  Arithmetic is float32; each output element is rounded once, to nearest
+ * even; inf and NaN propagate, and a float32 result beyond float16's largest finite value (65504) rounds to inf.
+ * Argument checks, empty shapes and the batch limit as the float32 entry points.
+ *   group_points_16: a copy, bit-equal to torch.gather of the same elements.  Two adjacent slots per 4-byte store when
+ *     the slot count is even (idx 8-byte and out 4-byte aligned).
+ *   three_interpolate_16: weight is float32; out[b,c,j] = round16(the float32 value pvn3d_three_interpolate gives for
+ *     the widened features), the same fma(p3,w3, fma(p1,w1, p2*w2)) order.
+ *   *_grad_16 (atomic): float32 atomics into `scratch`, b*c*n (group) or b*c*m (interpolate) floats the caller
+ *     allocates (8-byte aligned for paired rounding), zero-filled by the callee, then rounded once into grad_points.
+ *     Each element is within gamma_k * sum|t| of the exact sum (as the float32 grads above) plus half a 16-bit ulp of
+ *     the result.  No 16-bit atomics (those would round at every add).  Three launches (memset, scatter, round).
+ * ---------------------------------------------------------------------------------------- */
+#define PVN3D_F16 1
+#define PVN3D_BF16 2
+int pvn3d_group_points_16(int dtype, const void *points, const int *idx, int b, int c, int n, int npoints, int nsample,
+                          void *out, pvn3d_stream_t stream);
+int pvn3d_group_points_grad_16(int dtype, const void *grad_out, const int *idx, int b, int c, int n, int npoints,
+                               int nsample, float *scratch, void *grad_points, pvn3d_stream_t stream);
+int pvn3d_three_interpolate_16(int dtype, const void *points, const int *idx, const float *weight, int b, int c, int m,
+                               int n, void *out, pvn3d_stream_t stream);
+int pvn3d_three_interpolate_grad_16(int dtype, const void *grad_out, const int *idx, const float *weight, int b, int c,
+                                    int n, int m, float *scratch, void *grad_points, pvn3d_stream_t stream);
+
+/* ------------------------------------------------------------------------------------------
  * Fused forms of the same path (what QueryAndGroup.forward / PointnetFPModule.forward compose
  * from the ops above: pointnet2_utils.py:293-330, pointnet2_modules.py:183-190).
  * ---------------------------------------------------------------------------------------- */
@@ -847,6 +874,23 @@ int pvn3d_adaptive_avg_pool2d_backward(const float *grad_out, long long nc, int 
 int pvn3d_upsample_bilinear2d_backward(const float *grad_out, long long nc, int ih, int iw, int oh, int ow,
                                        int align_corners, double scale_h, double scale_w, float *grad_in,
                                        pvn3d_stream_t stream);
+
+/* 16-bit forms of the fixed-order grads and of the two PSPNet backward ops (dtype, element types, checks and the
+ * unknown-code refusal as pvn3d_group_points_16 above).  The same inverse index, workspace and launches as the float32
+ * calls: each element is the float32 sum of the widened 16-bit terms in the same ascending order, rounded once to
+ * nearest even, so it is bit-equal to round16(the float32 call on grad_out converted to float32), with the same bits
+ * on every call. */
+int pvn3d_group_points_grad_ordered_16(int dtype, const void *grad_out, const int *idx, int b, int c, int n,
+                                       int npoints, int nsample, void *grad_points, void *workspace,
+                                       size_t workspace_bytes, pvn3d_stream_t stream);
+int pvn3d_three_interpolate_grad_ordered_16(int dtype, const void *grad_out, const int *idx, const float *weight, int b,
+                                            int c, int n, int m, void *grad_points, void *workspace,
+                                            size_t workspace_bytes, pvn3d_stream_t stream);
+int pvn3d_adaptive_avg_pool2d_backward_16(int dtype, const void *grad_out, long long nc, int ih, int iw, int oh, int ow,
+                                          void *grad_in, pvn3d_stream_t stream);
+int pvn3d_upsample_bilinear2d_backward_16(int dtype, const void *grad_out, long long nc, int ih, int iw, int oh, int ow,
+                                          int align_corners, double scale_h, double scale_w, void *grad_in,
+                                          pvn3d_stream_t stream);
 
 #ifdef __cplusplus
 }

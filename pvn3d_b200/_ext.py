@@ -18,6 +18,14 @@ wrapper launches the forward kernel, interpolate.cpp:89-93 -- a training-only bu
 Under torch.use_deterministic_algorithms(True) (warn_only included) the three *_grad functions call the fixed-order
 entry points (pvn3d_*_grad_ordered, csrc/determinism.cu) instead of the atomic ones: the same values up to the order
 of the float additions, and the same bits on every call.
+
+Mixed precision (torch.autocast): group_points, group_points_grad, three_interpolate and three_interpolate_grad also
+take float16 and bfloat16 features / gradients and return that dtype (the pvn3d_*_16 entry points, chosen by the
+tensor's dtype; float32 calls run exactly what they ran before).  idx stays int32 and three_interpolate's weight stays
+float32; any other dtype raises the usual "<name> must be a float tensor".  Arithmetic is float32 and each output element
+is rounded once: group_points is a copy; three_interpolate is round16 of the float32 op on the widened features; the
+atomic grads scatter float32 atomics into a float32 scratch and round once; the ordered grads are round16 of the
+float32 ordered grads of the widened gradient, with the same bits on every call.
 """
 from __future__ import annotations
 
@@ -42,6 +50,15 @@ def _chk_contig(x, name):
 
 def _chk_float(x, name):
     if x.dtype != torch.float32:
+        raise RuntimeError(f"{name} must be a float tensor")
+
+
+_DTYPE16 = {torch.float16: 1, torch.bfloat16: 2}      # PVN3D_F16, PVN3D_BF16 (include/pvn3d_b200.h)
+
+
+def _chk_feat(x, name):
+    """float32, or one of the 16-bit dtypes autocast produces"""
+    if x.dtype != torch.float32 and x.dtype not in _DTYPE16:
         raise RuntimeError(f"{name} must be a float tensor")
 
 
@@ -138,15 +155,19 @@ def group_points(points: torch.Tensor, idx: torch.Tensor) -> torch.Tensor:
     """group_points.cpp:12-35 -- points [B,C,N], idx [B,M,S] -> [B,C,M,S]"""
     _chk_contig(points, "points")
     _chk_contig(idx, "idx")
-    _chk_float(points, "points")
+    _chk_feat(points, "points")
     _chk_int(idx, "idx")
     if points.is_cuda:
         _chk_cuda(idx, "idx")
     _need_cuda(points)
     b, c, n = points.shape
     m, s = idx.size(1), idx.size(2)
-    out = torch.empty((b, c, m, s), dtype=torch.float32, device=points.device)
-    call("pvn3d_group_points", points.device, ptr(points), ptr(idx), b, c, n, m, s, ptr(out))
+    out = torch.empty((b, c, m, s), dtype=points.dtype, device=points.device)
+    if points.dtype in _DTYPE16:
+        call("pvn3d_group_points_16", points.device, _DTYPE16[points.dtype], ptr(points), ptr(idx), b, c, n, m, s,
+             ptr(out))
+    else:
+        call("pvn3d_group_points", points.device, ptr(points), ptr(idx), b, c, n, m, s, ptr(out))
     return out
 
 
@@ -154,15 +175,24 @@ def group_points_grad(grad_out: torch.Tensor, idx: torch.Tensor, n: int) -> torc
     """group_points.cpp:37-60"""
     _chk_contig(grad_out, "grad_out")
     _chk_contig(idx, "idx")
-    _chk_float(grad_out, "grad_out")
+    _chk_feat(grad_out, "grad_out")
     _chk_int(idx, "idx")
     if grad_out.is_cuda:
         _chk_cuda(idx, "idx")
     _need_cuda(grad_out)
     b, c = grad_out.size(0), grad_out.size(1)
     m, s = idx.size(1), idx.size(2)
-    out = torch.empty((b, c, int(n)), dtype=torch.float32, device=grad_out.device)
-    if torch.are_deterministic_algorithms_enabled():
+    out = torch.empty((b, c, int(n)), dtype=grad_out.dtype, device=grad_out.device)
+    if grad_out.dtype in _DTYPE16:
+        code = _DTYPE16[grad_out.dtype]
+        if torch.are_deterministic_algorithms_enabled():
+            _ordered("pvn3d_group_points_grad_ordered_16", grad_out.device, b, int(n), m * s,
+                     code, ptr(grad_out), ptr(idx), b, c, int(n), m, s, ptr(out))
+        else:
+            scratch = torch.empty((b, c, int(n)), dtype=torch.float32, device=grad_out.device)
+            call("pvn3d_group_points_grad_16", grad_out.device, code, ptr(grad_out), ptr(idx), b, c, int(n), m, s,
+                 ptr(scratch), ptr(out))
+    elif torch.are_deterministic_algorithms_enabled():
         _ordered("pvn3d_group_points_grad_ordered", grad_out.device, b, int(n), m * s,
                  ptr(grad_out), ptr(idx), b, c, int(n), m, s, ptr(out))
     else:
@@ -251,7 +281,7 @@ def three_interpolate(points: torch.Tensor, idx: torch.Tensor, weight: torch.Ten
     _chk_contig(points, "points")
     _chk_contig(idx, "idx")
     _chk_contig(weight, "weight")
-    _chk_float(points, "points")
+    _chk_feat(points, "points")
     _chk_int(idx, "idx")
     _chk_float(weight, "weight")
     if points.is_cuda:
@@ -260,8 +290,12 @@ def three_interpolate(points: torch.Tensor, idx: torch.Tensor, weight: torch.Ten
     _need_cuda(points)
     b, c, m = points.shape
     n = idx.size(1)
-    out = torch.empty((b, c, n), dtype=torch.float32, device=points.device)
-    call("pvn3d_three_interpolate", points.device, ptr(points), ptr(idx), ptr(weight), b, c, m, n, ptr(out))
+    out = torch.empty((b, c, n), dtype=points.dtype, device=points.device)
+    if points.dtype in _DTYPE16:
+        call("pvn3d_three_interpolate_16", points.device, _DTYPE16[points.dtype], ptr(points), ptr(idx), ptr(weight),
+             b, c, m, n, ptr(out))
+    else:
+        call("pvn3d_three_interpolate", points.device, ptr(points), ptr(idx), ptr(weight), b, c, m, n, ptr(out))
     return out
 
 
@@ -270,7 +304,7 @@ def three_interpolate_grad(grad_out: torch.Tensor, idx: torch.Tensor, weight: to
     _chk_contig(grad_out, "grad_out")
     _chk_contig(idx, "idx")
     _chk_contig(weight, "weight")
-    _chk_float(grad_out, "grad_out")
+    _chk_feat(grad_out, "grad_out")
     _chk_int(idx, "idx")
     _chk_float(weight, "weight")
     if grad_out.is_cuda:
@@ -278,8 +312,17 @@ def three_interpolate_grad(grad_out: torch.Tensor, idx: torch.Tensor, weight: to
         _chk_cuda(weight, "weight")
     _need_cuda(grad_out)
     b, c, n = grad_out.shape
-    out = torch.empty((b, c, int(m)), dtype=torch.float32, device=grad_out.device)
-    if torch.are_deterministic_algorithms_enabled():
+    out = torch.empty((b, c, int(m)), dtype=grad_out.dtype, device=grad_out.device)
+    if grad_out.dtype in _DTYPE16:
+        code = _DTYPE16[grad_out.dtype]
+        if torch.are_deterministic_algorithms_enabled():
+            _ordered("pvn3d_three_interpolate_grad_ordered_16", grad_out.device, b, int(m), 3 * n,
+                     code, ptr(grad_out), ptr(idx), ptr(weight), b, c, n, int(m), ptr(out))
+        else:
+            scratch = torch.empty((b, c, int(m)), dtype=torch.float32, device=grad_out.device)
+            call("pvn3d_three_interpolate_grad_16", grad_out.device, code, ptr(grad_out), ptr(idx), ptr(weight), b, c,
+                 n, int(m), ptr(scratch), ptr(out))
+    elif torch.are_deterministic_algorithms_enabled():
         _ordered("pvn3d_three_interpolate_grad_ordered", grad_out.device, b, int(m), 3 * n,
                  ptr(grad_out), ptr(idx), ptr(weight), b, c, n, int(m), ptr(out))
     else:

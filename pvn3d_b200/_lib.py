@@ -153,9 +153,21 @@ _SIGNATURES = {
     "pvn3d_adaptive_avg_pool2d_backward": (c_int, [_P, ctypes.c_longlong, c_int, c_int, c_int, c_int, _P, _P]),
     "pvn3d_upsample_bilinear2d_backward": (c_int, [_P, ctypes.c_longlong, c_int, c_int, c_int, c_int, c_int, c_double,
                                                    c_double, _P, _P]),
+    "pvn3d_group_points_16": (c_int, [c_int, _P, _P, c_int, c_int, c_int, c_int, c_int, _P, _P]),
+    "pvn3d_group_points_grad_16": (c_int, [c_int, _P, _P, c_int, c_int, c_int, c_int, c_int, _P, _P, _P]),
+    "pvn3d_three_interpolate_16": (c_int, [c_int, _P, _P, _P, c_int, c_int, c_int, c_int, _P, _P]),
+    "pvn3d_three_interpolate_grad_16": (c_int, [c_int, _P, _P, _P, c_int, c_int, c_int, c_int, _P, _P, _P]),
+    "pvn3d_group_points_grad_ordered_16": (c_int, [c_int, _P, _P, c_int, c_int, c_int, c_int, c_int, _P, _P, c_size_t,
+                                                   _P]),
+    "pvn3d_three_interpolate_grad_ordered_16": (c_int, [c_int, _P, _P, _P, c_int, c_int, c_int, c_int, _P, _P, c_size_t,
+                                                        _P]),
+    "pvn3d_adaptive_avg_pool2d_backward_16": (c_int, [c_int, _P, ctypes.c_longlong, c_int, c_int, c_int, c_int, _P, _P]),
+    "pvn3d_upsample_bilinear2d_backward_16": (c_int, [c_int, _P, ctypes.c_longlong, c_int, c_int, c_int, c_int, c_int,
+                                                      c_double, c_double, _P, _P]),
 }
 FLAT_MS_MAX_PTS = 4096   # PVN3D_FLAT_MS_MAX_PTS
 EXPORTED_SYMBOLS = tuple(_SIGNATURES)
+PVN3D_F16, PVN3D_BF16 = 1, 2   # dtype codes of the *_16 entry points
 
 _lib = None
 

@@ -11,7 +11,10 @@
 //     walks its run in ascending slot order for a block of channels.
 //   * adaptive_avg_pool2d / upsample_bilinear2d backward: one thread per input element, which enumerates the output
 //     elements whose window (bin or four taps) holds it, in ascending output index.
+// The sums and PSP kernels are templated on the element type of the gradients (half_io.cuh): a 16-bit form reads
+// 16-bit terms, runs the same float32 sum in the same order and rounds each output element once.
 #include "common.cuh"
+#include "half_io.cuh"
 
 namespace pvn3d {
 namespace {
@@ -51,12 +54,13 @@ __global__ void run_starts_kernel(const Key *__restrict__ keys, long long total,
 
 // grad_points[f, l, i] = sum over the run of point (f, i), in ascending slot order, of the slot's term in channel l.
 // Terms: grad_out[f, l, s] (kGradGather), or fl(grad_out[f, l, s / 3] * weight[f, s]) (kGradInterp; the product is
-// rounded before the add: __fmul_rn keeps it out of an FMA).  src_len is grad_out's row length.
-template <int kMode>
+// rounded before the add: __fmul_rn keeps it out of an FMA).  src_len is grad_out's row length.  T is the element
+// type of grad_out and grad_points (one thread per point: the stores stay 2-byte for a 16-bit T).
+template <int kMode, typename T>
 __global__ void __launch_bounds__(kSumThreads)
-ordered_sum_kernel(const float *__restrict__ grad_out, const float *__restrict__ weight,
+ordered_sum_kernel(const T *__restrict__ grad_out, const float *__restrict__ weight,
                    const long long *__restrict__ starts, const int *__restrict__ sorted_slots, int c, int n,
-                   long long src_len, long long slots, float *__restrict__ grad_points) {
+                   long long src_len, long long slots, T *__restrict__ grad_points) {
   const int f = blockIdx.z;
   const int i = blockIdx.x * kSumThreads + threadIdx.x;
   if (i >= n) return;
@@ -65,7 +69,7 @@ ordered_sum_kernel(const float *__restrict__ grad_out, const float *__restrict__
   const float *w = weight + static_cast<size_t>(f) * slots;
   for (int l0 = blockIdx.y * kSumChannels; l0 < c; l0 += gridDim.y * kSumChannels) {
     const int nl = min(kSumChannels, c - l0);
-    const float *src = grad_out + (static_cast<size_t>(f) * c + l0) * src_len;
+    const T *src = grad_out + (static_cast<size_t>(f) * c + l0) * src_len;
     float acc[kSumChannels];
 #pragma unroll
     for (int k = 0; k < kSumChannels; ++k) acc[k] = 0.f;
@@ -76,16 +80,16 @@ ordered_sum_kernel(const float *__restrict__ grad_out, const float *__restrict__
         if (k < nl) {
           float t;
           if (kMode == kGradInterp)
-            t = __fmul_rn(__ldg(src + k * src_len + s / 3), __ldg(w + s));
+            t = __fmul_rn(to_f32(__ldg(src + k * src_len + s / 3)), __ldg(w + s));
           else
-            t = __ldg(src + k * src_len + s);
+            t = to_f32(__ldg(src + k * src_len + s));
           acc[k] = __fadd_rn(acc[k], t);
         }
       }
     }
 #pragma unroll
     for (int k = 0; k < kSumChannels; ++k)
-      if (k < nl) grad_points[(static_cast<size_t>(f) * c + l0 + k) * n + i] = acc[k];
+      if (k < nl) grad_points[(static_cast<size_t>(f) * c + l0 + k) * n + i] = from_f32<T>(acc[k]);
   }
 }
 
@@ -262,9 +266,9 @@ static int build_inverse(const int *idx, int b, int n, long long slots, const In
 }
 
 // the inverse index of idx (b frames of `slots` entries into [0, n)), then the ordered sums into grad_points
-template <int kMode>
-static int ordered_grad(const float *grad_out, const int *idx, const float *weight, int b, int c, int n,
-                        long long slots, long long src_len, float *grad_points, void *workspace,
+template <int kMode, typename T>
+static int ordered_grad(const T *grad_out, const int *idx, const float *weight, int b, int c, int n,
+                        long long slots, long long src_len, T *grad_points, void *workspace,
                         size_t workspace_bytes, cudaStream_t st) {
   const InverseLayout L = inverse_layout(b, n, slots);
   if (!workspace || workspace_bytes < L.total_bytes) return PVN3D_ERR_WORKSPACE;
@@ -276,7 +280,7 @@ static int ordered_grad(const float *grad_out, const int *idx, const float *weig
   const int gx = ceil_div(n, kSumThreads);
   int gy = ceil_div(4 * sm_count(), gx * b);
   gy = max(1, min(gy, min(ceil_div(c, kSumChannels), 65535)));
-  ordered_sum_kernel<kMode><<<dim3(gx, gy, b), kSumThreads, 0, st>>>(
+  ordered_sum_kernel<kMode, T><<<dim3(gx, gy, b), kSumThreads, 0, st>>>(
       grad_out, weight, reinterpret_cast<const long long *>(ws + L.starts),
       reinterpret_cast<const int *>(ws + L.vals[sorted]), c, n, src_len, slots, grad_points);
   return check_launch("ordered_sum_kernel");
@@ -301,11 +305,12 @@ __device__ __forceinline__ int bin_end(int o, int out, int in) {
          once; once = 0)
 
 // grad_in[p, y, x] = sum over the bins (oy, ox) holding (y, x), ascending, of (g[p, oy, ox] / kW) / kH
-__global__ void adaptive_avg_pool2d_backward_kernel(const float *__restrict__ grad_out, long long nc, int ih,
-                                                    int iw, int oh, int ow, float *__restrict__ grad_in) {
+template <typename T>
+__global__ void adaptive_avg_pool2d_backward_kernel(const T *__restrict__ grad_out, long long nc, int ih,
+                                                    int iw, int oh, int ow, T *__restrict__ grad_in) {
 
   PSP_FOR_EACH_ELEMENT(nc, ih, iw) {
-    const float *g = grad_out + plane * oh * ow;
+    const T *g = grad_out + plane * oh * ow;
     // the bins holding y: floor(y out / in) <= o < ceil((y + 1) out / in)
     const int oy0 = bin_start(y, ih, oh), oy1 = min(bin_end(y, ih, oh), oh);
     const int ox0 = bin_start(x, iw, ow), ox1 = min(bin_end(x, iw, ow), ow);
@@ -314,11 +319,11 @@ __global__ void adaptive_avg_pool2d_backward_kernel(const float *__restrict__ gr
       const float kh = static_cast<float>(bin_end(oy, oh, ih) - bin_start(oy, oh, ih));
       for (int ox = ox0; ox < ox1; ++ox) {
         const float kw = static_cast<float>(bin_end(ox, ow, iw) - bin_start(ox, ow, iw));
-        const float v = g[oy * ow + ox];
+        const float v = to_f32(g[oy * ow + ox]);
         acc = __fadd_rn(acc, __fdiv_rn(__fdiv_rn(v, kw), kh));   // width first, as torch's backward divides
       }
     }
-    grad_in[plane * ih * iw + pix] = acc;
+    grad_in[plane * ih * iw + pix] = from_f32<T>(acc);
   }
 }
 
@@ -361,11 +366,12 @@ __device__ __forceinline__ void tap_window(float scale, int v, int in, int out, 
 // grad_in[p, y, x] = sum over the outputs (oy, ox) in ascending order, and over their four taps in torch's order
 // (i1, j1), (i1, j1 + j1p), (i1 + i1p, j1), (i1 + i1p, j1 + j1p), of fl(fl(lambda_h lambda_w) g[p, oy, ox]) for the
 // taps that land on (y, x)
-__global__ void upsample_bilinear2d_backward_kernel(const float *__restrict__ grad_out, long long nc, int ih,
+template <typename T>
+__global__ void upsample_bilinear2d_backward_kernel(const T *__restrict__ grad_out, long long nc, int ih,
                                                     int iw, int oh, int ow, int align, float rh, float rw,
-                                                    float *__restrict__ grad_in) {
+                                                    T *__restrict__ grad_in) {
   PSP_FOR_EACH_ELEMENT(nc, ih, iw) {
-    const float *g = grad_out + plane * oh * ow;
+    const T *g = grad_out + plane * oh * ow;
     int oy0, oy1, ox0, ox1;
     tap_window(rh, y, ih, oh, align, oy0, oy1);
     tap_window(rw, x, iw, ow, align, ox0, ox1);
@@ -378,14 +384,14 @@ __global__ void upsample_bilinear2d_backward_kernel(const float *__restrict__ gr
         const Taps tw = bilinear_taps(rw, ox, iw, align);
         const bool w0 = tw.i1 == x, w1 = tw.i1 + tw.i1p == x;
         if (!w0 && !w1) continue;
-        const float v = g[oy * ow + ox];
+        const float v = to_f32(g[oy * ow + ox]);
         if (h0 && w0) acc = __fadd_rn(acc, __fmul_rn(__fmul_rn(th.l0, tw.l0), v));
         if (h0 && w1) acc = __fadd_rn(acc, __fmul_rn(__fmul_rn(th.l0, tw.l1), v));
         if (h1 && w0) acc = __fadd_rn(acc, __fmul_rn(__fmul_rn(th.l1, tw.l0), v));
         if (h1 && w1) acc = __fadd_rn(acc, __fmul_rn(__fmul_rn(th.l1, tw.l1), v));
       }
     }
-    grad_in[plane * ih * iw + pix] = acc;
+    grad_in[plane * ih * iw + pix] = from_f32<T>(acc);
   }
 }
 
@@ -468,7 +474,7 @@ extern "C" int pvn3d_adaptive_avg_pool2d_backward(const float *grad_out, long lo
   if (total == 0) return PVN3D_OK;
   if (!grad_out || !grad_in) return PVN3D_ERR_INVALID_ARG;
   if (!psp_sides_supported(ih, iw, oh, ow)) return PVN3D_ERR_UNSUPPORTED;
-  adaptive_avg_pool2d_backward_kernel<<<psp_grid(nc, ih * iw), 256, 0, as_stream(stream)>>>(grad_out, nc, ih, iw, oh,
+  adaptive_avg_pool2d_backward_kernel<float><<<psp_grid(nc, ih * iw), 256, 0, as_stream(stream)>>>(grad_out, nc, ih, iw, oh,
                                                                                             ow, grad_in);
   return check_launch("adaptive_avg_pool2d_backward_kernel");
 }
@@ -482,8 +488,80 @@ extern "C" int pvn3d_upsample_bilinear2d_backward(const float *grad_out, long lo
   if (!grad_out || !grad_in) return PVN3D_ERR_INVALID_ARG;
   const bool align = align_corners != 0;
   if (!psp_sides_supported(ih, iw, oh, ow)) return PVN3D_ERR_UNSUPPORTED;
-  upsample_bilinear2d_backward_kernel<<<psp_grid(nc, ih * iw), 256, 0, as_stream(stream)>>>(
+  upsample_bilinear2d_backward_kernel<float><<<psp_grid(nc, ih * iw), 256, 0, as_stream(stream)>>>(
       grad_out, nc, ih, iw, oh, ow, align ? 1 : 0, bilinear_scale(ih, oh, align, scale_h),
       bilinear_scale(iw, ow, align, scale_w), grad_in);
   return check_launch("upsample_bilinear2d_backward_kernel");
+}
+
+// ---- 16-bit forms (torch.autocast): the same inverse index and launches on __half / __nv_bfloat16 gradients --------
+extern "C" int pvn3d_group_points_grad_ordered_16(int dtype, const void *grad_out, const int *idx, int b, int c, int n,
+                                                  int npoints, int nsample, void *grad_points, void *workspace,
+                                                  size_t workspace_bytes, pvn3d_stream_t stream) {
+  return with_dtype16(dtype, [&](auto tag) -> int {
+    using T = decltype(tag);
+    if (b < 0 || c < 0 || n <= 0 || npoints < 0 || nsample < 0) return PVN3D_ERR_INVALID_ARG;
+    if (b == 0 || c == 0) return PVN3D_OK;
+    const long long slots = static_cast<long long>(npoints) * nsample;
+    if (!grad_points || (slots > 0 && (!grad_out || !idx))) return PVN3D_ERR_INVALID_ARG;
+    if (b > 65535 || slots > 0x7fffffffll) return PVN3D_ERR_UNSUPPORTED;
+    if (slots == 0) {
+      PVN3D_CUDA_TRY(cudaMemsetAsync(grad_points, 0, sizeof(T) * b * c * (size_t)n, as_stream(stream)), "memset");
+      return PVN3D_OK;
+    }
+    return ordered_grad<kGradGather>(static_cast<const T *>(grad_out), idx, nullptr, b, c, n, slots, slots,
+                                     static_cast<T *>(grad_points), workspace, workspace_bytes, as_stream(stream));
+  });
+}
+
+extern "C" int pvn3d_three_interpolate_grad_ordered_16(int dtype, const void *grad_out, const int *idx,
+                                                       const float *weight, int b, int c, int n, int m,
+                                                       void *grad_points, void *workspace, size_t workspace_bytes,
+                                                       pvn3d_stream_t stream) {
+  return with_dtype16(dtype, [&](auto tag) -> int {
+    using T = decltype(tag);
+    if (b < 0 || c < 0 || m <= 0 || n < 0) return PVN3D_ERR_INVALID_ARG;
+    if (b == 0 || c == 0) return PVN3D_OK;
+    if (!grad_points || (n > 0 && (!grad_out || !idx || !weight))) return PVN3D_ERR_INVALID_ARG;
+    if (b > 65535) return PVN3D_ERR_UNSUPPORTED;
+    if (n == 0) {
+      PVN3D_CUDA_TRY(cudaMemsetAsync(grad_points, 0, sizeof(T) * b * c * (size_t)m, as_stream(stream)), "memset");
+      return PVN3D_OK;
+    }
+    return ordered_grad<kGradInterp>(static_cast<const T *>(grad_out), idx, weight, b, c, m, 3ll * n, n,
+                                     static_cast<T *>(grad_points), workspace, workspace_bytes, as_stream(stream));
+  });
+}
+
+extern "C" int pvn3d_adaptive_avg_pool2d_backward_16(int dtype, const void *grad_out, long long nc, int ih, int iw,
+                                                     int oh, int ow, void *grad_in, pvn3d_stream_t stream) {
+  return with_dtype16(dtype, [&](auto tag) -> int {
+    using T = decltype(tag);
+    if (nc < 0 || ih < 0 || iw < 0 || oh <= 0 || ow <= 0) return PVN3D_ERR_INVALID_ARG;
+    const long long total = nc * ih * iw;
+    if (total == 0) return PVN3D_OK;
+    if (!grad_out || !grad_in) return PVN3D_ERR_INVALID_ARG;
+    if (!psp_sides_supported(ih, iw, oh, ow)) return PVN3D_ERR_UNSUPPORTED;
+    adaptive_avg_pool2d_backward_kernel<T><<<psp_grid(nc, ih * iw), 256, 0, as_stream(stream)>>>(
+        static_cast<const T *>(grad_out), nc, ih, iw, oh, ow, static_cast<T *>(grad_in));
+    return check_launch("adaptive_avg_pool2d_backward_kernel");
+  });
+}
+
+extern "C" int pvn3d_upsample_bilinear2d_backward_16(int dtype, const void *grad_out, long long nc, int ih, int iw,
+                                                     int oh, int ow, int align_corners, double scale_h, double scale_w,
+                                                     void *grad_in, pvn3d_stream_t stream) {
+  return with_dtype16(dtype, [&](auto tag) -> int {
+    using T = decltype(tag);
+    if (nc < 0 || ih < 0 || iw < 0 || oh <= 0 || ow <= 0) return PVN3D_ERR_INVALID_ARG;
+    const long long total = nc * ih * iw;
+    if (total == 0) return PVN3D_OK;
+    if (!grad_out || !grad_in) return PVN3D_ERR_INVALID_ARG;
+    const bool align = align_corners != 0;
+    if (!psp_sides_supported(ih, iw, oh, ow)) return PVN3D_ERR_UNSUPPORTED;
+    upsample_bilinear2d_backward_kernel<T><<<psp_grid(nc, ih * iw), 256, 0, as_stream(stream)>>>(
+        static_cast<const T *>(grad_out), nc, ih, iw, oh, ow, align ? 1 : 0, bilinear_scale(ih, oh, align, scale_h),
+        bilinear_scale(iw, ow, align, scale_w), static_cast<T *>(grad_in));
+    return check_launch("upsample_bilinear2d_backward_kernel");
+  });
 }

@@ -8,6 +8,7 @@
 // searched point set is staged through shared memory (bulk-copied by the TMA engine when
 // alignment allows) and read back as broadcasts, and global accesses are coalesced.
 #include "common.cuh"
+#include "half_io.cuh"
 
 namespace pvn3d {
 namespace {
@@ -140,22 +141,37 @@ ball_query_kernel(const float *__restrict__ new_xyz, const float *__restrict__ x
 
 // ------------------------------------------------------------------------------------------------
 // group_points: out[b,c,j,k] = points[b,c,idx[b,j,k]]            (group_points_gpu.cu:8-28)
-// One thread per (j,k) slot, looping over a slice of channels: idx is read once per slice, the
-// output is written coalesced along the slot axis.
+// One thread per (j,k) slot (kVec = 1), or per two adjacent slots stored as one 4-byte pair (kVec = 2, 16-bit T, an
+// even slot count), looping over a slice of channels: idx is read once per slice, the output is written coalesced
+// along the slot axis.  T = float, __half or __nv_bfloat16: a copy, so every form is bit-exact.
 // ------------------------------------------------------------------------------------------------
-__global__ void group_points_kernel(const float *__restrict__ points, const int *__restrict__ idx,
-                                    int c, int n, int slots, float *__restrict__ out) {
+template <typename T, int kVec>
+__global__ void group_points_kernel(const T *__restrict__ points, const int *__restrict__ idx,
+                                    int c, int n, int slots, T *__restrict__ out) {
   const int b = blockIdx.z;
-  const int s = blockIdx.x * blockDim.x + threadIdx.x;
-  if (s >= slots) return;
-  const int ii = idx[static_cast<size_t>(b) * slots + s];
-  for (int l = blockIdx.y; l < c; l += gridDim.y) {
-    const size_t row = static_cast<size_t>(b) * c + l;
-    stg_stream(out + row * slots + s, __ldg(points + row * n + ii));
+  if constexpr (kVec == 1) {
+    const int s = blockIdx.x * blockDim.x + threadIdx.x;
+    if (s >= slots) return;
+    const int ii = idx[static_cast<size_t>(b) * slots + s];
+    for (int l = blockIdx.y; l < c; l += gridDim.y) {
+      const size_t row = static_cast<size_t>(b) * c + l;
+      stg_stream(out + row * slots + s, __ldg(points + row * n + ii));
+    }
+  } else {
+    const int s = 2 * (blockIdx.x * blockDim.x + threadIdx.x);
+    if (s >= slots) return;
+    const int2 ii = *reinterpret_cast<const int2 *>(idx + static_cast<size_t>(b) * slots + s);
+    for (int l = blockIdx.y; l < c; l += gridDim.y) {
+      const size_t row = static_cast<size_t>(b) * c + l;
+      stg_stream2(out + row * slots + s, __ldg(points + row * n + ii.x), __ldg(points + row * n + ii.y));
+    }
   }
 }
 
-__global__ void group_points_grad_kernel(const float *__restrict__ grad_out,
+// grad_points[b,c,idx[b,s]] += grad_out[b,c,s] with float32 atomics; a 16-bit grad_out is widened on load and the
+// float32 grad_points is the scratch that round_to16_kernel rounds once
+template <typename T>
+__global__ void group_points_grad_kernel(const T *__restrict__ grad_out,
                                          const int *__restrict__ idx, int c, int n, int slots,
                                          float *__restrict__ grad_points) {
   const int b = blockIdx.z;
@@ -164,7 +180,7 @@ __global__ void group_points_grad_kernel(const float *__restrict__ grad_out,
   const int ii = idx[static_cast<size_t>(b) * slots + s];
   for (int l = blockIdx.y; l < c; l += gridDim.y) {
     const size_t row = static_cast<size_t>(b) * c + l;
-    atomicAdd(grad_points + row * n + ii, grad_out[row * slots + s]);  // group_points_gpu.cu:60
+    atomicAdd(grad_points + row * n + ii, to_f32(grad_out[row * slots + s]));  // group_points_gpu.cu:60
   }
 }
 
@@ -770,26 +786,45 @@ __global__ void __launch_bounds__(kBgWarps * 32) ball_grid_kernel(BallGridArgs a
 // three_interpolate: out[b,c,j] = sum_t points[b,c,idx[b,j,t]] * w[b,j,t]   (interpolate_gpu.cu:72-101)
 // contraction as in the reference SASS (oracle/_ref build, interpolate_gpu.o):
 //   t = p2*w2 (FMUL); t = fma(p1,w1,t); out = fma(p3,w3,t)  -- the MIDDLE product is the bare multiply
+// T = __half / __nv_bfloat16: the same float32 sum of the widened features, rounded once; kVec = 2 gives a thread two
+// adjacent points (an even n) and one 4-byte store per channel.
 // ------------------------------------------------------------------------------------------------
-__global__ void three_interpolate_kernel(const float *__restrict__ points,
+template <typename T>
+__device__ __forceinline__ float interp3(const T *row, int i1, int i2, int i3, float w1, float w2, float w3) {
+  return __fmaf_rn(to_f32(__ldg(row + i3)), w3,
+                   __fmaf_rn(to_f32(__ldg(row + i1)), w1, __fmul_rn(to_f32(__ldg(row + i2)), w2)));
+}
+
+template <typename T, int kVec>
+__global__ void three_interpolate_kernel(const T *__restrict__ points,
                                          const int *__restrict__ idx,
                                          const float *__restrict__ weight, int c, int m, int n,
-                                         float *__restrict__ out) {
+                                         T *__restrict__ out) {
   const int b = blockIdx.z;
-  const int j = blockIdx.x * blockDim.x + threadIdx.x;
+  const int j = kVec * (blockIdx.x * blockDim.x + threadIdx.x);
   if (j >= n) return;
   const size_t q = (static_cast<size_t>(b) * n + j) * 3;
   const float w1 = weight[q], w2 = weight[q + 1], w3 = weight[q + 2];
   const int i1 = idx[q], i2 = idx[q + 1], i3 = idx[q + 2];
-  for (int l = blockIdx.y; l < c; l += gridDim.y) {
-    const float *row = points + (static_cast<size_t>(b) * c + l) * m;
-    const float v = __fmaf_rn(__ldg(row + i3), w3,
-                              __fmaf_rn(__ldg(row + i1), w1, __fmul_rn(__ldg(row + i2), w2)));
-    out[(static_cast<size_t>(b) * c + l) * n + j] = v;
+  if constexpr (kVec == 1) {
+    for (int l = blockIdx.y; l < c; l += gridDim.y) {
+      const T *row = points + (static_cast<size_t>(b) * c + l) * m;
+      out[(static_cast<size_t>(b) * c + l) * n + j] = from_f32<T>(interp3(row, i1, i2, i3, w1, w2, w3));
+    }
+  } else {
+    const float v1 = weight[q + 3], v2 = weight[q + 4], v3 = weight[q + 5];
+    const int k1 = idx[q + 3], k2 = idx[q + 4], k3 = idx[q + 5];
+    for (int l = blockIdx.y; l < c; l += gridDim.y) {
+      const T *row = points + (static_cast<size_t>(b) * c + l) * m;
+      st_pair(out + (static_cast<size_t>(b) * c + l) * n + j, from_f32<T>(interp3(row, i1, i2, i3, w1, w2, w3)),
+              from_f32<T>(interp3(row, k1, k2, k3, v1, v2, v3)));
+    }
   }
 }
 
-__global__ void three_interpolate_grad_kernel(const float *__restrict__ grad_out,
+// float32 atomics of fl(g * w) into grad_points (a float32 scratch for a 16-bit grad_out, rounded afterwards)
+template <typename T>
+__global__ void three_interpolate_grad_kernel(const T *__restrict__ grad_out,
                                               const int *__restrict__ idx,
                                               const float *__restrict__ weight, int c, int n, int m,
                                               float *__restrict__ grad_points) {
@@ -800,7 +835,7 @@ __global__ void three_interpolate_grad_kernel(const float *__restrict__ grad_out
   const float w1 = weight[q], w2 = weight[q + 1], w3 = weight[q + 2];
   const int i1 = idx[q], i2 = idx[q + 1], i3 = idx[q + 2];
   for (int l = blockIdx.y; l < c; l += gridDim.y) {
-    const float g = grad_out[(static_cast<size_t>(b) * c + l) * n + j];
+    const float g = to_f32(grad_out[(static_cast<size_t>(b) * c + l) * n + j]);
     float *row = grad_points + (static_cast<size_t>(b) * c + l) * m;
     atomicAdd(row + i1, g * w1);  // interpolate_gpu.cu:139-141
     atomicAdd(row + i2, g * w2);
@@ -971,7 +1006,7 @@ extern "C" int pvn3d_group_points(const float *points, const int *idx, int b, in
   const int slots = static_cast<int>(slots_ll);
   const int gx = ceil_div(slots, 256);
   dim3 grid(gx, channel_slices(c, gx * b), b);
-  group_points_kernel<<<grid, 256, 0, as_stream(stream)>>>(points, idx, c, n, slots, out);
+  group_points_kernel<float, 1><<<grid, 256, 0, as_stream(stream)>>>(points, idx, c, n, slots, out);
   return check_launch("group_points_kernel");
 }
 
@@ -990,7 +1025,7 @@ extern "C" int pvn3d_group_points_grad(const float *grad_out, const int *idx, in
   const int slots = static_cast<int>(slots_ll);
   const int gx = ceil_div(slots, 256);
   dim3 grid(gx, channel_slices(c, gx * b), b);
-  group_points_grad_kernel<<<grid, 256, 0, as_stream(stream)>>>(grad_out, idx, c, n, slots,
+  group_points_grad_kernel<float><<<grid, 256, 0, as_stream(stream)>>>(grad_out, idx, c, n, slots,
                                                                 grad_points);
   return check_launch("group_points_grad_kernel");
 }
@@ -1167,7 +1202,7 @@ extern "C" int pvn3d_three_interpolate(const float *points, const int *idx, cons
   if (b > 65535) return PVN3D_ERR_UNSUPPORTED;
   const int gx = ceil_div(n, 256);
   dim3 grid(gx, channel_slices(c, gx * b), b);
-  three_interpolate_kernel<<<grid, 256, 0, as_stream(stream)>>>(points, idx, weight, c, m, n, out);
+  three_interpolate_kernel<float, 1><<<grid, 256, 0, as_stream(stream)>>>(points, idx, weight, c, m, n, out);
   return check_launch("three_interpolate_kernel");
 }
 
@@ -1184,9 +1219,122 @@ extern "C" int pvn3d_three_interpolate_grad(const float *grad_out, const int *id
   if (n == 0) return PVN3D_OK;
   const int gx = ceil_div(n, 256);
   dim3 grid(gx, channel_slices(c, gx * b), b);
-  three_interpolate_grad_kernel<<<grid, 256, 0, as_stream(stream)>>>(grad_out, idx, weight, c, n, m,
+  three_interpolate_grad_kernel<float><<<grid, 256, 0, as_stream(stream)>>>(grad_out, idx, weight, c, n, m,
                                                                      grad_points);
   return check_launch("three_interpolate_grad_kernel");
+}
+
+// ---- 16-bit forms (torch.autocast): the kernels above on __half / __nv_bfloat16 --------------------------------------
+// the one rounding of a 16-bit atomic grad: scratch [count] f32 -> out [count] 16-bit
+template <typename T>
+static int round_scratch(const float *scratch, long long count, T *out, cudaStream_t st) {
+  const bool pairs = aligned_to(scratch, 8) && aligned_to(out, 4);
+  const long long work = pairs ? (count + 1) / 2 : count;
+  const long long want = (work + 255) / 256, cap = 16ll * sm_count();
+  const unsigned grid = static_cast<unsigned>(want < cap ? want : cap);
+  if (pairs)
+    round_to16_kernel<T, 2><<<grid, 256, 0, st>>>(scratch, count, out);
+  else
+    round_to16_kernel<T, 1><<<grid, 256, 0, st>>>(scratch, count, out);
+  return check_launch("round_to16_kernel");
+}
+
+extern "C" int pvn3d_group_points_16(int dtype, const void *points, const int *idx, int b, int c, int n, int npoints,
+                                     int nsample, void *out, pvn3d_stream_t stream) {
+  return with_dtype16(dtype, [&](auto tag) -> int {
+    using T = decltype(tag);
+    if (!points || !idx || !out || b < 0 || c < 0 || n <= 0 || npoints < 0 || nsample < 0)
+      return PVN3D_ERR_INVALID_ARG;
+    const long long slots_ll = static_cast<long long>(npoints) * nsample;
+    if (b == 0 || c == 0 || slots_ll == 0) return PVN3D_OK;
+    if (b > 65535 || slots_ll > 0x7fffffffll) return PVN3D_ERR_UNSUPPORTED;
+    const int slots = static_cast<int>(slots_ll);
+    const T *src = static_cast<const T *>(points);
+    T *dst = static_cast<T *>(out);
+    if (slots % 2 == 0 && aligned_to(idx, 8) && aligned_to(out, 4)) {
+      const int gx = ceil_div(slots / 2, 256);
+      dim3 grid(gx, channel_slices(c, gx * b), b);
+      group_points_kernel<T, 2><<<grid, 256, 0, as_stream(stream)>>>(src, idx, c, n, slots, dst);
+    } else {
+      const int gx = ceil_div(slots, 256);
+      dim3 grid(gx, channel_slices(c, gx * b), b);
+      group_points_kernel<T, 1><<<grid, 256, 0, as_stream(stream)>>>(src, idx, c, n, slots, dst);
+    }
+    return check_launch("group_points_kernel");
+  });
+}
+
+extern "C" int pvn3d_group_points_grad_16(int dtype, const void *grad_out, const int *idx, int b, int c, int n,
+                                          int npoints, int nsample, float *scratch, void *grad_points,
+                                          pvn3d_stream_t stream) {
+  return with_dtype16(dtype, [&](auto tag) -> int {
+    using T = decltype(tag);
+    if (b < 0 || c < 0 || n <= 0 || npoints < 0 || nsample < 0) return PVN3D_ERR_INVALID_ARG;
+    if (b == 0 || c == 0) return PVN3D_OK;
+    const long long slots_ll = static_cast<long long>(npoints) * nsample;
+    if (!grad_points || (slots_ll > 0 && (!grad_out || !idx || !scratch))) return PVN3D_ERR_INVALID_ARG;
+    if (b > 65535 || slots_ll > 0x7fffffffll) return PVN3D_ERR_UNSUPPORTED;
+    const size_t count = static_cast<size_t>(b) * c * n;
+    cudaStream_t st = as_stream(stream);
+    if (slots_ll == 0) {
+      PVN3D_CUDA_TRY(cudaMemsetAsync(grad_points, 0, sizeof(T) * count, st), "memset");   // +0.0 in both formats
+      return PVN3D_OK;
+    }
+    PVN3D_CUDA_TRY(cudaMemsetAsync(scratch, 0, sizeof(float) * count, st), "memset");
+    const int slots = static_cast<int>(slots_ll);
+    const int gx = ceil_div(slots, 256);
+    dim3 grid(gx, channel_slices(c, gx * b), b);
+    group_points_grad_kernel<T><<<grid, 256, 0, st>>>(static_cast<const T *>(grad_out), idx, c, n, slots, scratch);
+    const int rc = check_launch("group_points_grad_kernel");
+    return rc != PVN3D_OK ? rc : round_scratch(scratch, static_cast<long long>(count), static_cast<T *>(grad_points), st);
+  });
+}
+
+extern "C" int pvn3d_three_interpolate_16(int dtype, const void *points, const int *idx, const float *weight, int b,
+                                          int c, int m, int n, void *out, pvn3d_stream_t stream) {
+  return with_dtype16(dtype, [&](auto tag) -> int {
+    using T = decltype(tag);
+    if (!points || !idx || !weight || !out || b < 0 || c < 0 || m <= 0 || n < 0) return PVN3D_ERR_INVALID_ARG;
+    if (b == 0 || c == 0 || n == 0) return PVN3D_OK;
+    if (b > 65535) return PVN3D_ERR_UNSUPPORTED;
+    const T *src = static_cast<const T *>(points);
+    T *dst = static_cast<T *>(out);
+    if (n % 2 == 0 && aligned_to(out, 4)) {
+      const int gx = ceil_div(n / 2, 256);
+      dim3 grid(gx, channel_slices(c, gx * b), b);
+      three_interpolate_kernel<T, 2><<<grid, 256, 0, as_stream(stream)>>>(src, idx, weight, c, m, n, dst);
+    } else {
+      const int gx = ceil_div(n, 256);
+      dim3 grid(gx, channel_slices(c, gx * b), b);
+      three_interpolate_kernel<T, 1><<<grid, 256, 0, as_stream(stream)>>>(src, idx, weight, c, m, n, dst);
+    }
+    return check_launch("three_interpolate_kernel");
+  });
+}
+
+extern "C" int pvn3d_three_interpolate_grad_16(int dtype, const void *grad_out, const int *idx, const float *weight,
+                                               int b, int c, int n, int m, float *scratch, void *grad_points,
+                                               pvn3d_stream_t stream) {
+  return with_dtype16(dtype, [&](auto tag) -> int {
+    using T = decltype(tag);
+    if (b < 0 || c < 0 || m <= 0 || n < 0) return PVN3D_ERR_INVALID_ARG;
+    if (b == 0 || c == 0) return PVN3D_OK;
+    if (!grad_points || (n > 0 && (!grad_out || !idx || !weight || !scratch))) return PVN3D_ERR_INVALID_ARG;
+    if (b > 65535) return PVN3D_ERR_UNSUPPORTED;
+    const size_t count = static_cast<size_t>(b) * c * m;
+    cudaStream_t st = as_stream(stream);
+    if (n == 0) {
+      PVN3D_CUDA_TRY(cudaMemsetAsync(grad_points, 0, sizeof(T) * count, st), "memset");
+      return PVN3D_OK;
+    }
+    PVN3D_CUDA_TRY(cudaMemsetAsync(scratch, 0, sizeof(float) * count, st), "memset");
+    const int gx = ceil_div(n, 256);
+    dim3 grid(gx, channel_slices(c, gx * b), b);
+    three_interpolate_grad_kernel<T><<<grid, 256, 0, st>>>(static_cast<const T *>(grad_out), idx, weight, c, n, m,
+                                                           scratch);
+    const int rc = check_launch("three_interpolate_grad_kernel");
+    return rc != PVN3D_OK ? rc : round_scratch(scratch, static_cast<long long>(count), static_cast<T *>(grad_points), st);
+  });
 }
 
 static int launch_transpose(const float *src, int b, int rows, int cols, float *dst,

@@ -4,9 +4,10 @@ torch has no deterministic CUDA backward for either op: under torch.use_determin
 `lib/pspnet.py` (nn.AdaptiveAvgPool2d, F.upsample(..., mode='bilinear'), nn.Upsample(scale_factor=2,
 mode='bilinear', align_corners=True)) raises at its first backward.  The autograd functions here run torch's own
 forward, so forward bits never change, and a backward that depends on the mode:
-  * deterministic mode on (warn_only included), a float32 CUDA NCHW gradient: pvn3d_adaptive_avg_pool2d_backward /
-    pvn3d_upsample_bilinear2d_backward (csrc/determinism.cu), which write every input-gradient element once, summing
-    its contributions in ascending output order;
+  * deterministic mode on (warn_only included), a float32, float16 or bfloat16 CUDA NCHW gradient:
+    pvn3d_adaptive_avg_pool2d_backward / pvn3d_upsample_bilinear2d_backward (csrc/determinism.cu; their *_16 forms for
+    the 16-bit gradients of torch.autocast), which write every input-gradient element once, summing its contributions
+    in ascending output order in float32 and rounding a 16-bit result once;
   * otherwise torch's own backward op, as if the module had never been wrapped.
 
 `compat.install(..., patch_deterministic=True)` routes the reference's PSPModule and PSPUpsample through them.
@@ -22,9 +23,17 @@ from torch import nn
 from ._lib import call, ptr
 
 
+_DTYPE16 = {torch.float16: 1, torch.bfloat16: 2}      # PVN3D_F16, PVN3D_BF16 (include/pvn3d_b200.h)
+
+
 def _ordered(g: torch.Tensor) -> bool:
-    return (torch.are_deterministic_algorithms_enabled() and g.is_cuda and g.dtype == torch.float32
-            and g.dim() == 4)
+    return (torch.are_deterministic_algorithms_enabled() and g.is_cuda
+            and (g.dtype == torch.float32 or g.dtype in _DTYPE16) and g.dim() == 4)
+
+
+def _entry(name: str, g: torch.Tensor):
+    """(entry point, leading arguments) of the float32 op or of its 16-bit form"""
+    return (name, ()) if g.dtype == torch.float32 else (name + "_16", (_DTYPE16[g.dtype],))
 
 
 def _pair(v):
@@ -46,7 +55,8 @@ class _AdaptiveAvgPool2d(torch.autograd.Function):
         n, c, oh, ow = g.shape
         ih, iw = x.shape[-2:]
         out = torch.empty((n, c, ih, iw), dtype=g.dtype, device=g.device)
-        call("pvn3d_adaptive_avg_pool2d_backward", g.device, ptr(g), n * c, ih, iw, oh, ow, ptr(out))
+        fn, lead = _entry("pvn3d_adaptive_avg_pool2d_backward", g)
+        call(fn, g.device, *lead, ptr(g), n * c, ih, iw, oh, ow, ptr(out))
         return out, None
 
 
@@ -69,8 +79,9 @@ class _UpsampleBilinear2d(torch.autograd.Function):
         g = g.contiguous()
         n, c, ih, iw = ctx.in_size
         out = torch.empty(ctx.in_size, dtype=g.dtype, device=g.device)
-        call("pvn3d_upsample_bilinear2d_backward", g.device, ptr(g), n * c, ih, iw, oh, ow, int(ctx.align),
-             float(sh or 0.0), float(sw or 0.0), ptr(out))
+        fn, lead = _entry("pvn3d_upsample_bilinear2d_backward", g)
+        call(fn, g.device, *lead, ptr(g), n * c, ih, iw, oh, ow, int(ctx.align), float(sh or 0.0), float(sw or 0.0),
+             ptr(out))
         return out, None, None, None
 
 
