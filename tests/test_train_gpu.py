@@ -114,28 +114,7 @@ def test_targets_k16_and_out_of_range_ids(cuda_dev):
 
 
 def _frames(b, h=480, w=640, seed=0):
-    rng = np.random.default_rng(seed)
-    yy, xx = np.mgrid[0:h, 0:w]
-    depth = np.zeros((b, h, w), np.float32)
-    label = np.zeros((b, h, w), np.int32)
-    for f in range(b):
-        depth[f] = 9000 + 500 * np.sin(xx / (60.0 + f)) + 300 * np.cos(yy / 50.0)
-        for c in (1, 4, 9, 4):
-            y0, x0 = rng.integers(0, h - 120), rng.integers(0, w - 150)
-            label[f, y0:y0 + 120, x0:x0 + 150] = c
-            depth[f, y0:y0 + 120, x0:x0 + 150] -= 500
-    depth[1] = 0
-    depth[1, 100:110, 100:130] = 8000                 # 300 valid pixels: ok = 0
-    K = np.tile(np.float32([[1066.778, 0, 312.9869], [0, 1067.487, 241.3109], [0, 0, 1]]), (b, 1, 1))
-    rgb = rng.integers(0, 256, (b, 3, h, w), dtype=np.uint8)
-    ids = np.zeros((b, 22), np.int64)
-    ids[:, :4] = [1, 4, 9, 4]
-    rts = np.zeros((b, 22, 3, 4))
-    for f in range(b):
-        for i in range(4):
-            q, _ = np.linalg.qr(rng.normal(size=(3, 3)))
-            rts[f, i] = np.concatenate([q, rng.normal(0, 0.2, (3, 1)) + [[0], [0], [0.9]]], 1)
-    return depth, K, np.full(b, 10000.0, np.float32), rgb, label, ids, rts
+    return R.raw_frames(b, h, w, seed, sparse=(1,))       # frame 1: 300 valid pixels, ok = 0
 
 
 def test_train_batch_end_to_end(cuda_dev):

@@ -189,3 +189,33 @@ def pvn3d_loss_ref(kp, seg, ctr, kp_targ, ctr_targ, labels, ok=None, weights=(2.
     r = pvn3d_loss_t(kp, seg, ctr, kp_targ, ctr_targ, labels, ok, weights, gamma)
     return (float(r["loss"]), r["parts"].numpy(), float(r["acc"]), r["d_kp"].numpy(), r["d_seg"].numpy(),
             r["d_ctr"].numpy())
+
+
+def raw_frames(b: int, h: int = 480, w: int = 640, seed: int = 0, sparse=()):
+    """raw frames for train_utils.train_batch: depth (mm) of a curved background with four objects (classes 1, 4, 9, 4)
+    0.5 m in front of it, their label image, a YCB camera, random colours and four poses -> (depth, K, cam_scale, rgb,
+    label, cls_ids, RTs) as numpy arrays.  The frames listed in `sparse` keep only 300 valid depth pixels, too few for
+    get_item (FrameInputBuilder's ok = 0); the random draws do not depend on `sparse`."""
+    rng = np.random.default_rng(seed)
+    yy, xx = np.mgrid[0:h, 0:w]
+    depth = np.zeros((b, h, w), np.float32)
+    label = np.zeros((b, h, w), np.int32)
+    for f in range(b):
+        depth[f] = 9000 + 500 * np.sin(xx / (60.0 + f)) + 300 * np.cos(yy / 50.0)
+        for c in (1, 4, 9, 4):
+            y0, x0 = rng.integers(0, h - 120), rng.integers(0, w - 150)
+            label[f, y0:y0 + 120, x0:x0 + 150] = c
+            depth[f, y0:y0 + 120, x0:x0 + 150] -= 500
+    for f in sparse:
+        depth[f] = 0
+        depth[f, 100:110, 100:130] = 8000
+    K = np.tile(np.float32([[1066.778, 0, 312.9869], [0, 1067.487, 241.3109], [0, 0, 1]]), (b, 1, 1))
+    rgb = rng.integers(0, 256, (b, 3, h, w), dtype=np.uint8)
+    ids = np.zeros((b, 22), np.int64)
+    ids[:, :4] = [1, 4, 9, 4]
+    rts = np.zeros((b, 22, 3, 4))
+    for f in range(b):
+        for i in range(4):
+            q, _ = np.linalg.qr(rng.normal(size=(3, 3)))
+            rts[f, i] = np.concatenate([q, rng.normal(0, 0.2, (3, 1)) + [[0], [0], [0.9]]], 1)
+    return depth, K, np.full(b, 10000.0, np.float32), rgb, label, ids, rts
