@@ -186,6 +186,14 @@ __device__ __forceinline__ void wgmma_tf32<128>(float (&d)[64], uint64_t adesc, 
       : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
       : "l"(adesc), "l"(bdesc), "r"(accumulate));
 }
+// One 32-column K chunk of a SWIZZLE_128B stage: four k8 steps, K = 8 tf32 = 32 bytes apart (+2 in the descriptors'
+// 16-byte units).  `acc`: add to d; otherwise the first step overwrites it.
+template <int N>
+__device__ __forceinline__ void wgmma_chunk_tf32(float (&d)[N / 2], uint64_t adesc, uint64_t bdesc, bool acc) {
+#pragma unroll
+  for (int k4 = 0; k4 < 4; ++k4)
+    wgmma_tf32<N>(d, adesc + static_cast<uint64_t>(k4 * 2), bdesc + static_cast<uint64_t>(k4 * 2), (acc || k4 > 0) ? 1u : 0u);
+}
 // D[64 x N] (+)= A[64 x 16] . B[N x 16]^T with bf16 operands, both K-major (no transpose) in shared memory, fp32
 // accumulate; the same fragment layout as wgmma_tf32.  K = 16 bf16 is 32 bytes, as K = 8 tf32 is.
 template <int N>
@@ -276,6 +284,23 @@ __host__ __device__ constexpr int mma_n(int n_pad) { return n_pad <= 16 ? 16 : n
 // byte offset of 16-byte chunk `c` (0..7) of row `r` inside a [rows x 128 B] SWIZZLE_128B tile
 __device__ __forceinline__ uint32_t sw128_off(int r, int c) {
   return static_cast<uint32_t>(r) * 128u + (static_cast<uint32_t>(c ^ (r & 7)) << 4);
+}
+// byte offset of column c of row frag_row in a K-major SWIZZLE_128B tile stored as K chunks of 32 columns,
+// `chunk_bytes` apart (rows x 128 B each)
+__device__ __forceinline__ uint32_t frag_off(int c, int frag_row, uint32_t chunk_bytes) {
+  return static_cast<uint32_t>(frag_row) * 128u + static_cast<uint32_t>(c >> 5) * chunk_bytes +
+         ((static_cast<uint32_t>(((c & 31) >> 2) ^ (frag_row & 7))) << 4) + (c & 3) * 4u;
+}
+// a lane's fragment values d4[0..3] (columns c, c + 1 of rows frag_row and frag_row + 8) into that tile as
+// tf32(act(value, e)), e = 0 / 1 the column c / c + 1
+template <typename Act>
+__device__ __forceinline__ void sts_frag_tf32(uint32_t tile, uint32_t chunk_bytes, int c, int frag_row, const float *d4, Act act) {
+  const uint32_t off = frag_off(c, frag_row, chunk_bytes);
+  asm volatile("st.shared.v2.f32 [%0], {%1,%2};" ::"r"(tile + off), "f"(to_tf32(act(d4[0], 0))), "f"(to_tf32(act(d4[1], 1)))
+               : "memory");
+  asm volatile("st.shared.v2.f32 [%0], {%1,%2};" ::"r"(tile + off + 8u * 128u), "f"(to_tf32(act(d4[2], 0))),
+               "f"(to_tf32(act(d4[3], 1)))
+               : "memory");
 }
 
 // ---- A-operand producers ---------------------------------------------------------------------------
@@ -456,10 +481,7 @@ __device__ __forceinline__ void mma_tile(uint32_t ring, uint32_t stage_bytes, in
     // this warpgroup's 64 rows of A start 64 x 128 B = 8 KB into the stage (a multiple of the 1 KB swizzle atom)
     const uint64_t adesc = smem_desc_sw128(sa + wg * 8192u), bdesc = smem_desc_sw128(sa + kMlpBM * 128u);
     wgmma_fence();
-#pragma unroll
-    for (int k4 = 0; k4 < 4; ++k4)  // K = 8 tf32 = 32 bytes per instruction: +2 in 16-byte units
-      wgmma_tf32<N>(d, adesc + static_cast<uint64_t>(k4 * 2), bdesc + static_cast<uint64_t>(k4 * 2),
-                    (kc > 0 || k4 > 0) ? 1u : 0u);
+    wgmma_chunk_tf32<N>(d, adesc, bdesc, kc > 0);
     wgmma_commit();
     if (prev >= 0) {
       wgmma_wait<1>();
@@ -1128,9 +1150,7 @@ __device__ __forceinline__ void sa2_layer2(const Sa2Args &g, uint32_t ring, uint
     const uint64_t adesc = smem_desc_sw128(ring + static_cast<uint32_t>(s) * kSa2StageBytes + wg * 8192u);
     const uint64_t bdesc = smem_desc_sw128(w2_s + static_cast<uint32_t>(kc * N2) * 128u);
     wgmma_fence();
-#pragma unroll
-    for (int k4 = 0; k4 < 4; ++k4)
-      wgmma_tf32<N2>(d, adesc + static_cast<uint64_t>(k4 * 2), bdesc + static_cast<uint64_t>(k4 * 2), (kc > 0 || k4 > 0) ? 1u : 0u);
+    wgmma_chunk_tf32<N2>(d, adesc, bdesc, kc > 0);
     wgmma_commit();
     if (prev >= 0) {
       wgmma_wait<1>();
@@ -1153,14 +1173,8 @@ __device__ __forceinline__ void sa2_layer2(const Sa2Args &g, uint32_t ring, uint
   for (int j = 0; j < N2 / 8; ++j) {
     if (8 * j < k3_pad) {
       const int c = 8 * j + 2 * static_cast<int>(lane & 3u);
-      const uint32_t off = static_cast<uint32_t>(c >> 5) * (kMlpBM * 128u) + static_cast<uint32_t>(frag_row) * 128u +
-                           ((static_cast<uint32_t>(((c & 31) >> 2) ^ (frag_row & 7))) << 4) + (c & 3) * 4u;
-      asm volatile("st.shared.v2.f32 [%0], {%1,%2};" ::"r"(h_s + off), "f"(to_tf32(fmaxf(d[4 * j] + bv[j].x, 0.f))),
-                   "f"(to_tf32(fmaxf(d[4 * j + 1] + bv[j].y, 0.f)))
-                   : "memory");
-      asm volatile("st.shared.v2.f32 [%0], {%1,%2};" ::"r"(h_s + off + 8u * 128u), "f"(to_tf32(fmaxf(d[4 * j + 2] + bv[j].x, 0.f))),
-                   "f"(to_tf32(fmaxf(d[4 * j + 3] + bv[j].y, 0.f)))
-                   : "memory");
+      sts_frag_tf32(h_s, kMlpBM * 128u, c, frag_row, d + 4 * j,
+                    [&](float x, int e) { return fmaxf(x + (e ? bv[j].y : bv[j].x), 0.f); });
     }
   }
   fence_proxy_async_smem();   // generic-proxy stores of H -> visible to the tensor core
@@ -1275,9 +1289,7 @@ __global__ void __launch_bounds__(kSa2Threads, 1) mlp_sa_fact2_kernel(const __gr
         const uint64_t adesc = smem_desc_sw128(h_wg + static_cast<uint32_t>(kc) * (kMlpBM * 128u));
         const uint64_t bdesc = smem_desc_sw128(base + L.w3 + static_cast<uint32_t>(kc * N3) * 128u);
         wgmma_fence();
-#pragma unroll
-        for (int k4 = 0; k4 < 4; ++k4)
-          wgmma_tf32<N3>(d, adesc + static_cast<uint64_t>(k4 * 2), bdesc + static_cast<uint64_t>(k4 * 2), (kc > 0 || k4 > 0) ? 1u : 0u);
+        wgmma_chunk_tf32<N3>(d, adesc, bdesc, kc > 0);
         wgmma_commit();
       }
       wgmma_wait<0>();
@@ -1421,6 +1433,22 @@ static inline __host__ __device__ Sa2wSmem sa2w_smem(int k2_pad, int k3_pad, int
 // interleaved -- (2p, 0) (2p+1, 0) (2p, 1) (2p+1, 1) ..; chunk kc of block 2p + q is item kc * cnt + q of the pair.
 __device__ __forceinline__ int sa2w_pair_blocks(int nb, int pp) { return nb - pp < 2 ? nb - pp : 2; }
 
+// The loader warp's lane 0: the weight chunks of one layer (nb column blocks of 128, kcs K chunks, through `map`) by TMA
+// into the ring in that order, each once its stage is free.  `it` counts the ring items across layers and tiles.
+__device__ __forceinline__ void load_weight_blocks(int &it, const CUtensorMap *map, int nb, int kcs, uint32_t base,
+                                                   uint32_t ring, int S, uint64_t *full, uint64_t *empty) {
+  for (int pp = 0; pp < nb; pp += 2) {
+    const int cnt = sa2w_pair_blocks(nb, pp);
+    for (int kc = 0; kc < kcs; ++kc)
+      for (int q = 0; q < cnt; ++q, ++it) {
+        const int s = it % S;
+        mbar_wait(&empty[s], static_cast<unsigned>(((it / S) & 1) ^ 1));
+        mbar_expect_tx(&full[s], kSa2wStageBytes);   // rows past n_pad arrive as zeros and count too
+        tma_load_2d(base + ring + static_cast<uint32_t>(s) * kSa2wStageBytes, map, kc * 32, (pp + q) * 128, &full[s]);
+      }
+  }
+}
+
 // One 64 x 128 block of a layer for the calling warpgroup: K chunks of `a_tile` (64 rows each) x the weight chunks
 // of the ring into registers, each ring stage released once the MMAs that read it have retired -- except the last
 // one with `keep_last`, which the caller releases (returned).  With `a_bars`, K chunk kc of the A tile is waited for
@@ -1440,9 +1468,7 @@ __device__ __forceinline__ int sa2w_block(float (&d)[64], uint32_t a_tile, uint3
     const uint64_t adesc = smem_desc_sw128(a_tile + static_cast<uint32_t>(kc) * kSa2wChunk);
     const uint64_t bdesc = smem_desc_sw128(ring + static_cast<uint32_t>(s) * kSa2wStageBytes);
     wgmma_fence();
-#pragma unroll
-    for (int k4 = 0; k4 < 4; ++k4)
-      wgmma_tf32<128>(d, adesc + static_cast<uint64_t>(k4 * 2), bdesc + static_cast<uint64_t>(k4 * 2), (kc > 0 || k4 > 0) ? 1u : 0u);
+    wgmma_chunk_tf32<128>(d, adesc, bdesc, kc > 0);
     wgmma_commit();
     if (prev >= 0) {
       wgmma_wait<1>();
@@ -1502,23 +1528,10 @@ __global__ void __launch_bounds__(kSa2wThreads, 1) mlp_sa_fact2w_kernel(const __
     // ================= loader: every weight chunk of every tile, in ring order ===============================
     if (lane == 0) {
       int it = 0;
-      for (int tile = blockIdx.x; tile < tiles; tile += gridDim.x) {
-        for (int layer = 0; layer < 2; ++layer) {
-          const CUtensorMap *map = layer ? &g.tmap3 : &a.tmap;
-          const int nb = layer ? nb3 : nb2, kcs = layer ? kc3 : kc2;
-          for (int pp = 0; pp < nb; pp += 2) {
-            const int cnt = sa2w_pair_blocks(nb, pp);
-            for (int kc = 0; kc < kcs; ++kc)
-              for (int q = 0; q < cnt; ++q, ++it) {
-                const int s = it % S;
-                mbar_wait(&ctl.empty[s], static_cast<unsigned>(((it / S) & 1) ^ 1));
-                mbar_expect_tx(&ctl.full[s], kSa2wStageBytes);   // rows past n_pad arrive as zeros and count too
-                tma_load_2d(base + L.ring + static_cast<uint32_t>(s) * kSa2wStageBytes, map, kc * 32, (pp + q) * 128,
-                            &ctl.full[s]);
-              }
-          }
-        }
-      }
+      for (int tile = blockIdx.x; tile < tiles; tile += gridDim.x)
+        for (int layer = 0; layer < 2; ++layer)
+          load_weight_blocks(it, layer ? &g.tmap3 : &a.tmap, layer ? nb3 : nb2, layer ? kc3 : kc2, base, L.ring, S, ctl.full,
+                             ctl.empty);
     }
   } else {
     // ================= MMA + epilogue: warpgroup wg, warp w4 of it holds rows 16 w4 .. +15 of the tile ======
@@ -1754,37 +1767,46 @@ __device__ __forceinline__ int4 lds128i(uint32_t addr) {
   return v;
 }
 
+// three_interpolate of columns k .. k+3 of known_feat for the producer's 8 rows, from their row state in shared memory
+// (fp2_rows_store): fma(p3,w3, fma(p1,w1, p2*w2)) as pn2_ops.cu contracts it, dead rows zero, into the swizzled operand
+// tile at `sa`.  ROUND: TF32-rounded, as an operand is staged; otherwise unrounded.
+template <bool ROUND>
+__device__ __forceinline__ void interp_rows(const MlpArgs &a, int k, uint32_t rst, int r_first, int sub, uint32_t sa) {
+  const float *kf = a.known_feat + k;
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {  // two halves: 12 LDG.128 in flight each
+    float4 p1[4], p2[4], p3[4];
+#pragma unroll
+    for (int jj = 0; jj < 4; ++jj) {
+      const int4 gi = lds128i(rst + 128u * (h * 4 + jj));
+      p1[jj] = ldg128(kf + static_cast<size_t>(gi.x) * a.c2);
+      p2[jj] = ldg128(kf + static_cast<size_t>(gi.y) * a.c2);
+      p3[jj] = ldg128(kf + static_cast<size_t>(gi.z) * a.c2);
+    }
+#pragma unroll
+    for (int jj = 0; jj < 4; ++jj) {
+      const int j = h * 4 + jj;
+      const float4 w = lds128(rst + 128u * j + 16u);
+      float4 v;
+      v.x = __fmaf_rn(p3[jj].x, w.z, __fmaf_rn(p1[jj].x, w.x, __fmul_rn(p2[jj].x, w.y)));
+      v.y = __fmaf_rn(p3[jj].y, w.z, __fmaf_rn(p1[jj].y, w.x, __fmul_rn(p2[jj].y, w.y)));
+      v.z = __fmaf_rn(p3[jj].z, w.z, __fmaf_rn(p1[jj].z, w.x, __fmul_rn(p2[jj].z, w.y)));
+      v.w = __fmaf_rn(p3[jj].w, w.z, __fmaf_rn(p1[jj].w, w.x, __fmul_rn(p2[jj].w, w.y)));
+      if (w.w == 0.f) v = make_float4(0.f, 0.f, 0.f, 0.f);
+      if constexpr (ROUND) sts_tf32(sa + sw128_off(r_first + 4 * j, sub), v);
+      else sts128(sa + sw128_off(r_first + 4 * j, sub), v.x, v.y, v.z, v.w);
+    }
+  }
+}
+
 // K chunk k0 / 32 of the producer's 8 rows of A = [interpolated known | skip | 0], row state from shared memory
-// (fp2_rows_store): three_interpolate's fma(p3,w3, fma(p1,w1, p2*w2)) (pn2_ops.cu), TF32 rounding, dead rows zero
+// (fp2_rows_store), TF32 rounding, dead rows zero
 __device__ __forceinline__ void fp2_stage_chunk(const MlpArgs &a, uint32_t rst, long long p_first, int r_first, int sub,
                                                 int k0, uint32_t sa, bool vec_ok) {
   const int k = k0 + 4 * sub;
   const float4 zero = make_float4(0.f, 0.f, 0.f, 0.f);
   if (vec_ok && k + 4 <= a.c2) {
-    const float *kf = a.known_feat + k;
-#pragma unroll
-    for (int h = 0; h < 2; ++h) {  // two halves: 12 LDG.128 in flight each
-      float4 p1[4], p2[4], p3[4];
-#pragma unroll
-      for (int jj = 0; jj < 4; ++jj) {
-        const int4 gi = lds128i(rst + 128u * (h * 4 + jj));
-        p1[jj] = ldg128(kf + static_cast<size_t>(gi.x) * a.c2);
-        p2[jj] = ldg128(kf + static_cast<size_t>(gi.y) * a.c2);
-        p3[jj] = ldg128(kf + static_cast<size_t>(gi.z) * a.c2);
-      }
-#pragma unroll
-      for (int jj = 0; jj < 4; ++jj) {
-        const int j = h * 4 + jj;
-        const float4 w = lds128(rst + 128u * j + 16u);
-        float4 v;
-        v.x = __fmaf_rn(p3[jj].x, w.z, __fmaf_rn(p1[jj].x, w.x, __fmul_rn(p2[jj].x, w.y)));
-        v.y = __fmaf_rn(p3[jj].y, w.z, __fmaf_rn(p1[jj].y, w.x, __fmul_rn(p2[jj].y, w.y)));
-        v.z = __fmaf_rn(p3[jj].z, w.z, __fmaf_rn(p1[jj].z, w.x, __fmul_rn(p2[jj].z, w.y)));
-        v.w = __fmaf_rn(p3[jj].w, w.z, __fmaf_rn(p1[jj].w, w.x, __fmul_rn(p2[jj].w, w.y)));
-        if (w.w == 0.f) v = zero;
-        sts_tf32(sa + sw128_off(r_first + 4 * j, sub), v);
-      }
-    }
+    interp_rows<true>(a, k, rst, r_first, sub, sa);
     return;
   }
   const bool skip_vec = (a.c2 % 4 == 0) && (a.lds % 4 == 0) && ((reinterpret_cast<uintptr_t>(a.skip) & 15u) == 0);
@@ -1843,9 +1865,7 @@ __device__ __forceinline__ void fp2_layer1_block(float (&d)[64], uint32_t aring,
     const uint64_t adesc = smem_desc_sw128(aring + static_cast<uint32_t>(sa) * kFp2AStageBytes);
     const uint64_t bdesc = smem_desc_sw128(wring + static_cast<uint32_t>(sw) * kFp2WStageBytes);
     wgmma_fence();
-#pragma unroll
-    for (int k4 = 0; k4 < 4; ++k4)
-      wgmma_tf32<128>(d, adesc + static_cast<uint64_t>(k4 * 2), bdesc + static_cast<uint64_t>(k4 * 2), (kc > 0 || k4 > 0) ? 1u : 0u);
+    wgmma_chunk_tf32<128>(d, adesc, bdesc, kc > 0);
     wgmma_commit();
     if (pa >= 0) {
       wgmma_wait<1>();
@@ -1923,23 +1943,10 @@ __global__ void __launch_bounds__(kFp2Threads, 1) mlp_fp2_kernel(const __grid_co
     // ================= loader: every weight chunk of every tile, in ring order ===============================
     if (lane == 0) {
       int it = 0;
-      for (int tile = blockIdx.x; tile < tiles; tile += gridDim.x) {
-        for (int layer = 0; layer < 2; ++layer) {
-          const CUtensorMap *map = layer ? &g.tmap2 : &a.tmap;
-          const int nb = layer ? nb2 : nb1, kcs = layer ? kc2 : kc1;
-          for (int pp = 0; pp < nb; pp += 2) {
-            const int cnt = sa2w_pair_blocks(nb, pp);
-            for (int kc = 0; kc < kcs; ++kc)
-              for (int q = 0; q < cnt; ++q, ++it) {
-                const int s = it % SW;
-                mbar_wait(&ctl.w_empty[s], static_cast<unsigned>(((it / SW) & 1) ^ 1));
-                mbar_expect_tx(&ctl.w_full[s], kFp2WStageBytes);
-                tma_load_2d(base + L.wring + static_cast<uint32_t>(s) * kFp2WStageBytes, map, kc * 32, (pp + q) * 128,
-                            &ctl.w_full[s]);
-              }
-          }
-        }
-      }
+      for (int tile = blockIdx.x; tile < tiles; tile += gridDim.x)
+        for (int layer = 0; layer < 2; ++layer)
+          load_weight_blocks(it, layer ? &g.tmap2 : &a.tmap, layer ? nb2 : nb1, layer ? kc2 : kc1, base, L.wring, SW,
+                             ctl.w_full, ctl.w_empty);
     }
   } else {
     // ================= MMA + epilogues: warpgroup wg, warp w4 of it holds rows 16 w4 .. +15 of the tile ======
@@ -2113,35 +2120,6 @@ int fpf2_stages(int ks_pad, int ns_pad, int k2_pad, int n2_pad) {
   return stages >= 2 ? stages : 0;
 }
 
-// K chunk k0 / 32 of the producer's 8 rows: sum_t w_t P[idx_t] with the contraction of three_interpolate (pn2_ops.cu),
-// fma(p3,w3, fma(p1,w1, p2*w2)), stored unrounded (the MMA warpgroup adds S, applies the ReLU and rounds); dead rows 0
-__device__ __forceinline__ void fpf2_stage_chunk(const MlpArgs &a, uint32_t rst, int r_first, int sub, int k0, uint32_t sa) {
-  const float *kf = a.known_feat + k0 + 4 * sub;
-#pragma unroll
-  for (int h = 0; h < 2; ++h) {  // two halves: 12 LDG.128 in flight each
-    float4 p1[4], p2[4], p3[4];
-#pragma unroll
-    for (int jj = 0; jj < 4; ++jj) {
-      const int4 gi = lds128i(rst + 128u * (h * 4 + jj));
-      p1[jj] = ldg128(kf + static_cast<size_t>(gi.x) * a.c2);
-      p2[jj] = ldg128(kf + static_cast<size_t>(gi.y) * a.c2);
-      p3[jj] = ldg128(kf + static_cast<size_t>(gi.z) * a.c2);
-    }
-#pragma unroll
-    for (int jj = 0; jj < 4; ++jj) {
-      const int j = h * 4 + jj;
-      const float4 w = lds128(rst + 128u * j + 16u);
-      float4 v;
-      v.x = __fmaf_rn(p3[jj].x, w.z, __fmaf_rn(p1[jj].x, w.x, __fmul_rn(p2[jj].x, w.y)));
-      v.y = __fmaf_rn(p3[jj].y, w.z, __fmaf_rn(p1[jj].y, w.x, __fmul_rn(p2[jj].y, w.y)));
-      v.z = __fmaf_rn(p3[jj].z, w.z, __fmaf_rn(p1[jj].z, w.x, __fmul_rn(p2[jj].z, w.y)));
-      v.w = __fmaf_rn(p3[jj].w, w.z, __fmaf_rn(p1[jj].w, w.x, __fmul_rn(p2[jj].w, w.y)));
-      if (w.w == 0.f) v = make_float4(0.f, 0.f, 0.f, 0.f);
-      sts128(sa + sw128_off(r_first + 4 * j, sub), v.x, v.y, v.z, v.w);
-    }
-  }
-}
-
 template <int OUT>
 __global__ void __launch_bounds__(kFpf2Threads, 1) mlp_fp_fact2_kernel(const __grid_constant__ FpFact2Args g) {
   const MlpArgs &a = g.a;
@@ -2183,7 +2161,8 @@ __global__ void __launch_bounds__(kFpf2Threads, 1) mlp_fp_fact2_kernel(const __g
         __syncwarp();
       }
       mbar_wait(&ctl.empty[s], static_cast<unsigned>(((it / S) & 1) ^ 1));
-      fpf2_stage_chunk(a, rst, r_first, sub, kc * 32, base + L.a + static_cast<uint32_t>(s) * kFpf2ABytes + kc * kFpf2AChunk);
+      // unrounded: the MMA warpgroup adds S, applies the ReLU and rounds
+      interp_rows<false>(a, kc * 32 + 4 * sub, rst, r_first, sub, base + L.a + static_cast<uint32_t>(s) * kFpf2ABytes + kc * kFpf2AChunk);
       mbar_arrive(&ctl.a_full[s]);
     }
   } else if (warp == kFpf2LoaderWarp) {
@@ -2218,9 +2197,7 @@ __global__ void __launch_bounds__(kFpf2Threads, 1) mlp_fp_fact2_kernel(const __g
       {
         const uint64_t tdesc = smem_desc_sw128(base + L.t + static_cast<uint32_t>(s) * kFpf2TBytes);
         wgmma_fence();
-#pragma unroll
-        for (int k4 = 0; k4 < 4; ++k4)
-          wgmma_tf32<128>(d, tdesc + static_cast<uint64_t>(k4 * 2), ws_desc + static_cast<uint64_t>(k4 * 2), k4 > 0 ? 1u : 0u);
+        wgmma_chunk_tf32<128>(d, tdesc, ws_desc, false);
         wgmma_commit();
         wgmma_wait<0>();
         acc_fence(d);
@@ -2233,8 +2210,7 @@ __global__ void __launch_bounds__(kFpf2Threads, 1) mlp_fp_fact2_kernel(const __g
       for (int j = 0; j < 16; ++j) {
         const int c = 8 * j + 2 * static_cast<int>(lane & 3u);
         const float b0 = __ldg(g.bias_s + c), b1 = __ldg(g.bias_s + c + 1);
-        const uint32_t off = static_cast<uint32_t>(c >> 5) * kFpf2AChunk + static_cast<uint32_t>(frag_row) * 128u +
-                             ((static_cast<uint32_t>(((c & 31) >> 2) ^ (frag_row & 7))) << 4) + (c & 3) * 4u;
+        const uint32_t off = frag_off(c, frag_row, kFpf2AChunk);
         float x0, x1, y0, y1;
         asm volatile("ld.shared.v2.f32 {%0,%1}, [%2];" : "=f"(x0), "=f"(x1) : "r"(a_s + off));
         asm volatile("ld.shared.v2.f32 {%0,%1}, [%2];" : "=f"(y0), "=f"(y1) : "r"(a_s + off + 8u * 128u));
@@ -2253,9 +2229,7 @@ __global__ void __launch_bounds__(kFpf2Threads, 1) mlp_fp_fact2_kernel(const __g
       for (int kc = 0; kc < 4; ++kc) {
         const uint64_t adesc = smem_desc_sw128(a_s + static_cast<uint32_t>(kc) * kFpf2AChunk);
         const uint64_t bdesc = smem_desc_sw128(base + L.w2 + static_cast<uint32_t>(kc) * 128u * 128u);
-#pragma unroll
-        for (int k4 = 0; k4 < 4; ++k4)
-          wgmma_tf32<128>(d, adesc + static_cast<uint64_t>(k4 * 2), bdesc + static_cast<uint64_t>(k4 * 2), (kc > 0 || k4 > 0) ? 1u : 0u);
+        wgmma_chunk_tf32<128>(d, adesc, bdesc, kc > 0);
       }
       wgmma_commit();
       wgmma_wait<0>();
@@ -2566,9 +2540,7 @@ __global__ void __launch_bounds__(kPspThreads, 1) psp_tail_kernel(const __grid_c
         const uint32_t slot = base + L.ring + static_cast<uint32_t>(s) * kPspStage;
         const uint64_t adesc = smem_desc_sw128(slot + wg * 64u * 128u), bdesc = smem_desc_sw128(slot + kPspAStage);
         wgmma_fence();
-#pragma unroll
-        for (int k4 = 0; k4 < 4; ++k4)
-          wgmma_tf32<64>(d1, adesc + static_cast<uint64_t>(k4 * 2), bdesc + static_cast<uint64_t>(k4 * 2), (kc > 0 || k4 > 0) ? 1u : 0u);
+        wgmma_chunk_tf32<64>(d1, adesc, bdesc, kc > 0);
         wgmma_commit();
         if (prev >= 0) {
           wgmma_wait<1>();
@@ -2605,9 +2577,7 @@ __global__ void __launch_bounds__(kPspThreads, 1) psp_tail_kernel(const __grid_c
       for (int kc = 0; kc < 2; ++kc) {
         const uint64_t adesc = smem_desc_sw128(h_s + static_cast<uint32_t>(kc) * kPspAStage + wg * 64u * 128u);
         const uint64_t bdesc = smem_desc_sw128(base + L.w2 + static_cast<uint32_t>(kc) * kPspN2 * 128u);
-#pragma unroll
-        for (int k4 = 0; k4 < 4; ++k4)
-          wgmma_tf32<128>(d, adesc + static_cast<uint64_t>(k4 * 2), bdesc + static_cast<uint64_t>(k4 * 2), (kc > 0 || k4 > 0) ? 1u : 0u);
+        wgmma_chunk_tf32<128>(d, adesc, bdesc, kc > 0);
       }
       wgmma_commit();
       wgmma_wait<0>();
