@@ -689,6 +689,81 @@ int pvn3d_depth_fill(const float *depth, const float *cam_scale, float scale_2_8
                      float *stages, int *top_rows, void *workspace, size_t workspace_bytes, pvn3d_stream_t stream);
 
 /* ------------------------------------------------------------------------------------------
+ * Training augmentation: get_item's ColorJitter, rgb_add_noise and add_real_back
+ * (ycb_dataset.py:84-177,191-204, linemod_dataset.py:103-188,211-240) from a per-frame record
+ * ---------------------------------------------------------------------------------------- */
+#define PVN3D_AUG_YCB 0
+#define PVN3D_AUG_LINEMOD 1
+/* frame kinds: YCB 0 real, 1 syn; LineMOD 0 real png, 1 render, 2 fuse */
+
+/* One rgb_add_noise pass (80 B).  Only the fields of the pass's dataset are drawn; the others are 0. */
+typedef struct {
+  double s_factor, v_factor; /* HSV S and V factors: YCB U[1.25,1.45], U[1.15,1.35]; LineMOD U[.75,1.25], U[.85,1.15] */
+  double sharpen_w;          /* sharpen centre weight rand*3+9 (YCB)                                             */
+  double sigma;              /* GaussianBlur sigma rand()                                                         */
+  int32_t sharpen;           /* p = 0.2 (YCB)                                                                     */
+  int32_t motion;            /* p = 0.2                                                                           */
+  int32_t angle, length;     /* int(rand*360), int(rand*15)+1                                                     */
+  int32_t gauss;             /* p = 0.2                                                                           */
+  int32_t ksize;             /* 3 (p = 0.8) or 5                                                                  */
+  int32_t noise_sigma;       /* YCB: randint(15) (p = 0.8) else randint(25)                                       */
+  int32_t extra;             /* YCB: the extra sigma-7 noise, p = 0.2                                             */
+  uint64_t noise_key, extra_key; /* Philox keys of the two standard-normal fields                                 */
+} pvn3d_augment_pass_t;
+
+/* The record of one frame (208 B). */
+typedef struct {
+  int32_t kind;                       /* as given to the draw                                                     */
+  int32_t jitter;                     /* ColorJitter runs: every YCB frame, LineMOD real png frames               */
+  int32_t order[4];                   /* torch.randperm(4): 0 brightness, 1 contrast, 2 saturation, 3 hue          */
+  float brightness, contrast, saturation; /* U[0.8, 1.2]                                                          */
+  float hue;                          /* U[-0.05, 0.05]                                                           */
+  int32_t n_pass;                     /* rgb_add_noise passes: 0, or on YCB syn / LineMOD render 1 + (p = 0.2)    */
+  int32_t back;                       /* add_real_back runs after the first pass                                  */
+  pvn3d_augment_pass_t passes[2];
+} pvn3d_augment_params_t;
+
+/* pvn3d_augment_draw: records [B] of the frames kinds[B] (device i32) of `dataset`, from Philox4x32-10 keyed by
+ * seed with frame b's stream at subsequence b: the reference's decision structure and distributions, not its random
+ * streams.  One launch, no host sync. */
+int pvn3d_augment_draw(unsigned long long seed, const int32_t *kinds, int b, int dataset,
+                       pvn3d_augment_params_t *params, pvn3d_stream_t stream);
+
+/* pvn3d_augment_apply: get_item's augmentation of B frames from their records (device), in its order --
+ *   YCB      jitter (RGB); if n_pass: pass 1, add_real_back, [pass 2]
+ *   LineMOD  jitter if record.jitter; flip to BGR; if n_pass: pass 1, add_real_back (background flipped), [pass 2]
+ * A pass is rgb_add_noise: cv2 BGR2HSV 8U (YCB feeds it RGB), S and V times the float64 factors truncated into
+ * uint16 and clipped, HSV2BGR 8U (truncating in cv2's 32-pixel vector loop, rounding in the last W % 32 pixels
+ * of a row, as cv2 4.13's AVX2 dispatch does); [YCB: sharpen filter2D]; [motion blur filter2D]; [GaussianBlur 8U fixed point];
+ * YCB: + N(0,1) * noise_sigma, clip, uint8 truncation; [+ N(0,1) * 7, clip, truncation] -- float32, the normals
+ * from Philox keyed by (key, pixel y*W+x), channel c the c-th of curand_normal4.  The jitter is PIL 12.2's
+ * Image.blend in float32 and RGB<->HSV; every colour conversion, the Gaussian blur and the composite are
+ * bit-exact to cv2 / PIL, filter2D sums its float32 taps in row-major order (cv2 is within 1).
+ * Inputs: rgb [B,H,W,3] u8 RGB, depth [B,H,W] f32, labels [B,H,W] u8 (0 = background), back_rgb [B,H,W,3] u8
+ * RGB, back_labels [B,H,W,back_label_channels] u8 (1 or 3; the reference's mask test per channel), back_depth
+ * [B,H,W] f32.  Outputs: rgb_out [B,3,H,W] u8 (YCB RGB, LineMOD BGR), depth_out [B,H,W] f32.  Optional debug
+ * outputs (NULL to skip): stages [B,12,H,W,3] u8 = after the jitter (and flip), pass 1's hsv, sharpen, motion,
+ * gauss, noise, the composite, pass 2's five (a step that does not run repeats its input); noise [B,2,2,H,W,3] f32
+ * = per pass the noise and extra fields (written where the pass adds them).
+ * Workspace pvn3d_augment_workspace_bytes(b, h, w), 256-B aligned; 0 = unsupported (B*H*W*3 >= 2^31).
+ * 18 launches, no host sync; capturable in a CUDA graph once one call has run on the device. */
+size_t pvn3d_augment_workspace_bytes(int b, int h, int w);
+int pvn3d_augment_apply(const uint8_t *rgb, const float *depth, const uint8_t *labels, const uint8_t *back_rgb,
+                        const uint8_t *back_labels, int back_label_channels, const float *back_depth,
+                        const pvn3d_augment_params_t *params, int b, int h, int w, int dataset, uint8_t *rgb_out,
+                        float *depth_out, uint8_t *stages, float *noise, void *workspace, size_t workspace_bytes,
+                        pvn3d_stream_t stream);
+
+/* pvn3d_augment_probe: the augmentation's building blocks one at a time, for checking them exhaustively.
+ *   op 0..4  colour ops on n u8 triples in -> out: 0 cv2 BGR2HSV, 1 cv2 HSV2BGR, 2 PIL RGB->HSV, 3 PIL HSV->RGB,
+ *            4 PIL convert("L") (one byte out per triple), 7 cv2 HSV2BGR as its per-pixel row tail computes it
+ *   op 5     GaussianBlur's fixed-point taps: in n (double ksize, double sigma) -> out n x 5 i32 (ksize used)
+ *   op 6     the motion-blur line: in n (i32 angle, i32 length) -> out n x 64 i32: a, tap count, then each tap
+ *            row * 256 + col in row-major order
+ * One launch. */
+int pvn3d_augment_probe(int op, const void *in, long long n, void *out, pvn3d_stream_t stream);
+
+/* ------------------------------------------------------------------------------------------
  * Callers either side of the path (SURVEY section 8 f4)
  * ---------------------------------------------------------------------------------------- */
 

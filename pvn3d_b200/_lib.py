@@ -138,7 +138,12 @@ _SIGNATURES = {
                                   _P]),
     "pvn3d_depth_fill_workspace_bytes": (c_size_t, [c_int, c_int, c_int]),
     "pvn3d_depth_fill": (c_int, [_P, _P, c_float, c_int, c_int, c_int, _P, _P, _P, _P, c_size_t, _P]),
-    "pvn3d_train_targets": (c_int, [_P, _P, _P, _P, c_int, c_int, c_int, _P, _P, c_int, c_int, _P, _P, _P, _P, _P]),
+    "pvn3d_augment_draw": (c_int, [ctypes.c_ulonglong, _P, c_int, c_int, _P, _P]),
+    "pvn3d_augment_workspace_bytes": (c_size_t, [c_int, c_int, c_int]),
+    "pvn3d_augment_apply": (c_int, [_P, _P, _P, _P, _P, c_int, _P, _P, c_int, c_int, c_int, c_int, _P, _P, _P, _P, _P,
+                                    c_size_t, _P]),
+    "pvn3d_augment_probe": (c_int, [c_int, _P, ctypes.c_longlong, _P, _P]),
+    "pvn3d_train_targets":(c_int, [_P, _P, _P, _P, c_int, c_int, c_int, _P, _P, c_int, c_int, _P, _P, _P, _P, _P]),
     "pvn3d_train_loss_workspace_bytes": (c_size_t, [ctypes.POINTER(LossArgs)]),
     "pvn3d_train_loss_forward": (c_int, [ctypes.POINTER(LossArgs), _P, _P, _P, _P, _P, _P, c_size_t, _P]),
     "pvn3d_train_loss_backward": (c_int, [ctypes.POINTER(LossArgs), _P, _P, _P, _P, _P, _P, _P, c_size_t, _P]),

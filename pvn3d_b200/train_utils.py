@@ -8,8 +8,8 @@
   * TrainTargets.compute is the target block of get_item (ycb_dataset.py:241-278, linemod_dataset.py:275-310) on the
     sampled cloud: pvn3d_train_targets, one launch.
   * train_batch fixes model_fn's 11-tuple (train_ycb_pvn3d.py:165-166) in one place: FrameInputBuilder.build with the
-    label image, then the targets.  The DataLoader workers keep loading and augmenting on the CPU (CUDA cannot start
-    in forked workers); the main process calls train_batch on the collated batch.
+    label image, then the targets.  The DataLoader workers keep loading and decoding on the CPU (CUDA cannot start
+    in forked workers); the main process augments the collated batch (augment.FrameAugmenter) and calls train_batch.
   * FocalLoss and OFLoss are drop-ins for lib/loss.py with its constructors and forward signatures, PVN3DLoss is
     model_fn's weighted sum of the three terms plus the accuracy; each is one torch.autograd.Function over
     pvn3d_train_loss_forward (two launches) and pvn3d_train_loss_backward (one launch), with no host sync.  They take
