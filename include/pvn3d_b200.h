@@ -907,6 +907,38 @@ int pvn3d_vis_draw_poses(uint8_t *img, int b, int h, int w, const float *mesh_pt
 int pvn3d_vis_draw_p2ds(uint8_t *img, int h, int w, int *p2ds, int n, int r, unsigned color, void *workspace,
                         size_t workspace_bytes, pvn3d_stream_t stream);
 
+/* ---- mesh rasteriser (csrc/render.cu): LineMOD's synthetic render / fuse frames ----------------------------------- */
+
+/* Workspace of pvn3d_render_meshes for b frames of h x w over packed meshes of n_vtx vertices and n_faces faces: the
+ * per-pixel depth keys (b*h*w u64), the snapped vertex records (b*n_vtx x 16 B), the fragment-count scan of the b*n_faces
+ * face slots and its block offsets, 256-byte aligned pieces.  0 = refused sizes (any size < 1, h or w > 4096, b > 65535,
+ * b*n_faces or b*n_vtx >= 2^31).  Host only. */
+size_t pvn3d_render_workspace_bytes(int b, int h, int w, int n_vtx, int n_faces);
+
+/* Rasterise vertex-coloured triangle meshes at per-frame poses into rgb [b,h,w,3] u8, depth [b,h,w] f32 (the pose's
+ * units; metres for LineMOD, cam_scale = 1) and labels [b,h,w] u8 (the visible surface's class id):
+ *   vtx [n_vtx,3] f32, colors [n_vtx,3] u8, faces [n_faces,3] i32 packed vertex indices; vtx_off / face_off [n_cls+1]
+ *   i32, class c owning vertices [vtx_off[c], vtx_off[c+1]) and faces [face_off[c], face_off[c+1]) (faces packed by
+ *   class, then by face index); poses [b,n_cls,3,4] f32 (poses_f64 = 0) or f64 (1); present [b,n_cls] u8; k [b,3,3]
+ *   f64; all on the device.  Class c of frame f is drawn when 1 <= c < n_cls and present[f,c] != 0; class 0 and classes
+ *   without faces draw nothing.
+ * The contract (the header comment of csrc/render.cu has it in full): float64 vertex stage without FMA, q = R p + t,
+ * sx = (fx q0) / q2 + cx, sy = (fy q1) / q2 + cy, so pixel (v, u) samples the ray ((u - cx) / fx, (v - cy) / fy, 1);
+ * snapped to 1/256 px half to even; exact int64 edge functions with a top-left fill rule; perspective-correct 1/z and
+ * colour from those edge functions in float64, depth rounded to f32, colour rint and clamped; the smallest f32 depth
+ * wins, then the lower packed face index.  Triangles are skipped with zero snapped area, a vertex with z < z_near, a
+ * vertex outside +-16384 px, or a vertex index outside the face's class.  Uncovered pixels are 0 in all three outputs,
+ * or take back_rgb [b,h,w,3] u8 and back_depth [b,h,w] f32 (both or neither) with label 0.
+ * Refused: null pointers, n_cls < 2, sizes < 1, z_near not finite and > 0, only one background buffer, an unaligned
+ * workspace (PVN3D_ERR_INVALID_ARG); n_cls > 256, h or w > 4096, sizes pvn3d_render_workspace_bytes refuses
+ * (PVN3D_ERR_UNSUPPORTED); a short workspace (PVN3D_ERR_WORKSPACE).  A memset and five launches, no host sync, no
+ * allocation: it can be captured in a CUDA graph.  Work grows with the faces' clipped bounding-box areas. */
+int pvn3d_render_meshes(const float *vtx, const uint8_t *colors, const int *faces, const int *vtx_off,
+                        const int *face_off, int n_cls, int n_vtx, int n_faces, const void *poses, int poses_f64,
+                        const uint8_t *present, const double *k, int b, int h, int w, double z_near,
+                        const uint8_t *back_rgb, const float *back_depth, uint8_t *rgb, float *depth, uint8_t *labels,
+                        void *workspace, size_t workspace_bytes, pvn3d_stream_t stream);
+
 /* ---- fixed-order backward (csrc/determinism.cu): torch.use_deterministic_algorithms ------------------------------- */
 
 /* Workspace of the three *_grad_ordered calls below for b frames of `slots` index entries into n points (gather: m,

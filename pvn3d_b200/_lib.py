@@ -151,7 +151,10 @@ _SIGNATURES = {
     "pvn3d_vis_draw_poses": (c_int, [_P, c_int, c_int, c_int, _P, _P, c_int, c_int, _P, c_int, _P, _P, c_int, _P,
                                      c_double, _P, c_int, _P, c_size_t, _P]),
     "pvn3d_vis_draw_p2ds": (c_int, [_P, c_int, c_int, _P, c_int, c_int, c_uint, _P, c_size_t, _P]),
-    "pvn3d_ordered_grad_workspace_bytes": (c_size_t, [c_int, c_int, ctypes.c_longlong]),
+    "pvn3d_render_workspace_bytes": (c_size_t, [c_int, c_int, c_int, c_int, c_int]),
+    "pvn3d_render_meshes": (c_int, [_P, _P, _P, _P, _P, c_int, c_int, c_int, _P, c_int, _P, _P, c_int, c_int, c_int,
+                                    c_double, _P, _P, _P, _P, _P, _P, c_size_t, _P]),
+    "pvn3d_ordered_grad_workspace_bytes":(c_size_t, [c_int, c_int, ctypes.c_longlong]),
     "pvn3d_gather_points_grad_ordered": (c_int, [_P, _P, c_int, c_int, c_int, c_int, _P, _P, c_size_t, _P]),
     "pvn3d_group_points_grad_ordered": (c_int, [_P, _P, c_int, c_int, c_int, c_int, c_int, _P, _P, c_size_t, _P]),
     "pvn3d_three_interpolate_grad_ordered": (c_int, [_P, _P, _P, c_int, c_int, c_int, c_int, _P, _P, c_size_t, _P]),

@@ -21,7 +21,7 @@ OBJ = os.path.join(HERE, "_build")
 LIB = os.path.join(HERE, "libpvn3d_b200.so")
 SOURCES = ["runtime.cu", "fps.cu", "pn2_ops.cu", "query_group.cu", "meanshift.cu", "poses.cu", "mlp_tc.cu", "metrics.cu",
            "icp.cu", "flat_meanshift.cu", "normals.cu", "depth_fill.cu", "train.cu",
-           "vis.cu", "determinism.cu", "augment.cu"]
+           "vis.cu", "determinism.cu", "augment.cu", "render.cu"]
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a",
