@@ -30,6 +30,61 @@ def _vertices(vtx, vtx_off, pose_b, k, z_near):
     return sx, sy, ok, iz, q
 
 
+def faces_setup(vtx, faces, vtx_off, face_off, pose_b, present_b, k, h, w, z_near=1e-3, snap=True):
+    """the triangle stage of one frame: the drawn faces that survive the skip rules, in packed order -> dict of fi
+    (packed face ids), tri (packed vertex ids, vertices 1 and 2 swapped where the area was negative), X, Y, area, iz
+    (per vertex), ua, va (the candidate box's first column and row), bw, bh (its width and height, <= 0 when the box
+    misses the frame) and cnt (candidate pixels per face: the kernel's per-slot count)."""
+    n_cls = vtx_off.size - 1
+    cls_f = np.repeat(np.arange(n_cls), np.diff(face_off))
+    sx, sy, ok, iz, _ = _vertices(vtx, vtx_off, pose_b, k, z_near)
+    drawn = (cls_f > 0) & (np.asarray(present_b).reshape(-1)[cls_f] != 0)
+    fi = np.nonzero(drawn)[0]
+    tri = faces[fi].astype(np.int64)
+    lo, hi = vtx_off[cls_f[fi]], vtx_off[cls_f[fi] + 1]
+    inr = ((tri >= lo[:, None]) & (tri < hi[:, None])).all(1)
+    fi, tri = fi[inr], tri[inr]
+    fi, tri = fi[ok[tri].all(1)], tri[ok[tri].all(1)]
+    if snap:
+        X = np.rint(sx[tri] * 256.0).astype(np.int64)
+        Y = np.rint(sy[tri] * 256.0).astype(np.int64)
+    else:
+        X, Y = sx[tri] * 256.0, sy[tri] * 256.0
+    area = (X[:, 1] - X[:, 0]) * (Y[:, 2] - Y[:, 0]) - (Y[:, 1] - Y[:, 0]) * (X[:, 2] - X[:, 0])
+    keep = area != 0
+    fi, tri, X, Y, area = fi[keep], tri[keep], X[keep], Y[keep], area[keep]
+    sw = area < 0
+    for a in (tri, X, Y):
+        a[sw, 1], a[sw, 2] = a[sw, 2].copy(), a[sw, 1].copy()
+    area = np.abs(area)
+    if snap:
+        ua = np.maximum(-((-X.min(1)) >> 8), 0)
+        ub = np.minimum(X.max(1) >> 8, w - 1)
+        va = np.maximum(-((-Y.min(1)) >> 8), 0)
+        vb = np.minimum(Y.max(1) >> 8, h - 1)
+    else:
+        ua = np.maximum(np.ceil(X.min(1) / 256.0), 0).astype(np.int64)
+        ub = np.minimum(np.floor(X.max(1) / 256.0), w - 1).astype(np.int64)
+        va = np.maximum(np.ceil(Y.min(1) / 256.0), 0).astype(np.int64)
+        vb = np.minimum(np.floor(Y.max(1) / 256.0), h - 1).astype(np.int64)
+    bw, bh = ub - ua + 1, vb - va + 1
+    cnt = np.where((bw > 0) & (bh > 0), bw * bh, 0)
+    return dict(fi=fi, tri=tri, X=X, Y=Y, area=area, iz=iz, ua=ua, va=va, bw=bw, bh=bh, cnt=cnt)
+
+
+def slot_counts(vtx, faces, vtx_off, face_off, poses, present, K, h, w, z_near=1e-3):
+    """[B, n_faces] int64: the candidate-pixel count of every (frame, face) slot of the kernel's scan, in slot order
+    (frame-major); undrawn and skipped faces count 0"""
+    poses = np.asarray(poses)
+    b = poses.shape[0]
+    K = np.broadcast_to(np.asarray(K, np.float64), (b, 3, 3))
+    out = np.zeros((b, faces.shape[0]), np.int64)
+    for f in range(b):
+        s = faces_setup(vtx, faces, vtx_off, face_off, poses[f], present[f], K[f], h, w, z_near)
+        out[f, s["fi"]] = s["cnt"]
+    return out
+
+
 def raster(vtx, col, faces, vtx_off, face_off, poses, present, K, h, w, z_near=1e-3, background=None, *,
            centre=0.0, top_left=True, perspective=True, low_wins=True, snap=True, frags=False):
     """-> (rgb [B,h,w,3] u8, depth [B,h,w] f32, labels [B,h,w] u8, face [B,h,w] i64 (-1 = uncovered)); with
@@ -48,38 +103,9 @@ def raster(vtx, col, faces, vtx_off, face_off, poses, present, K, h, w, z_near=1
         depth[:] = background[1]
     all_frags = []
     for f in range(b):
-        sx, sy, ok, iz, _ = _vertices(vtx, vtx_off, poses[f], K[f], z_near)
-        drawn = (cls_f > 0) & (np.asarray(present[f]).reshape(-1)[cls_f] != 0)
-        fi = np.nonzero(drawn)[0]
-        tri = faces[fi].astype(np.int64)
-        lo, hi = vtx_off[cls_f[fi]], vtx_off[cls_f[fi] + 1]
-        inr = ((tri >= lo[:, None]) & (tri < hi[:, None])).all(1)
-        fi, tri = fi[inr], tri[inr]
-        fi, tri = fi[ok[tri].all(1)], tri[ok[tri].all(1)]
-        if snap:
-            X = np.rint(sx[tri] * 256.0).astype(np.int64)
-            Y = np.rint(sy[tri] * 256.0).astype(np.int64)
-        else:
-            X, Y = sx[tri] * 256.0, sy[tri] * 256.0
-        area = (X[:, 1] - X[:, 0]) * (Y[:, 2] - Y[:, 0]) - (Y[:, 1] - Y[:, 0]) * (X[:, 2] - X[:, 0])
-        keep = area != 0
-        fi, tri, X, Y, area = fi[keep], tri[keep], X[keep], Y[keep], area[keep]
-        sw = area < 0
-        for a in (tri, X, Y):
-            a[sw, 1], a[sw, 2] = a[sw, 2].copy(), a[sw, 1].copy()
-        area = np.abs(area)
-        if snap:
-            ua = np.maximum(-((-X.min(1)) >> 8), 0)
-            ub = np.minimum(X.max(1) >> 8, w - 1)
-            va = np.maximum(-((-Y.min(1)) >> 8), 0)
-            vb = np.minimum(Y.max(1) >> 8, h - 1)
-        else:
-            ua = np.maximum(np.ceil(X.min(1) / 256.0), 0).astype(np.int64)
-            ub = np.minimum(np.floor(X.max(1) / 256.0), w - 1).astype(np.int64)
-            va = np.maximum(np.ceil(Y.min(1) / 256.0), 0).astype(np.int64)
-            vb = np.minimum(np.floor(Y.max(1) / 256.0), h - 1).astype(np.int64)
-        bw, bh = ub - ua + 1, vb - va + 1
-        cnt = np.where((bw > 0) & (bh > 0), bw * bh, 0)
+        s = faces_setup(vtx, faces, vtx_off, face_off, poses[f], present[f], K[f], h, w, z_near, snap)
+        fi, tri, X, Y, area, iz = s["fi"], s["tri"], s["X"], s["Y"], s["area"], s["iz"]
+        ua, va, bw, cnt = s["ua"], s["va"], s["bw"], s["cnt"]
         sel = np.repeat(np.arange(fi.size), cnt)
         local = np.arange(sel.size) - np.repeat(np.cumsum(cnt) - cnt, cnt)
         u = ua[sel] + local % bw[sel]
